@@ -240,6 +240,16 @@ int svb_conv1d_run(const float *x_nct_dev, const float *w_host, const float *bia
                    int32_t B, int32_t Cin, int32_t Cout, int32_t T, int32_t K, int32_t dil,
                    int32_t transposed_stride, float in_slope, float out_scale, int32_t precision, int32_t iters,
                    float *y_nct_dev, float *avg_ms, void *stream);
+/* Backward of the same layer (no residual, out_scale 1) through the launchers and argument mappings of the
+ * generator's backward: for y = conv(leaky_relu(x, in_slope)) + bias and dy [B,Cout,T or T*u],
+ *   dw_dev [Cout,Cin,K] (transposed: [Cin,Cout,K]) and db_dev [Cout] are ACCUMULATED (device buffers the caller
+ *   zeroes), dx_nct_dev [B,Cin,T] is written (the leaky-relu derivative of x included).
+ * Stride 1: weight gradient on the wgmma kernel in the tensor-core precisions (split bf16) when the shape allows it,
+ * data gradient = the forward kernel of `precision` on the flipped, transposed weights.  Transposed: fp32 kernels.
+ * w_host as svb_conv1d_run.  Synchronises `stream`. */
+int svb_conv1d_backward_run(const float *x_nct_dev, const float *w_host, const float *dy_nct_dev, int32_t B, int32_t Cin,
+                            int32_t Cout, int32_t T, int32_t K, int32_t dil, int32_t transposed_stride, float in_slope,
+                            int32_t precision, float *dx_nct_dev, float *dw_dev, float *db_dev, void *stream);
 
 /* ---- discriminator-side operators of the vocoder losses (forward; fp32 CUDA cores) ------------ */
 

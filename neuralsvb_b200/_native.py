@@ -136,6 +136,8 @@ _PROTOS = {
                                             ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double)]),
     'svb_conv1d_run': (ctypes.c_int, [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, ctypes.c_float,
                                       ctypes.c_float, _I32, _I32, _P, ctypes.POINTER(ctypes.c_float), _P]),
+    'svb_conv1d_backward_run': (ctypes.c_int, [_P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, ctypes.c_float, _I32,
+                                               _P, _P, _P, _P]),
     'svb_conv_nct_forward': (ctypes.c_int, [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32,
                                             ctypes.c_float, _P]),
     'svb_avgpool1d_4_2_1': (ctypes.c_int, [_P, _P, _I64, _I32, _P]),

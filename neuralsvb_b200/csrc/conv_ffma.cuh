@@ -51,5 +51,10 @@ int launch_conv_post_tanh(const float *x, int B, int C, int T, int Tp, const flo
 // host-side weight packing (layer_api.cu)
 std::vector<float> pack_conv_weights(const float *w, int Cout, int Cin, int K);
 std::vector<float> pack_convT_weights(const float *w, int Cin, int Cout, int K, int u, int pad, int *KS_out);
+// data gradient of a Conv1d with weight [Cout][Cin][K]: the Conv1d over dy with weight Wd[ci][co][K-1-k] = W[co][ci][k],
+// in the FFMA packing [K][Cout][Cin]
+std::vector<float> pack_dgrad_weights(const float *w, int Cout, int Cin, int K);
+// ConvTranspose1d weight [Cin][Cout][K] -> [K][Cout][Cin] (launch_convT_dgrad)
+std::vector<float> pack_convT_dgrad_weights(const float *w, int Cin, int Cout, int K);
 
 }  // namespace svb

@@ -20,13 +20,7 @@ using namespace svb;
 namespace {
 
 int pack_dgrad(svb_gen *g, const HostTensor &w, int C, int K, int dil, ConvLayer *L) {
-    // forward  y[t][co] = sum_k sum_ci W[co][ci][k] x[t + (k - (K-1)/2) dil][ci]
-    // backward dx[t][ci] = sum_k' sum_co W[co][ci][K-1-k'] dy[t + (k' - (K-1)/2) dil][co]   -> a Conv1d with weight Wd[ci][co][k']
-    std::vector<float> wd((size_t)C * C * K);
-    for (int co = 0; co < C; ++co)
-        for (int ci = 0; ci < C; ++ci)
-            for (int k = 0; k < K; ++k) wd[((size_t)ci * C + co) * K + (K - 1 - k)] = w.data[((size_t)co * C + ci) * K + k];
-    const std::vector<float> p = pack_conv_weights(wd.data(), C, C, K);
+    const std::vector<float> p = pack_dgrad_weights(w.data.data(), C, C, K);
     L->Cin = C, L->Cout = C, L->CoutP = C, L->KS = K, L->dil = dil, L->ups_u = 0;
     L->macs_per_row = (double)C * C * K;
     SVB_TRY(gen_upload(g, p, &L->w));
@@ -44,13 +38,8 @@ int bwd_skip() {
 
 int run_dgrad(svb_gen *g, const ConvLayer &L, const float *in, float *out, int Tp, int B, int Tq, cudaStream_t st) {
     if (bwd_skip() & 2) return SVB_OK;
-    ConvArgs a;
-    a.in = in, a.w = L.w, a.bias = L.b, a.res = nullptr, a.out = out;
-    a.B = B, a.Cin = L.Cin, a.in_Tp = Tp, a.Cout = L.Cout, a.out_Tp = Tp, a.CoutP = L.CoutP, a.Tq = Tq;
-    a.KS = L.KS, a.dil = L.dil, a.ups_u = 0, a.in_slope = 1.f, a.out_scale = 1.f, a.accumulate = 0;
     g->bwd_launches += 1;
-    if (g->cfg.precision != SVB_PREC_FP32 && tc_supported(L.tc, a)) return launch_conv_tc(L.tc, a, g->cfg.precision, st);
-    return launch_conv_ffma(a, st);
+    return launch_conv_dgrad(L.w, L.tc, L.b, in, out, B, L.Cin, L.Cout, Tp, Tq, L.KS, L.dil, g->cfg.precision, st);
 }
 
 // ---- device-side re-packing after an optimizer step -----------------------------------------------------------
@@ -87,14 +76,6 @@ int add_copy_job(svb_gen *g, const std::string &src, float *dst, size_t n) {
     return SVB_OK;
 }
 
-std::vector<float> flip_transpose(const std::vector<float> &w, int C, int K) {   // as pack_dgrad
-    std::vector<float> wd((size_t)C * C * K);
-    for (int co = 0; co < C; ++co)
-        for (int ci = 0; ci < C; ++ci)
-            for (int k = 0; k < K; ++k) wd[((size_t)ci * C + co) * K + (K - 1 - k)] = w[((size_t)co * C + ci) * K + k];
-    return wd;
-}
-
 int build_jobs(svb_gen *g) {
     for (void *p : g->job_allocs) cudaFree(p);
     g->job_allocs.clear(), g->jobs.clear();
@@ -112,13 +93,7 @@ int build_jobs(svb_gen *g) {
         SVB_TRY(add_job(g, up + ".weight", s.up.w, pack_convT_weights(iota1((size_t)Cin * C * K).data(), Cin, C, K, u, (K - u) / 2, &KS),
                         &s.up.tc));
         SVB_TRY(add_copy_job(g, up + ".bias", s.up.b, C));
-        {
-            std::vector<float> m((size_t)K * C * Cin);
-            for (int ci = 0; ci < Cin; ++ci)
-                for (int co = 0; co < C; ++co)
-                    for (int k = 0; k < K; ++k) m[((size_t)k * C + co) * Cin + ci] = (float)(((size_t)ci * C + co) * K + k + 1);
-            SVB_TRY(add_job(g, up + ".weight", bs.up_wt, m, nullptr));
-        }
+        SVB_TRY(add_job(g, up + ".weight", bs.up_wt, pack_convT_dgrad_weights(iota1((size_t)Cin * C * K).data(), Cin, C, K), nullptr));
         if (c.use_pitch_embed) {
             const std::string nc = "noise_convs." + std::to_string(i);
             std::vector<float> m((size_t)s.noise.K * C);
@@ -131,7 +106,7 @@ int build_jobs(svb_gen *g) {
             const int rk = c.resblock_kernel_sizes[j];
             const std::vector<float> id = iota1((size_t)C * C * rk);
             const std::vector<float> fw = pack_conv_weights(id.data(), C, C, rk);
-            const std::vector<float> bw = pack_conv_weights(flip_transpose(id, C, rk).data(), C, C, rk);
+            const std::vector<float> bw = pack_dgrad_weights(id.data(), C, C, rk);
             const std::string base = "resblocks." + std::to_string(i * c.n_resblock_kernels + j);
             for (int m = 0; m < c.n_dilations; ++m) {
                 if (c.resblock == 1) {
@@ -223,11 +198,7 @@ int svb::gen_build_bwd_layers(svb_gen *g) {
             const int Cin = s.up.Cin, Cout = s.C, K = c.upsample_kernel_sizes[i];
             const HostTensor *w;
             SVB_TRY(gen_get_w(g, "ups." + std::to_string(i) + ".weight", {Cin, Cout, K}, &w));
-            std::vector<float> wt((size_t)K * Cout * Cin);
-            for (int ci = 0; ci < Cin; ++ci)
-                for (int co = 0; co < Cout; ++co)
-                    for (int k = 0; k < K; ++k) wt[((size_t)k * Cout + co) * Cin + ci] = w->data[((size_t)ci * Cout + co) * K + k];
-            SVB_TRY(gen_upload(g, wt, &bs.up_wt));
+            SVB_TRY(gen_upload(g, pack_convT_dgrad_weights(w->data.data(), Cin, Cout, K), &bs.up_wt));
         }
     }
     {
@@ -387,12 +358,7 @@ extern "C" int svb_gen_backward(svb_gen_t *g, const float *dwav_dev, void *strea
         if (bwd_skip() & 1) return SVB_OK;
         SVB_TRY(need_grad(prefix + ".weight", &dw));
         SVB_TRY(need_grad(prefix + ".bias", &db));
-        WgradArgs a;
-        a.A = x, a.G = gy, a.out = dw, a.B = B, a.Tq = Tq, a.Ca = C_in, a.TpA = Tp, a.Cg = C_out, a.TpG = Tp, a.K = K;
-        a.sa = 1, a.da = dil, a.pa = (K - 1) / 2 * dil, a.sb = 1, a.db = 0, a.pb = 0, a.slope = slope;
-        a.s_co = (long long)C_in * K, a.s_ci = K, a.s_k = 1;
-        a.allow_tc = g->cfg.precision != SVB_PREC_FP32;
-        SVB_TRY(launch_wgrad(a, st));
+        SVB_TRY(launch_wgrad(conv_wgrad_args(x, gy, dw, B, C_in, C_out, Tp, Tq, K, dil, slope, g->cfg.precision != SVB_PREC_FP32), st));
         SVB_TRY(launch_colsum(gy, B, C_out, Tq, Tp, db, st));
         g->bwd_launches += 2;
         return SVB_OK;
@@ -461,11 +427,7 @@ extern "C" int svb_gen_backward(svb_gen_t *g, const float *dwav_dev, void *strea
             float *dw, *db;
             SVB_TRY(need_grad("ups." + std::to_string(i) + ".weight", &dw));
             SVB_TRY(need_grad("ups." + std::to_string(i) + ".bias", &db));
-            WgradArgs a;
-            a.A = xin, a.G = dX, a.out = dw, a.B = B, a.Tq = Tin, a.Ca = Cin, a.TpA = Tin_p, a.Cg = C, a.TpG = Tip, a.K = K;
-            a.sa = 1, a.da = 0, a.pa = 0, a.sb = s.u, a.db = 1, a.pb = pad, a.slope = 0.1f;
-            a.s_ci = (long long)C * K, a.s_co = K, a.s_k = 1;
-            SVB_TRY(launch_wgrad(a, st));
+            SVB_TRY(launch_wgrad(convT_wgrad_args(xin, dX, dw, B, Cin, Tin_p, Tin, C, Tip, K, s.u, pad, 0.1f), st));
             SVB_TRY(launch_colsum(dX, B, C, Ti, Tip, db, st));
         }
         SVB_CUDA(cudaMemsetAsync(dS_next, 0, c4t_floats(B, Cin, Tin) * 4, st));

@@ -204,11 +204,7 @@ extern "C" int svb_tc_layer_create(int32_t Cin, int32_t Cout, int32_t K, int32_t
     // forward: natural [Cout][Ce][KS] -> FFMA packing [KS][Ce][Cout]
     const std::vector<float> pf = pack_conv_weights(id.data(), Cout, Ce, KS);
     // data gradient: a Conv1d with weight Wd[ce][co][KS-1-k] = W[co][ce][k]
-    std::vector<float> wd(n);
-    for (int co = 0; co < Cout; ++co)
-        for (int ce = 0; ce < Ce; ++ce)
-            for (int k = 0; k < KS; ++k) wd[((size_t)ce * Cout + co) * KS + (KS - 1 - k)] = id[((size_t)co * Ce + ce) * KS + k];
-    const std::vector<float> pb = pack_conv_weights(wd.data(), Ce, Cout, KS);
+    const std::vector<float> pb = pack_dgrad_weights(id.data(), Cout, Ce, KS);
     int rc;
     auto setup = [&](ConvLayer &cl, int ci, int co, const std::vector<float> &pk, int **map) -> int {
         cl.Cin = ci, cl.Cout = co, cl.CoutP = co, cl.KS = KS, cl.dil = 1, cl.ups_u = 0, cl.macs_per_row = (double)ci * co * KS;

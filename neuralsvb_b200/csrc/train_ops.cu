@@ -371,6 +371,35 @@ int launch_wgrad(const WgradArgs &a, cudaStream_t st) {
     return SVB_OK;
 }
 
+WgradArgs conv_wgrad_args(const float *x, const float *dy, float *dw, int B, int Cin, int Cout, int Tp, int Tq, int K, int dil,
+                          float slope, bool allow_tc) {
+    WgradArgs a;
+    a.A = x, a.G = dy, a.out = dw, a.B = B, a.Tq = Tq, a.Ca = Cin, a.TpA = Tp, a.Cg = Cout, a.TpG = Tp, a.K = K;
+    a.sa = 1, a.da = dil, a.pa = (K - 1) / 2 * dil, a.sb = 1, a.db = 0, a.pb = 0, a.slope = slope;
+    a.s_co = (long long)Cin * K, a.s_ci = K, a.s_k = 1;
+    a.allow_tc = allow_tc ? 1 : 0;
+    return a;
+}
+
+WgradArgs convT_wgrad_args(const float *x, const float *dy, float *dw, int B, int Cin, int TpIn, int Tin, int Cout, int TpOut, int K,
+                           int u, int pad, float slope) {
+    WgradArgs a;
+    a.A = x, a.G = dy, a.out = dw, a.B = B, a.Tq = Tin, a.Ca = Cin, a.TpA = TpIn, a.Cg = Cout, a.TpG = TpOut, a.K = K;
+    a.sa = 1, a.da = 0, a.pa = 0, a.sb = u, a.db = 1, a.pb = pad, a.slope = slope;
+    a.s_ci = (long long)Cout * K, a.s_co = K, a.s_k = 1;
+    return a;
+}
+
+int launch_conv_dgrad(const float *w, const TcWeights &tc, const float *zero_bias, const float *dy, float *dx, int B, int Cy, int Cx,
+                      int Tp, int Tq, int K, int dil, int precision, cudaStream_t st) {
+    ConvArgs a;
+    a.in = dy, a.w = w, a.bias = zero_bias, a.res = nullptr, a.out = dx;
+    a.B = B, a.Cin = Cy, a.in_Tp = Tp, a.Cout = Cx, a.out_Tp = Tp, a.CoutP = Cx, a.Tq = Tq;
+    a.KS = K, a.dil = dil, a.ups_u = 0, a.in_slope = 1.f, a.out_scale = 1.f, a.accumulate = 0;
+    if (precision != SVB_PREC_FP32 && tc_supported(tc, a)) return launch_conv_tc(tc, a, precision, st);
+    return launch_conv_ffma(a, st);
+}
+
 int launch_colsum(const float *G, int B, int C, int T, int Tp, float *db, cudaStream_t st) {
     const int groups = c4t_groups(C), chunks = (T + 255) / 256;
     const int ns = std::min(B * chunks, std::max(1, 132 * 4 / groups));

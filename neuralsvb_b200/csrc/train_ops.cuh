@@ -1,6 +1,7 @@
 // Backward (training) kernels of the generator on the G32T layout.  See train_ops.cu.
 #pragma once
 #include "common.cuh"
+#include "conv_tc.cuh"
 
 namespace svb {
 
@@ -27,6 +28,21 @@ struct WgradArgs {
 int launch_wgrad(const WgradArgs &a, cudaStream_t st);
 bool wgrad_tc_supported(const WgradArgs &a);
 int launch_wgrad_tc(const WgradArgs &a, cudaStream_t st);
+
+// The gradient mappings of the generator's convolutions, shared by generator_bwd.cu and svb_conv1d_backward_run.
+// Conv1d(Cin, Cout, K, dilation dil, padding dil*(K-1)/2) of leaky_relu(x, slope), weight [Cout][Cin][K]: A = x, G = dy,
+// both G32T with Tp padded / Tq valid rows.  allow_tc: the wgmma kernel may take it (the tensor-core precision modes).
+WgradArgs conv_wgrad_args(const float *x, const float *dy, float *dw, int B, int Cin, int Cout, int Tp, int Tq, int K, int dil,
+                          float slope, bool allow_tc);
+// ConvTranspose1d(Cin, Cout, K, stride u, padding pad) of leaky_relu(x, slope), weight [Cin][Cout][K]: x has Tin valid rows
+// (TpIn padded), dy has Tin * u (TpOut padded).  The strided G runs on the fp32 kernel.
+WgradArgs convT_wgrad_args(const float *x, const float *dy, float *dw, int B, int Cin, int TpIn, int Tin, int Cout, int TpOut, int K,
+                           int u, int pad, float slope);
+// Data gradient of that Conv1d before the leaky-relu mask: the forward kernel over dy (Cy channels) with the weights of
+// pack_dgrad_weights (`w`: FFMA packing, `tc`: its wgmma tiles), writing Cx channels.  On the tensor cores when
+// precision != fp32 and the shape allows it, else on the fp32 CUDA-core kernel.
+int launch_conv_dgrad(const float *w, const TcWeights &tc, const float *zero_bias, const float *dy, float *dx, int B, int Cy, int Cx,
+                      int Tp, int Tq, int K, int dil, int precision, cudaStream_t st);
 
 // db[c] += sum_{b,t<T} G[b][t][c]
 int launch_colsum(const float *G, int B, int C, int T, int Tp, float *db, cudaStream_t st);

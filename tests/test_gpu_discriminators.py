@@ -169,3 +169,53 @@ def test_grouped_polyphase_tc_layers_match_torch(layer, T):
     # and the fp32 CUDA-core kernel agrees (the path USE_TC_GROUPED = False takes)
     got32 = D.conv_nct(x.cuda(), w.cuda(), b.cuda(), k, stride=s, pad=p, groups=g, slope=0.1)
     assert rel(got32, ref) < 2e-5
+
+
+# the dense MPD layers on wgmma (k5 s3 p2: tap-major expansion, wgrad_tc with K = 1, col2im; k5 s1 p2: the generator's
+# kernel as is) with the input lengths a 600-sample column gives along the stack
+DENSE_TC_LAYERS = [(32, 128, 5, 3, 2, 600), (128, 512, 5, 3, 2, 200), (512, 1024, 5, 3, 2, 67), (1024, 1024, 5, 1, 2, 23)]
+
+
+@pytest.mark.parametrize('W', [1, 2, 3, 5, 7, 11, 13])          # 13 > the 11 period columns of one output tile: W slices
+@pytest.mark.parametrize('layer', range(len(DENSE_TC_LAYERS)))
+def test_dense_tc_layers_match_torch(layer, W):
+    """The dense (groups = 1) discriminator layers through svb_tc_layer_create: forward, data / weight / bias gradients
+    against torch fp64 F.conv2d with a (K, 1) kernel over W period columns (F.conv1d for W = 1)."""
+    import torch.nn.functional as F
+    from neuralsvb_b200.modules.hifigan import discriminators as D
+    cin, cout, k, s, p, T = DENSE_TC_LAYERS[layer]
+    assert D.tc_eligible(cin, cout, k, s, 1, p, 1)
+    B = 2
+    gen = torch.Generator().manual_seed(200 + 10 * layer + W)
+    x = torch.randn((B, cin, T) + ((W,) if W > 1 else ()), generator=gen)
+    w = torch.randn(cout, cin, k, generator=gen) * (1.0 / (cin * k) ** 0.5)
+    b = torch.randn(cout, generator=gen) * 0.1
+    xr, wr, br = (t.double().cuda().requires_grad_(True) for t in (x, w, b))
+    if W > 1:
+        ref_lin = F.conv2d(xr, wr[..., None], br, stride=(s, 1), padding=(p, 0))
+    else:
+        ref_lin = F.conv1d(xr, wr, br, stride=s, padding=p)
+    ref = F.leaky_relu(ref_lin, 0.1)
+    cot = torch.randn(ref.shape, generator=gen).cuda()
+    xc, wc, bc = (t.cuda().requires_grad_(True) for t in (x, w, b))
+    got = D.conv_tc(xc, wc, bc, D.TcLayer(), k, s, p, 0.1, W, 1)
+    assert got.shape == ref.shape
+    rel = lambda a, r: (float((a.detach().double() - r.detach()).norm() / r.detach().norm()),
+                        float((a.detach().double() - r.detach()).abs().max() / r.detach().abs().max()))
+    e_y = rel(got, ref)
+    (got * cot).sum().backward()
+    # the reference takes the leaky-relu mask of the CUDA forward (see test_grouped_polyphase_tc_layers_match_torch)
+    mask = torch.where(got.detach() > 0, 1.0, 0.1).double()
+    flips = int((mask != torch.where(ref.detach() > 0, 1.0, 0.1)).sum())
+    assert flips <= 1e-4 * mask.numel(), flips
+    (ref_lin * (cot.double() * mask)).sum().backward()
+    e = {'y': e_y, 'dx': rel(xc.grad, xr.grad), 'dw': rel(wc.grad, wr.grad), 'db': rel(bc.grad, br.grad)}
+    print('MEASURED', DENSE_TC_LAYERS[layer], W, {n: f'{a:.2e}/{b:.2e}' for n, (a, b) in e.items()})
+    bad = {n: v for n, v in e.items() if v[0] > DENSE_TOL[n][0] or v[1] > DENSE_TOL[n][1]}
+    assert not bad, f'{DENSE_TC_LAYERS[layer]} W {W}: (rel L2, rel L-inf) {bad}'
+
+
+# (relative L2, relative L-inf) per tensor, split-bf16 on wgmma (bf16x3, the discriminators' mode): about 5x the worst
+# measured on an H100 80GB HBM3 (400 W power limit) -- y 1.7e-5 / 2.2e-5 and dx 1.8e-5 / 2.1e-5 (both on the 1024 -> 1024
+# layer: 5120 products per output), dw 4.1e-6 / 5.2e-6, db 1.5e-7 / 1.9e-7
+DENSE_TOL = {'y': (9e-5, 1.1e-4), 'dx': (9e-5, 1.1e-4), 'dw': (2.5e-5, 3e-5), 'db': (1e-6, 1e-6)}

@@ -84,6 +84,23 @@ def test_training_entry_points_validate_arguments_without_gpu(built):
     assert l.svb_conv_nct_backward(None, None, None, None, 1, 1, 1, 8, 1, 3, 1, 1, 1, 1, f(0.1), None, None, None, None, None) < 0
     assert l.svb_loss_grad_dev(None, None, 0, f(1.0), None, None, 8, 0, None) < 0
     assert l.svb_cond_net_forward(None, None, None, 1, 80, 8, 512, 256, 128, None, None) < 0
+    # single-layer backward: (x, w, dy, B, Cin, Cout, T, K, dil, u, slope, precision, dx, dw, db, stream); host buffers
+    # stand in for every pointer, the call must refuse before it touches one
+    import numpy as np
+    buf = np.zeros(1 << 16, np.float32)
+    p = ctypes.c_void_p(buf.ctypes.data)
+    bwd = lambda Cin, Cout, K, dil, u, prec, x=p, db=p: l.svb_conv1d_backward_run(x, p, p, 2, Cin, Cout, 16, K, dil, u, f(0.1), prec,
+                                                                                  p, p, db, None)
+    assert bwd(32, 32, 3, 1, 0, 3, x=None) < 0 and b'bad argument' in l.svb_last_error()
+    assert bwd(32, 32, 3, 1, 0, 3, db=None) < 0 and b'bad argument' in l.svb_last_error()
+    assert bwd(32, 32, 3, 1, -1, 3) < 0 and b'bad argument' in l.svb_last_error()
+    assert bwd(32, 32, 3, 1, 0, 4) < 0 and b'bad precision' in l.svb_last_error()
+    assert bwd(30, 32, 3, 1, 0, 0) < 0 and b'multiples of 4' in l.svb_last_error()
+    assert bwd(32, 32, 4, 1, 0, 0) < 0 and b'odd kernel' in l.svb_last_error()
+    assert bwd(32, 32, 3, 0, 0, 0) < 0 and b'odd kernel' in l.svb_last_error()          # dilation 0
+    assert bwd(32, 32, 11, 13, 0, 3) < 0 and b'halo' in l.svb_last_error()             # 5 * 13 = 65 rows > 64
+    assert bwd(32, 32, 4, 0, 8, 0) < 0 and b'transposed kernel' in l.svb_last_error()  # K < u
+    assert bwd(32, 32, 15, 0, 8, 0) < 0 and b'transposed kernel' in l.svb_last_error() # odd K - u
     h = ctypes.c_void_p()
     # 33 -> 64 channels is not a tensor-core shape; a stride-1 layer needs 'same' padding
     assert l.svb_tc_layer_create(33, 64, 5, 1, 2, 3, 0, ctypes.byref(h)) < 0 and b'tensor-core shape' in l.svb_last_error()
