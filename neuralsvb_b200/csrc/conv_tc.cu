@@ -1,20 +1,21 @@
 // wgmma implicit-GEMM 1-D convolution on the G32T activation layout (sm_90a).
 //
-//   D[128 time rows x N columns] (fp32, registers of two warpgroups) += A[128 x K] (smem) * B[K x N] (smem)
+//   D[MT x 128 time rows x N columns] (fp32, registers of two warpgroups) += A[MT x 128 x K] (smem) * B[K x N] (smem)
 //
-// GEMM mapping: M = time (128 rows per CTA tile, 64 per warpgroup), N = output channels (<= 128 per CTA),
-// K = taps x Cin.
+// GEMM mapping: M = time (items of MT = 1 or 2 tiles of 128 rows; math warpgroup w owns the m64 blocks w and w + 2),
+// N = output channels (<= 128 per CTA), K = taps x Cin.  Both blocks of a warpgroup read the same weight tile, so a
+// two-tile item streams each weight tile once per 256 rows.
 // * A operand = the activation slab.  G32T keeps, per 32-channel group, consecutive time steps as
 //   consecutive 128-byte rows, so the [rows x 32 ch] slab is one contiguous span fetched with ONE
 //   cp.async.bulk (TMA) straight into the operand slot.  The transform warps rewrite it IN
 //   PLACE into the MMA operand: leaky-relu pre-activation, hi/lo split (or tf32 rounding) and the
 //   SWIZZLE_128B chunk permutation; one 128-byte K-major row per time step.  A conv tap at
 //   dilation d is a ROW SHIFT of that operand = +128*k*d bytes on the descriptor start address,
-//   so one slab (128 + halo rows) feeds all KS taps of the tile.
+//   so one slab (MT x 128 + halo rows) feeds all KS taps of the item.
 // * B operand = weights, packed and pre-swizzled on the host per (column block, input-channel
 //   chunk, tap), streamed through a ring of bulk copies (or kept resident for narrow layers).
-// * Persistent, warp-specialised: TMA producer warp, 8 operand-transform warps and two math
-//   warpgroups (wgmma into register accumulators, then bias / residual / scale / accumulate ->
+// * Persistent, warp-specialised, three warpgroups: TMA producer warp, 3 operand-transform warps and two
+//   math warpgroups (wgmma into register accumulators, then bias / residual / scale / accumulate ->
 //   G32T stores).  HBM tensors stay exact fp32; rounding happens only on the operand copy in smem.
 // * One launch runs a WORK LIST: items (layer, column block, clip, first row, tiles) in the order
 //   each CTA executes them.  A single layer uses the implicit round-robin list; the generator hands
@@ -25,6 +26,7 @@
 #include <cmath>
 #include <cstring>
 #include <cstdlib>
+#include <type_traits>
 #include <vector>
 
 #include <cuda_bf16.h>
@@ -74,12 +76,13 @@ struct TcArgs {
 
 constexpr int kMaxW = 8;
 constexpr int kMaxDevices = 64;     // per-device caches of function attributes / SM counts
-// Warp roles: warps 0-7 the two math warpgroups (rows 0-63 / 64-127 of the tile), 8-14 operand transform,
-// 15 TMA producer.  16 warps = 4 per SM sub-partition, which leaves 128 registers per thread (a 17th warp would
-// cap them at 96 and spill the N = 128 accumulators).
-constexpr int kTcThreadsP = 512;
-constexpr int kWarpProducer = 15, kWarpTransform0 = 8;
-constexpr int kMathWarps = 8, kTransformWarps = 7;
+// Warp roles, three warpgroups: warp 0 TMA producer, warps 1-3 operand transform, warps 4-11 the two math warpgroups.
+// 12 warps leave 168 registers per thread (65,536 / 384): two m64 blocks of N = 128 fp32 accumulators (128 registers)
+// plus the loop state fit without spilling.  (setmaxnreg 40 / 232 between the roles was tried: ptxas ignores it for
+// this kernel, C7507, and at 48 / 224 it spills.)
+constexpr int kTcThreadsP = 384;
+constexpr int kWarpProducer = 0, kWarpTransform0 = 1, kWarpMath0 = 4;
+constexpr int kMathWarps = 8, kTransformWarps = 3;
 constexpr int kTrRows = kTransformWarps * 32 / 8;   // rows one pass of the transform warps covers (8 lanes per row)
 constexpr int kBiasBytes = 4096;        // bias of the layer(s) (<= 1024 floats; wider layers take 12 KB)
 
@@ -120,8 +123,8 @@ __device__ __forceinline__ void conv_tap_mma(float *d, uint32_t a_row, uint32_t 
     }
 }
 
-// Persistent kernel: one CTA per SM walks its work items (one 128-row tile of one clip for one column block of
-// one layer).  Every stage is decoupled by mbarriers, so the TMA producer runs ahead into the next items and the
+// Persistent kernel: one CTA per SM walks its work items (one or two 128-row tiles of one clip for one column block
+// of one layer).  Every stage is decoupled by mbarriers, so the TMA producer runs ahead into the next items and the
 // transform warps prepare operands while the warpgroups multiply the previous chunk.
 template <int MODE, int N>
 __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __grid_constant__ TcArgs p) {
@@ -159,10 +162,12 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
             if (threadIdx.x == 0) *n_items_s = n;
         } else {                                                     // implicit: groups blockIdx.x, + gridDim.x, ... of layer 0
             const int n = ((int)blockIdx.x < p.total_groups) ? (p.total_groups - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
+            const int tiles = (a.Tq + kTcM - 1) / kTcM;
             for (int i = threadIdx.x; i < n; i += kTcThreadsP) {
                 const int g = blockIdx.x + i * gridDim.x;
                 const int tg = g % p.groups_per_b, r = g / p.groups_per_b;
-                it_w[i] = make_int4(((r / a.B) << 8) | (p.MT << 24), r % a.B, tg * (kTcM * p.MT), 0);
+                const int mt = min(p.MT, tiles - tg * p.MT);          // the last group of a clip with an odd tile count has one
+                it_w[i] = make_int4(((r / a.B) << 8) | (mt << 24), r % a.B, tg * (kTcM * p.MT), 0);
             }
             if (threadIdx.x == 0) *n_items_s = n;
         }
@@ -215,13 +220,13 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
                 }
             }
         }
-    } else if (warp >= kWarpTransform0) {
-        // ====================== operand transform warps (224 threads) =================
+    } else if (warp < kWarpMath0) {
+        // ====================== operand transform warps (96 threads) ==================
         // In place, 8 lanes per 128-byte row (one 16-byte chunk = 4 channels each): conflict-free
         // LDS.128 / STS.128.  Row r, logical chunk j is stored at chunk position j ^ (r & 7)
         // (SWIZZLE_128B).  bf16 mode: lane pairs exchange halves so the even lane writes the
         // 8-channel hi chunk (j = c/2) and the odd lane the lo chunk (4 + c/2).
-        const int tid = threadIdx.x - kWarpTransform0 * 32;     // 0..223
+        const int tid = threadIdx.x - kWarpTransform0 * 32;     // 0..95
         const int cl = tid & 7;                                 // chunk of the row this lane reads
         const bool odd = cl & 1;
         const float slope = a.in_slope;                         // 0 <= slope <= 1: lrelu(x) = max(x, slope * x)
@@ -299,11 +304,12 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
             }
         }
     } else {
-        // ================================ math warpgroups (warps 0-7) =================
-        // Warpgroup wg multiplies rows 64*wg .. 64*wg + 63 of the tile into N / 2 accumulator registers per thread.
-        // The wgmma group of one tap stays in flight while the next is issued; a weight tile / operand slot is
-        // released once the group that read it has completed (wait_group 1).
-        const int wg = warp >> 2;
+        // ================================ math warpgroups (warps 4-11) ================
+        // Warpgroup wg multiplies the m64 blocks wg and wg + 2 of the item (rows 64*wg .. 64*wg + 63 of each tile) into
+        // N / 2 accumulator registers per block and thread.  Both blocks of a tap read the same weight tile.  The wgmma
+        // group of one tap stays in flight while the next is issued; a weight tile / operand slot is released once the
+        // group that read it has completed (wait_group 1).
+        const int wg = (warp - kWarpMath0) >> 2;
         const uint32_t hi = desc_hi_sw128();
         const uint32_t a_lo_plane = (X3 ? p.op_bytes / 2 : 64u) >> 4;      // lo plane / half-row
         const uint32_t b_lo_plane = (X3 ? p.wtile_bytes / 2 : 64u) >> 4;
@@ -311,10 +317,11 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
         // multiple of 16 bytes and the sum stays inside shared memory, so the field cannot overflow)
         const uint32_t op_base = desc_lo(smem_u32(op0)) + (uint32_t)wg * ((64 * 128) >> 4), w_base = desc_lo(smem_u32(wring));
         const uint32_t op_step = p.op_bytes >> 4, wtile_step = p.wtile_bytes >> 4;
+        constexpr uint32_t tile_step = (kTcM * 128) >> 4;                  // the second tile of an item starts 128 rows on
         const int gout = c4t_groups(a.Cout);
         const int r_lo = 64 * wg + 16 * (warp & 3) + (lane >> 2);           // first accumulator row of this thread
         const int c_lo = 2 * (lane & 3);                                    // first accumulator column of this thread
-        float acc[N / 2];
+        float acc0[N / 2], acc1[N / 2];                                     // blocks wg and wg + 2
         int sA = 0, phA = 0, sW = 0, phW = 0;
         int pend_w = -1, pend_a = -1;                                       // slots read by the wgmma group in flight
         auto release = [&]() {
@@ -324,42 +331,9 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
             }
             pend_w = -1, pend_a = -1;
         };
-        if (p.w_resident && n_items > 0) mbar_wait(w_full, 0);
-        for (int n = 0; n < n_items; ++n) {
-            const TcItem it = item_decode(items[n]);
-            const TcLayer &L = Ls[it.layer];
-            const int KS = L.KS;
-            const uint32_t tap_step = (uint32_t)L.dil * (128 >> 4);       // a tap is a row shift of the operand
-            uint32_t scale = 0;                                             // first MMA of the item overwrites
-            for (int c = 0; c < p.n_chunks; ++c) {
-                mbar_wait(a_ready + sA, phA);
-                uint32_t a_tap = op_base + sA * op_step;
-                uint32_t b_tap = w_base + (L.w_res_off >> 4);               // resident tiles (single chunk)
-                for (int k = 0; k < KS; ++k) {
-                    if (!p.w_resident) {
-                        mbar_wait(w_full + sW, phW);
-                        b_tap = w_base + sW * wtile_step;
-                    }
-                    wgmma_fence();
-                    conv_tap_mma<MODE, N>(acc, a_tap, b_tap, a_lo_plane, b_lo_plane, hi, scale);
-                    wgmma_commit();
-                    wgmma_wait<1>();
-                    release();                                              // the previous tap's group has completed
-                    if (!p.w_resident) {
-                        pend_w = sW;
-                        if (++sW == p.nW) sW = 0, phW ^= 1;
-                    }
-                    if (k == KS - 1) pend_a = sA;
-                    scale = 1;
-                    a_tap += tap_step, b_tap += wtile_step;
-                }
-                if (++sA == p.nA) sA = 0, phA ^= 1;
-            }
-            wgmma_wait<0>();
-            wgmma_keep<N>(acc);
-            release();
-            // ---- epilogue straight from the accumulator fragment: each thread owns column pairs of two rows, i.e.
-            // float2 loads / stores; the four threads of a row quad cover one 32-byte sector
+        // ---- epilogue straight from the accumulator fragment of one block (first row `row0` of the item): each thread owns
+        // column pairs of two rows, i.e. float2 loads / stores; the four threads of a row quad cover one 32-byte sector
+        auto epilogue = [&](const TcItem &it, const TcLayer &L, const float *acc, int row0) {
             float *out = L.out;
             const float *res = L.res;
             const float out_scale = L.out_scale;
@@ -367,7 +341,7 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
             const float *bias_s = reinterpret_cast<const float *>(smem + p.off_bias) + L.bias_off;
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-                const int q = it.t0 + r_lo + 8 * h;                         // GEMM row = output time step (before upsampling)
+                const int q = it.t0 + row0 + r_lo + 8 * h;                  // GEMM row = output time step (before upsampling)
                 if (q >= a.Tq) continue;
 #pragma unroll
                 for (int j = 0; j < N / 8; ++j) {
@@ -391,6 +365,52 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
                     *dst = o;
                 }
             }
+        };
+        // one item of one (TWO = false) or two (TWO = true) tiles; per output element the MMAs accumulate in the same
+        // order either way (chunk, tap, then the split terms)
+        auto run_item = [&](auto two, const TcItem &it) {
+            constexpr bool TWO = decltype(two)::value;
+            const TcLayer &L = Ls[it.layer];
+            const int KS = L.KS;
+            const uint32_t tap_step = (uint32_t)L.dil * (128 >> 4);       // a tap is a row shift of the operand
+            uint32_t scale = 0;                                             // first MMA of the item overwrites
+            for (int c = 0; c < p.n_chunks; ++c) {
+                mbar_wait(a_ready + sA, phA);
+                uint32_t a_tap = op_base + sA * op_step;
+                uint32_t b_tap = w_base + (L.w_res_off >> 4);               // resident tiles (single chunk)
+                for (int k = 0; k < KS; ++k) {
+                    if (!p.w_resident) {
+                        mbar_wait(w_full + sW, phW);
+                        b_tap = w_base + sW * wtile_step;
+                    }
+                    wgmma_fence();
+                    conv_tap_mma<MODE, N>(acc0, a_tap, b_tap, a_lo_plane, b_lo_plane, hi, scale);
+                    if (TWO) conv_tap_mma<MODE, N>(acc1, a_tap + tile_step, b_tap, a_lo_plane, b_lo_plane, hi, scale);
+                    wgmma_commit();
+                    wgmma_wait<1>();
+                    release();                                              // the previous tap's group has completed
+                    if (!p.w_resident) {
+                        pend_w = sW;
+                        if (++sW == p.nW) sW = 0, phW ^= 1;
+                    }
+                    if (k == KS - 1) pend_a = sA;
+                    scale = 1;
+                    a_tap += tap_step, b_tap += wtile_step;
+                }
+                if (++sA == p.nA) sA = 0, phA ^= 1;
+            }
+            wgmma_wait<0>();
+            wgmma_keep<N>(acc0);
+            if (TWO) wgmma_keep<N>(acc1);
+            release();
+            epilogue(it, L, acc0, 0);
+            if (TWO) epilogue(it, L, acc1, kTcM);
+        };
+        if (p.w_resident && n_items > 0) mbar_wait(w_full, 0);
+        for (int n = 0; n < n_items; ++n) {
+            const TcItem it = item_decode(items[n]);
+            if (it.mt == 2) run_item(std::true_type(), it);
+            else run_item(std::false_type(), it);
         }
     }
 }
@@ -568,9 +588,11 @@ static int sm_count() {
     return n[slot];
 }
 
-// Shape-class plan of one launch: operand slots, weight ring / residency and the shared-memory carve-up.  `a[0..n)` are layers of the same shape class (channels, rows, upsampling) that may
-// differ in taps / dilation / pointers; slots are sized for the largest halo.
-static int tc_plan(int n, const TcWeights *const *w, const ConvArgs *a, int precision, TcArgs &p, size_t &smem) {
+// Shape-class plan of one launch: tiles per item, operand slots, weight ring / residency and the shared-memory carve-up.
+// `a[0..n)` are layers of the same shape class (channels, rows, upsampling) that may differ in taps / dilation / pointers;
+// slots are sized for the largest halo.  `grid` > 0: the launch runs the implicit round-robin list on that many CTAs;
+// 0: a host-built work list (tc_schedule balances it).
+static int tc_plan(int n, const TcWeights *const *w, const ConvArgs *a, int precision, int grid, TcArgs &p, size_t &smem) {
     SVB_CHECK(n >= 1 && n <= kTcMaxLayers, SVB_ERR_INVALID, "tc conv: %d layers in one launch", n);
     const ConvArgs &a0 = a[0];
     for (int l = 1; l < n; ++l)
@@ -593,37 +615,36 @@ static int tc_plan(int n, const TcWeights *const *w, const ConvArgs *a, int prec
     p.wtile_bytes = (uint32_t)p.n_tile * 128 * planes;
     p.pdl = 1;
     if (const char *e = getenv("SVB_TC_PDL")) p.pdl = atoi(e) != 0;
-    // ---- one 128-row tile per work item: the accumulators of both warpgroups (N / 2 registers per thread) hold
-    // exactly one tile; slabs and the weight ring must fit shared memory.
+    // ---- items of MT tiles: MT = 2 (each weight tile feeds 256 rows; the two math warpgroups hold two m64 blocks each)
+    // when a clip has 2 tiles and the 256-row slabs fit shared memory next to a weight ring of 2 tiles (or the resident
+    // weights), else MT = 1.  Work lists may still carry one-tile items (odd tile counts, balance splits).
     smem = 0;
     const size_t bias_bytes = (size_t)n * a0.Cout <= 1024 ? kBiasBytes : 3 * kBiasBytes;
     SVB_CHECK((size_t)n * a0.Cout * 4 <= bias_bytes, SVB_ERR_INVALID, "tc conv: %d layers x %d biases exceed the shared-memory bias area", n, a0.Cout);
     const size_t budget = 227 * 1024 - bias_bytes;
-    p.MT = 1;
-    {
-        const int R = kTcM + 2 * halo;
-        p.op_bytes = (uint32_t)round_up(R, 8) * 128 * planes;
-        // operand slots double as TMA targets: 3 of them keep two slab copies in flight behind the MMAs
-        p.nA = 3;
-        if (const char *e = getenv("SVB_TC_NA")) p.nA = std::max(2, std::min(4, atoi(e)));
+    // operand slots double as TMA targets: 3 of them keep two slab copies in flight behind the MMAs
+    int nA_pref = 3;
+    if (const char *e = getenv("SVB_TC_NA")) nA_pref = std::max(2, std::min(4, atoi(e)));
+    // narrow layers (one chunk, one column block): every layer's tiles stay resident
+    const size_t res_bytes = (size_t)ks_sum * p.wtile_bytes;
+    const bool can_res = p.n_chunks == 1 && p.col_blocks == 1;
+    auto fit = [&](int mt) {
+        p.MT = mt;
+        p.op_bytes = (uint32_t)round_up(mt * kTcM + 2 * halo, 8) * 128 * planes;
         p.off_op = 1024 + kItemBytes;
-        // narrow layers (one chunk, one column block): every layer's tiles stay resident
-        const size_t res_bytes = (size_t)ks_sum * p.wtile_bytes;
-        const bool can_res = p.n_chunks == 1 && p.col_blocks == 1;
         p.w_resident = 0;
-        for (int nA : {p.nA, 2}) {
+        for (int nA : {nA_pref, 2}) {
             if (can_res && p.off_op + (size_t)nA * p.op_bytes + res_bytes <= budget) {
                 p.nA = nA, p.w_resident = 1;
                 break;
             }
         }
-        p.off_w = p.off_op + (uint32_t)p.nA * p.op_bytes;
-        if (!p.w_resident && p.off_w + 2 * (size_t)p.wtile_bytes > budget) {
-            p.nA = 2;
-            p.off_w = p.off_op + (uint32_t)p.nA * p.op_bytes;
+        if (!p.w_resident) {
+            p.nA = nA_pref;
+            if (p.off_op + (size_t)p.nA * p.op_bytes + 2 * (size_t)p.wtile_bytes > budget) p.nA = 2;
+            if (p.off_op + (size_t)p.nA * p.op_bytes + (size_t)(mt == 2 ? 2 : 1) * p.wtile_bytes > budget) return false;
         }
-        SVB_CHECK(p.w_resident || p.off_w + (size_t)p.wtile_bytes <= budget, SVB_ERR_INVALID,
-                  "tc conv: tile does not fit shared memory (N %d)", p.n_tile);
+        p.off_w = p.off_op + (uint32_t)p.nA * p.op_bytes;
         const size_t avail = budget - p.off_w;
         size_t w_area;
         if (p.w_resident) {
@@ -634,7 +655,16 @@ static int tc_plan(int n, const TcWeights *const *w, const ConvArgs *a, int prec
         }
         p.off_bias = p.off_w + (uint32_t)round_up((int)w_area, 1024);
         smem = (size_t)p.off_bias + bias_bytes;
+        return true;
+    };
+    bool two = tiles >= 2 && fit(2);
+    if (two && grid > 0) {
+        // implicit round-robin list over `grid` CTAs: keep MT = 2 only if its makespan (in tiles) is no longer
+        const long long per = (long long)a0.B * (a0.CoutP / p.n_tile);
+        const long long g1 = per * tiles, g2 = per * ((tiles + 1) / 2);
+        two = 2 * ((g2 + grid - 1) / grid) <= (g1 + grid - 1) / grid;
     }
+    if (!two) SVB_CHECK(fit(1), SVB_ERR_INVALID, "tc conv: tile does not fit shared memory (N %d)", p.n_tile);
     SVB_CHECK(smem <= 227 * 1024, SVB_ERR_INVALID, "tc conv: no tiling fits (N %d, %d layers)", p.n_tile, n);
     uint32_t res_off = 0;
     for (int l = 0; l < n; ++l) {
@@ -647,8 +677,8 @@ static int tc_plan(int n, const TcWeights *const *w, const ConvArgs *a, int prec
     }
     for (int l = n; l < kTcMaxLayers; ++l) p.L[l] = p.L[0];
     if (getenv("SVB_TC_VERBOSE"))
-        fprintf(stderr, "[tc] %d layer(s) Cin %d CoutP %d KS %d.. halo %d Tq %d | n_tile %d nA %d nW %d resident %d smem %zu\n", n,
-                a0.Cin, a0.CoutP, a0.KS, halo, a0.Tq, p.n_tile, p.nA, p.nW, p.w_resident, smem);
+        fprintf(stderr, "[tc] %d layer(s) Cin %d CoutP %d KS %d.. halo %d Tq %d | n_tile %d MT %d nA %d nW %d resident %d smem %zu\n", n,
+                a0.Cin, a0.CoutP, a0.KS, halo, a0.Tq, p.n_tile, p.MT, p.nA, p.nW, p.w_resident, smem);
     p.groups_per_b = (tiles + p.MT - 1) / p.MT;
     p.total_groups = p.groups_per_b * a0.B * p.col_blocks;
     return SVB_OK;
@@ -678,8 +708,9 @@ int launch_conv_tc(const TcWeights &w, const ConvArgs &a, int precision, cudaStr
     TcArgs p;
     size_t smem = 0;
     const TcWeights *wp = &w;
-    SVB_TRY(tc_plan(1, &wp, &a, precision, p, smem));
-    const int grid = std::min(p.total_groups, max_ctas > 0 ? std::min(max_ctas, sm_count()) : sm_count());
+    const int ctas = max_ctas > 0 ? std::min(max_ctas, sm_count()) : sm_count();
+    SVB_TRY(tc_plan(1, &wp, &a, precision, ctas, p, smem));
+    const int grid = std::min(p.total_groups, ctas);
     if ((p.total_groups + grid - 1) / grid > kMaxItems) {
         // more items per CTA than the shared-memory list holds: run the batch in slices of clips
         const int per_b = p.groups_per_b * p.col_blocks;
@@ -698,9 +729,10 @@ int launch_conv_tc(const TcWeights &w, const ConvArgs &a, int precision, cudaStr
     return tc_dispatch(p, precision, grid, smem, st);
 }
 
-// whether `n` layers of this shape class fit one merged launch: the per-CTA item list lives in shared memory
+// whether `n` layers of this shape class fit one merged launch: the per-CTA item list lives in shared memory.  Counted
+// in one-tile items: the plan may pick MT = 1, and tc_schedule may split two-tile units back into one-tile items.
 bool tc_merge_fits(int n, int B, int Tq, int Cout, int n_tile) {
-    const int tiles = (Tq + kTcM - 1) / kTcM, groups = tiles * B * std::max(1, Cout / std::max(1, n_tile));   // one tile per item
+    const int tiles = (Tq + kTcM - 1) / kTcM, groups = tiles * B * std::max(1, Cout / std::max(1, n_tile));
     return (long long)groups * n <= (long long)(kMaxItems * 8 / 10) * sm_count();
 }
 
@@ -738,11 +770,13 @@ int tc_schedule(int n, const int *KS, const int *has_res, const int *accum, int 
                     for (int l = 0; l < n; ++l) units.push_back({unit_cost(l, mt), nblk, b, t * kTcM, mt, l});
                 }
             }
-    // longest processing time first onto the least-loaded CTA.  SVB_TC_SPLIT=1: when the units are too coarse for the
-    // SMs (a few per CTA), split the cheapest two-tile units into one-tile halves and redo the schedule.
+    // longest processing time first onto the least-loaded CTA.  When the units are too coarse for the SMs (balance below
+    // 0.95, e.g. a few two-tile units per CTA), split the cheapest two-tile units into one-tile halves and redo the
+    // schedule; a split is kept only if it improves the balance.
     std::vector<double> load;
-    std::vector<std::vector<int>> mine;
-    double balance = 0;
+    std::vector<std::vector<int>> mine, best_mine;
+    std::vector<Unit> best_units;
+    double balance = -1;
     for (int round = 0; round < 4; ++round) {
         std::stable_sort(units.begin(), units.end(), [](const Unit &x, const Unit &y) { return x.cost > y.cost; });
         load.assign(grid, 0.0);
@@ -756,8 +790,10 @@ int tc_schedule(int n, const int *KS, const int *has_res, const int *accum, int 
         }
         double mx = 0, sum = 0;
         for (double v : load) mx = std::max(mx, v), sum += v;
-        balance = sum / grid / mx;
-        if (balance >= 0.95 || !getenv("SVB_TC_SPLIT")) break;
+        const double bal = sum / grid / mx;
+        if (bal <= balance) break;
+        balance = bal, best_units = units, best_mine = mine;
+        if (balance >= 0.95) break;
         // split up to `grid` of the cheapest two-tile units (they sit at the end of the sorted list)
         int split = 0;
         for (size_t u = units.size(); u-- > 0 && split < grid;) {
@@ -771,6 +807,7 @@ int tc_schedule(int n, const int *KS, const int *has_res, const int *accum, int 
         }
         if (!split) break;
     }
+    units.swap(best_units), mine.swap(best_mine);
     std::vector<int4> &items = *items_out;
     std::vector<int> &off = *off_out;
     items.clear();
@@ -821,7 +858,7 @@ int tc_schedule(int n, const int *KS, const int *has_res, const int *accum, int 
 int tc_worklist_build(int n, const TcWeights *const *w, const ConvArgs *a, int precision, bool chain_ordered, TcWorkList *out) {
     TcArgs p;
     size_t smem = 0;
-    SVB_TRY(tc_plan(n, w, a, precision, p, smem));
+    SVB_TRY(tc_plan(n, w, a, precision, 0, p, smem));
     const int grid = sm_count();
     int KS[kTcMaxLayers], has_res[kTcMaxLayers], accum[kTcMaxLayers];
     for (int l = 0; l < n; ++l) KS[l] = a[l].KS, has_res[l] = a[l].res != nullptr, accum[l] = a[l].accumulate;
@@ -844,7 +881,7 @@ int launch_conv_tc_multi(int n, const TcWeights *const *w, const ConvArgs *a, in
     SVB_CHECK(precision >= SVB_PREC_TF32 && precision <= SVB_PREC_BF16X3, SVB_ERR_INVALID, "tc conv: bad precision %d", precision);
     TcArgs p;
     size_t smem = 0;
-    SVB_TRY(tc_plan(n, w, a, precision, p, smem));
+    SVB_TRY(tc_plan(n, w, a, precision, 0, p, smem));
     SVB_CHECK(wl.items && wl.n_layers == n && wl.MT == p.MT && wl.grid == sm_count(), SVB_ERR_STATE,
               "tc conv: work list was built for another plan (layers %d / %d, MT %d / %d)", wl.n_layers, n, wl.MT, p.MT);
     p.work = wl.items, p.work_off = wl.off;
