@@ -312,6 +312,7 @@ extern "C" int svb_cond_net_backward(const float *mel_dev, const float *dy_dev, 
     SVB_CHECK(mel_dev && dy_dev && dw_dev && db_dev && B > 0 && C > 0 && T > 0 && K > 0 && stride > 0 && pad >= 0, SVB_ERR_INVALID,
               "cond_net_backward: bad argument");
     const long long Tout = (long long)(T - 1) * stride - 2 * pad + K;
+    SVB_CHECK(Tout > 0, SVB_ERR_INVALID, "cond_net_backward: empty output");
     cond_net_bwd_kernel<<<C, 256, 0, as_stream(stream)>>>(mel_dev, dy_dev, B, C, T, K, stride, pad, Tout, dw_dev, db_dev);
     SVB_CUDA(cudaGetLastError());
     return SVB_OK;
@@ -382,6 +383,10 @@ extern "C" int svb_conv_nct_backward(const float *x_dev, const float *w_dev, con
                   stride > 0 && dil > 0 && groups > 0 && Cin % groups == 0 && Cout % groups == 0 && pad >= 0,
               SVB_ERR_INVALID, "conv_nct_backward: bad argument");
     SVB_CHECK(out_slope == 1.f || y_dev, SVB_ERR_INVALID, "conv_nct_backward: the activation mask needs the forward output");
+    // every reject before the first launch: a refused call leaves dz, dx, dw and db untouched
+    SVB_CHECK(!dx_dev || stride <= 4, SVB_ERR_INVALID, "conv_nct_backward: stride %d unsupported", stride);
+    SVB_CHECK(!dw_dev || K == 1 || K == 3 || K == 5 || K == 7 || K == 15 || K == 41, SVB_ERR_INVALID,
+              "conv_nct_backward: kernel size %d has no weight-gradient instance", K);
     cudaStream_t st = as_stream(stream);
     GBwdArgs a;
     a.x = x_dev, a.w = w_dev, a.dz = dz_scratch_dev, a.dx = dx_dev, a.dw = dw_dev;
@@ -390,10 +395,7 @@ extern "C" int svb_conv_nct_backward(const float *x_dev, const float *w_dev, con
     SVB_CHECK(a.Tout > 0, SVB_ERR_INVALID, "conv_nct_backward: empty output");
     mask_bias_kernel<<<dim3(Cout, B), 256, 0, st>>>(dy_dev, out_slope == 1.f ? nullptr : y_dev, out_slope, B, Cout,
                                                      (long long)a.Tout * W, dz_scratch_dev, db_dev);
-    if (dx_dev) {
-        SVB_CHECK(stride <= 4, SVB_ERR_INVALID, "conv_nct_backward: stride %d unsupported", stride);
-        SVB_TRY(launch_dgrad(a, st));
-    }
+    if (dx_dev) SVB_TRY(launch_dgrad(a, st));
     if (dw_dev) {
         switch (K) {
             case 1: SVB_TRY(launch_wgrad_k<1>(a, st)); break;
@@ -401,8 +403,7 @@ extern "C" int svb_conv_nct_backward(const float *x_dev, const float *w_dev, con
             case 5: SVB_TRY(launch_wgrad_k<5>(a, st)); break;
             case 7: SVB_TRY(launch_wgrad_k<7>(a, st)); break;
             case 15: SVB_TRY(launch_wgrad_k<15>(a, st)); break;
-            case 41: SVB_TRY(launch_wgrad_k<41>(a, st)); break;
-            default: SVB_CHECK(false, SVB_ERR_INVALID, "conv_nct_backward: kernel size %d has no weight-gradient instance", K);
+            default: SVB_TRY(launch_wgrad_k<41>(a, st)); break;     // K == 41: the only instance left after the check above
         }
     }
     SVB_CUDA(cudaGetLastError());

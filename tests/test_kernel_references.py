@@ -1,0 +1,72 @@
+"""CPU: the float64 references of the kernel-level GPU tests (tests/test_gpu_stft_kernels.py, test_gpu_disc_kernels.py)
+against the oracle (oracle/hifigan.py, oracle/frontend.py), which is pinned to the reference fixtures.  A wrong reference
+would let a wrong kernel pass its test; here it fails without a GPU."""
+import numpy as np
+import torch
+
+from neuralsvb_b200.utils import synthetic as S
+from oracle import frontend as FE
+from oracle import hifigan as O
+from tests import test_gpu_disc_kernels as D
+from tests import test_gpu_stft_kernels as T
+
+
+def _rel(a, b):
+    a, b = torch.as_tensor(a).double(), torch.as_tensor(b).double()
+    return float((a - b).abs().max() / b.abs().max())
+
+
+def test_stft_reference_matches_the_oracle_mel_spectrogram_stft_and_wav2spec():
+    hp = S.hifigan_config()
+    y = T.make_wave(2, 8192, 'oracle', 'loud')                # clamp_input matters: samples beyond +-1
+    # mel loss: clamp, half reflect pad, hann(win), sqrt(|X|^2 + 1e-9), fmin 80 / fmax 7600 basis, ln(clamp(1e-5))
+    cfg = (hp['fft_size'], hp['hop_size'], hp['win_size'], T.HALF, T.LN_MEL, 1, 80, 0, 1e-5)
+    ref, _ = T.stft_reference(y, cfg, T.make_basis('loss80', hp['fft_size'], 80))
+    assert _rel(ref, O.mel_spectrogram(y, hp)) < 1e-5
+    # MR-STFT magnitude: torch.stft defaults (centre, reflect), sqrt(clamp(|X|^2, 1e-7)), frames-major
+    x = T.make_wave(2, 8192, 'oracle-mag')
+    ref, _ = T.stft_reference(x, (1024, 120, 600, T.REFLECT, T.MAG, 0, 0, 1, 1e-7), None)
+    assert _rel(ref, O.stft_mag(x, 1024, 120, 600)) < 1e-5
+    # wav2spec: librosa.stft(centre, zero pad) -> |.| -> mel -> log10(max(eps, .))
+    cfg = (hp['fft_size'], hp['hop_size'], hp['win_size'], T.ZERO, T.LOG10_MEL, 0, 80, 1, 1e-10)
+    ref, _ = T.stft_reference(x[:1], cfg, T.make_basis('loss80', hp['fft_size'], 80))
+    _, mel = FE.wav2spec(x[0].numpy(), hp)
+    assert _rel(ref[0], mel) < 1e-5
+
+
+def test_cond_net_reference_matches_the_oracle():
+    g = torch.Generator().manual_seed(5)
+    t = 128
+    mel = torch.randn(2, 80, 7, generator=g, dtype=torch.float64)
+    x = torch.randn(2, 1, 7 * t, generator=g, dtype=torch.float64)
+    w = {'d.cond_net.weight': torch.randn(80, 1, 2 * t, generator=g, dtype=torch.float64),
+         'd.cond_net.bias': torch.randn(1, generator=g, dtype=torch.float64)}
+    ref = D.cond_net_reference(mel, w['d.cond_net.weight'], w['d.cond_net.bias'], t)
+    assert torch.equal(O._cond(x, w, 'd', mel)[:, :1], ref)
+
+
+def _grad(f, a):
+    a = a.clone().requires_grad_(True)
+    f(a).backward()
+    return a.grad
+
+
+def test_loss_gradient_references_match_the_oracle_losses(monkeypatch):
+    """Each svb_loss_grad kind, at the scale its call site passes, is the gradient of the oracle loss it replaces."""
+    g = torch.Generator().manual_seed(9)
+    n = 1000
+    a = torch.exp(torch.randn(n, generator=g, dtype=torch.float64))
+    b = torch.exp(torch.randn(n, generator=g, dtype=torch.float64))
+    b[::7] = a[::7]                                            # ties: sign(0) = 0 on both sides
+    kind = lambda k, scale, b_=b: _grad(lambda t: D.loss_expr(k, t, b_, scale), a)
+    # feature_loss (2 * mean |r - g|, w.r.t. g), generator_loss, discriminator_loss (real / generated terms)
+    assert _rel(kind(0, 2 / n), _grad(lambda t: O.feature_loss([[b]], [[t]]), a)) < 1e-12
+    assert _rel(kind(1, 2 / n), _grad(lambda t: O.generator_loss([t]), a)) < 1e-12
+    assert _rel(kind(1, 2 / n), _grad(lambda t: O.discriminator_loss([t], [b])[0], a)) < 1e-12
+    assert _rel(kind(2, 2 / n), _grad(lambda t: O.discriminator_loss([b], [t])[1], a)) < 1e-12
+    # the STFT losses on given magnitudes: spectral convergence (kind 3) and log-magnitude L1 (kind 4), w.r.t. the prediction
+    monkeypatch.setattr(O, 'stft_mag', lambda x, *args: x)
+    sc_scale = float(1 / ((b - a).norm() * b.norm()))
+    assert _rel(kind(3, sc_scale), _grad(lambda t: O.stft_loss(t, b, 0, 0, 0)[0], a)) < 1e-12
+    assert _rel(kind(4, 1 / n), _grad(lambda t: O.stft_loss(t, b, 0, 0, 0)[1], a)) < 1e-12
+    assert (kind(4, 1 / n)[::7] == 0).all() and (kind(0, 1.0)[::7] == 0).all()

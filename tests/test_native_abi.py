@@ -101,6 +101,15 @@ def test_training_entry_points_validate_arguments_without_gpu(built):
     assert bwd(32, 32, 11, 13, 0, 3) < 0 and b'halo' in l.svb_last_error()             # 5 * 13 = 65 rows > 64
     assert bwd(32, 32, 4, 0, 8, 0) < 0 and b'transposed kernel' in l.svb_last_error()  # K < u
     assert bwd(32, 32, 15, 0, 8, 0) < 0 and b'transposed kernel' in l.svb_last_error() # odd K - u
+    # discriminator conv backward: (x, w, y, dy, B, Cin, Cout, Tin, W, K, stride, dil, pad, groups, slope, dz, dx, dw, db, stream);
+    # every reject comes before the first launch, so dz / dx / dw / db are never written
+    nct = lambda K, stride, dx=p, dw=p: l.svb_conv_nct_backward(p, p, p, p, 1, 4, 4, 64, 1, K, stride, 1, 0, 1, f(0.1), p, dx, dw, p, None)
+    assert nct(3, 5) < 0 and b'stride 5 unsupported' in l.svb_last_error()
+    assert nct(9, 1) < 0 and b'kernel size 9 has no weight-gradient instance' in l.svb_last_error()
+    assert nct(9, 5, dw=None) < 0 and b'stride 5 unsupported' in l.svb_last_error()
+    assert nct(9, 5, dx=None) < 0 and b'kernel size 9' in l.svb_last_error()
+    # cond_net backward with an empty output: (T - 1) * stride - 2 * pad + K = 0
+    assert l.svb_cond_net_backward(p, p, 1, 80, 1, 2, 1, 1, p, p, None) < 0 and b'empty output' in l.svb_last_error()
     h = ctypes.c_void_p()
     # 33 -> 64 channels is not a tensor-core shape; a stride-1 layer needs 'same' padding
     assert l.svb_tc_layer_create(33, 64, 5, 1, 2, 3, 0, ctypes.byref(h)) < 0 and b'tensor-core shape' in l.svb_last_error()
