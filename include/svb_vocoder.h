@@ -363,6 +363,33 @@ int svb_fvae_decoder_create(int32_t latent_channels, int32_t hidden_channels, in
                             int32_t gin_channels, int32_t stride, int32_t precision, int32_t device, svb_wn_t **out);
 int svb_fvae_decoder_forward(svb_wn_t *w, const float *z_dev, const float *mask_dev, const float *g_dev, int32_t B, int32_t T,
                              float *out_dev, void *stream);
+/* Training of a WN / decoder handle (replaces torch autograd through fs2_vae.py:62-94 / :147-152).
+ *   svb_wn_set_training(w, 1): builds the data-gradient packings, one gradient buffer per folded tensor (the names of
+ *     svb_wn_set_weight) and a device copy of every folded tensor; set_training(w, 0) keeps them (eval forwards between steps).
+ *   The tape is CALLER-OWNED, one per call, so several training forwards may run before their backwards:
+ *     svb_wn_tape_bytes(w, B, T) is its size (-1 on a bad argument); svb_wn_forward_train / svb_fvae_decoder_forward_train
+ *     compute what svb_wn_forward / svb_fvae_decoder_forward compute (bit for bit) and fill the tape;
+ *     svb_wn_backward / svb_fvae_decoder_backward(w, tape, B, T, dout, ...) read it back.  B and T must be those of the
+ *     forward that wrote the tape.  dx [B, H, T] / dz [B, latent, T / stride] / dg [B, gin, T] are written (each may be NULL;
+ *     dg needs a conditioned forward); the weight / bias gradients ACCUMULATE (svb_wn_zero_grad clears them).
+ *   svb_wn_get_grad copies one gradient to a device buffer of exactly svb_wn_grad_numel(w, name) floats.
+ *   After an optimizer step: svb_wn_set_weight_dev(w, name, folded tensor) for the changed tensors, then
+ *     svb_wn_update_weights_dev(w) rebuilds every packing (forward, data-gradient twins, wgmma tiles) on the device. */
+int svb_wn_set_training(svb_wn_t *w, int32_t on);
+int64_t svb_wn_tape_bytes(const svb_wn_t *w, int32_t B, int32_t T);
+int svb_wn_forward_train(svb_wn_t *w, const float *x_dev, const float *mask_dev, const float *g_dev, int32_t B, int32_t T,
+                         float *out_dev, void *tape_dev, void *stream);
+int svb_fvae_decoder_forward_train(svb_wn_t *w, const float *z_dev, const float *mask_dev, const float *g_dev, int32_t B, int32_t T,
+                                   float *out_dev, void *tape_dev, void *stream);
+int svb_wn_backward(svb_wn_t *w, const void *tape_dev, int32_t B, int32_t T, const float *dout_dev, float *dx_dev, float *dg_dev,
+                    void *stream);
+int svb_fvae_decoder_backward(svb_wn_t *w, const void *tape_dev, int32_t B, int32_t T, const float *dout_dev, float *dz_dev,
+                              float *dg_dev, void *stream);
+int svb_wn_zero_grad(svb_wn_t *w, void *stream);
+int64_t svb_wn_grad_numel(const svb_wn_t *w, const char *name);
+int svb_wn_get_grad(svb_wn_t *w, const char *name, float *dst_dev, int64_t n, void *stream);
+int svb_wn_set_weight_dev(svb_wn_t *w, const char *name, const float *src_dev, int64_t n, void *stream);
+int svb_wn_update_weights_dev(svb_wn_t *w, void *stream);
 
 /* ---- PPG extractor (VCASR, modules/voice_conversion/vc_modules.py:56-80) pieces that are not convolutions, on [B, C, T] tensors.
  * nn.LayerNorm(C) of EncoderLayer (modules/fastspeech/conformer/layers.py:167-178): statistics over the channel axis per (b, t). */

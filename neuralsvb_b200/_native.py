@@ -159,6 +159,17 @@ _PROTOS = {
     'svb_wn_forward': (ctypes.c_int, [_P, _P, _P, _P, _I32, _I32, _P, _P]),
     'svb_fvae_decoder_create': (ctypes.c_int, [_I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, ctypes.POINTER(_P)]),
     'svb_fvae_decoder_forward': (ctypes.c_int, [_P, _P, _P, _P, _I32, _I32, _P, _P]),
+    'svb_wn_set_training': (ctypes.c_int, [_P, _I32]),
+    'svb_wn_tape_bytes': (_I64, [_P, _I32, _I32]),
+    'svb_wn_forward_train': (ctypes.c_int, [_P, _P, _P, _P, _I32, _I32, _P, _P, _P]),
+    'svb_fvae_decoder_forward_train': (ctypes.c_int, [_P, _P, _P, _P, _I32, _I32, _P, _P, _P]),
+    'svb_wn_backward': (ctypes.c_int, [_P, _P, _I32, _I32, _P, _P, _P, _P]),
+    'svb_fvae_decoder_backward': (ctypes.c_int, [_P, _P, _I32, _I32, _P, _P, _P, _P]),
+    'svb_wn_zero_grad': (ctypes.c_int, [_P, _P]),
+    'svb_wn_grad_numel': (_I64, [_P, ctypes.c_char_p]),
+    'svb_wn_get_grad': (ctypes.c_int, [_P, ctypes.c_char_p, _P, _I64, _P]),
+    'svb_wn_set_weight_dev': (ctypes.c_int, [_P, ctypes.c_char_p, _P, _I64, _P]),
+    'svb_wn_update_weights_dev': (ctypes.c_int, [_P, _P]),
     'svb_tc_schedule_probe': (_I64, [_I32, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _I64, _P, ctypes.POINTER(ctypes.c_double)]),
     'svb_layer_norm_nct': (ctypes.c_int, [_P, _P, _P, _I32, _I32, _I32, ctypes.c_float, _P, _P]),
     'svb_relpos_attention_nct': (ctypes.c_int, [_P, _P, _P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _P, _P]),

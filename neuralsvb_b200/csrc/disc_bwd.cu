@@ -385,7 +385,7 @@ extern "C" int svb_conv_nct_backward(const float *x_dev, const float *w_dev, con
     SVB_CHECK(out_slope == 1.f || y_dev, SVB_ERR_INVALID, "conv_nct_backward: the activation mask needs the forward output");
     // every reject before the first launch: a refused call leaves dz, dx, dw and db untouched
     SVB_CHECK(!dx_dev || stride <= 4, SVB_ERR_INVALID, "conv_nct_backward: stride %d unsupported", stride);
-    SVB_CHECK(!dw_dev || K == 1 || K == 3 || K == 5 || K == 7 || K == 15 || K == 41, SVB_ERR_INVALID,
+    SVB_CHECK(!dw_dev || K == 1 || K == 3 || K == 5 || K == 7 || K == 8 || K == 15 || K == 41, SVB_ERR_INVALID,
               "conv_nct_backward: kernel size %d has no weight-gradient instance", K);
     cudaStream_t st = as_stream(stream);
     GBwdArgs a;
@@ -402,6 +402,7 @@ extern "C" int svb_conv_nct_backward(const float *x_dev, const float *w_dev, con
             case 3: SVB_TRY(launch_wgrad_k<3>(a, st)); break;
             case 5: SVB_TRY(launch_wgrad_k<5>(a, st)); break;
             case 7: SVB_TRY(launch_wgrad_k<7>(a, st)); break;
+            case 8: SVB_TRY(launch_wgrad_k<8>(a, st)); break;       // the GlobalFVAE's pre_net / g_pre_net (k 8, stride 4)
             case 15: SVB_TRY(launch_wgrad_k<15>(a, st)); break;
             default: SVB_TRY(launch_wgrad_k<41>(a, st)); break;     // K == 41: the only instance left after the check above
         }

@@ -42,29 +42,12 @@ int run_dgrad(svb_gen *g, const ConvLayer &L, const float *in, float *out, int T
     return launch_conv_dgrad(L.w, L.tc, L.b, in, out, B, L.Cin, L.Cout, Tp, Tq, L.KS, L.dil, g->cfg.precision, st);
 }
 
-// ---- device-side re-packing after an optimizer step -----------------------------------------------------------
-// Every packed array is a permutation (with zeros) of one folded tensor, so the host packers are run ONCE on an
-// index tensor (values i + 1, exact in fp32 up to 2^24 elements) and the result is kept as a gather map.
-__global__ void gather_kernel(float *__restrict__ dst, const float *__restrict__ nat, const int *__restrict__ idx, size_t n) {
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-        dst[i] = idx ? (idx[i] ? nat[idx[i] - 1] : 0.f) : nat[i];
-}
-
-std::vector<float> iota1(size_t n) {
-    std::vector<float> v(n);
-    for (size_t i = 0; i < n; ++i) v[i] = (float)(i + 1);
-    return v;
-}
-
+// ---- device-side re-packing after an optimizer step (gather maps, train_ops.cuh) ----------------------------------
 int add_job(svb_gen *g, const std::string &src, float *dst, const std::vector<float> &coded, const TcWeights *tc) {
-    std::vector<int> idx(coded.size());
-    for (size_t i = 0; i < coded.size(); ++i) idx[i] = (int)coded[i];
     int *d = nullptr;
-    SVB_CUDA(cudaMalloc((void **)&d, std::max<size_t>(idx.size(), 1) * sizeof(int)));
-    g->job_allocs.push_back(d);
-    SVB_CUDA(cudaMemcpy(d, idx.data(), idx.size() * sizeof(int), cudaMemcpyHostToDevice));
+    SVB_TRY(upload_gather_map(coded, &g->job_allocs, &d));
     PackJob j;
-    j.src = src, j.dst = dst, j.idx = d, j.n = idx.size(), j.tc = (tc && tc->ok) ? tc : nullptr;
+    j.src = src, j.dst = dst, j.idx = d, j.n = coded.size(), j.tc = (tc && tc->ok) ? tc : nullptr;
     g->jobs.push_back(j);
     return SVB_OK;
 }
@@ -281,8 +264,7 @@ extern "C" int svb_gen_update_weights_dev(svb_gen_t *g, void *stream) {
     for (const PackJob &j : g->jobs) {
         GradBuf *b;
         SVB_TRY(nat_buffer(g, j.src, &b));
-        const int blocks = (int)std::min<size_t>((j.n + 255) / 256, 132 * 8);
-        gather_kernel<<<blocks, 256, 0, st>>>(j.dst, b->p, j.idx, j.n);
+        SVB_TRY(launch_gather(j.dst, b->p, j.idx, j.n, st));
         if (j.tc) SVB_TRY(tc_repack_weights_dev(j.dst, *j.tc, st));
     }
     SVB_CUDA(cudaGetLastError());

@@ -101,11 +101,6 @@ __global__ void __launch_bounds__(256) col2im_to_nctw_kernel(const float *__rest
     dx[(((size_t)b * C + c) * T) * W + e] = acc;
 }
 
-__global__ void gather_w_kernel(float *__restrict__ dst, const float *__restrict__ nat, const int *__restrict__ idx, size_t n) {
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-        dst[i] = idx[i] ? nat[idx[i] - 1] : 0.f;
-}
-
 // one scratch arena per device, shared by every layer handle.  Contract (include/svb_vocoder.h, "ownership / threading"): the
 // svb_tc_layer_* calls of one device are issued from ONE host thread on ONE stream -- the arena is reused by consecutive calls in
 // stream order and is not guarded against concurrent streams; the mutex below only keeps a (re)allocation from racing with another
@@ -133,8 +128,6 @@ int arena_get(int device, size_t bytes, char **out) {
     *out = a.p;
     return SVB_OK;
 }
-
-int blocks_for(long long total) { return (int)std::min<long long>((total + 255) / 256, 132 * 32); }
 
 void launch_expand(const float *x, const float *mask, float slope, int B, int C, int T, int W, int KE, int s, int p, int Tq, int Tp,
                    float *out, cudaStream_t st) {
@@ -327,9 +320,9 @@ extern "C" int svb_tc_layer_set_weight_dev(svb_tc_layer_t *L, const float *w_dev
     SVB_CHECK(L && w_dev && bias_dev, SVB_ERR_INVALID, "tc_layer_set_weight: null argument");
     SVB_CUDA(cudaSetDevice(L->device));
     cudaStream_t st = as_stream(stream);
-    gather_w_kernel<<<blocks_for((long long)L->n_f), 256, 0, st>>>(L->fwd.w, w_dev, L->map_f, L->n_f);
+    SVB_TRY(launch_gather(L->fwd.w, w_dev, L->map_f, L->n_f, st));
     SVB_TRY(tc_repack_weights_dev(L->fwd.w, L->fwd.tc, st));
-    gather_w_kernel<<<blocks_for((long long)L->n_b), 256, 0, st>>>(L->bwd.w, w_dev, L->map_b, L->n_b);
+    SVB_TRY(launch_gather(L->bwd.w, w_dev, L->map_b, L->n_b, st));
     SVB_TRY(tc_repack_weights_dev(L->bwd.w, L->bwd.tc, st));
     SVB_CUDA(cudaMemcpyAsync(L->bias, bias_dev, (size_t)L->Cout * 4, cudaMemcpyDeviceToDevice, st));
     SVB_CUDA(cudaGetLastError());

@@ -351,7 +351,37 @@ __global__ void __launch_bounds__(256) nsf_linear_bwd_kernel(const float *__rest
     }
 }
 
+__global__ void gather_kernel(float *__restrict__ dst, const float *__restrict__ nat, const int *__restrict__ idx, size_t n) {
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+        dst[i] = idx ? (idx[i] ? nat[idx[i] - 1] : 0.f) : nat[i];
+}
+
 }  // namespace
+
+std::vector<float> iota1(size_t n) {
+    std::vector<float> v(n);
+    for (size_t i = 0; i < n; ++i) v[i] = (float)(i + 1);
+    return v;
+}
+
+int upload_gather_map(const std::vector<float> &coded, std::vector<void *> *allocs, int **out) {
+    std::vector<int> idx(coded.size());
+    for (size_t i = 0; i < coded.size(); ++i) idx[i] = (int)coded[i];
+    int *d = nullptr;
+    SVB_CUDA(cudaMalloc((void **)&d, std::max<size_t>(idx.size(), 1) * sizeof(int)));
+    allocs->push_back(d);
+    SVB_CUDA(cudaMemcpy(d, idx.data(), idx.size() * sizeof(int), cudaMemcpyHostToDevice));
+    *out = d;
+    return SVB_OK;
+}
+
+int launch_gather(float *dst, const float *nat, const int *idx, size_t n, cudaStream_t st) {
+    if (n == 0) return SVB_OK;
+    const int blocks = (int)std::min<size_t>((n + 255) / 256, 132 * 8);
+    gather_kernel<<<blocks, 256, 0, st>>>(dst, nat, idx, n);
+    SVB_CUDA(cudaGetLastError());
+    return SVB_OK;
+}
 
 int launch_wgrad(const WgradArgs &a, cudaStream_t st) {
     SVB_CHECK(a.A && a.G && a.out && a.B > 0 && a.Tq > 0 && a.K >= 1, SVB_ERR_INVALID, "wgrad: bad argument");

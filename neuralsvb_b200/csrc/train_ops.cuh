@@ -1,5 +1,7 @@
 // Backward (training) kernels of the generator on the G32T layout.  See train_ops.cu.
 #pragma once
+#include <vector>
+
 #include "common.cuh"
 #include "conv_tc.cuh"
 
@@ -46,6 +48,14 @@ int launch_conv_dgrad(const float *w, const TcWeights &tc, const float *zero_bia
 
 // db[c] += sum_{b,t<T} G[b][t][c]
 int launch_colsum(const float *G, int B, int C, int T, int Tp, float *db, cudaStream_t st);
+
+// Device-side re-packing after an optimizer step.  Every packed weight array is a permutation (with zeros) of one folded
+// tensor, so the host packers are run ONCE on an index tensor (values i + 1, exact in fp32 up to 2^24 elements) and the
+// result is kept as a gather map:  dst[i] = idx ? (idx[i] ? nat[idx[i] - 1] : 0) : nat[i]   (idx == nullptr: plain copy)
+std::vector<float> iota1(size_t n);
+// the gather map of a packing of iota1 (`coded`), uploaded to a new device array (appended to `allocs`)
+int upload_gather_map(const std::vector<float> &coded, std::vector<void *> *allocs, int **out);
+int launch_gather(float *dst, const float *nat, const int *idx, size_t n, cudaStream_t st);
 
 // out = (add ? add : 0) + alpha * a * (mask ? (mask >= 0 ? 1 : slope) : 1)   over n4 float4 (whole G32T buffers:
 // the zero padding stays zero)
