@@ -36,6 +36,24 @@ const char *get_error();
         if (_s != SVB_OK) return _s;                                                           \
     } while (0)
 
+// ---- the dynamic shared-memory limit of a kernel ----------------------------------------------
+// cudaFuncSetAttribute is per device and one process may drive several GPUs, so each launcher keeps its cache of the limit
+// it has set with one entry per device.  The last entry stands for every device from kSmemCacheDevices - 1 up and is
+// always re-applied.  Sizes up to `floor` launch without setting the attribute (48 KB: the default limit).
+constexpr int kSmemCacheDevices = 64;
+template <typename Kernel>
+inline int raise_smem_limit(Kernel kern, size_t smem, size_t (&configured)[kSmemCacheDevices], size_t floor = 48 * 1024) {
+    if (smem <= floor) return SVB_OK;
+    int dev = 0;
+    SVB_CUDA(cudaGetDevice(&dev));
+    dev = dev < kSmemCacheDevices ? dev : kSmemCacheDevices - 1;
+    if (smem > configured[dev] || dev == kSmemCacheDevices - 1) {
+        SVB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        configured[dev] = smem;
+    }
+    return SVB_OK;
+}
+
 // ---- activation layout: "G32T" ----------------------------------------------------------------
 // Generator activations live in HBM in channel groups of 32, time-major inside a group:
 //     buf[b][c / 32][PAD + t][c % 32]         (fp32, one "row" = 32 channels = 128 bytes)

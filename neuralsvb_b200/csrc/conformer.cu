@@ -119,11 +119,8 @@ extern "C" int svb_layer_norm_nct(const float *x_dev, const float *gamma_dev, co
     SVB_CHECK(x_dev && gamma_dev && beta_dev && y_dev && B > 0 && C > 0 && T > 0, SVB_ERR_INVALID, "layer_norm_nct: bad argument");
     const size_t smem = (size_t)C * 32 * 4;
     SVB_CHECK(smem <= 200 * 1024, SVB_ERR_INVALID, "layer_norm_nct: %d channels do not fit shared memory", C);
-    static size_t configured = 48 * 1024;
-    if (smem > configured) {
-        SVB_CUDA(cudaFuncSetAttribute(layer_norm_nct_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        configured = smem;
-    }
+    static size_t configured[kSmemCacheDevices] = {};
+    SVB_TRY(raise_smem_limit(layer_norm_nct_kernel, smem, configured));
     layer_norm_nct_kernel<<<dim3((T + 31) / 32, B), 256, smem, as_stream(stream)>>>(x_dev, gamma_dev, beta_dev, C, T, eps, y_dev);
     SVB_CUDA(cudaGetLastError());
     return SVB_OK;
@@ -137,11 +134,8 @@ extern "C" int svb_relpos_attention_nct(const float *q_dev, const float *k_dev, 
     const int dk = C / n_head;
     const size_t smem = (size_t)kAttWarps * (3 * dk + T) * 4;
     SVB_CHECK(smem <= 200 * 1024, SVB_ERR_INVALID, "relpos_attention_nct: T %d does not fit the score rows in shared memory", T);
-    static size_t configured = 48 * 1024;
-    if (smem > configured) {
-        SVB_CUDA(cudaFuncSetAttribute(relpos_attention_nct_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        configured = smem;
-    }
+    static size_t configured[kSmemCacheDevices] = {};
+    SVB_TRY(raise_smem_limit(relpos_attention_nct_kernel, smem, configured));
     relpos_attention_nct_kernel<<<dim3((T + kAttWarps - 1) / kAttWarps, n_head, B), 32 * kAttWarps, smem, as_stream(stream)>>>(
         q_dev, k_dev, v_dev, p_dev, bias_u_dev, bias_v_dev, mask_dev, C, T, dk, out_dev);
     SVB_CUDA(cudaGetLastError());

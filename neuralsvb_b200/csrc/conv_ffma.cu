@@ -129,11 +129,8 @@ static int launch_conv_t(const ConvArgs &a, cudaStream_t st) {
     const int rows = kTileT + 2 * halo;
     const size_t smem = (size_t)4 * rows * 16 + (size_t)KS * kCK * (8 * CPT) * 4;
     auto kern = conv1d_c4_ffma_kernel<KS, CPT>;
-    static size_t configured = 0;
-    if (smem > configured) {
-        SVB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        configured = smem;
-    }
+    static size_t configured[kSmemCacheDevices] = {};
+    SVB_TRY(raise_smem_limit(kern, smem, configured, 0));      // sets the exact size on first use, also below 48 KB
     dim3 grid((a.Tq + kTileT - 1) / kTileT, (a.CoutP + 8 * CPT - 1) / (8 * CPT), a.B);
     kern<<<grid, 256, smem, st>>>(a);
     SVB_CUDA(cudaGetLastError());
@@ -278,11 +275,8 @@ int launch_conv_post_tanh(const float *x, int B, int C, int T, int Tp, const flo
     const int rows = 256 + (K - 1);
     const size_t smem = (size_t)(C / 4) * (rows + K) * 16;
     SVB_CHECK(smem <= 200 * 1024, SVB_ERR_INVALID, "conv_post: %d channels do not fit shared memory", C);
-    static size_t configured = 48 * 1024;
-    if (smem > configured) {
-        SVB_CUDA(cudaFuncSetAttribute(conv_post_tanh_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        configured = smem;
-    }
+    static size_t configured[kSmemCacheDevices] = {};
+    SVB_TRY(raise_smem_limit(conv_post_tanh_kernel, smem, configured));
     dim3 grid((T + 255) / 256, B);
     conv_post_tanh_kernel<<<grid, 256, smem, st>>>(reinterpret_cast<const float4 *>(x), C, T, Tp,
                                                    reinterpret_cast<const float4 *>(wq), bias, K, slope, wav);

@@ -553,15 +553,12 @@ static int launch_mode(const TcArgs &p, int grid, size_t smem, cudaStream_t st) 
     auto kern = conv1d_c4_tc_kernel<MODE, N>;
     // function attributes are per device: one process may drive several GPUs (the reference's mp.spawn gives one each,
     // but nothing in the C ABI forbids a handle per device in one process)
-    static size_t configured[kMaxDevices] = {};
+    static size_t configured[kSmemCacheDevices] = {};
+    SVB_TRY(raise_smem_limit(kern, smem, configured, 0));      // sets the exact size on first use, also below 48 KB
     static bool carve[kMaxDevices] = {};
     int dev = 0;
     SVB_CUDA(cudaGetDevice(&dev));
     dev = dev < kMaxDevices ? dev : kMaxDevices - 1;
-    if (smem > configured[dev] || dev == kMaxDevices - 1) {
-        SVB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        configured[dev] = smem;
-    }
     if (!carve[dev]) {   // keep the SM's smem/L1 split fixed across the differently-sized launches of a forward
         SVB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
         carve[dev] = true;

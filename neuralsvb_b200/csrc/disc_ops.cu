@@ -169,11 +169,8 @@ static int launch_gconv(const GConvArgs &a, cudaStream_t st) {
     constexpr int TX = 256 / COQ, kGT = 4 * TX, kGC = 4 * COQ;
     const int span = (kGT - 1) * a.stride + (a.K - 1) * a.dil + 1;
     const size_t smem = ((size_t)kGCI * span + (size_t)kGCI * a.K * kGC) * 4;
-    static size_t configured = 48 * 1024;
-    if (smem > configured) {
-        SVB_CUDA(cudaFuncSetAttribute(gconv_kernel<COQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        configured = smem;
-    }
+    static size_t configured[kSmemCacheDevices] = {};
+    SVB_TRY(raise_smem_limit(gconv_kernel<COQ>, smem, configured));
     const int cout_g = a.Cout / a.groups;
     dim3 grid((a.Tout + kGT - 1) / kGT, ((cout_g + kGC - 1) / kGC) * a.groups, a.B * a.W);
     gconv_kernel<COQ><<<grid, 256, smem, st>>>(a);

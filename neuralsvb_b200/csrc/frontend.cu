@@ -543,14 +543,8 @@ int launch_stft_v2(const StftArgs &a, bool want_mel, const ClipTable &ct, int n_
         pack_cap = (int)std::min<size_t>(n_val, 4096);
     }
     const size_t smem = ((size_t)2 * kFPB * (a.n_fft / 2) + a.n_fft + a.win + (size_t)kFPB * a.n_bins + pack_cap) * sizeof(float);
-    static size_t configured[64] = {};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    dev = dev < 64 ? dev : 63;
-    if (smem > 48 * 1024 && (smem > configured[dev] || dev == 63)) {
-        SVB_CUDA(cudaFuncSetAttribute(stft_mel_v2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        configured[dev] = smem;
-    }
+    static size_t configured[kSmemCacheDevices] = {};
+    SVB_TRY(raise_smem_limit(stft_mel_v2_kernel, smem, configured));
     stft_mel_v2_kernel<<<total_blocks, 256, smem, st>>>(a, ct, n_clips, mp, pack_cap);
     SVB_CUDA(cudaGetLastError());
     if (ws) SVB_CUDA(cudaFreeAsync(ws, st));
@@ -659,11 +653,8 @@ extern "C" int svb_stft_backward(const svb_stft_config *cfg, const float *wav_de
     StftBwdArgs g;
     g.dout = dout_dev, g.dwav = dwav_dev;
     const size_t smem = (size_t)(3 * a.n_fft + a.n_bins + (want_mel ? a.n_mels : 0)) * sizeof(float);
-    static size_t configured = 48 * 1024;
-    if (smem > configured) {
-        SVB_CUDA(cudaFuncSetAttribute(stft_mel_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        configured = smem;
-    }
+    static size_t configured[kSmemCacheDevices] = {};
+    SVB_TRY(raise_smem_limit(stft_mel_bwd_kernel, smem, configured));
     stft_mel_bwd_kernel<<<dim3(a.frames, B), 256, smem, as_stream(stream)>>>(a, g);
     SVB_CUDA(cudaGetLastError());
     return SVB_OK;
@@ -687,11 +678,8 @@ extern "C" int svb_denoise(const svb_stft_config *cfg, const float *wav_dev, int
     cudaStream_t st = as_stream(stream);
     SVB_CUDA(cudaMemsetAsync(out_dev, 0, (size_t)B * out_len * sizeof(float), st));
     const size_t smem = (size_t)(3 * a.n_fft) * sizeof(float);
-    static size_t configured = 48 * 1024;
-    if (smem > configured) {
-        SVB_CUDA(cudaFuncSetAttribute(denoise_frames_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        configured = smem;
-    }
+    static size_t configured[kSmemCacheDevices] = {};
+    SVB_TRY(raise_smem_limit(denoise_frames_kernel, smem, configured));
     denoise_frames_kernel<<<dim3(a.frames, B), 256, smem, st>>>(a, v, out_dev, out_len);
     const long long tot = (long long)B * out_len;
     denoise_norm_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(out_dev, out_len, B, c.n_fft, c.hop, c.win, a.frames);

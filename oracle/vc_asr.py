@@ -41,8 +41,8 @@ def shifted_bd(bd):
     """rel_shift (espnet_transformer_attn.py:127-145) written as the index map it performs on bd [B, h, T, T]:
     out[i][j] = bd[i][T-1-(i-j)] for j <= i ; 0 for j == i+1 ; bd[i+1][j-i-2] for j >= i+2."""
     T = bd.shape[-1]
-    i = torch.arange(T)[:, None]
-    j = torch.arange(T)[None, :]
+    i = torch.arange(T, device=bd.device)[:, None]
+    j = torch.arange(T, device=bd.device)[None, :]
     past = j <= i
     row = torch.where(past, i, (i + 1).clamp(max=T - 1)).expand(T, T)
     col = torch.where(past, T - 1 - (i - j), (j - i - 2).clamp(min=0))
@@ -93,7 +93,7 @@ def conformer_forward(w, pre, x, n_layers, n_head=4, K=31, last_norm=False):
     """ConformerLayers.forward (conformer.py:37-52) with EncoderLayer.forward (layers.py:181-260, macaron, normalize_before)."""
     B, T, H = x.shape
     key_mask = x.abs().sum(-1) > 0
-    pos_emb = rel_positions(T, H)
+    pos_emb = rel_positions(T, H).to(x.dtype)
     x = x * math.sqrt(H)
     for l in range(n_layers):
         e = f'{pre}.encoder_layers.{l}'

@@ -31,30 +31,3 @@ def test_vc_asr_h_content_matches_reference_fixture():
     rel = float(np.abs(h - ref).max() / np.abs(ref).max())
     assert rel < 1e-4, rel                    # fp32 kernels throughout; the north-star asks 1e-3 relative L-inf on spectral features
     assert np.all(h[1, -9 // 2:] == 0.0)      # padded frames stay exactly zero (conformer.py:51)
-
-
-def test_layer_norm_and_attention_kernels_against_torch():
-    from neuralsvb_b200.modules.voice_conversion import vc_modules as V
-    from oracle import vc_asr as OV
-    torch.manual_seed(3)
-    x = torch.randn(3, 256, 77).cuda()
-    ln = torch.nn.LayerNorm(256).cuda()
-    with torch.no_grad():
-        ln.weight.uniform_(0.5, 1.5), ln.bias.uniform_(-0.2, 0.2)
-        y = V.layer_norm_nct(x, ln)
-        ref = ln(x.transpose(1, 2)).transpose(1, 2)
-    assert float((y - ref).abs().max()) < 2e-5
-    # attention core vs the oracle's index-mapped rel_shift (bit-checked against the reference on CPU)
-    B, H, T, nh = 2, 256, 45, 4
-    w = {k: v for k, v in S.make_vc_asr_state_dict(1234).items() if '.encoder_layers.0.self_attn.' in k}
-    pre = 'content_encoder.encoder_layers.0.self_attn'
-    xs = torch.randn(B, T, H)
-    mask = torch.ones(B, T, dtype=torch.bool)
-    mask[1, T - 6:] = False
-    with torch.no_grad():
-        ref = OV.attention(w, pre, xs, OV.rel_positions(T, H), mask, nh)
-    m = _model()
-    a = m.content_encoder.encoder_layers[0].self_attn
-    with torch.no_grad():
-        out = m._attention(a, xs.transpose(1, 2).contiguous().cuda(), V.rel_positions(T, H, 'cuda'), mask.float().cuda())
-    assert float((out.transpose(1, 2).cpu() - ref).abs().max()) < 1e-4 * float(ref.abs().max())

@@ -1,12 +1,18 @@
-"""CPU: the float64 references of the kernel-level GPU tests (tests/test_gpu_stft_kernels.py, test_gpu_disc_kernels.py)
-against the oracle (oracle/hifigan.py, oracle/frontend.py), which is pinned to the reference fixtures.  A wrong reference
+"""CPU: the float64 references of the kernel-level GPU tests (tests/test_gpu_stft_kernels.py, test_gpu_disc_kernels.py,
+test_gpu_acoustic_kernels.py) against the oracle (oracle/hifigan.py, oracle/frontend.py, oracle/vc_asr.py), which is pinned to
+the reference fixtures.  A wrong reference
 would let a wrong kernel pass its test; here it fails without a GPU."""
+import os
+
 import numpy as np
 import torch
+import torch.nn.functional as F
 
 from neuralsvb_b200.utils import synthetic as S
 from oracle import frontend as FE
 from oracle import hifigan as O
+from oracle import vc_asr as OV
+from tests import test_gpu_acoustic_kernels as A
 from tests import test_gpu_disc_kernels as D
 from tests import test_gpu_stft_kernels as T
 
@@ -70,3 +76,47 @@ def test_loss_gradient_references_match_the_oracle_losses(monkeypatch):
     assert _rel(kind(3, sc_scale), _grad(lambda t: O.stft_loss(t, b, 0, 0, 0)[0], a)) < 1e-12
     assert _rel(kind(4, 1 / n), _grad(lambda t: O.stft_loss(t, b, 0, 0, 0)[1], a)) < 1e-12
     assert (kind(4, 1 / n)[::7] == 0).all() and (kind(0, 1.0)[::7] == 0).all()
+
+
+def _rel_shift(x):
+    """espnet's rel_shift as written: prepend a zero column, view [T, T + 1] as [T + 1, T], drop the first row."""
+    *lead, T, _ = x.shape
+    padded = torch.cat([x.new_zeros(*lead, T, 1), x], -1).view(*lead, T + 1, T)
+    return padded[..., 1:, :].reshape(x.shape)
+
+
+def test_shifted_bd_is_rel_shift():
+    for T in (1, 2, 3, 8):
+        x = torch.randn(2, 3, T, T, generator=torch.Generator().manual_seed(T), dtype=torch.float64)
+        assert torch.equal(OV.shifted_bd(x), _rel_shift(x)), T
+
+
+def test_attention_reference_matches_the_oracle_attention():
+    """The float64 attention core of test_gpu_acoustic_kernels on the fixture's weights and shape (B 2, T' 48, the shorter
+    clip's last 4 keys masked), against oracle.vc_asr.attention in fp32 with linear_out set to the identity."""
+    B, T, H, nh = 2, 48, 256, 4
+    pre = 'content_encoder.encoder_layers.0.self_attn'
+    w = {k: v for k, v in S.make_vc_asr_state_dict(1234).items() if k.startswith(pre)}
+    w[pre + '.linear_out.weight'], w[pre + '.linear_out.bias'] = torch.eye(H), torch.zeros(H)
+    x = torch.randn(B, T, H, generator=torch.Generator().manual_seed(11))
+    mask = torch.ones(B, T, dtype=torch.bool)
+    mask[1, T - 4:] = False
+    pos = OV.rel_positions(T, H)
+    with torch.no_grad():
+        ctx = OV.attention(w, pre, x, pos, mask, nh)
+        q, k, v = (F.linear(x, w[f'{pre}.linear_{n}.weight'], w[f'{pre}.linear_{n}.bias']).transpose(1, 2).contiguous() for n in 'qkv')
+        p = F.linear(pos, w[pre + '.linear_pos.weight']).t().contiguous()
+        ref = A.attention_reference(q, k, v, p, w[pre + '.pos_bias_u'], w[pre + '.pos_bias_v'], mask.float(), nh)
+    assert ref.dtype == torch.float64
+    assert _rel(ref.transpose(1, 2), ctx) < 1e-5
+
+
+def test_vc_asr_oracle_runs_in_float64_and_matches_the_fixture():
+    """The float64 PPG-extractor reference of test_gpu_acoustic_kernels is the oracle run on double weights and mel."""
+    g = np.load(os.path.join(os.path.dirname(__file__), 'golden', 'vc_asr.npz'))
+    B, T = [int(v) for v in g['params']]
+    w = {k: v.double() for k, v in S.make_vc_asr_state_dict(1234).items()}
+    with torch.no_grad():
+        h = OV.vc_asr_h_content(w, S.make_vc_asr_mel(B, T, 1234).double())
+    assert h.dtype == torch.float64
+    assert _rel(h, g['h_content']) < 1e-5
