@@ -402,6 +402,21 @@ int svb_relpos_attention_nct(const float *q_dev, const float *k_dev, const float
                              const float *bias_v_dev, const float *mask_dev, int32_t B, int32_t C, int32_t T, int32_t n_head,
                              float *out_dev, void *stream);
 
+/* ---- Mel reconstruction loss of the SVB acoustic step (the `ssim:0.5|l1:0.5` recipe: FastSpeech2Task.l1_loss and
+ * ssim_loss(bias), tasks/tts/fs2.py:158-175, ssim(..., size_average=False), modules/commons/ssim.py:319-351).
+ * pred / target [B, T, M] (M <= 128); a frame's weight is 1 when its target row has a non-zero element, else 0:
+ *   l1 = sum w |pred - target| / sum w,   ssim = sum w (1 - SSIM(pred + bias, target + bias)) / sum w   (sums over B*T*M pixels)
+ * with the 11x11 Gaussian window (sigma 1.5) over the whole [T, M] image (padding frames included), zero padding outside it.
+ * svb_mel_loss_workspace_bytes: size of the caller-owned partial-sum buffer (-1 on a bad shape).
+ * svb_mel_loss_forward writes out3_dev (double[3]) = {l1, ssim, sum w}; NaN for both losses when sum w = 0, like the reference.
+ * svb_mel_loss_backward writes dpred = g_l1 * d l1 / d pred + g_ssim * d ssim / d pred, reading the upstream gradients from the
+ * device scalars g_l1_dev / g_ssim_dev (NULL = 0) and sum w from the forward's out3_dev.  No gradient to the target. */
+int64_t svb_mel_loss_workspace_bytes(int32_t B, int32_t T, int32_t M);
+int svb_mel_loss_forward(const float *pred_dev, const float *target_dev, int32_t B, int32_t T, int32_t M, float bias,
+                         double *workspace_dev, double *out3_dev, void *stream);
+int svb_mel_loss_backward(const float *pred_dev, const float *target_dev, int32_t B, int32_t T, int32_t M, float bias,
+                          const double *out3_dev, const float *g_l1_dev, const float *g_ssim_dev, float *dpred_dev, void *stream);
+
 /* Host-only view of the schedule of a merged tensor-core launch (csrc/conv_tc.cu: tc_schedule; no CUDA call, usable without a GPU):
  * `n_layers` convolutions of one shape class (taps KS[l], residual / accumulate flags) over B clips x Tq rows, tiles of 128 rows in
  * items of up to MT tiles, `col_blocks` column blocks, `grid` CTAs.  items_out receives 5 ints per item (layer, column block, clip,

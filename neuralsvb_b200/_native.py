@@ -16,7 +16,7 @@ CSRC = os.path.join(_HERE, 'csrc')
 LIB_PATH = os.path.join(_HERE, 'libsvb_vocoder.so')
 HEADER = os.path.join(_ROOT, 'include', 'svb_vocoder.h')
 SOURCES = ['wn.cu', 'conformer.cu', 'api.cu', 'conv_ffma.cu', 'conv_tc.cu', 'nsf_source.cu', 'frontend.cu', 'generator.cu', 'layer_api.cu', 'disc_ops.cu',
-           'train_ops.cu', 'generator_bwd.cu', 'disc_bwd.cu', 'tc_layer.cu', 'wgrad_tc.cu']
+           'train_ops.cu', 'generator_bwd.cu', 'disc_bwd.cu', 'tc_layer.cu', 'wgrad_tc.cu', 'mel_loss.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '-Xcompiler', '-fPIC', '-shared']
 
@@ -173,6 +173,9 @@ _PROTOS = {
     'svb_tc_schedule_probe': (_I64, [_I32, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _I64, _P, ctypes.POINTER(ctypes.c_double)]),
     'svb_layer_norm_nct': (ctypes.c_int, [_P, _P, _P, _I32, _I32, _I32, ctypes.c_float, _P, _P]),
     'svb_relpos_attention_nct': (ctypes.c_int, [_P, _P, _P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _P, _P]),
+    'svb_mel_loss_workspace_bytes': (_I64, [_I32, _I32, _I32]),
+    'svb_mel_loss_forward': (ctypes.c_int, [_P, _P, _I32, _I32, _I32, ctypes.c_float, _P, _P, _P]),
+    'svb_mel_loss_backward': (ctypes.c_int, [_P, _P, _I32, _I32, _I32, ctypes.c_float, _P, _P, _P, _P, _P]),
 }
 
 

@@ -224,10 +224,12 @@ class WN(_NativeStack):
     def forward(self, x, x_mask=None, g=None, **kwargs):
         """fs2_vae.py:62-94.  x [B, H, T] ([B, T, H] with is_BTC), x_mask [B, 1, T], g [B, gin, T]."""
         train = torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()) and self.training
+        # a trainable stack also tapes in eval mode when an input needs a gradient (a frozen stack between trainable layers)
+        train = train or (self.trainable and torch.is_grad_enabled() and (x.requires_grad or (g is not None and g.requires_grad)))
         if train and not self.trainable:
             raise RuntimeError('neuralsvb_b200 WN is inference only: call .eval() and run under torch.no_grad() '
                                '(or construct it with trainable=True)')
-        if train and self.p_dropout > 0:
+        if train and self.training and self.p_dropout > 0:
             raise NotImplementedError(f'WN training with p_dropout={self.p_dropout}: the native stack has no dropout '
                                       '(the SVB configurations use 0)')
         if not x.is_cuda:
@@ -324,10 +326,13 @@ class FVAEDecoder(_NativeStack):
     def forward(self, x, x_mask, g):
         """x [B, latent, T / s]; x_mask [B, 1, T] (or the scalar 1 the reference passes at inference); g [B, gin, T] or None."""
         train = torch.is_grad_enabled() and self.training
+        # a trainable decoder also tapes in eval mode when an input needs a gradient: the mapping step differentiates the mel
+        # through the frozen eval-mode decoder (it has no dropout or BatchNorm, so the taped forward is the eval computation)
+        train = train or (self.trainable and torch.is_grad_enabled() and (x.requires_grad or (torch.is_tensor(g) and g.requires_grad)))
         if train and not self.trainable:
             raise RuntimeError('neuralsvb_b200 FVAEDecoder is inference only: call .eval() and run under torch.no_grad() '
                                '(or construct it with trainable=True)')
-        if train and self.wn.p_dropout > 0:
+        if train and self.training and self.wn.p_dropout > 0:
             raise NotImplementedError(f'FVAEDecoder training with p_dropout={self.wn.p_dropout}: the native stack has no dropout '
                                       '(the SVB configurations use 0)')
         if not x.is_cuda:

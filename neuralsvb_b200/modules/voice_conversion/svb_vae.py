@@ -9,7 +9,15 @@
 Same constructor (``dict_size`` + hparams) and ``state_dict`` names as the reference.  Every Conv1d / Linear runs as a native kernel
 (``svb_conv_nct_forward``; the WN stacks and the PPG extractor through their own entry points, see ``modules/fastspeech/fs2_vae.py`` and
 ``vc_modules.py``); embedding lookup, GroupNorm / BatchNorm(eval) affine maps, nearest up-sampling, gathers and concatenations are torch
-ops on the same device tensors.  No training path (the acoustic model's DDP step, BASELINE cfg 4, is not part of this package)."""
+ops on the same device tensors.
+
+Training is opt-in: ``MleSVBVAE(..., trainable=True)`` makes the generator and the latent map differentiable (the phase-2 generator
+step and the phase-3 mapping step of ``SVBVAEMleTask``, tasks/singing/svb_vae_task.py:543-676).  Every convolution then runs as an
+autograd node with a native backward (``_conv`` -> ``_TcConvFn`` / ``_ConvNctFn``, the GlobalFVAE through ``_WNTrainFn`` /
+``_FVAEDecTrainFn``); the BatchNorms of ``upsample_layer`` and of the latent map use batch statistics in ``train()`` mode and update
+their running statistics as ``nn.BatchNorm1d`` does; ``vc_asr`` always runs without grad (the reference ``.detach()``es its output).
+The mel reconstruction loss is ``neuralsvb_b200.modules.commons.mel_loss.mel_l1_ssim_loss``; the DDP step (BASELINE cfg 4) is not part
+of this package."""
 import torch
 import torch.nn.functional as F
 from torch import nn
@@ -21,6 +29,11 @@ from neuralsvb_b200.modules.voice_conversion.vc_modules import VCASR, _bn_affine
 def _linear_btc(x, lin):
     """nn.Linear on [B, T, C] as a native 1x1 convolution on [B, C, T]."""
     return _conv(x.transpose(1, 2).contiguous(), lin.weight, lin.bias).transpose(1, 2)
+
+
+def _bn_train(m):
+    """Batch-statistics BatchNorm (running statistics updated, as nn.BatchNorm1d in train mode) for a trainable module in training."""
+    return m.trainable and m.training and torch.is_grad_enabled()
 
 
 class _ConvStacks(nn.Module):
@@ -47,10 +60,12 @@ class _ConvStacks(nn.Module):
 
 
 class _GlobalLatentMap(nn.Module):
-    """``GlobalLatentMap`` (modules/voice_conversion/vae_models.py:149-172): 1x1 convs on the [B, latent, 1] latent, eval-mode BatchNorm."""
+    """``GlobalLatentMap`` (modules/voice_conversion/vae_models.py:149-172): 1x1 convs on the [B, latent, 1] latent, eval-mode BatchNorm
+    (batch statistics in ``train()`` mode with grad enabled when ``trainable``)."""
 
-    def __init__(self, latent):
+    def __init__(self, latent, trainable=False):
         super().__init__()
+        self.trainable = trainable
         self.convs = nn.Sequential(nn.Conv1d(latent, latent, 1), nn.BatchNorm1d(latent), nn.ReLU(), nn.Conv1d(latent, latent, 1),
                                    nn.BatchNorm1d(latent), nn.ReLU(), nn.Conv1d(latent, latent, 1))
         self.spk_proj = nn.Sequential(nn.Conv1d(256, latent, 1), nn.ReLU(), nn.Conv1d(latent, latent, 1))
@@ -60,20 +75,23 @@ class _GlobalLatentMap(nn.Module):
         s = _conv(_conv(s, self.spk_proj[0].weight, self.spk_proj[0].bias, relu=True), self.spk_proj[2].weight, self.spk_proj[2].bias)
         x = (x + s).contiguous()
         c = self.convs
-        x = torch.relu(_bn_affine(c[1], _conv(x, c[0].weight, c[0].bias))).contiguous()
-        x = torch.relu(_bn_affine(c[4], _conv(x, c[3].weight, c[3].bias))).contiguous()
+        bn = (lambda m, y: m(y)) if _bn_train(self) else _bn_affine
+        x = torch.relu(bn(c[1], _conv(x, c[0].weight, c[0].bias))).contiguous()
+        x = torch.relu(bn(c[4], _conv(x, c[3].weight, c[3].bias))).contiguous()
         return _conv(x, c[6].weight, c[6].bias)
 
 
 class MleSVBVAE(nn.Module):
-    def __init__(self, dict_size=None, hp=None, precision='bf16x3'):
+    def __init__(self, dict_size=None, hp=None, precision='bf16x3', trainable=False):
         super().__init__()
+        self.trainable = bool(trainable)
         if hp is None:
             from neuralsvb_b200.utils.hparams import hparams as hp
         H = self.hidden_size = hp['hidden_size']
         self.c_content = self.c_out = hp['audio_num_mel_bins']
         self.vae_model = GlobalFVAE(self.c_content, hp['fvae_enc_dec_hidden'], hp['latent_size'], hp['fvae_kernel_size'],
-                                    hp['fvae_enc_n_layers'], hp['fvae_dec_n_layers'], H, [4], False, precision=precision)
+                                    hp['fvae_enc_n_layers'], hp['fvae_dec_n_layers'], H, [4], False, precision=precision,
+                                    trainable=self.trainable)
         self.pitch_embed = nn.Embedding(300, H, 0)
         self.pitch_encoder = _ConvStacks(H, 3)
         self.vc_asr = VCASR(dict_size, self.c_content, hidden_size=H, asr_enc_layers=hp['asr_enc_layers'], mel_strides=hp['mel_strides'],
@@ -84,7 +102,7 @@ class MleSVBVAE(nn.Module):
                                               [nn.Conv1d(H, H, 5, padding=2)]))
         self.spk_embed_proj = nn.Linear(256, H)
         self.encoded_embed_proj = nn.Linear(3 * H, H)
-        self.z_mapping_function = _GlobalLatentMap(hp['latent_size'])
+        self.z_mapping_function = _GlobalLatentMap(hp['latent_size'], self.trainable)
 
     def load_state_dict(self, state_dict, strict=True):
         sd = {k: v for k, v in state_dict.items() if not k.startswith(('vc_asr.asr_decoder.', 'vc_asr.token_embed.'))}
@@ -93,12 +111,15 @@ class MleSVBVAE(nn.Module):
     def prepare_condition(self, mels_content=None, pitch=None, spk_ids=None):
         """svb_vae.py:57-84."""
         T = pitch.shape[1]
-        h_pitch = self.pitch_encoder(F.embedding(pitch, self.pitch_embed.weight))
-        h = self.vc_asr(mels_content)['h_content'].transpose(1, 2)
+        # padding_idx 0 as the reference's Embedding(300, H, 0): unvoiced / padding frames (pitch 0) give row 0 no gradient
+        h_pitch = self.pitch_encoder(F.embedding(pitch, self.pitch_embed.weight, padding_idx=0))
+        with torch.no_grad():                                       # the reference detaches h_content (svb_vae.py:68)
+            h = self.vc_asr(mels_content)['h_content'].transpose(1, 2)
+        bn = (lambda m, y: m(y)) if _bn_train(self) else _bn_affine
         for m in self.upsample_layer:
-            if isinstance(m, nn.Sequential):                        # Upsample(nearest) -> Conv1d -> ReLU -> BatchNorm1d (eval)
+            if isinstance(m, nn.Sequential):                        # Upsample(nearest) -> Conv1d -> ReLU -> BatchNorm1d
                 s = int(m[0].scale_factor)
-                h = _bn_affine(m[3], _conv(h.repeat_interleave(s, dim=2).contiguous(), m[1].weight, m[1].bias, K=2 * s + 1, pad=s, relu=True))
+                h = bn(m[3], _conv(h.repeat_interleave(s, dim=2).contiguous(), m[1].weight, m[1].bias, K=2 * s + 1, pad=s, relu=True))
             else:
                 h = _conv(h.contiguous(), m.weight, m.bias, K=5, pad=2)
         h_content = h.transpose(1, 2)[:, :mels_content.shape[1]]
@@ -120,8 +141,10 @@ class MleSVBVAE(nn.Module):
     def forward(self, amateur_mel=None, prof_mel=None, amateur_pitch=None, prof_pitch=None, amateur_spk_id=None, prof_spk_id=None,
                 a2p_alignment=None, p2a_alignment=None, infer=False, disable_map=False, eps=None, **kwargs):
         """svb_vae.py:258-312.  ``eps`` [B, latent, 1] replaces the posterior noise (parity tests); default torch.randn_like."""
-        if torch.is_grad_enabled() and self.training:
+        if torch.is_grad_enabled() and self.training and not self.trainable:
             raise RuntimeError('neuralsvb_b200 MleSVBVAE is inference only: call .eval() and run under torch.no_grad()')
+        if self.trainable and not amateur_mel.is_cuda:
+            raise RuntimeError('neuralsvb_b200 has no CPU path: move the module and its inputs to a CUDA device')
         ways = kwargs['concurrent_ways']
         ret = {}
         ac = self.prepare_condition(amateur_mel, amateur_pitch, spk_ids=amateur_spk_id)

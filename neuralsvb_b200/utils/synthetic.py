@@ -439,6 +439,18 @@ def make_svb_state_dict(seed=1234, hidden=256, latent=128, n_mel=80):
     return sd
 
 
+def make_mel_pair(B, T, pad, seed=1234, n_mel=80):
+    """(mel_out, target) [B, T, n_mel] for the mel reconstruction loss: a log10-mel-range target whose clip b has its last pad[b]
+    frames zero (padding; pad[b] = T is an all-padding clip) and a prediction = target + noise everywhere, padding frames included."""
+    rs = np.random.RandomState(seed + 47)
+    tgt = (rs.randn(B, T, n_mel) * 1.2 - 2.5).clip(-6, 1.5)
+    out = tgt + rs.randn(B, T, n_mel) * 0.3
+    for b, p in enumerate(pad):
+        if p:
+            tgt[b, T - p:] = 0.0
+    return torch.from_numpy(out.astype(np.float32)), torch.from_numpy(tgt.astype(np.float32))
+
+
 def make_svb_batch(B=2, Ta=96, Tp=120, seed=1234, n_mel=80):
     """A PopBuTFy-shaped batch (SURVEY 8(d) cfg 4 / 5): amateur / professional mels [B, T, 80] (zero frames = padding), coarse pitch
     ids in [1, 255] (0 = padding), one speaker embedding [B, 256], the a2p alignment [B, Tp] into the amateur frames."""
