@@ -425,6 +425,13 @@ int svb_mel_loss_backward(const float *pred_dev, const float *target_dev, int32_
 int64_t svb_tc_schedule_probe(int32_t n_layers, const int32_t *KS, const int32_t *has_res, const int32_t *accumulate, int32_t Cin, int32_t B,
                               int32_t Tq, int32_t MT, int32_t col_blocks, int32_t chain_ordered, int32_t grid, int32_t *items_out,
                               int64_t items_capacity, int32_t *off_out, double *balance_out);
+/* The same for the fused ResBlock1 launches (one item = c1 and c2 of one dilation step of chain l for P output rows): c1 taps KS1[l]
+ * at dilation dil1[l], c2 taps KS2[l], c2 accumulate flags, Cin channels (one column block), items of 256 c1 rows.  items_out
+ * receives 7 ints per item: the 5 of svb_tc_schedule_probe, then the first padded row and the row count of the item's c1 slab copy
+ * (padded rows of a clip: [0, round_up(Tq, 256) + 128)).  P_out receives P. */
+int64_t svb_tc_fused_schedule_probe(int32_t n_layers, const int32_t *KS1, const int32_t *dil1, const int32_t *KS2, const int32_t *accumulate,
+                                    int32_t Cin, int32_t B, int32_t Tq, int32_t chain_ordered, int32_t grid, int32_t *items_out,
+                                    int64_t items_capacity, int32_t *off_out, int32_t *P_out, double *balance_out);
 
 #ifdef __cplusplus
 }

@@ -171,6 +171,8 @@ _PROTOS = {
     'svb_wn_set_weight_dev': (ctypes.c_int, [_P, ctypes.c_char_p, _P, _I64, _P]),
     'svb_wn_update_weights_dev': (ctypes.c_int, [_P, _P]),
     'svb_tc_schedule_probe': (_I64, [_I32, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _I64, _P, ctypes.POINTER(ctypes.c_double)]),
+    'svb_tc_fused_schedule_probe': (_I64, [_I32, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _P, _I64, _P, _P,
+                                           ctypes.POINTER(ctypes.c_double)]),
     'svb_layer_norm_nct': (ctypes.c_int, [_P, _P, _P, _I32, _I32, _I32, ctypes.c_float, _P, _P]),
     'svb_relpos_attention_nct': (ctypes.c_int, [_P, _P, _P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _P, _P]),
     'svb_mel_loss_workspace_bytes': (_I64, [_I32, _I32, _I32]),

@@ -59,8 +59,10 @@ struct TcLayer {                // what differs between the layers of one launch
 
 struct TcArgs {
     ConvArgs a;                 // the shape class (B, channels, rows, in_slope, ups_u ...); per-layer fields live in L[]
-    TcLayer L[kTcMaxLayers];
+    TcLayer L[2 * kTcMaxLayers];    // fused launches: L[j] = c1 and L[n_layers + j] = c2 of ResBlock chain j
     int n_layers;
+    int fused_P;                // fused launches: output rows per item (the same for every layer of the launch)
+    uint32_t off_inter, inter_bytes;    // fused: the c1 -> c2 intermediate in dynamic smem, bytes per 32-channel chunk
     const int4 *work;           // explicit work list (device) or nullptr: implicit round-robin over the groups of layer 0
     const int *work_off;        // [grid + 1] item ranges per CTA
     int n_tile, n_chunks, MT, nW, nA;
@@ -85,6 +87,16 @@ constexpr int kWarpProducer = 0, kWarpTransform0 = 1, kWarpMath0 = 4;
 constexpr int kMathWarps = 8, kTransformWarps = 3;
 constexpr int kTrRows = kTransformWarps * 32 / 8;   // rows one pass of the transform warps covers (8 lanes per row)
 constexpr int kBiasBytes = 4096;        // bias of the layer(s) (<= 1024 floats; wider layers take 12 KB)
+
+static_assert(512 + 2 * kTcMaxLayers * sizeof(TcLayer) <= 1024, "the layer table lives in smem bytes 512 .. 1023");
+
+// Slab of a fused item (output rows [t0, t0 + P) of a clip): c1 runs over the 256 rows from t0 - h2, so its slab starts
+// at padded row kPad + t0 - h2 - h1.  The copy stops at the clip's last padded row (in_Tp): a bulk copy never reads the
+// next channel group or past the allocation.  The rows it leaves stale feed only c1 rows >= Tq, which are zeroed.
+__host__ __device__ inline void tc_fused_slab(int t0, int h1, int h2, int in_Tp, int *row0, int *rows) {
+    *row0 = kPad + t0 - h2 - h1;
+    *rows = min(2 * kTcM + 2 * h1, in_Tp - *row0);
+}
 
 // a work item, as staged in shared memory: x = layer | column block << 8 | tiles << 24, y = clip, z = first row
 struct TcItem {
@@ -126,7 +138,15 @@ __device__ __forceinline__ void conv_tap_mma(float *d, uint32_t a_row, uint32_t 
 // Persistent kernel: one CTA per SM walks its work items (one or two 128-row tiles of one clip for one column block
 // of one layer).  Every stage is decoupled by mbarriers, so the TMA producer runs ahead into the next items and the
 // transform warps prepare operands while the warpgroups multiply the previous chunk.
-template <int MODE, int N>
+//
+// FUSED: an item is one step x <- x + c2(lrelu(c1(lrelu(x)))) of ResBlock chain `layer` for the output rows
+// [t0, t0 + P).  c1 runs as a two-tile item over the 256 rows from t0 - h2 (h2 = c2's halo); its epilogue adds the
+// bias, writes zero for rows outside [0, Tq) (c2's zero padding), applies the leaky relu and stores c2's operand into
+// the shared-memory intermediate; c2 then reads that intermediate at row shifts 0 .. 2 h2 and runs the usual epilogue
+// for the first P rows.  Per output element both convolutions accumulate in the same order as two separate launches,
+// and the intermediate holds the same values c2's transform makes from c1's exact fp32 output: the results are
+// bit-identical.
+template <int MODE, int N, bool FUSED>
 __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __grid_constant__ TcArgs p) {
     extern __shared__ __align__(1024) unsigned char smem[];
     constexpr bool BF = MODE == SVB_PREC_BF16X3;
@@ -152,9 +172,10 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
     }
     {   // constant data (not produced by the previous kernel): staged once, before the PDL wait
         float *sb = reinterpret_cast<float *>(smem + p.off_bias);
-        for (int l = 0; l < p.n_layers; ++l)
+        const int n_tab = FUSED ? 2 * p.n_layers : p.n_layers;
+        for (int l = 0; l < n_tab; ++l)
             for (int i = threadIdx.x; i < a.Cout; i += kTcThreadsP) sb[p.L[l].bias_off + i] = __ldg(p.L[l].bias + i);
-        if (threadIdx.x < p.n_layers) Ls[threadIdx.x] = p.L[threadIdx.x];
+        if (threadIdx.x < n_tab) Ls[threadIdx.x] = p.L[threadIdx.x];
         int4 *it_w = reinterpret_cast<int4 *>(smem + 1024);
         if (p.work) {                                                // explicit list: this CTA's range
             const int i0 = __ldg(p.work_off + blockIdx.x), n = __ldg(p.work_off + blockIdx.x + 1) - i0;
@@ -199,8 +220,14 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
                 const TcItem it = item_decode(items[n]);
                 const TcLayer &L = Ls[it.layer];
                 const int halo = (L.KS - 1) / 2 * L.dil;
-                const uint32_t raw_bytes = (uint32_t)(it.mt * kTcM + 2 * halo) * 128;
+                uint32_t raw_bytes = (uint32_t)(it.mt * kTcM + 2 * halo) * 128;
                 const float *in_c = L.in + (((size_t)it.b * gin + (size_t)it.nblk * p.blk_chunk_step) * a.in_Tp + (kPad + it.t0 - halo)) * 32;
+                if (FUSED) {                                                      // c1 rows start h2 early; the copy stops at the clip's last padded row
+                    int row0, rows;
+                    tc_fused_slab(it.t0, halo, (Ls[p.n_layers + it.layer].KS - 1) / 2, a.in_Tp, &row0, &rows);
+                    raw_bytes = (uint32_t)rows * 128;
+                    in_c = L.in + ((size_t)it.b * gin * a.in_Tp + row0) * 32;
+                }
                 const unsigned char *w_k = L.w + (size_t)it.nblk * p.n_chunks * L.KS * p.wtile_bytes;
                 for (int c = 0; c < p.n_chunks; ++c) {
                     mbar_wait(a_empty + sA, phA);                                 // MMAs of the slot's previous slab retired
@@ -216,6 +243,17 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
                             w_k += p.wtile_bytes;
                             if (++sW == p.nW) sW = 0, phW ^= 1;
                         }
+                    }
+                }
+                if (FUSED) {                                                      // then c2's tiles, (chunk, tap) in order
+                    const TcLayer &L2 = Ls[p.n_layers + it.layer];
+                    w_k = L2.w + (size_t)it.nblk * p.n_chunks * L2.KS * p.wtile_bytes;
+                    for (int k = 0; k < p.n_chunks * L2.KS; ++k) {
+                        mbar_wait(w_empty + sW, phW);
+                        mbar_expect_tx(w_full + sW, p.wtile_bytes);
+                        bulk_g2s(wring + sW * p.wtile_bytes, w_k, p.wtile_bytes, w_full + sW);
+                        w_k += p.wtile_bytes;
+                        if (++sW == p.nW) sW = 0, phW ^= 1;
                     }
                 }
             }
@@ -343,6 +381,8 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
             for (int h = 0; h < 2; ++h) {
                 const int q = it.t0 + row0 + r_lo + 8 * h;                  // GEMM row = output time step (before upsampling)
                 if (q >= a.Tq) continue;
+                if (FUSED && row0 + r_lo + 8 * h >= p.fused_P) continue;    // the next item's rows
+
 #pragma unroll
                 for (int j = 0; j < N / 8; ++j) {
                     const int cop = it.nblk * N + 8 * j + c_lo;             // a column pair never straddles an upsampler phase
@@ -368,9 +408,8 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
         };
         // one item of one (TWO = false) or two (TWO = true) tiles; per output element the MMAs accumulate in the same
         // order either way (chunk, tap, then the split terms)
-        auto run_item = [&](auto two, const TcItem &it) {
+        auto run_mma_slab = [&](auto two, const TcLayer &L) {
             constexpr bool TWO = decltype(two)::value;
-            const TcLayer &L = Ls[it.layer];
             const int KS = L.KS;
             const uint32_t tap_step = (uint32_t)L.dil * (128 >> 4);       // a tap is a row shift of the operand
             uint32_t scale = 0;                                             // first MMA of the item overwrites
@@ -403,13 +442,88 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
             wgmma_keep<N>(acc0);
             if (TWO) wgmma_keep<N>(acc1);
             release();
+        };
+        auto run_item = [&](auto two, const TcItem &it) {
+            const TcLayer &L = Ls[it.layer];
+            run_mma_slab(two, L);
             epilogue(it, L, acc0, 0);
-            if (TWO) epilogue(it, L, acc1, kTcM);
+            if (decltype(two)::value) epilogue(it, L, acc1, kTcM);
+        };
+        // ---- fused items: c1's epilogue stores c2's operand for the item's rows 0 .. 255 (time tq0 + row) into the
+        // intermediate, in the layout the transform warps give a slab (hi / lo split or tf32 rounding, SWIZZLE_128B)
+        unsigned char *inter = smem + p.off_inter;
+        auto stage_intermediate = [&](const TcLayer &L1, const float *acc, int row0, int tq0) {
+            const float *bias_s = reinterpret_cast<const float *>(smem + p.off_bias) + L1.bias_off;
+            const float slope = a.in_slope;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int i = row0 + r_lo + 8 * h, q = tq0 + i;
+                const bool live = q >= 0 && q < a.Tq;                       // else c2's zero padding
+                const int sw = i & 7;
+#pragma unroll
+                for (int j = 0; j < N / 8; ++j) {
+                    const int co = 8 * j + c_lo;
+                    float x0 = live ? acc[4 * j + 2 * h] + bias_s[co] : 0.f, x1 = live ? acc[4 * j + 2 * h + 1] + bias_s[co + 1] : 0.f;
+                    x0 = fmaxf(x0, x0 * slope), x1 = fmaxf(x1, x1 * slope);
+                    unsigned char *row = inter + (size_t)(co >> 5) * p.inter_bytes + (size_t)i * 128;
+                    if (BF) {
+                        const __nv_bfloat162 hv = __floats2bfloat162_rn(x0, x1);
+                        const uint32_t hb = *reinterpret_cast<const uint32_t *>(&hv);
+                        const __nv_bfloat162 lv = __floats2bfloat162_rn(x0 - __uint_as_float(hb << 16), x1 - __uint_as_float(hb & 0xffff0000u));
+                        const int ch = (co & 31) >> 3, off = (co & 7) * 2;
+                        *reinterpret_cast<uint32_t *>(row + ((ch ^ sw) << 4) + off) = hb;
+                        *reinterpret_cast<uint32_t *>(row + (((4 + ch) ^ sw) << 4) + off) = *reinterpret_cast<const uint32_t *>(&lv);
+                    } else {
+                        const int ch = (co & 31) >> 2, off = (co & 3) * 4;
+                        const float h0 = to_tf32(x0), h1 = to_tf32(x1);
+                        *reinterpret_cast<float2 *>(row + ((ch ^ sw) << 4) + off) = make_float2(h0, h1);
+                        if (X3) *reinterpret_cast<float2 *>(row + p.inter_bytes / 2 + ((ch ^ sw) << 4) + off) = make_float2(to_tf32(x0 - h0), to_tf32(x1 - h1));
+                    }
+                }
+            }
+        };
+        auto run_fused = [&](const TcItem &it) {
+            const TcLayer &L1 = Ls[it.layer], &L2 = Ls[p.n_layers + it.layer];
+            const int h2 = (L2.KS - 1) / 2;
+            run_mma_slab(std::true_type(), L1);
+            // the other warpgroup's c2 wgmmas of the previous item have retired: the intermediate may be overwritten
+            named_bar_sync(1, kMathWarps * 32);
+            stage_intermediate(L1, acc0, 0, it.t0 - h2);
+            stage_intermediate(L1, acc1, kTcM, it.t0 - h2);
+            fence_proxy_async();                                            // generic-proxy writes -> visible to the tensor core
+            named_bar_sync(1, kMathWarps * 32);                             // c2's tap shifts read rows the other warpgroup wrote
+            const uint32_t inter_lo_plane = (X3 ? p.inter_bytes / 2 : 64u) >> 4;
+            const uint32_t inter_base = desc_lo(smem_u32(inter)) + (uint32_t)wg * ((64 * 128) >> 4);
+            uint32_t scale = 0;
+            for (int c = 0; c < p.n_chunks; ++c) {
+                uint32_t a_tap = inter_base + (uint32_t)c * (p.inter_bytes >> 4);
+                for (int k = 0; k < L2.KS; ++k) {
+                    mbar_wait(w_full + sW, phW);
+                    const uint32_t b_tap = w_base + sW * wtile_step;
+                    wgmma_fence();
+                    conv_tap_mma<MODE, N>(acc0, a_tap, b_tap, inter_lo_plane, b_lo_plane, hi, scale);
+                    conv_tap_mma<MODE, N>(acc1, a_tap + tile_step, b_tap, inter_lo_plane, b_lo_plane, hi, scale);
+                    wgmma_commit();
+                    wgmma_wait<1>();
+                    release();
+                    pend_w = sW;
+                    if (++sW == p.nW) sW = 0, phW ^= 1;
+                    scale = 1;
+                    a_tap += 128 >> 4;
+                }
+            }
+            wgmma_wait<0>();
+            wgmma_keep<N>(acc0);
+            wgmma_keep<N>(acc1);
+            release();
+            epilogue(it, L2, acc0, 0);
+            epilogue(it, L2, acc1, kTcM);
         };
         if (p.w_resident && n_items > 0) mbar_wait(w_full, 0);
         for (int n = 0; n < n_items; ++n) {
             const TcItem it = item_decode(items[n]);
-            if (it.mt == 2) run_item(std::true_type(), it);
+            if constexpr (FUSED) run_fused(it);
+            else if (it.mt == 2) run_item(std::true_type(), it);
             else run_item(std::false_type(), it);
         }
     }
@@ -548,9 +662,9 @@ bool tc_supported(const TcWeights &w, const ConvArgs &a) {
            (a.ups_u == 0 || a.Cout % 32 == 0) && a.Cout <= 3072;
 }
 
-template <int MODE, int N>
+template <int MODE, int N, bool FUSED>
 static int launch_mode(const TcArgs &p, int grid, size_t smem, cudaStream_t st) {
-    auto kern = conv1d_c4_tc_kernel<MODE, N>;
+    auto kern = conv1d_c4_tc_kernel<MODE, N, FUSED>;
     // function attributes are per device: one process may drive several GPUs (the reference's mp.spawn gives one each,
     // but nothing in the C ABI forbids a handle per device in one process)
     static size_t configured[kSmemCacheDevices] = {};
@@ -672,7 +786,8 @@ static int tc_plan(int n, const TcWeights *const *w, const ConvArgs *a, int prec
         L.bias_off = l * a0.Cout, L.w_res_off = res_off;
         res_off += (uint32_t)a[l].KS * p.wtile_bytes;
     }
-    for (int l = n; l < kTcMaxLayers; ++l) p.L[l] = p.L[0];
+    for (int l = n; l < 2 * kTcMaxLayers; ++l) p.L[l] = p.L[0];
+    p.fused_P = 0, p.off_inter = 0, p.inter_bytes = 0;
     if (getenv("SVB_TC_VERBOSE"))
         fprintf(stderr, "[tc] %d layer(s) Cin %d CoutP %d KS %d.. halo %d Tq %d | n_tile %d MT %d nA %d nW %d resident %d smem %zu\n", n,
                 a0.Cin, a0.CoutP, a0.KS, halo, a0.Tq, p.n_tile, p.MT, p.nA, p.nW, p.w_resident, smem);
@@ -681,21 +796,81 @@ static int tc_plan(int n, const TcWeights *const *w, const ConvArgs *a, int prec
     return SVB_OK;
 }
 
+// Plan of a fused launch over n ResBlock chains: a[0..n) are the c1 layers, a[n..2n) the c2 layers of the same step.
+// Every item is 256 c1 rows; the c1 slab slots, the intermediate (256 + 2 max h2 rows per 32-channel chunk), a weight
+// ring of at least 2 tiles (c1's and c2's tiles stream through it in order) and the biases of all 2n layers share the
+// shared memory.  Returns false when the shape is not one a fused launch runs or the layout does not fit.
+static bool tc_plan_fused(int n, const TcWeights *const *w, const ConvArgs *a, int precision, TcArgs &p, size_t &smem) {
+    if (n < 1 || n > kTcMaxLayers) return false;
+    const ConvArgs &a0 = a[0];
+    for (int l = 0; l < 2 * n; ++l) {
+        if (a[l].B != a0.B || a[l].Cin != a0.Cin || a[l].Cout != a0.Cin || a[l].CoutP != a0.Cin || a[l].Tq != a0.Tq ||
+            a[l].in_Tp != a0.in_Tp || a[l].out_Tp != a0.in_Tp || a[l].ups_u != 0 || a[l].cin_blk != 0 ||
+            a[l].in_slope != a0.in_slope || !w[l]->ok || w[l]->n_tile != a0.Cin || (l >= n && a[l].dil != 1))
+            return false;
+    }
+    if (a0.Cin != 32 && a0.Cin != 64) return false;
+    const int planes = precision == SVB_PREC_TF32X3 ? 2 : 1;
+    int h1 = 0, h2 = 0;
+    for (int l = 0; l < n; ++l) h1 = std::max(h1, (a[l].KS - 1) / 2 * a[l].dil), h2 = std::max(h2, (a[n + l].KS - 1) / 2);
+    if (h1 + h2 > kPad || 2 * h2 >= kTcM) return false;           // the shifted slab starts inside the zero padding
+    p.a = a0, p.n_layers = n;
+    p.work = nullptr, p.work_off = nullptr;
+    p.n_tile = a0.Cin, p.n_chunks = a0.Cin / kTcCK, p.blk_chunk_step = 0, p.col_blocks = 1;
+    p.MT = 2, p.w_resident = 0, p.w_res_bytes = 0;
+    p.wtile_bytes = (uint32_t)p.n_tile * 128 * planes;
+    p.pdl = 1;
+    if (const char *e = getenv("SVB_TC_PDL")) p.pdl = atoi(e) != 0;
+    p.fused_P = 2 * kTcM - 2 * h2;
+    p.op_bytes = (uint32_t)round_up(2 * kTcM + 2 * h1, 8) * 128 * planes;
+    p.inter_bytes = (uint32_t)round_up(2 * kTcM + 2 * h2, 8) * 128 * planes;
+    const size_t bias_bytes = kBiasBytes;                       // 2n x Cout <= 6 x 64 floats
+    const size_t budget = 227 * 1024 - bias_bytes;
+    int nA_pref = 3;
+    if (const char *e = getenv("SVB_TC_NA")) nA_pref = std::max(2, std::min(4, atoi(e)));
+    p.off_op = 1024 + kItemBytes;
+    const size_t inter_area = (size_t)p.n_chunks * p.inter_bytes;
+    p.nA = nA_pref;
+    if (p.off_op + (size_t)p.nA * p.op_bytes + inter_area + 2 * (size_t)p.wtile_bytes > budget) p.nA = 2;
+    if (p.off_op + (size_t)p.nA * p.op_bytes + inter_area + 2 * (size_t)p.wtile_bytes > budget) return false;
+    p.off_inter = p.off_op + (uint32_t)p.nA * p.op_bytes;
+    p.off_w = p.off_inter + (uint32_t)inter_area;
+    p.nW = std::min((int)((budget - p.off_w) / p.wtile_bytes), kMaxW);
+    p.off_bias = p.off_w + (uint32_t)round_up(p.nW * (int)p.wtile_bytes, 1024);
+    smem = (size_t)p.off_bias + bias_bytes;
+    if (smem > 227 * 1024) return false;
+    for (int l = 0; l < 2 * n; ++l) {
+        TcLayer &L = p.L[l];
+        L.in = a[l].in, L.res = a[l].res, L.out = a[l].out, L.bias = a[l].bias;
+        L.w = reinterpret_cast<const unsigned char *>(w[l]->blob[precision]);
+        L.KS = a[l].KS, L.dil = a[l].dil, L.out_scale = a[l].out_scale, L.accumulate = a[l].accumulate;
+        L.bias_off = l * a0.Cout, L.w_res_off = 0;
+    }
+    for (int l = 2 * n; l < 2 * kTcMaxLayers; ++l) p.L[l] = p.L[0];
+    p.groups_per_b = (a0.Tq + p.fused_P - 1) / p.fused_P;
+    p.total_groups = p.groups_per_b * a0.B;
+    return true;
+}
+
 template <int MODE>
-static int launch_n(const TcArgs &p, int grid, size_t smem, cudaStream_t st) {
+static int launch_n(const TcArgs &p, bool fused, int grid, size_t smem, cudaStream_t st) {
+    if (fused) {                // fused ResBlock steps: C = 32 or 64 only
+        SVB_CHECK(p.n_tile == 32 || p.n_tile == 64, SVB_ERR_INVALID, "tc conv: fused launch with %d columns per tile", p.n_tile);
+        return p.n_tile == 32 ? launch_mode<MODE, 32, true>(p, grid, smem, st) : launch_mode<MODE, 64, true>(p, grid, smem, st);
+    }
     switch (p.n_tile) {
-        case 32: return launch_mode<MODE, 32>(p, grid, smem, st);
-        case 64: return launch_mode<MODE, 64>(p, grid, smem, st);
-        case 96: return launch_mode<MODE, 96>(p, grid, smem, st);
-        default: return launch_mode<MODE, 128>(p, grid, smem, st);
+        case 32: return launch_mode<MODE, 32, false>(p, grid, smem, st);
+        case 64: return launch_mode<MODE, 64, false>(p, grid, smem, st);
+        case 96: return launch_mode<MODE, 96, false>(p, grid, smem, st);
+        default: return launch_mode<MODE, 128, false>(p, grid, smem, st);
     }
 }
 
-static int tc_dispatch(TcArgs &p, int precision, int grid, size_t smem, cudaStream_t st) {
+static int tc_dispatch(TcArgs &p, int precision, int grid, size_t smem, cudaStream_t st, bool fused = false) {
     switch (precision) {
-        case SVB_PREC_TF32: return launch_n<SVB_PREC_TF32>(p, grid, smem, st);
-        case SVB_PREC_TF32X3: return launch_n<SVB_PREC_TF32X3>(p, grid, smem, st);
-        default: return launch_n<SVB_PREC_BF16X3>(p, grid, smem, st);
+        case SVB_PREC_TF32: return launch_n<SVB_PREC_TF32>(p, fused, grid, smem, st);
+        case SVB_PREC_TF32X3: return launch_n<SVB_PREC_TF32X3>(p, fused, grid, smem, st);
+        default: return launch_n<SVB_PREC_BF16X3>(p, fused, grid, smem, st);
     }
 }
 
@@ -741,9 +916,11 @@ void tc_worklist_free(TcWorkList *wl) {
 }
 
 // The schedule itself is plain host code (no CUDA call): exposed for the CPU tests through svb_tc_schedule_probe.
-int tc_schedule(int n, const int *KS, const int *has_res, const int *accum, int Cin, int B, int Tq, int MT, int col_blocks, bool chain_ordered,
-                int grid, std::vector<int4> *items_out, std::vector<int> *off_out, double *balance_out) {
+// fused_P > 0: fused items (KS2 = c2's taps per layer) of fused_P output rows each, always 256 c1 rows, never split.
+int tc_schedule(int n, const int *KS, const int *KS2, const int *has_res, const int *accum, int Cin, int B, int Tq, int MT, int fused_P,
+                int col_blocks, bool chain_ordered, int grid, std::vector<int4> *items_out, std::vector<int> *off_out, double *balance_out) {
     const int tiles = (Tq + kTcM - 1) / kTcM;
+    const bool fused = fused_P > 0;
     // cost of an item in "taps of one tile": the MMA work plus a constant for the memory-bound part (slab, epilogue)
     const double beta = 160.0 / std::max(32, Cin);
     struct Unit {
@@ -751,20 +928,21 @@ int tc_schedule(int n, const int *KS, const int *has_res, const int *accum, int 
         int nblk, b, t0, mt, layer;     // layer < 0: all layers in order (chain-ordered unit)
     };
     auto unit_cost = [&](int layer, int mt) {
-        if (layer >= 0) return mt * (KS[layer] + beta + (has_res[layer] ? 1.0 : 0.0));
+        auto taps = [&](int l) { return KS[l] + (fused ? KS2[l] : 0); };
+        if (layer >= 0) return mt * (taps(layer) + beta + (has_res[layer] ? 1.0 : 0.0));
         double c = 0;
-        for (int l = 0; l < n; ++l) c += mt * (KS[l] + beta + (has_res[l] ? 1.0 : 0.0) + (accum[l] ? 1.0 : 0.0));
+        for (int l = 0; l < n; ++l) c += mt * (taps(l) + beta + (has_res[l] ? 1.0 : 0.0) + (accum[l] ? 1.0 : 0.0));
         return c;
     };
     std::vector<Unit> units;
     for (int nblk = 0; nblk < col_blocks; ++nblk)
         for (int b = 0; b < B; ++b)
-            for (int t = 0; t < tiles; t += MT) {
-                const int mt = std::min(MT, tiles - t);
+            for (int t0 = 0; t0 < (fused ? Tq : tiles * kTcM); t0 += (fused ? fused_P : MT * kTcM)) {
+                const int mt = fused ? 2 : std::min(MT, tiles - t0 / kTcM);
                 if (chain_ordered) {
-                    units.push_back({unit_cost(-1, mt), nblk, b, t * kTcM, mt, -1});
+                    units.push_back({unit_cost(-1, mt), nblk, b, t0, mt, -1});
                 } else {
-                    for (int l = 0; l < n; ++l) units.push_back({unit_cost(l, mt), nblk, b, t * kTcM, mt, l});
+                    for (int l = 0; l < n; ++l) units.push_back({unit_cost(l, mt), nblk, b, t0, mt, l});
                 }
             }
     // longest processing time first onto the least-loaded CTA.  When the units are too coarse for the SMs (balance below
@@ -790,7 +968,7 @@ int tc_schedule(int n, const int *KS, const int *has_res, const int *accum, int 
         const double bal = sum / grid / mx;
         if (bal <= balance) break;
         balance = bal, best_units = units, best_mine = mine;
-        if (balance >= 0.95) break;
+        if (balance >= 0.95 || fused) break;
         // split up to `grid` of the cheapest two-tile units (they sit at the end of the sorted list)
         int split = 0;
         for (size_t u = units.size(); u-- > 0 && split < grid;) {
@@ -852,37 +1030,71 @@ int tc_schedule(int n, const int *KS, const int *has_res, const int *accum, int 
     return SVB_OK;
 }
 
-int tc_worklist_build(int n, const TcWeights *const *w, const ConvArgs *a, int precision, bool chain_ordered, TcWorkList *out) {
+// plan of a merged (fused = false: n layers) or fused (n chains, 2n layers) launch
+static int tc_plan_multi(int n, const TcWeights *const *w, const ConvArgs *a, int precision, bool fused, TcArgs &p, size_t &smem) {
+    if (!fused) return tc_plan(n, w, a, precision, 0, p, smem);
+    SVB_CHECK(tc_plan_fused(n, w, a, precision, p, smem), SVB_ERR_INVALID, "tc conv: no fused layout for %d chains of C = %d", n, a[0].Cin);
+    return SVB_OK;
+}
+
+// Fused launches over the n chains of a step (c1 layers a[0..n), c2 layers a[n..2n)): the layout fits shared memory,
+// there are at least 4 items per CTA (fused items are never split, so fewer leave SMs idle where the two-launch path
+// balances with one-tile items), and both work lists of a stage (plain and chain-ordered) fit the per-CTA item table.
+// Bounds of the LPT schedule: a CTA's load ends at most one unit above the mean, so it holds at most
+// (mean + max cost) / min cost units.
+bool tc_fused_fits(int n, const TcWeights *const *w, const ConvArgs *a, int precision) {
     TcArgs p;
     size_t smem = 0;
-    SVB_TRY(tc_plan(n, w, a, precision, 0, p, smem));
+    if (!tc_plan_fused(n, w, a, precision, p, smem)) return false;
     const int grid = sm_count();
-    int KS[kTcMaxLayers], has_res[kTcMaxLayers], accum[kTcMaxLayers];
-    for (int l = 0; l < n; ++l) KS[l] = a[l].KS, has_res[l] = a[l].res != nullptr, accum[l] = a[l].accumulate;
+    const double units = (double)a[0].B * p.groups_per_b, beta = 160.0 / std::max(32, a[0].Cin);
+    if (units * n < 4.0 * grid) return false;
+    double sum = 0, mx = 0, mn = 1e30;
+    for (int l = 0; l < n; ++l) {
+        const double c = 2 * (a[l].KS + a[n + l].KS + beta + 1.0);
+        sum += c, mx = std::max(mx, c), mn = std::min(mn, c);
+    }
+    const double plain = (units * sum / grid + mx) / mn, chained = n * std::ceil(units / grid);
+    return plain <= kMaxItems && chained <= kMaxItems;
+}
+
+int tc_worklist_build(int n, const TcWeights *const *w, const ConvArgs *a, int precision, bool chain_ordered, TcWorkList *out, bool fused) {
+    TcArgs p;
+    size_t smem = 0;
+    SVB_TRY(tc_plan_multi(n, w, a, precision, fused, p, smem));
+    const int grid = sm_count();
+    const ConvArgs *ao = fused ? a + n : a;                      // the layers whose epilogue writes the output
+    int KS[kTcMaxLayers], KS2[kTcMaxLayers], has_res[kTcMaxLayers], accum[kTcMaxLayers];
+    for (int l = 0; l < n; ++l) KS[l] = a[l].KS, KS2[l] = ao[l].KS, has_res[l] = ao[l].res != nullptr, accum[l] = ao[l].accumulate;
     std::vector<int4> items;
     std::vector<int> off;
     double balance = 0;
-    SVB_TRY(tc_schedule(n, KS, has_res, accum, a[0].Cin, a[0].B, a[0].Tq, p.MT, p.col_blocks, chain_ordered, grid, &items, &off, &balance));
+    SVB_TRY(tc_schedule(n, KS, fused ? KS2 : nullptr, has_res, accum, a[0].Cin, a[0].B, a[0].Tq, p.MT, p.fused_P, p.col_blocks,
+                        chain_ordered, grid, &items, &off, &balance));
     tc_worklist_free(out);
     SVB_CUDA(cudaMalloc((void **)&out->items, std::max<size_t>(items.size(), 1) * sizeof(int4)));
     SVB_CUDA(cudaMalloc((void **)&out->off, off.size() * sizeof(int)));
     SVB_CUDA(cudaMemcpy(out->items, items.data(), items.size() * sizeof(int4), cudaMemcpyHostToDevice));
     SVB_CUDA(cudaMemcpy(out->off, off.data(), off.size() * sizeof(int), cudaMemcpyHostToDevice));
     out->grid = grid, out->n_items = (int)items.size(), out->MT = p.MT, out->n_layers = n, out->chain_ordered = chain_ordered;
+    out->fused = fused;
     if (getenv("SVB_TC_VERBOSE"))
         fprintf(stderr, "[tc] work list: %d layers, %zu items over %d CTAs, balance %.3f (mean / max load)\n", n, items.size(), grid, balance);
     return SVB_OK;
 }
 
-int launch_conv_tc_multi(int n, const TcWeights *const *w, const ConvArgs *a, int precision, cudaStream_t st, const TcWorkList &wl) {
+int launch_conv_tc_multi(int n, const TcWeights *const *w, const ConvArgs *a, int precision, cudaStream_t st, const TcWorkList &wl, bool fused) {
     SVB_CHECK(precision >= SVB_PREC_TF32 && precision <= SVB_PREC_BF16X3, SVB_ERR_INVALID, "tc conv: bad precision %d", precision);
     TcArgs p;
     size_t smem = 0;
-    SVB_TRY(tc_plan(n, w, a, precision, 0, p, smem));
-    SVB_CHECK(wl.items && wl.n_layers == n && wl.MT == p.MT && wl.grid == sm_count(), SVB_ERR_STATE,
+    SVB_TRY(tc_plan_multi(n, w, a, precision, fused, p, smem));
+    SVB_CHECK(wl.items && wl.n_layers == n && wl.MT == p.MT && wl.fused == fused && wl.grid == sm_count(), SVB_ERR_STATE,
               "tc conv: work list was built for another plan (layers %d / %d, MT %d / %d)", wl.n_layers, n, wl.MT, p.MT);
     p.work = wl.items, p.work_off = wl.off;
-    return tc_dispatch(p, precision, wl.grid, smem, st);
+    if (fused && getenv("SVB_TC_VERBOSE"))
+        fprintf(stderr, "[tc] fused %d chain(s) C %d KS %d.. dil %d.. Tq %d | P %d nA %d nW %d smem %zu\n", n, a[0].Cin, a[0].KS, a[0].dil,
+                a[0].Tq, p.fused_P, p.nA, p.nW, smem);
+    return tc_dispatch(p, precision, wl.grid, smem, st, fused);
 }
 
 }  // namespace svb
@@ -899,7 +1111,7 @@ extern "C" int64_t svb_tc_schedule_probe(int32_t n_layers, const int32_t *KS, co
     std::vector<int> off;
     int ks[svb::kTcMaxLayers], hr[svb::kTcMaxLayers], ac[svb::kTcMaxLayers];
     for (int l = 0; l < n_layers; ++l) ks[l] = KS[l], hr[l] = has_res[l], ac[l] = accumulate[l];
-    SVB_TRY(svb::tc_schedule(n_layers, ks, hr, ac, Cin, B, Tq, MT, col_blocks, chain_ordered != 0, grid, &items, &off, balance_out));
+    SVB_TRY(svb::tc_schedule(n_layers, ks, nullptr, hr, ac, Cin, B, Tq, MT, 0, col_blocks, chain_ordered != 0, grid, &items, &off, balance_out));
     SVB_CHECK((int64_t)items.size() <= items_capacity, SVB_ERR_INVALID, "tc_schedule_probe: %zu items, capacity %lld", items.size(),
               (long long)items_capacity);
     for (size_t i = 0; i < items.size(); ++i) {
@@ -907,5 +1119,38 @@ extern "C" int64_t svb_tc_schedule_probe(int32_t n_layers, const int32_t *KS, co
         o[0] = items[i].x & 0xff, o[1] = (items[i].x >> 8) & 0xffff, o[2] = items[i].y, o[3] = items[i].z, o[4] = items[i].x >> 24;
     }
     for (int c = 0; c <= grid; ++c) off_out[c] = off[c];
+    return (int64_t)items.size();
+}
+
+// Host-only view of a fused schedule (ResBlock steps c1 + c2 in one item): the items as svb_tc_schedule_probe gives them,
+// each followed by the first padded row and the row count of its c1 slab copy (two more int32 per item, 7 in all).  The
+// output rows per item, P = 256 - 2 max((KS2 - 1) / 2), go to *P_out.
+extern "C" int64_t svb_tc_fused_schedule_probe(int32_t n_layers, const int32_t *KS1, const int32_t *dil1, const int32_t *KS2,
+                                               const int32_t *accumulate, int32_t Cin, int32_t B, int32_t Tq, int32_t chain_ordered,
+                                               int32_t grid, int32_t *items_out, int64_t items_capacity, int32_t *off_out,
+                                               int32_t *P_out, double *balance_out) {
+    SVB_CHECK(n_layers >= 1 && n_layers <= svb::kTcMaxLayers && KS1 && dil1 && KS2 && accumulate && B > 0 && Tq > 0 && grid >= 1 &&
+                  items_out && off_out && P_out && balance_out,
+              SVB_ERR_INVALID, "tc_fused_schedule_probe: bad argument");
+    int ks1[svb::kTcMaxLayers], ks2[svb::kTcMaxLayers], hr[svb::kTcMaxLayers], ac[svb::kTcMaxLayers], h2 = 0;
+    for (int l = 0; l < n_layers; ++l) {
+        SVB_CHECK(KS1[l] >= 1 && KS2[l] >= 1 && dil1[l] >= 1 && (KS1[l] - 1) / 2 * dil1[l] + (KS2[l] - 1) / 2 <= svb::kPad && KS2[l] < svb::kTcM,
+                  SVB_ERR_INVALID, "tc_fused_schedule_probe: layer %d: taps %d / %d, dilation %d", l, KS1[l], KS2[l], dil1[l]);
+        ks1[l] = KS1[l], ks2[l] = KS2[l], hr[l] = 1, ac[l] = accumulate[l], h2 = std::max(h2, (KS2[l] - 1) / 2);
+    }
+    const int P = 2 * svb::kTcM - 2 * h2;
+    std::vector<int4> items;
+    std::vector<int> off;
+    SVB_TRY(svb::tc_schedule(n_layers, ks1, ks2, hr, ac, Cin, B, Tq, 2, P, 1, chain_ordered != 0, grid, &items, &off, balance_out));
+    SVB_CHECK((int64_t)items.size() <= items_capacity, SVB_ERR_INVALID, "tc_fused_schedule_probe: %zu items, capacity %lld", items.size(),
+              (long long)items_capacity);
+    for (size_t i = 0; i < items.size(); ++i) {
+        int32_t *o = items_out + 7 * i;
+        const int l = items[i].x & 0xff;
+        o[0] = l, o[1] = (items[i].x >> 8) & 0xffff, o[2] = items[i].y, o[3] = items[i].z, o[4] = items[i].x >> 24;
+        svb::tc_fused_slab(items[i].z, (ks1[l] - 1) / 2 * dil1[l], (ks2[l] - 1) / 2, svb::c4t_rows(Tq), &o[5], &o[6]);
+    }
+    for (int c = 0; c <= grid; ++c) off_out[c] = off[c];
+    *P_out = P;
     return (int64_t)items.size();
 }

@@ -33,13 +33,21 @@ struct TcWorkList {
     int *off = nullptr;
     int grid = 0, n_items = 0, MT = 0, n_layers = 0;
     bool chain_ordered = false;
+    bool fused = false;
 };
-int tc_worklist_build(int n, const TcWeights *const *w, const ConvArgs *a, int precision, bool chain_ordered, TcWorkList *out);
+// fused = true: n ResBlock chains, w / a hold the c1 layers [0, n) and the c2 layers [n, 2n) of one step, and every item
+// runs c1 and c2 of one chain for P output rows (conv_tc.cu: conv1d_c4_tc_kernel, FUSED)
+int tc_worklist_build(int n, const TcWeights *const *w, const ConvArgs *a, int precision, bool chain_ordered, TcWorkList *out,
+                      bool fused = false);
 void tc_worklist_free(TcWorkList *wl);
 // the per-CTA item list of a merged launch is bounded (shared memory): very long batches fall back to one launch per layer
 bool tc_merge_fits(int n, int B, int Tq, int Cout, int n_tile);
+// whether one step of n ResBlock1 chains (w / a as for fused work lists) runs as a fused launch: C = 32 or 64, and the
+// layout fits shared memory (not in tf32x3) and the item table
+bool tc_fused_fits(int n, const TcWeights *const *w, const ConvArgs *a, int precision);
 // one persistent launch over `n` layers that share channels / rows / upsampling (taps, dilation and pointers may differ)
-int launch_conv_tc_multi(int n, const TcWeights *const *w, const ConvArgs *a, int precision, cudaStream_t st, const TcWorkList &wl);
+int launch_conv_tc_multi(int n, const TcWeights *const *w, const ConvArgs *a, int precision, cudaStream_t st, const TcWorkList &wl,
+                         bool fused = false);
 // max_ctas > 0 caps the persistent grid (used to run independent ResBlock chains side by side on SM subsets)
 int launch_conv_tc(const TcWeights &w, const ConvArgs &a, int precision, cudaStream_t st, int max_ctas = 0);
 

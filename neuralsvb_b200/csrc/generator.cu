@@ -78,6 +78,36 @@ struct Plan {
     }
 };
 
+ConvArgs resblock_args(const ConvLayer &L, const float *in, float *out, const float *res, float scale, int accumulate, int B, int Tq,
+                       int Tp, float in_slope) {
+    ConvArgs a;
+    a.in = in, a.w = L.w, a.bias = L.b, a.res = res, a.out = out;
+    a.B = B, a.Cin = L.Cin, a.in_Tp = Tp, a.Cout = L.Cout, a.out_Tp = Tp, a.CoutP = L.CoutP, a.Tq = Tq;
+    a.KS = L.KS, a.dil = L.dil, a.ups_u = 0, a.in_slope = in_slope, a.out_scale = scale, a.accumulate = accumulate;
+    return a;
+}
+
+// Inference runs every ResBlock1 step x <- x + c2(lrelu(c1(lrelu(x)))) of a C <= 64 stage as ONE launch over its chains
+// (conv_tc.cu: fused items; c1's output stays in shared memory instead of a round trip through HBM) when the fused layout
+// fits.  Training keeps two launches per step: its tape needs every c1 input in HBM.
+bool stage_fused(const svb_gen *g, const Stage &s, int B, int Ti) {
+    const int nk = g->cfg.n_resblock_kernels, nd = g->cfg.n_dilations;
+    if (!g->fuse || !g->merge || g->chains > 1 || g->training || g->cfg.resblock != 1 || g->cfg.precision == SVB_PREC_FP32 || s.C > 64 ||
+        nk > kTcMaxLayers)
+        return false;
+    for (int m = 0; m < nd; ++m) {
+        ConvArgs a[2 * kTcMaxLayers];
+        const TcWeights *w[2 * kTcMaxLayers];
+        for (int j = 0; j < nk; ++j) {
+            a[j] = resblock_args(s.c1[j][m], nullptr, nullptr, nullptr, 1.f, 0, B, Ti, c4t_rows(Ti), 0.1f);
+            a[nk + j] = resblock_args(s.c2[j][m], nullptr, nullptr, nullptr, 1.f, 0, B, Ti, c4t_rows(Ti), 0.1f);
+            w[j] = &s.c1[j][m].tc, w[nk + j] = &s.c2[j][m].tc;
+        }
+        if (!tc_fused_fits(nk, w, a, g->cfg.precision)) return false;
+    }
+    return true;
+}
+
 Buffers plan_workspace(const svb_gen *g, int B, int T, size_t *total) {
     Plan p;
     Buffers b;
@@ -91,12 +121,15 @@ Buffers plan_workspace(const svb_gen *g, int B, int T, size_t *total) {
         const size_t n = c4t_floats(B, s.C, Ti) * 4;
         b.X.push_back(p.take(n)), b.S.push_back(p.take(n));
         b.A.emplace_back(), b.R.emplace_back();
+        const bool fused = stage_fused(g, s, B, Ti);
         for (int j = 0; j < g->cfg.n_resblock_kernels; ++j) {
-            // inference: one A / R buffer per chain, reused by every dilation; training: every conv input is kept (the tape)
-            std::vector<size_t> a(g->cfg.n_dilations), r(g->cfg.n_dilations);
+            // inference: one A / R buffer per chain, reused by every dilation; training: every conv input is kept (the tape).
+            // Fused steps have no A, and their x ping-pongs between two R buffers: an item reads its input rows plus a halo
+            // that other CTAs' items of the same launch write.
+            std::vector<size_t> a(fused ? 0 : g->cfg.n_dilations), r(g->cfg.n_dilations);
             for (int m = 0; m < g->cfg.n_dilations; ++m) {
-                a[m] = (m == 0 || g->training) ? p.take(n) : a[0];
-                r[m] = (m == 0 || g->training) ? p.take(n) : r[0];
+                if (!fused) a[m] = (m == 0 || g->training) ? p.take(n) : a[0];
+                r[m] = fused ? (m < 2 ? p.take(n) : r[m - 2]) : (m == 0 || g->training) ? p.take(n) : r[0];
             }
             b.A.back().push_back(a), b.R.back().push_back(r);
         }
@@ -154,17 +187,17 @@ int run_conv(svb_gen *g, const ConvLayer &L, const float *in, int in_Tp, float *
 
 // One merged launch over the nk layers `Ls` (same shape class): layer j reads in[j], writes out[j], adds res[j].
 // chain_ordered: later layers accumulate into the output of earlier ones (the ResBlock sum), see TcWorkList.
+// fused: the 2 nk entries are the c1 layers of nk chains, then their c2 layers (conv_tc.cuh: tc_worklist_build); the launch
+// is profiled with the bytes and FLOPs of the 2 nk convolutions it replaces, so the byte model stays the same across paths.
 int run_conv_multi(svb_gen *g, int stage, int nk, const ConvLayer *const *Ls, const float *const *in, float *const *out,
                    const float *const *res, const float *scale, const int *accumulate, bool chain_ordered, int B, int Tq, int Tp,
-                   float in_slope, cudaStream_t st) {
-    ConvArgs a[kTcMaxLayers];
-    const TcWeights *w[kTcMaxLayers];
+                   float in_slope, cudaStream_t st, bool fused = false) {
+    ConvArgs a[2 * kTcMaxLayers];
+    const TcWeights *w[2 * kTcMaxLayers];
     double bytes = 0, flops = 0;
-    for (int j = 0; j < nk; ++j) {
+    for (int j = 0; j < (fused ? 2 * nk : nk); ++j) {
         const ConvLayer &L = *Ls[j];
-        a[j].in = in[j], a[j].w = L.w, a[j].bias = L.b, a[j].res = res[j], a[j].out = out[j];
-        a[j].B = B, a[j].Cin = L.Cin, a[j].in_Tp = Tp, a[j].Cout = L.Cout, a[j].out_Tp = Tp, a[j].CoutP = L.CoutP, a[j].Tq = Tq;
-        a[j].KS = L.KS, a[j].dil = L.dil, a[j].ups_u = 0, a[j].in_slope = in_slope, a[j].out_scale = scale[j], a[j].accumulate = accumulate[j];
+        a[j] = resblock_args(L, in[j], out[j], res[j], scale[j], accumulate[j], B, Tq, Tp, in_slope);
         w[j] = &L.tc;
         bytes += 4.0 * ((double)B * Tq * L.Cin + (double)B * Tq * L.Cout * (1 + (res[j] ? 1 : 0) + (accumulate[j] ? 1 : 0)));
         flops += 2.0 * L.macs_per_row * (double)B * Tq;
@@ -174,10 +207,10 @@ int run_conv_multi(svb_gen *g, int stage, int nk, const ConvLayer *const *Ls, co
     ProfScope ps(g, st, "conv1d_c4_tc (resblock)", bytes, flops);
     // the list depends on the plan (MT) of this layer set: try the cached one, rebuild on a plan mismatch
     for (int attempt = 0; attempt < 2; ++attempt) {
-        const int key = stage * 4 + (chain_ordered ? 2 : 0) + attempt;
+        const int key = stage * 8 + (fused ? 4 : 0) + (chain_ordered ? 2 : 0) + attempt;
         TcWorkList &wl = g->worklists[key];
-        if (!wl.items) SVB_TRY(tc_worklist_build(nk, w, a, g->cfg.precision, chain_ordered, &wl));
-        const int rc = launch_conv_tc_multi(nk, w, a, g->cfg.precision, st, wl);
+        if (!wl.items) SVB_TRY(tc_worklist_build(nk, w, a, g->cfg.precision, chain_ordered, &wl, fused));
+        const int rc = launch_conv_tc_multi(nk, w, a, g->cfg.precision, st, wl, fused);
         if (rc != SVB_ERR_STATE) return rc;
     }
     set_error("merged launch: no cached work list matches the plan of stage %d", stage);
@@ -277,8 +310,27 @@ int forward_impl(svb_gen *g, const float *mel, bool mel_frame_major, const float
         const bool par = g->chains > 1 && nk > 1 && nk <= 3 && g->cfg.precision != SVB_PREC_FP32 && !g->profile;
         int sms = 0;
         SVB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, g->device));
+        const bool fused = stage_fused(g, s, B, Ti);
+        if (fused) {
+            for (int m = 0; m < nd; ++m) {
+                const bool last = m == nd - 1;
+                const ConvLayer *L[2 * kTcMaxLayers];
+                const float *xin[2 * kTcMaxLayers], *res[2 * kTcMaxLayers];
+                float *dst[2 * kTcMaxLayers], scl[2 * kTcMaxLayers];
+                int acc[2 * kTcMaxLayers];
+                for (int j = 0; j < nk; ++j) {
+                    L[j] = &s.c1[j][m], L[nk + j] = &s.c2[j][m];
+                    xin[j] = m == 0 ? X : F(bf.R[i][j][m - 1]), xin[nk + j] = nullptr;
+                    res[j] = nullptr, res[nk + j] = xin[j];
+                    dst[j] = nullptr, dst[nk + j] = last ? S : F(bf.R[i][j][m]);
+                    scl[j] = 1.f, scl[nk + j] = last ? 1.f / nk : 1.f;
+                    acc[j] = 0, acc[nk + j] = (last && j > 0) ? 1 : 0;
+                }
+                SVB_TRY(run_conv_multi(g, (int)i, nk, L, xin, dst, res, scl, acc, last, B, Ti, Tip, 0.1f, st, true));
+            }
+        }
         // merged schedule: step m of all nk chains in ONE persistent launch (the chains only share their input)
-        bool merged = g->merge && !par && nk > 1 && nk <= kTcMaxLayers && g->cfg.precision != SVB_PREC_FP32 &&
+        bool merged = !fused && g->merge && !par && nk > 1 && nk <= kTcMaxLayers && g->cfg.precision != SVB_PREC_FP32 &&
                       s.c1[0][0].tc.ok && tc_merge_fits(nk, B, Ti, s.C, s.c1[0][0].tc.n_tile);
         for (int j = 0; merged && j < nk; ++j)
             for (int m = 0; m < nd; ++m) {
@@ -318,7 +370,7 @@ int forward_impl(svb_gen *g, const float *mel, bool mel_frame_major, const float
             }
         }
         if (par) SVB_CUDA(cudaEventRecord(g->ev_fork, st));
-        for (int j = 0; j < nk && !merged; ++j) {
+        for (int j = 0; j < nk && !merged && !fused; ++j) {
             cudaStream_t cs = par ? g->side[j] : st;
             // SM share of a chain ~ its cost: kernel size plus a constant for the memory-bound part
             int cap = 0;
@@ -412,6 +464,7 @@ extern "C" int svb_gen_create(const svb_gen_config *cfg, int device, svb_gen_t *
     }
     if (const char *e = getenv("SVB_CHAINS")) g->chains = atoi(e);
     if (const char *e = getenv("SVB_MERGE")) g->merge = atoi(e) != 0;
+    if (const char *e = getenv("SVB_FUSE")) g->fuse = atoi(e) != 0;
     if (const char *e = getenv("SVB_CHAIN_BIAS")) g->chain_bias = atof(e);
     *out = g;
     return SVB_OK;

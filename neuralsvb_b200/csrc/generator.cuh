@@ -141,6 +141,8 @@ struct svb_gen {
     // merged launches: the ResBlock chains of a stage step together in one persistent launch (conv_tc.cuh: TcWorkList).
     // Lists depend on the stage, the batch / length and the plan's MT; cached per (stage, chain_ordered, MT).
     bool merge = true;              // SVB_MERGE=0: one launch per convolution (round-1 schedule)
+    bool fuse = true;               // SVB_FUSE=0: two launches per ResBlock1 step also where the fused launch fits (the
+                                    // reference path of the bit-identity tests)
     std::map<int, svb::TcWorkList> worklists;
 
     bool profile = false;

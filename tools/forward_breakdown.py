@@ -6,7 +6,9 @@
 svb_gen_enable_timing(handle, 2) records one CUDA-event pair around every launch, in launch order (the NSF source
 then runs on the main stream, so the records are serial).  Each record is labelled from the generator config:
 mel layout, NSF source, conv_pre, and per upsampling stage the upsampler, noise_conv_add and, per dilation step m,
-the merged c1 and c2 launches of the three ResBlock chains; conv_post last.  Per launch class it prints:
+the merged c1 and c2 launches of the three ResBlock chains -- or, in the C <= 64 stages, ONE fused launch per step that
+runs c1 and c2 (not in tf32x3, whose layout does not fit; SVB_FUSE=0 labels a build or handle without fused launches);
+conv_post last.  Per launch class it prints:
 
 * ms (mean over the timed forwards);
 * tensor fraction: algorithmic FLOPs / (ms x the operand mode's dense peak), the peak (H100 SXM data sheet, 989 TFLOP/s
@@ -14,7 +16,8 @@ the merged c1 and c2 launches of the three ResBlock chains; conv_post last.  Per
 * GB/s of the layer-streaming byte model (input once, output once, residual / running sum once);
 * modelled L2 -> shared-memory weight bytes: every work item streams the (column block, input chunk, tap) tiles
   of its layer once, so the bytes scale with 1 / tiles per item (MT, `--mt`; balance splits into one-tile items are
-  not modelled); resident-weight launches (C = 32) load each layer's tiles once per CTA.
+  not modelled); resident-weight launches (C = 32) load each layer's tiles once per CTA.  A fused item (P = 246
+  output rows, 256 c1 rows) streams the tiles of both convolutions through the ring.
 """
 import argparse
 import contextlib
@@ -57,8 +60,16 @@ def weight_bytes(precision, cin, coutp, ks_list, B, rows, mt, grid=132):
     return sum(items * chunks * k * tile for k in ks_list)
 
 
-def labels(h, B, T, precision, mt):
-    """(label, class, modelled weight bytes) per record, in the generator's launch order (every stage merged)."""
+def fused_weight_bytes(precision, C, ks_list, B, rows, P=246):
+    """Modelled L2 -> smem weight bytes of one fused launch: every item streams c1's and c2's tiles once."""
+    tile = C * 128 * PLANES[precision]
+    items = B * ((rows + P - 1) // P)
+    return sum(items * (C // 32) * 2 * k * tile for k in ks_list)
+
+
+def labels(h, B, T, precision, mt, fuse=True):
+    """(label, class, modelled weight bytes) per record, in the generator's launch order (every stage merged; the C <= 64
+    stages fused unless `fuse` is off or the precision is tf32x3)."""
     out = [('mel layout', 'mel layout', 0.0), ('nsf source', 'nsf source', 0.0)]
     C0 = h['upsample_initial_channel']
     out.append(('conv_pre', 'conv_pre', weight_bytes(precision, h['audio_num_mel_bins'], C0, [7], B, T, mt)))
@@ -70,6 +81,9 @@ def labels(h, B, T, precision, mt):
         out.append((f'stage{i} noise_conv_add', 'noise_conv_add', 0.0))
         Ti = Tin * u
         for m, _ in enumerate(h['resblock_dilation_sizes'][0]):
+            if fuse and C <= 64 and precision != 'tf32x3':
+                out.append((f'stage{i} m{m} c1+c2', f'stage{i} (C={C}) c1+c2 fused', fused_weight_bytes(precision, C, ks, B, Ti)))
+                continue
             wb = weight_bytes(precision, C, C, ks, B, Ti, mt)
             out.append((f'stage{i} m{m} c1', f'stage{i} (C={C}) c1', wb))
             out.append((f'stage{i} m{m} c2', f'stage{i} (C={C}) c2', wb))
@@ -99,7 +113,7 @@ def main():
     model = model.eval().to(dev)
     lib, handle = _native.lib(), model.native_handle(dev)
     mel, f0 = (t.to(dev) for t in S.make_mel_f0(B_CLIPS, T_FRAMES, 1234))
-    lab = labels(h, B_CLIPS, T_FRAMES, args.precision, args.mt)
+    lab = labels(h, B_CLIPS, T_FRAMES, args.precision, args.mt, fuse=os.environ.get('SVB_FUSE', '1') != '0')
     name = ctypes.create_string_buffer(64)
     ms, by, fl = ctypes.c_float(), ctypes.c_double(), ctypes.c_double()
     rec = None
