@@ -407,6 +407,16 @@ int forward_impl(svb_gen *g, const float *mel, bool mel_frame_major, const float
         }
         if (par) SVB_CUDA(cudaStreamWaitEvent(st, g->ev_chain[nk - 1], 0));
         g->taps["stage" + std::to_string(i)] = Tap{S, s.C, Ti, Tip, false};
+        // The tape as taps: every leaky-relu input of the ResBlocks, x{m} (input of step m; x0 is ups{i}) and, for ResBlock1,
+        // t{m} (c1's output).  Only training keeps one buffer per step; inference reuses A / R across the steps.
+        for (int j = 0; j < nk && g->training; ++j) {
+            const std::string rb = "resblocks." + std::to_string(i * nk + j);
+            for (int m = 0; m < nd; ++m) {
+                const size_t xm = m == 0 ? bf.X[i] : (g->cfg.resblock == 1 || m % 2) ? bf.R[i][j][m - 1] : bf.A[i][j][m - 1];
+                g->taps[rb + ".x" + std::to_string(m)] = Tap{F(xm), s.C, Ti, Tip, false};
+                if (g->cfg.resblock == 1) g->taps[rb + ".t" + std::to_string(m)] = Tap{F(bf.A[i][j][m]), s.C, Ti, Tip, false};
+            }
+        }
         x_in = S, Tin = Ti, Tin_p = Tip;
     }
     // x = tanh(conv_post(leaky_relu(x)))   default slope 0.01   :165-167

@@ -83,33 +83,42 @@ def source_module(f0_up, w, rand_ini, noise, sr=22050):
 
 
 # ------------------------------------------------------------------ generator
-def resblock1(x, w, prefix, k, dil):
-    """ResBlock1.forward (hifigan.py:54-61)."""
+def _leaky_relu(site, x, slope):
+    return F.leaky_relu(x, slope)
+
+
+def resblock1(x, w, prefix, k, dil, act=_leaky_relu):
+    """ResBlock1.forward (hifigan.py:54-61).  ``act(site, x, slope)`` is every leaky relu; the sites are
+    ``{prefix}.x{m}`` (the input of step m) and ``{prefix}.t{m}`` (convs1's output)."""
     for m, d in enumerate(dil):
-        xt = F.leaky_relu(x, LRELU_SLOPE)
+        xt = act(f'{prefix}.x{m}', x, LRELU_SLOPE)
         xt = F.conv1d(xt, w[f'{prefix}.convs1.{m}.weight'], w[f'{prefix}.convs1.{m}.bias'],
                       dilation=d, padding=get_padding(k, d))
-        xt = F.leaky_relu(xt, LRELU_SLOPE)
+        xt = act(f'{prefix}.t{m}', xt, LRELU_SLOPE)
         xt = F.conv1d(xt, w[f'{prefix}.convs2.{m}.weight'], w[f'{prefix}.convs2.{m}.bias'],
                       padding=get_padding(k, 1))
         x = xt + x
     return x
 
 
-def resblock2(x, w, prefix, k, dil):
-    """ResBlock2.forward (hifigan.py:81-86)."""
+def resblock2(x, w, prefix, k, dil, act=_leaky_relu):
+    """ResBlock2.forward (hifigan.py:81-86); ``act`` as in resblock1, sites ``{prefix}.x{m}``."""
     for m, d in enumerate(dil):
-        xt = F.leaky_relu(x, LRELU_SLOPE)
+        xt = act(f'{prefix}.x{m}', x, LRELU_SLOPE)
         xt = F.conv1d(xt, w[f'{prefix}.convs.{m}.weight'], w[f'{prefix}.convs.{m}.bias'],
                       dilation=d, padding=get_padding(k, d))
         x = xt + x
     return x
 
 
-def generator_forward(w, h, mel, f0=None, rand_ini=None, noise=None, taps=None):
+def generator_forward(w, h, mel, f0=None, rand_ini=None, noise=None, taps=None, act=_leaky_relu):
     """HifiGanGenerator.forward (hifigan.py:144-169) on FOLDED weights ``w``
     (see fold_weight_norm).  mel [B,80,T]; f0 [B,T] Hz or None.  ``taps``: an
-    optional dict that receives named intermediates for layer-level checks."""
+    optional dict that receives named intermediates for layer-level checks.
+    ``act(site, x, slope)`` is called at every leaky relu, named after the tap
+    that holds its input: ``conv_pre`` and ``stage{i}`` (upsampler inputs, the
+    last stage's at slope 0.01 before conv_post) and the ResBlock sites of
+    resblock1 / resblock2."""
     rates = h['upsample_rates']
     ksz = h['upsample_kernel_sizes']
     nk = len(h['resblock_kernel_sizes'])
@@ -125,7 +134,7 @@ def generator_forward(w, h, mel, f0=None, rand_ini=None, noise=None, taps=None):
     if taps is not None:
         taps['conv_pre'] = x
     for i, (u, k) in enumerate(zip(rates, ksz)):
-        x = F.leaky_relu(x, LRELU_SLOPE)
+        x = act('conv_pre' if i == 0 else f'stage{i - 1}', x, LRELU_SLOPE)
         x = F.conv_transpose1d(x, w[f'ups.{i}.weight'], w[f'ups.{i}.bias'], stride=u, padding=(k - u) // 2)
         if har is not None:
             if i + 1 < len(rates):
@@ -139,12 +148,12 @@ def generator_forward(w, h, mel, f0=None, rand_ini=None, noise=None, taps=None):
         xs = None
         for j, (rk, dil) in enumerate(zip(h['resblock_kernel_sizes'], h['resblock_dilation_sizes'])):
             fn = resblock1 if h['resblock'] == '1' else resblock2
-            r = fn(x, w, f'resblocks.{i * nk + j}', rk, dil)
+            r = fn(x, w, f'resblocks.{i * nk + j}', rk, dil, act)
             xs = r if xs is None else xs + r
         x = xs / nk
         if taps is not None:
             taps[f'stage{i}'] = x
-    x = F.leaky_relu(x)                       # default slope 0.01 (hifigan.py:165, SURVEY D9)
+    x = act(f'stage{len(rates) - 1}', x, 0.01)   # F.leaky_relu's default slope (hifigan.py:165, SURVEY D9)
     x = F.conv1d(x, w['conv_post.weight'], w['conv_post.bias'], padding=3)
     return torch.tanh(x)
 

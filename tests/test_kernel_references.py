@@ -1,6 +1,6 @@
 """CPU: the float64 references of the kernel-level GPU tests (tests/test_gpu_stft_kernels.py, test_gpu_disc_kernels.py,
-test_gpu_acoustic_kernels.py) against the oracle (oracle/hifigan.py, oracle/frontend.py, oracle/vc_asr.py), which is pinned to
-the reference fixtures.  A wrong reference
+test_gpu_acoustic_kernels.py, test_gpu_generator_backward.py) against the oracle (oracle/hifigan.py, oracle/frontend.py,
+oracle/vc_asr.py), which is pinned to the reference fixtures.  A wrong reference
 would let a wrong kernel pass its test; here it fails without a GPU."""
 import os
 
@@ -14,6 +14,7 @@ from oracle import hifigan as O
 from oracle import vc_asr as OV
 from tests import test_gpu_acoustic_kernels as A
 from tests import test_gpu_disc_kernels as D
+from tests import test_gpu_generator_backward as G
 from tests import test_gpu_stft_kernels as T
 
 
@@ -120,3 +121,32 @@ def test_vc_asr_oracle_runs_in_float64_and_matches_the_fixture():
         h = OV.vc_asr_h_content(w, S.make_vc_asr_mel(B, T, 1234).double())
     assert h.dtype == torch.float64
     assert _rel(h, g['h_content']) < 1e-5
+
+
+def test_masked_generator_reference_with_its_own_masks_is_autograd():
+    """test_gpu_generator_backward's reference (leaky relus at given masks, NSF sines passed in) fed the masks of its own
+    pre-activations is plain float64 autograd through the oracle: the same waveform and every gradient to 1e-12."""
+    h = S.small_config(True)
+    B, T, hop = 2, 24, 16
+    sd = S.make_generator_state_dict(h, 1234)
+    mel, f0 = (t.double() for t in S.make_mel_f0(B, T, 1234))
+    ri, nz = (t.double() for t in S.make_nsf_noise(B, T * hop, 1234))
+    cot = torch.randn(B, 1, T * hop, generator=torch.Generator().manual_seed(7), dtype=torch.float64)
+    pre = {}
+
+    def record(site, x, slope):
+        assert site not in pre, site
+        pre[site] = x.detach()
+        return F.leaky_relu(x, slope)
+    p = {k: v.double().requires_grad_(True) for k, v in sd.items()}
+    y = O.generator_forward(O.fold_weight_norm(p), h, mel, f0, ri, nz, act=record)
+    (y * cot).sum().backward()
+    nk, nd, n_ups = len(h['resblock_kernel_sizes']), len(h['resblock_dilation_sizes'][0]), len(h['upsample_rates'])
+    assert len(pre) == 1 + n_ups + n_ups * nk * nd * 2
+    with torch.no_grad():
+        assert torch.equal(y, O.generator_forward(O.fold_weight_norm(p), h, mel, f0, ri, nz))
+    y_m, _, g_m, _ = G.reference(h, sd, mel, f0, G.nsf_sines(h, f0, ri, nz), cot, G.masked_act(pre.__getitem__))
+    assert _rel(y_m, y.detach()) < 1e-12
+    assert set(g_m) == set(p)
+    for k, t in p.items():
+        assert _rel(g_m[k], t.grad) < 1e-12, k
