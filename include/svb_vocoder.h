@@ -190,6 +190,16 @@ int svb_tc_layer_create(int32_t Cin, int32_t Cout, int32_t K, int32_t stride, in
  * 32-channel chunks (pairs of narrow groups share a tile). */
 int svb_tc_layer_create_grouped(int32_t Cin, int32_t Cout, int32_t K, int32_t stride, int32_t pad, int32_t groups,
                                 int32_t precision, int device, svb_tc_layer_t **out);
+/* 2-D convolutions: Conv2d(Cin, Cout, (KH, KW), stride (SH, SW), padding (PH, PW)) of the mel discriminator
+ * (modules/fastspeech/multi_window_disc.py:16-30, 3x3 / stride 2 / padding 1 on 128 -> 128 channels).  One K = 1 GEMM over the
+ * Cin*KH*KW im2col channels c*KH*KW + kh*KW + kw (the natural flatten of the [Cout, Cin, KH, KW] weight, which set_weight_dev
+ * takes as is).  With this handle the svb_tc_layer_* calls below read T as the height and W as the width of x [B, Cin, T, W]
+ * and write y [B, Cout, T', W'],
+ *     T' = (T + 2*PH - KH) / SH + 1 (= svb_tc_layer_out_len),   W' = (W + 2*PW - KW) / SW + 1;
+ * dy / y of backward are [B, Cout, T', W'], dx [B, Cin, T, W], dw [Cout, Cin, KH, KW].  Needs 2*PH <= KH, 2*PW <= KW and
+ * Cin*KH*KW, Cout tensor-core shapes as svb_tc_layer_create (multiples of 32, Cin*KH*KW <= 3072, Cout <= 1024). */
+int svb_tc_layer_create_2d(int32_t Cin, int32_t Cout, int32_t KH, int32_t KW, int32_t SH, int32_t SW, int32_t PH, int32_t PW,
+                           int32_t precision, int device, svb_tc_layer_t **out);
 void svb_tc_layer_destroy(svb_tc_layer_t *layer);
 int svb_tc_layer_set_weight_dev(svb_tc_layer_t *layer, const float *w_dev, const float *bias_dev, void *stream);
 int64_t svb_tc_layer_out_len(const svb_tc_layer_t *layer, int64_t T);
@@ -197,6 +207,36 @@ int svb_tc_layer_forward(svb_tc_layer_t *layer, const float *x_dev, int32_t B, i
                          float *y_dev, void *stream);
 int svb_tc_layer_backward(svb_tc_layer_t *layer, const float *x_dev, const float *y_dev, const float *dy_dev, int32_t B,
                           int32_t T, int32_t W, float out_slope, float *dx_dev, float *dw_dev, float *db_dev, void *stream);
+
+/* ---- mel discriminator (modules/fastspeech/multi_window_disc.py): fp32 operators ------------------------------------
+ * svb_conv2d_forward: y[b, co] = scale[b, co] * leaky_relu(conv2d(x, w) + bias, out_slope) on [B, C, H, W] device tensors,
+ *   w [Cout, Cin, KH, KW]; H' = (H + 2*PH - KH) / SH + 1, W' likewise; bias and scale [B, Cout] (a Dropout2d mask: 0 or
+ *   1/(1-p) per plane) may be NULL.  Needs 2*PH <= KH and 2*PW <= KW.
+ * svb_conv2d_backward: y = the forward's output (mask source, may be NULL when out_slope == 1), same scale, dy = gradient
+ *   w.r.t. y.  dz_scratch [B, Cout, H', W'] receives the masked gradient; dx is written, dw / db are ACCUMULATED (the caller
+ *   zeroes them); each may be NULL.
+ * svb_drop_inorm_forward: Dropout2d + InstanceNorm2d(C, affine=True) over planes of N = H*W elements:
+ *   u = scale[b, c] * v (scale NULL = all ones), y = gamma[c] (u - mean) / sqrt(var + eps) + beta[c] with the biased variance
+ *   of the plane; mean / rstd [B, C] are kept for the backward.  A dropped or constant plane gives beta.
+ * svb_drop_inorm_backward: dv (written; may be NULL) and dgamma / dbeta [C] (ACCUMULATED; each may be NULL) from dy.
+ * svb_linear1_forward: adv_layer = Linear(N, 1): y[b] = x[b, :] . w + bias[0], x [B, N].
+ * svb_linear1_backward: dx [B, N] written, dw [N] / db [1] ACCUMULATED (each may be NULL); dy [B] on the device. */
+int svb_conv2d_forward(const float *x_dev, const float *w_dev, const float *bias_dev, const float *scale_dev, float *y_dev, int32_t B,
+                       int32_t Cin, int32_t Cout, int32_t H, int32_t W, int32_t KH, int32_t KW, int32_t SH, int32_t SW, int32_t PH,
+                       int32_t PW, float out_slope, void *stream);
+int svb_conv2d_backward(const float *x_dev, const float *w_dev, const float *y_dev, const float *scale_dev, const float *dy_dev,
+                        int32_t B, int32_t Cin, int32_t Cout, int32_t H, int32_t W, int32_t KH, int32_t KW, int32_t SH, int32_t SW,
+                        int32_t PH, int32_t PW, float out_slope, float *dz_scratch_dev, float *dx_dev, float *dw_dev, float *db_dev,
+                        void *stream);
+int svb_drop_inorm_forward(const float *v_dev, const float *scale_dev, const float *gamma_dev, const float *beta_dev, int32_t B,
+                           int32_t C, int32_t N, float eps, float *y_dev, float *mean_dev, float *rstd_dev, void *stream);
+int svb_drop_inorm_backward(const float *v_dev, const float *scale_dev, const float *gamma_dev, const float *mean_dev,
+                            const float *rstd_dev, const float *dy_dev, int32_t B, int32_t C, int32_t N, float *dv_dev,
+                            float *dgamma_dev, float *dbeta_dev, void *stream);
+int svb_linear1_forward(const float *x_dev, const float *w_dev, const float *bias_dev, int32_t B, int32_t N, float *y_dev,
+                        void *stream);
+int svb_linear1_backward(const float *x_dev, const float *w_dev, const float *dy_dev, int32_t B, int32_t N, float *dx_dev,
+                         float *dw_dev, float *db_dev, void *stream);
 
 /* ---- training: backward of the generator -------------------------------------------------------------
  * Replaces torch autograd through HifiGanGenerator.forward (modules/hifigan/hifigan.py:144-169; ResBlock1/2

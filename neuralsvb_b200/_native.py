@@ -16,7 +16,7 @@ CSRC = os.path.join(_HERE, 'csrc')
 LIB_PATH = os.path.join(_HERE, 'libsvb_vocoder.so')
 HEADER = os.path.join(_ROOT, 'include', 'svb_vocoder.h')
 SOURCES = ['wn.cu', 'conformer.cu', 'api.cu', 'conv_ffma.cu', 'conv_tc.cu', 'nsf_source.cu', 'frontend.cu', 'generator.cu', 'layer_api.cu', 'disc_ops.cu',
-           'train_ops.cu', 'generator_bwd.cu', 'disc_bwd.cu', 'tc_layer.cu', 'wgrad_tc.cu', 'mel_loss.cu']
+           'train_ops.cu', 'generator_bwd.cu', 'disc_bwd.cu', 'tc_layer.cu', 'wgrad_tc.cu', 'mel_loss.cu', 'mel_disc.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '-Xcompiler', '-fPIC', '-shared']
 
@@ -115,6 +115,7 @@ _PROTOS = {
     'svb_loss_grad_dev': (ctypes.c_int, [_P, _P, _I32, ctypes.c_float, _P, _P, _I64, _I32, _P]),
     'svb_tc_layer_create': (ctypes.c_int, [_I32, _I32, _I32, _I32, _I32, _I32, ctypes.c_int, ctypes.POINTER(_P)]),
     'svb_tc_layer_create_grouped': (ctypes.c_int, [_I32, _I32, _I32, _I32, _I32, _I32, _I32, ctypes.c_int, ctypes.POINTER(_P)]),
+    'svb_tc_layer_create_2d': (ctypes.c_int, [_I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, ctypes.c_int, ctypes.POINTER(_P)]),
     'svb_tc_layer_destroy': (None, [_P]),
     'svb_tc_layer_set_weight_dev': (ctypes.c_int, [_P, _P, _P, _P]),
     'svb_tc_layer_out_len': (_I64, [_P, _I64]),
@@ -178,6 +179,14 @@ _PROTOS = {
     'svb_mel_loss_workspace_bytes': (_I64, [_I32, _I32, _I32]),
     'svb_mel_loss_forward': (ctypes.c_int, [_P, _P, _I32, _I32, _I32, ctypes.c_float, _P, _P, _P]),
     'svb_mel_loss_backward': (ctypes.c_int, [_P, _P, _I32, _I32, _I32, ctypes.c_float, _P, _P, _P, _P, _P]),
+    'svb_conv2d_forward': (ctypes.c_int, [_P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32,
+                                          ctypes.c_float, _P]),
+    'svb_conv2d_backward': (ctypes.c_int, [_P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32,
+                                           ctypes.c_float, _P, _P, _P, _P, _P]),
+    'svb_drop_inorm_forward': (ctypes.c_int, [_P, _P, _P, _P, _I32, _I32, _I32, ctypes.c_float, _P, _P, _P, _P]),
+    'svb_drop_inorm_backward': (ctypes.c_int, [_P, _P, _P, _P, _P, _P, _I32, _I32, _I32, _P, _P, _P, _P]),
+    'svb_linear1_forward': (ctypes.c_int, [_P, _P, _P, _I32, _I32, _P, _P]),
+    'svb_linear1_backward': (ctypes.c_int, [_P, _P, _P, _I32, _I32, _P, _P, _P, _P]),
 }
 
 

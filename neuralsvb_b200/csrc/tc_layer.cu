@@ -7,6 +7,8 @@
 //                                is x[c][to*s + j - pad]), which turns the conv into ONE K = 1 GEMM over Cin*K
 //                                channels on the UNPERMUTED weight tensor [Cout][Cin*K]; its data gradient is the
 //                                transposed GEMM followed by a gather (col2im).
+//   2-D (svb_tc_layer_create_2d): the same K = 1 GEMM over Cin*KH*KW im2col channels (c*KH*KW + kh*KW + kw, the natural
+//                                flatten of a [Cout, Cin, KH, KW] weight), one G32T row per output pixel (h', w') of a clip.
 // Reference: the Conv2d((5,1),(3,1)) / Conv1d stacks of modules/hifigan/hifigan.py:193-199, :262-271 (layers with
 // groups == 1 and >= 32 channels: 98 % of the discriminators' FLOPs).
 #include <algorithm>
@@ -101,6 +103,54 @@ __global__ void __launch_bounds__(256) col2im_to_nctw_kernel(const float *__rest
     dx[(((size_t)b * C + c) * T) * W + e] = acc;
 }
 
+// 2-D im2col: out[b][(c*KK + kh*KW + kw)][ho*Wo + wo] = x[b][c][ho*SH + kh - PH][wo*SW + kw - PW] (zero outside), every row of
+// the allocation written.  Same grid and thread ownership as expand_to_g32t_kernel, clips = B.
+__global__ void __launch_bounds__(256) expand2d_to_g32t_kernel(const float *__restrict__ x, int C, int H, int W, int KH, int KW, int SH,
+                                                               int SW, int PH, int PW, int Wo, int Tq, int Tp, float *__restrict__ out) {
+    const int lane = threadIdx.x & 31, wrp = threadIdx.x >> 5;
+    const int grp = blockIdx.y, b = blockIdx.z, groups = gridDim.y, KK = KH * KW;
+    const int cc = grp * 32 + lane;
+    const int c = cc / KK, j = cc - c * KK, kh = j / KW, kw = j - kh * KW;
+    const bool ch_ok = cc < C * KK;
+    const float *xb = x + ((size_t)b * C + (ch_ok ? c : 0)) * H * W;
+    float *ob = out + ((size_t)b * groups + grp) * Tp * 32 + lane;
+    const int r1 = min(Tp, (int)(blockIdx.x + 1) * kExpRows);
+    for (int row = blockIdx.x * kExpRows + wrp; row < r1; row += 8) {
+        const int to = row - kPad;
+        float v = 0.f;
+        if (ch_ok && to >= 0 && to < Tq) {
+            const int ho = to / Wo, wo = to - ho * Wo;
+            const int h = ho * SH + kh - PH, w = wo * SW + kw - PW;
+            if (h >= 0 && h < H && w >= 0 && w < W) v = __ldg(xb + (size_t)h * W + w);
+        }
+        ob[(size_t)row * 32] = v;
+    }
+}
+
+// dx[b][c][h][w] = sum over taps (kh, kw) with (h + PH - kh) % SH == 0 and (w + PW - kw) % SW == 0 of
+//                  g[b][c*KK + kh*KW + kw][((h + PH - kh) / SH) * Wo + (w + PW - kw) / SW]
+__global__ void __launch_bounds__(256) col2im2d_to_nctw_kernel(const float *__restrict__ g, int C, int H, int W, int KH, int KW, int SH,
+                                                               int SW, int PH, int PW, int Ho, int Wo, int Tp, float *__restrict__ dx) {
+    const int c = blockIdx.y, b = blockIdx.z, KK = KH * KW;
+    const int groups = c4t_groups(C * KK);
+    const int e = blockIdx.x * 256 + threadIdx.x;
+    if (e >= H * W) return;
+    const int h = e / W, w = e - h * W;
+    const size_t base = (size_t)b * groups;
+    float acc = 0.f;
+    for (int kh = (h + PH) % SH; kh < KH && kh <= h + PH; kh += SH) {
+        const int ho = (h + PH - kh) / SH;
+        if (ho >= Ho) continue;
+        for (int kw = (w + PW) % SW; kw < KW && kw <= w + PW; kw += SW) {
+            const int wo = (w + PW - kw) / SW;
+            if (wo >= Wo) continue;
+            const int cc = c * KK + kh * KW + kw;
+            acc += g[((base + (cc >> 5)) * Tp + kPad + ho * Wo + wo) * 32 + (cc & 31)];
+        }
+    }
+    dx[((size_t)b * C + c) * H * W + e] = acc;
+}
+
 // one scratch arena per device, shared by every layer handle.  Contract (include/svb_vocoder.h, "ownership / threading"): the
 // svb_tc_layer_* calls of one device are issued from ONE host thread on ONE stream -- the arena is reused by consecutive calls in
 // stream order and is not guarded against concurrent streams; the mutex below only keeps a (re)allocation from racing with another
@@ -144,6 +194,17 @@ void launch_col2im(const float *g, int B, int C, int T, int W, int KE, int s, in
     col2im_to_nctw_kernel<<<grid, 256, 0, st>>>(g, C, T, W, KE, s, p, Tq, Tp, dx);
 }
 
+void launch_expand2d(const float *x, int B, int C, int H, int W, int KH, int KW, int SH, int SW, int PH, int PW, int Wo, int Tq, int Tp,
+                     float *out, cudaStream_t st) {
+    const dim3 grid((Tp + kExpRows - 1) / kExpRows, c4t_groups(C * KH * KW), B);
+    expand2d_to_g32t_kernel<<<grid, 256, 0, st>>>(x, C, H, W, KH, KW, SH, SW, PH, PW, Wo, Tq, Tp, out);
+}
+void launch_col2im2d(const float *g, int B, int C, int H, int W, int KH, int KW, int SH, int SW, int PH, int PW, int Ho, int Wo, int Tp,
+                     float *dx, cudaStream_t st) {
+    const dim3 grid((H * W + 255) / 256, C, B);
+    col2im2d_to_nctw_kernel<<<grid, 256, 0, st>>>(g, C, H, W, KH, KW, SH, SW, PH, PW, Ho, Wo, Tp, dx);
+}
+
 }  // namespace
 
 struct svb_tc_layer {
@@ -159,6 +220,9 @@ struct svb_tc_layer {
     // grouped layers (svb_tc_layer_create_grouped): polyphase form, see below
     bool poly = false;
     int groups = 1, KSp = 1, halo = 0, cin_blk_f = 0, cin_blk_b = 0;
+    // 2-D layers (svb_tc_layer_create_2d): KE = KH*KW, T is the height, W the width
+    bool two_d = false;
+    int KH = 1, KW = 1, SH = 1, SW = 1, PH = 0, PW = 0;
 };
 
 static std::vector<int> to_idx(const std::vector<float> &v) {
@@ -309,6 +373,23 @@ extern "C" int svb_tc_layer_create_grouped(int32_t Cin, int32_t Cout, int32_t K,
     return SVB_OK;
 }
 
+// ---- 2-D convolutions: Conv2d(Cin, Cout, (KH, KW), (SH, SW), (PH, PW)) of the mel discriminator ----------------------------
+// The packings are those of a strided 1-D layer with K = KH*KW taps (the tap-major expansion, weight [Cout][Cin*KH*KW], one
+// K = 1 GEMM): only the gather differs, so the handle is built by svb_tc_layer_create with those taps and then marked 2-D.
+extern "C" int svb_tc_layer_create_2d(int32_t Cin, int32_t Cout, int32_t KH, int32_t KW, int32_t SH, int32_t SW, int32_t PH, int32_t PW,
+                                      int32_t precision, int device, svb_tc_layer_t **out) {
+    SVB_CHECK(out && Cin > 0 && Cout > 0 && KH >= 1 && KW >= 1 && SH >= 1 && SW >= 1 && PH >= 0 && PW >= 0 && 2 * PH <= KH &&
+                  2 * PW <= KW && (long long)KH * KW <= 64,
+              SVB_ERR_INVALID, "tc_layer_create_2d: bad geometry (kernel %dx%d, stride %dx%d, padding %dx%d)", KH, KW, SH, SW, PH, PW);
+    svb_tc_layer_t *L = nullptr;
+    SVB_TRY(svb_tc_layer_create(Cin, Cout, KH * KW, 2, 0, precision, device, &L));      // stride > 1: the K-expanded packing
+    L->two_d = true, L->KH = KH, L->KW = KW, L->SH = SH, L->SW = SW, L->PH = PH, L->PW = PW;
+    *out = L;
+    return SVB_OK;
+}
+
+static int out_width_2d(const svb_tc_layer *L, int W) { return (W + 2 * L->PW - L->KW) / L->SW + 1; }
+
 extern "C" void svb_tc_layer_destroy(svb_tc_layer_t *L) {
     if (!L) return;
     cudaSetDevice(L->device);
@@ -343,6 +424,7 @@ static int run_tc(const svb_tc_layer *L, const ConvLayer &cl, const float *in, f
 
 extern "C" int64_t svb_tc_layer_out_len(const svb_tc_layer_t *L, int64_t T) {
     if (!L) return -1;
+    if (L->two_d) return (T + 2 * L->PH - L->KH) / L->SH + 1;
     return (T + 2 * L->pad - (L->K - 1) - 1) / L->stride + 1;
 }
 
@@ -351,6 +433,20 @@ extern "C" int svb_tc_layer_forward(svb_tc_layer_t *L, const float *x_dev, int32
     SVB_CHECK(L && L->has_w && x_dev && y_dev && B > 0 && T > 0 && W > 0, SVB_ERR_INVALID, "tc_layer_forward: bad argument");
     SVB_CUDA(cudaSetDevice(L->device));
     cudaStream_t st = as_stream(stream);
+    if (L->two_d) {                             // [B, Cin, T, W] -> [B, Cout, T', W']: one clip per b, one row per output pixel
+        const int Ho = (int)svb_tc_layer_out_len(L, T), Wo = out_width_2d(L, W), Ce = L->Cin * L->KE;
+        SVB_CHECK(Ho > 0 && Wo > 0 && (long long)Ho * Wo < (1 << 24), SVB_ERR_INVALID, "tc_layer_forward: bad 2-D output %d x %d", Ho, Wo);
+        const int Tq = Ho * Wo, Tp = c4t_rows(Tq);
+        const size_t n_x = c4t_floats(B, Ce, Tq), n_y = c4t_floats(B, L->Cout, Tq);
+        char *base;
+        SVB_TRY(arena_get(L->device, (n_x + n_y) * 4, &base));
+        float *xe = reinterpret_cast<float *>(base), *yg = xe + n_x;
+        launch_expand2d(x_dev, B, L->Cin, T, W, L->KH, L->KW, L->SH, L->SW, L->PH, L->PW, Wo, Tq, Tp, xe, st);
+        SVB_TRY(run_tc(L, L->fwd, xe, yg, Tp, B, Tq, st));
+        launch_g32t_to_nctw(yg, B, L->Cout, Tq, 1, Tp, out_slope, y_dev, 0, st);
+        SVB_CUDA(cudaGetLastError());
+        return SVB_OK;
+    }
     if (L->poly) {                              // grouped / polyphase layer
         const int To = (int)svb_tc_layer_out_len(L, T), Tr = To + 2 * L->halo, Tp = c4t_rows(Tr), clips = B * W, Ce = L->Cin * L->KE;
         SVB_CHECK(To > 0, SVB_ERR_INVALID, "tc_layer_forward: empty output");
@@ -386,6 +482,33 @@ extern "C" int svb_tc_layer_backward(svb_tc_layer_t *L, const float *x_dev, cons
     SVB_CHECK(out_slope == 1.f || y_dev, SVB_ERR_INVALID, "tc_layer_backward: the activation mask needs the forward output");
     SVB_CUDA(cudaSetDevice(L->device));
     cudaStream_t st = as_stream(stream);
+    if (L->two_d) {
+        const int Ho = (int)svb_tc_layer_out_len(L, T), Wo = out_width_2d(L, W), Ce = L->Cin * L->KE;
+        SVB_CHECK(Ho > 0 && Wo > 0 && (long long)Ho * Wo < (1 << 24), SVB_ERR_INVALID, "tc_layer_backward: bad 2-D output %d x %d", Ho, Wo);
+        const int Tq = Ho * Wo, Tp = c4t_rows(Tq);
+        const size_t n_x = c4t_floats(B, Ce, Tq), n_y = c4t_floats(B, L->Cout, Tq);
+        char *base;
+        SVB_TRY(arena_get(L->device, (2 * n_x + n_y) * 4, &base));
+        float *xe = reinterpret_cast<float *>(base), *dxe = xe + n_x, *dzg = dxe + n_x;
+        // dy [B, Cout, T', W'] is a [B, Cout, T'*W'] signal: the 1-D gather with the leaky-relu mask from the stored output
+        launch_expand(dy_dev, out_slope == 1.f ? nullptr : y_dev, out_slope, B, L->Cout, Tq, 1, 1, 1, 0, Tq, Tp, dzg, st);
+        if (db_dev) SVB_TRY(launch_colsum(dzg, B, L->Cout, Tq, Tp, db_dev, st));
+        if (dw_dev) {
+            launch_expand2d(x_dev, B, L->Cin, T, W, L->KH, L->KW, L->SH, L->SW, L->PH, L->PW, Wo, Tq, Tp, xe, st);
+            WgradArgs a;
+            a.A = xe, a.G = dzg, a.out = dw_dev, a.B = B, a.Tq = Tq, a.Ca = Ce, a.TpA = Tp, a.Cg = L->Cout, a.TpG = Tp, a.K = 1;
+            a.sa = 1, a.da = 1, a.pa = 0, a.sb = 1, a.db = 0, a.pb = 0, a.slope = 1.f;
+            a.s_co = Ce, a.s_ci = 1, a.s_k = 1;         // natural [Cout][Cin][KH][KW] = [Cout][Ce]
+            a.allow_tc = 1;
+            SVB_TRY(launch_wgrad(a, st));
+        }
+        if (dx_dev) {
+            SVB_TRY(run_tc(L, L->bwd, dzg, dxe, Tp, B, Tq, st));
+            launch_col2im2d(dxe, B, L->Cin, T, W, L->KH, L->KW, L->SH, L->SW, L->PH, L->PW, Ho, Wo, Tp, dx_dev, st);
+        }
+        SVB_CUDA(cudaGetLastError());
+        return SVB_OK;
+    }
     if (L->poly) {                              // grouped / polyphase layer
         const int To = (int)svb_tc_layer_out_len(L, T), Tr = To + 2 * L->halo, Tp = c4t_rows(Tr), clips = B * W, Ce = L->Cin * L->KE;
         const size_t n_x = c4t_floats(clips, Ce, Tr), n_y = c4t_floats(clips, L->Cout, Tr);

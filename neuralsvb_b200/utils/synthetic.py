@@ -471,3 +471,39 @@ def make_svb_batch(B=2, Ta=96, Tp=120, seed=1234, n_mel=80):
     align = torch.from_numpy(np.minimum((np.arange(Tp)[None, :] * Ta / Tp).astype(np.int64) + rs.randint(0, 2, size=(B, Tp)), Ta - 1))
     return dict(amateur_mel=a_mel, prof_mel=p_mel, amateur_pitch=a_pitch, prof_pitch=p_pitch, amateur_spk_id=spk, prof_spk_id=spk,
                 a2p_alignment=align)
+
+
+def make_mel_disc_state_dict(seed=1234, wins=(32, 64, 128), hidden=128, n_mel=80):
+    """state_dict of the reference's mel discriminator (modules/fastspeech/multi_window_disc.py, Discriminator with
+    norm_type 'in', c_in 1, kernel 3x3; tasks/tts/fs2_adv.py:22-34): per window three Conv2d blocks, InstanceNorm2d affine
+    parameters on blocks 2 and 3, adv_layer = Linear(hidden * win/8 * ceil(n_mel/8), 1).  Uniform weights at PyTorch's default
+    fan-in bounds, norm scales around 1."""
+    rs = np.random.RandomState(seed + 53)
+    sd = OrderedDict()
+
+    def t(a):
+        return torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32))
+    for i, win in enumerate(wins):
+        p = f'discriminator.conv_layers.{i}.'
+        for j in range(3):
+            cin = 1 if j == 0 else hidden
+            b = 1.0 / np.sqrt(cin * 9)
+            sd[f'{p}model.{j}.0.weight'] = t(_uniform(rs, (hidden, cin, 3, 3), b))
+            sd[f'{p}model.{j}.0.bias'] = t(_uniform(rs, (hidden,), b))
+            if j > 0:
+                sd[f'{p}model.{j}.3.weight'] = t(rs.uniform(0.7, 1.3, hidden))
+                sd[f'{p}model.{j}.3.bias'] = t(_uniform(rs, (hidden,), 0.1))
+        n = hidden * (win // 8) * ((n_mel + 7) // 8)
+        sd[p + 'adv_layer.weight'] = t(_uniform(rs, (1, n), 1.0 / np.sqrt(n)))
+        sd[p + 'adv_layer.bias'] = t(_uniform(rs, (1,), 1.0 / np.sqrt(n)))
+    return sd
+
+
+def make_disc_mel(B, T, pad, seed=1234, n_mel=80):
+    """A log10-mel-range mel [B, T, n_mel] whose clip b has its last pad[b] frames zero (padding, not counted by x_len)."""
+    rs = np.random.RandomState(seed + 59)
+    m = (rs.randn(B, T, n_mel) * 1.2 - 2.5).clip(-6, 1.5)
+    for b, p in enumerate(pad):
+        if p:
+            m[b, T - p:] = 0.0
+    return torch.from_numpy(m.astype(np.float32))
