@@ -457,6 +457,44 @@ int svb_mel_loss_forward(const float *pred_dev, const float *target_dev, int32_t
 int svb_mel_loss_backward(const float *pred_dev, const float *target_dev, int32_t B, int32_t T, int32_t M, float bias,
                           const double *out3_dev, const float *g_l1_dev, const float *g_ssim_dev, float *dpred_dev, void *stream);
 
+/* ---- Shape-aware DTW pitch alignment (csrc/sadtw.cu): SADTW (modules/voice_conversion/dtw/shape_aware_dtw.py) and EHSADTW
+ * (enhance_sadtw.py) over time_warp / align_from_distances (align.py).  A batch of n pairs is ragged: the amateur f0 of every pair
+ * concatenated in src_f0_dev (pair p has src_len[p] frames), the professional f0 in tgt_f0_dev (tgt_len[p] frames), float32 or
+ * float64 (dtype), lengths on the host.  The professional histogram uses the scale factor tgt_scale[p] (NULL: tgt_len / src_len,
+ * cal_shape_dist's), the amateur one 1.0.
+ * svb_sadtw_workspace_bytes: size of the caller-owned workspace (-1 on bad lengths); offsets_host (5 entries, NULL = not wanted)
+ *   receives the byte offsets of its sections: [0] per-sequence and [1] per-pair metadata, [2] histograms float32 [rows, 48] (the
+ *   amateur frames of all pairs, then the professional ones), [3] costs float32 and [4] direction bytes (0 up, 1 left, 2 diagonal),
+ *   pair p's R x C cells (R = tgt_len[p], C = src_len[p]) after those of the pairs before it, anti-diagonal-major: cell (i, j) at
+ *   (number of cells with i' + j' < i + j) + i - max(0, i + j - C + 1).
+ * svb_sadtw_align writes alignment_dev int64 [sum tgt_len] (pair p's rows after the pairs before it): for each professional frame the
+ *   amateur frame align_from_distances picks; path_cost_dev (NULL = not wanted) float32 [n] = the pair's DTW value at its last cell.
+ *   stage_ms_host (NULL = not wanted) receives 4 CUDA-event times (histogram, cost, DTW, backtrack) and makes the call synchronise.
+ *   Rejected before any launch (SVB_ERR_INVALID): a length below 2, min(S, T) > 8192, a frame whose slope windows are all empty
+ *   after scaling (the reference divides by zero), a bad dtype / variant / scale or a short workspace.  f0 must be finite (the
+ *   reference exits otherwise); that is the caller's check. */
+typedef enum svb_sadtw_variant { SVB_SADTW = 0, SVB_EHSADTW = 1 } svb_sadtw_variant;
+typedef enum svb_sadtw_dtype { SVB_SADTW_F32 = 0, SVB_SADTW_F64 = 1 } svb_sadtw_dtype;
+int64_t svb_sadtw_workspace_bytes(int32_t n_pairs, const int32_t *src_len_host, const int32_t *tgt_len_host, int64_t *offsets_host);
+int svb_sadtw_align(const void *src_f0_dev, const void *tgt_f0_dev, int32_t dtype, int32_t variant, int32_t n_pairs,
+                    const int32_t *src_len_host, const int32_t *tgt_len_host, const double *tgt_scale_host, void *workspace_dev,
+                    int64_t workspace_bytes, int64_t *alignment_dev, float *path_cost_dev, float *stage_ms_host, void *stream);
+/* The histogram kernel alone (cal_hist_of_f0(f, max_window=64, scale_factor=scale[k])): n_seq sequences concatenated in f0_dev,
+ * hist_dev float32 [sum len, 48] = k / total (normalize_hist=True), counts_dev int32 [sum len, 48] = k (NULL = not wanted).
+ * The workspace holds the per-sequence metadata (svb_sadtw_histogram_workspace_bytes). */
+int64_t svb_sadtw_histogram_workspace_bytes(int32_t n_seq);
+int svb_sadtw_histogram(const void *f0_dev, int32_t dtype, int32_t variant, int32_t n_seq, const int32_t *len_host, const double *scale_host,
+                        void *workspace_dev, int64_t workspace_bytes, float *hist_dev, int32_t *counts_dev, void *stream);
+/* cal_hist_dist(hist_a, hist_b): dist_dev float32 [n_a, n_b] row-major, sum_m 0.5 (b_m - a_m)^2 / (b_m + a_m + 1e-8) over the 48
+ * bins in order.  Histograms float32 [n, 48], 16-byte aligned. */
+int svb_sadtw_cost(const float *hist_a_dev, int32_t n_a, const float *hist_b_dev, int32_t n_b, float *dist_dev, void *stream);
+/* time_warp / align_from_distances on an arbitrary cost [rows, cols] (row-major, float32 or float64; min(rows, cols) <= 8192):
+ * alignment_dev int64 [rows] (NULL = not wanted), path_cost_dev one element of the cost's type (NULL = not wanted), dtw_dev the
+ * whole DTW matrix [rows, cols] in the cost's type (NULL = not wanted).  svb_dtw_workspace_bytes: -1 on a bad shape. */
+int64_t svb_dtw_workspace_bytes(int32_t dtype, int32_t rows, int32_t cols);
+int svb_dtw_align(const void *cost_dev, int32_t dtype, int32_t rows, int32_t cols, void *workspace_dev, int64_t workspace_bytes,
+                  int64_t *alignment_dev, void *path_cost_dev, void *dtw_dev, void *stream);
+
 /* Host-only view of the schedule of a merged tensor-core launch (csrc/conv_tc.cu: tc_schedule; no CUDA call, usable without a GPU):
  * `n_layers` convolutions of one shape class (taps KS[l], residual / accumulate flags) over B clips x Tq rows, tiles of 128 rows in
  * items of up to MT tiles, `col_blocks` column blocks, `grid` CTAs.  items_out receives 5 ints per item (layer, column block, clip,

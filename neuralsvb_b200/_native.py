@@ -16,7 +16,7 @@ CSRC = os.path.join(_HERE, 'csrc')
 LIB_PATH = os.path.join(_HERE, 'libsvb_vocoder.so')
 HEADER = os.path.join(_ROOT, 'include', 'svb_vocoder.h')
 SOURCES = ['wn.cu', 'conformer.cu', 'api.cu', 'conv_ffma.cu', 'conv_tc.cu', 'nsf_source.cu', 'frontend.cu', 'generator.cu', 'layer_api.cu', 'disc_ops.cu',
-           'train_ops.cu', 'generator_bwd.cu', 'disc_bwd.cu', 'tc_layer.cu', 'wgrad_tc.cu', 'mel_loss.cu', 'mel_disc.cu']
+           'train_ops.cu', 'generator_bwd.cu', 'disc_bwd.cu', 'tc_layer.cu', 'wgrad_tc.cu', 'mel_loss.cu', 'mel_disc.cu', 'sadtw.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '-Xcompiler', '-fPIC', '-shared']
 
@@ -187,6 +187,13 @@ _PROTOS = {
     'svb_drop_inorm_backward': (ctypes.c_int, [_P, _P, _P, _P, _P, _P, _I32, _I32, _I32, _P, _P, _P, _P]),
     'svb_linear1_forward': (ctypes.c_int, [_P, _P, _P, _I32, _I32, _P, _P]),
     'svb_linear1_backward': (ctypes.c_int, [_P, _P, _P, _I32, _I32, _P, _P, _P, _P]),
+    'svb_sadtw_workspace_bytes': (_I64, [_I32, _P, _P, _P]),
+    'svb_sadtw_align': (ctypes.c_int, [_P, _P, _I32, _I32, _I32, _P, _P, _P, _P, _I64, _P, _P, _P, _P]),
+    'svb_sadtw_histogram_workspace_bytes': (_I64, [_I32]),
+    'svb_sadtw_histogram': (ctypes.c_int, [_P, _I32, _I32, _I32, _P, _P, _P, _I64, _P, _P, _P]),
+    'svb_sadtw_cost': (ctypes.c_int, [_P, _I32, _P, _I32, _P, _P]),
+    'svb_dtw_workspace_bytes': (_I64, [_I32, _I32, _I32]),
+    'svb_dtw_align': (ctypes.c_int, [_P, _I32, _I32, _I32, _P, _I64, _P, _P, _P, _P]),
 }
 
 

@@ -1,0 +1,559 @@
+// Shape-aware DTW pitch alignment (the paper's pitch correction: SADTW, modules/voice_conversion/dtw/shape_aware_dtw.py, and
+// EHSADTW, enhance_sadtw.py, over time_warp / align_from_distances, align.py) on a ragged batch of amateur / professional f0 pairs.
+//
+// Per pair (S amateur frames, T professional frames):
+//   1. histogram: 48 bins per frame (8 slope windows x 6 regions) of the amateur contour at scale 1 and the professional one at
+//      scale T / S (sadtw_hist_kernel; 8 lanes per frame, one window each);
+//   2. cost[i, j] = sum_m 0.5 (b_m - a_m)^2 / (b_m + a_m + 1e-8), a = amateur histogram j, b = professional histogram i, summed
+//      sequentially over m, written in anti-diagonal-major ("skewed") order so the wavefront reads contiguous memory;
+//   3. DTW over the [T, S] matrix: one CTA per pair walks the anti-diagonals with the three live diagonals in shared memory and
+//      writes one direction byte per cell (0 up, 1 left, 2 diagonal: the first minimum in the backtrack's order);
+//   4. backtrack: one thread per pair follows the direction bytes from the last cell (align_from_distances).
+// The float DTW matrix never goes to HBM on this path.  Nothing is accumulated across pairs and there are no atomics, so a pair's
+// result does not depend on the batch it is in.
+//
+// Numerics follow the reference's Python / numpy / torch arithmetic bit for bit: every division and product is an explicit
+// round-to-nearest intrinsic (no FMA contraction can move a slope across a region threshold), the f0 arithmetic runs in the input's
+// type (float32 or float64), a bin is (float)((double)k / (double)n) (Python's division, then torch.tensor's float32), and the DTW
+// minimum is Python's min(): the first operand unless a later one is strictly smaller.
+#include <algorithm>
+#include <cmath>
+#include <vector>
+
+#include "common.cuh"
+
+using namespace svb;
+
+namespace {
+
+constexpr int kBins = 48, kRegions = 6, kWindows = 8;
+constexpr int kHistThreads = 256;           // 32 frames x 8 windows
+constexpr int kCostThreads = 128;           // 4 warps, one 32 x 32 block of a cost tile each
+constexpr int kDtwPer = 8;                  // cells per thread per anti-diagonal
+constexpr int kDtwMaxThreads = 1024;
+constexpr int kMaxDiag = kDtwPer * kDtwMaxThreads;   // longest anti-diagonal = min(rows, cols)
+constexpr int kMaxPairs = 65535;            // grid.y of the histogram and cost launches
+
+const int kWin[2][kWindows][2] = {
+    {{-64, -32}, {-32, -16}, {-16, -8}, {-8, 0}, {0, 8}, {8, 16}, {16, 32}, {32, 64}},          // SADTW (max_window = 64)
+    {{-64, -48}, {-48, -32}, {-32, -16}, {-16, 0}, {0, 16}, {16, 32}, {32, 48}, {48, 64}},      // EHSADTW
+};
+
+struct SeqMeta {
+    int64_t f0_off;                 // first frame in its f0 array
+    int64_t hist_row;               // first row in the histogram buffer
+    int32_t len;
+    int32_t lo[kWindows], hi[kWindows];   // window w of frame t covers [clamp(t + lo[w]), clamp(t + hi[w]))
+    int32_t pad_;
+};
+
+struct PairMeta {
+    int64_t src_row, tgt_row;       // first histogram row of the amateur / professional frames
+    int64_t cell_off;               // first cell of the skewed cost and direction matrices
+    int64_t out_row;                // first alignment entry
+    int32_t R, C;                   // rows = professional frames (T), columns = amateur frames (S)
+};
+
+inline size_t align_up(size_t x) { return (x + 255) & ~(size_t)255; }
+
+// cells (i, j) of an R x C matrix with i + j < d: the offset of anti-diagonal d in the skewed layout
+__host__ __device__ __forceinline__ int64_t tri(int64_t x) { return x > 0 ? x * (x + 1) / 2 : 0; }
+__host__ __device__ __forceinline__ int64_t diag_start(int64_t d, int R, int C) {
+    return d * (d + 1) / 2 - tri(d - R) - tri(d - C) + tri(d - R - C);
+}
+__host__ __device__ __forceinline__ int diag_lo(int d, int C) { return d - C + 1 > 0 ? d - C + 1 : 0; }
+__host__ __device__ __forceinline__ int64_t skew_index(int i, int j, int R, int C) {
+    return diag_start(i + j, R, C) + i - diag_lo(i + j, C);
+}
+
+// int(b * scale) (truncation toward zero), then a left boundary of 0 becomes 1 (cal_hist_of_f0)
+void scaled_windows(int variant, double scale, int32_t *lo, int32_t *hi) {
+    for (int w = 0; w < kWindows; ++w) {
+        lo[w] = (int32_t)((double)kWin[variant][w][0] * scale);
+        hi[w] = (int32_t)((double)kWin[variant][w][1] * scale);
+        if (lo[w] == 0) lo[w] = 1;
+    }
+}
+
+// every frame t in [0, L) has a non-empty window: window w is non-empty at t iff max(0, lo + t) < min(L, hi + t), i.e. for
+// t in [1 - hi, L - lo) when lo < hi.  The reference divides by a zero total otherwise.
+bool every_frame_has_a_window(int L, const int32_t *lo, const int32_t *hi) {
+    int64_t covered = 0;
+    for (bool moved = true; moved && covered < L;) {
+        moved = false;
+        for (int w = 0; w < kWindows; ++w) {
+            if (lo[w] >= hi[w]) continue;
+            const int64_t a = std::max<int64_t>(0, 1 - (int64_t)hi[w]), b = std::min<int64_t>(L, (int64_t)L - lo[w]);
+            if (a <= covered && covered < b) covered = b, moved = true;
+        }
+    }
+    return covered >= L;
+}
+
+int make_seq(int variant, int64_t f0_off, int64_t hist_row, int32_t len, double scale, const char *what, int idx, SeqMeta &s) {
+    SVB_CHECK(len >= 2, SVB_ERR_INVALID, "sadtw: %s %d has %d frames (at least 2 are needed)", what, idx, len);
+    SVB_CHECK(std::isfinite(scale) && scale > 0.0 && scale < 1e6, SVB_ERR_INVALID, "sadtw: %s %d: bad scale factor %g", what, idx,
+              scale);
+    s.f0_off = f0_off, s.hist_row = hist_row, s.len = len, s.pad_ = 0;
+    scaled_windows(variant, scale, s.lo, s.hi);
+    SVB_CHECK(every_frame_has_a_window(len, s.lo, s.hi), SVB_ERR_INVALID,
+              "sadtw: %s %d (%d frames, scale factor %g): a frame has no neighbour in any slope window (empty histogram)", what, idx,
+              len, scale);
+    return SVB_OK;
+}
+
+// ---- round-to-nearest arithmetic in the f0 type ---------------------------------------------------------------------------
+__device__ __forceinline__ float sub_rn(float a, float b) { return __fsub_rn(a, b); }
+__device__ __forceinline__ double sub_rn(double a, double b) { return __dsub_rn(a, b); }
+__device__ __forceinline__ float div_rn(float a, float b) { return __fdiv_rn(a, b); }
+__device__ __forceinline__ double div_rn(double a, double b) { return __ddiv_rn(a, b); }
+__device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
+__device__ __forceinline__ double mul_rn(double a, double b) { return __dmul_rn(a, b); }
+__device__ __forceinline__ float add_rn(float a, float b) { return __fadd_rn(a, b); }
+__device__ __forceinline__ double add_rn(double a, double b) { return __dadd_rn(a, b); }
+template <typename T> __device__ __forceinline__ T inf_of();
+template <> __device__ __forceinline__ float inf_of<float>() { return __int_as_float(0x7f800000); }
+template <> __device__ __forceinline__ double inf_of<double>() { return __longlong_as_double(0x7ff0000000000000ll); }
+
+// EHSADTW's slope weights (windows 0/7, 1/6, 2/5; the rest 1) and the region thresholds, in the f0 type
+template <typename T> __device__ __forceinline__ T eh_weight(int w) {
+    const int e = w < 4 ? w : 7 - w;
+    return e == 0 ? (T)0.5 : e == 1 ? (T)0.75 : e == 2 ? (T)0.9 : (T)1;
+}
+
+// grid (ceil(max len / 32), n_seq): 8 lanes per frame, lane w counts window w into 6 regions; the frame's total is the sum over
+// its 8 lanes.  hist [rows, 48] float32 = k / total; counts [rows, 48] int32 (optional) = k.
+template <typename T>
+__global__ void __launch_bounds__(kHistThreads) sadtw_hist_kernel(const T *__restrict__ f0_a, const T *__restrict__ f0_b, int n_a,
+                                                                  const SeqMeta *__restrict__ seqs, int eh, float *__restrict__ hist,
+                                                                  int32_t *__restrict__ counts) {
+    const SeqMeta &s = seqs[blockIdx.y];
+    const int len = s.len, w = threadIdx.x & 7, t = blockIdx.x * (kHistThreads / 8) + (threadIdx.x >> 3);
+    if (blockIdx.x * (kHistThreads / 8) >= len) return;       // the whole CTA: no frame of this sequence
+    const T *f = ((int)blockIdx.y < n_a ? f0_a : f0_b) + s.f0_off;
+    int c0 = 0, c1 = 0, c2 = 0, c3 = 0, c4 = 0, c5 = 0;
+    if (t < len) {
+        const int lb = min(max(0, s.lo[w] + t), len), rb = min(max(0, s.hi[w] + t), len);
+        const T ft = f[t], k = eh ? eh_weight<T>(w) : (T)1;
+        const T th1 = (T)0.57735, th2 = (T)1.73205;
+        for (int i = lb; i < rb; ++i) {
+            const T d = sub_rn(f[i], ft);
+            T tn = div_rn(d, (T)(i - t));
+            if (eh) tn = mul_rn(tn, k);
+            const T a = fabs(tn);
+            const bool up = d >= (T)0;
+            if (a < th1) up ? ++c2 : ++c3;
+            else if (a < th2) up ? ++c1 : ++c4;
+            else up ? ++c0 : ++c5;
+        }
+    }
+    int n = c0 + c1 + c2 + c3 + c4 + c5;
+    n += __shfl_xor_sync(0xffffffffu, n, 1);
+    n += __shfl_xor_sync(0xffffffffu, n, 2);
+    n += __shfl_xor_sync(0xffffffffu, n, 4);
+    if (t >= len) return;
+    const int64_t o = (s.hist_row + t) * kBins + w * kRegions;
+    const double dn = (double)n;
+    auto put = [&](int r, int k) {
+        hist[o + r] = __double2float_rn(__ddiv_rn((double)k, dn));
+        if (counts) counts[o + r] = k;
+    };
+    put(0, c0), put(1, c1), put(2, c2), put(3, c3), put(4, c4), put(5, c5);
+}
+
+// 0.5 (b - a)^2 / (b + a + 1e-8) summed over the 48 bins in order (a, b: 16-byte aligned, global or shared).  A bin with b = a
+// adds +0 / (positive) = +0 to a sum that is >= +0, which leaves it unchanged, so the division is skipped there; most bins of
+// two histograms are both zero.
+__device__ __forceinline__ float chi_square(const float *a, const float *b) {
+    const float4 *a4 = reinterpret_cast<const float4 *>(a), *b4 = reinterpret_cast<const float4 *>(b);
+    float s = 0.f;
+#pragma unroll
+    for (int q = 0; q < kBins / 4; ++q) {
+        const float4 x = a4[q], y = b4[q];
+        const float av[4] = {x.x, x.y, x.z, x.w}, bv[4] = {y.x, y.y, y.z, y.w};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const float d = __fsub_rn(bv[e], av[e]);
+            if (d != 0.f) s = __fadd_rn(s, __fdiv_rn(__fmul_rn(0.5f, __fmul_rn(d, d)), __fadd_rn(__fadd_rn(bv[e], av[e]), 1e-8f)));
+        }
+    }
+    return s;
+}
+
+// grid (tiles of the largest pair, n_pairs): a CTA computes a tile of 32 professional x 128 amateur frames from histogram rows
+// staged in shared memory (rows padded to 52 floats: float4 reads without bank conflicts).  Warp w takes columns
+// [32 w, 32 w + 32) of the tile; at step dd lane k computes cell (k, (dd - k) mod 32), so a warp's 32 cells lie on two
+// anti-diagonals, consecutive rows on each: two contiguous runs of the skewed layout per store.
+constexpr int kTileI = 32, kTileJ = 128, kRowStride = 52;
+__global__ void __launch_bounds__(kCostThreads) sadtw_cost_kernel(const float *__restrict__ hist, const PairMeta *__restrict__ pairs,
+                                                                  float *__restrict__ cost) {
+    __shared__ __align__(16) float sb[kTileI * kRowStride], sa[kTileJ * kRowStride];
+    const PairMeta p = pairs[blockIdx.y];
+    const int R = p.R, C = p.C, tiles_j = (C + kTileJ - 1) / kTileJ;
+    if ((int)blockIdx.x >= tiles_j * ((R + kTileI - 1) / kTileI)) return;
+    const int i0 = (blockIdx.x / tiles_j) * kTileI, j0 = (blockIdx.x % tiles_j) * kTileJ;
+    const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int q = threadIdx.x; q < (kTileI + kTileJ) * (kBins / 4); q += kCostThreads) {
+        const int r = q / (kBins / 4), c = q - r * (kBins / 4);
+        const bool is_b = r < kTileI;
+        const int rr = is_b ? r : r - kTileI, f = is_b ? i0 + rr : j0 + rr;
+        const bool in = f < (is_b ? R : C);
+        const float4 v = in ? __ldg(reinterpret_cast<const float4 *>(hist + ((is_b ? p.tgt_row : p.src_row) + f) * kBins) + c) : zero;
+        *reinterpret_cast<float4 *>((is_b ? sb : sa) + rr * kRowStride + 4 * c) = v;
+    }
+    __syncthreads();
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, i = i0 + lane;
+    if (i >= R) return;
+    for (int dd = 0; dd < 32; ++dd) {
+        const int jj = w * 32 + ((dd - lane) & 31), j = j0 + jj;
+        if (j < C) cost[p.cell_off + skew_index(i, j, R, C)] = chi_square(sa + jj * kRowStride, sb + lane * kRowStride);
+    }
+}
+
+// cal_hist_dist: dist [n_a, n_b] row-major, dist[j, i] = chi_square(a_j, b_i)
+__global__ void __launch_bounds__(kCostThreads) sadtw_dist_kernel(const float *__restrict__ ha, int n_a, const float *__restrict__ hb,
+                                                                  int n_b, float *__restrict__ dist) {
+    const int64_t cells = (int64_t)n_a * n_b;
+    for (int64_t q = (int64_t)blockIdx.x * kCostThreads + threadIdx.x; q < cells; q += (int64_t)gridDim.x * kCostThreads) {
+        const int64_t j = q / n_b, i = q - j * n_b;
+        dist[q] = chi_square(ha + j * kBins, hb + i * kBins);
+    }
+}
+
+// row-major [R, C] -> skewed
+template <typename T>
+__global__ void skew_kernel(const T *__restrict__ src, int R, int C, T *__restrict__ dst) {
+    const int64_t cells = (int64_t)R * C;
+    for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < cells; q += (int64_t)gridDim.x * blockDim.x) {
+        const int i = (int)(q / C), j = (int)(q - (int64_t)i * C);
+        dst[skew_index(i, j, R, C)] = src[q];
+    }
+}
+
+// one CTA per pair (blockIdx.x): dtw[0,0] = 0, the rest of row 0 and column 0 = inf, dtw[i,j] = cost[i,j] + min(up, left, diag).
+// Shared memory: the anti-diagonals d - 2, d - 1 and d (indexed by i - lo(d)), 3 x maxdiag elements.  Each thread keeps the costs
+// of its cells of the next diagonal in registers, so the load is in flight during the current step.  dirs: one byte per cell
+// (i, j >= 1), skewed.  path_cost[pair] = dtw[R-1, C-1].  FULL: also the whole matrix, row-major, to dtw_full (time_warp).
+template <typename T, bool FULL>
+__global__ void __launch_bounds__(kDtwMaxThreads) dtw_kernel(const T *__restrict__ cost, const PairMeta *__restrict__ pairs, PairMeta single,
+                                                             int maxdiag, uint8_t *__restrict__ dirs, T *__restrict__ path_cost,
+                                                             T *__restrict__ dtw_full) {
+    extern __shared__ __align__(16) unsigned char dtw_smem[];
+    const PairMeta p = pairs ? pairs[blockIdx.x] : single;
+    const int R = p.R, C = p.C, D = R + C - 1, nt = blockDim.x;
+    const T *cp = cost + p.cell_off;
+    uint8_t *dp = dirs + p.cell_off;
+    T *b2 = reinterpret_cast<T *>(dtw_smem), *b1 = b2 + maxdiag, *b0 = b1 + maxdiag;
+    T nxt[kDtwPer];
+    {
+        const int n = min(0, R - 1) - diag_lo(0, C) + 1;
+#pragma unroll
+        for (int k = 0; k < kDtwPer; ++k) {
+            const int c = threadIdx.x + k * nt;
+            nxt[k] = c < n ? cp[c] : (T)0;
+        }
+    }
+    for (int d = 0; d < D; ++d) {
+        T cur[kDtwPer];
+#pragma unroll
+        for (int k = 0; k < kDtwPer; ++k) cur[k] = nxt[k];
+        const int lo = diag_lo(d, C), n = min(d, R - 1) - lo + 1;
+        const int64_t start = diag_start(d, R, C);
+        if (d + 1 < D) {
+            const int n1 = min(d + 1, R - 1) - diag_lo(d + 1, C) + 1;
+            const int64_t s1 = start + n;
+#pragma unroll
+            for (int k = 0; k < kDtwPer; ++k) {
+                const int c = threadIdx.x + k * nt;
+                if (c < n1) nxt[k] = cp[s1 + c];
+            }
+        }
+        const int lo1 = diag_lo(d - 1, C), lo2 = diag_lo(d - 2, C);
+#pragma unroll
+        for (int k = 0; k < kDtwPer; ++k) {
+            const int c = threadIdx.x + k * nt;
+            if (c >= n) break;
+            const int i = lo + c, j = d - i;
+            T v;
+            if (i == 0 || j == 0) {
+                v = (i == 0 && j == 0) ? (T)0 : inf_of<T>();
+            } else {
+                const T up = b1[i - 1 - lo1], left = b1[i - lo1], dg = b2[i - 1 - lo2];
+                T m = up;
+                uint8_t dir = 0;
+                if (left < m) m = left, dir = 1;
+                if (dg < m) m = dg, dir = 2;
+                v = add_rn(cur[k], m);
+                dp[start + c] = dir;
+            }
+            b0[c] = v;
+            if (FULL) dtw_full[(int64_t)i * C + j] = v;
+            if (i == R - 1 && j == C - 1 && path_cost) path_cost[blockIdx.x] = v;
+        }
+        __syncthreads();
+        T *t = b2;
+        b2 = b1, b1 = b0, b0 = t;
+    }
+}
+
+// one thread per pair: align_from_distances.  results[i] = j while i > 0 and j > 0, then the first minimum of up, left, diagonal
+// (the direction byte); rows the walk never reached stay 0.
+__global__ void backtrack_kernel(const uint8_t *__restrict__ dirs, const PairMeta *__restrict__ pairs, PairMeta single, int n_pairs,
+                                 int64_t *__restrict__ out) {
+    const int pid = blockIdx.x * blockDim.x + threadIdx.x;
+    if (pid >= n_pairs) return;
+    const PairMeta p = pairs ? pairs[pid] : single;
+    const int R = p.R, C = p.C;
+    const uint8_t *dp = dirs + p.cell_off;
+    int64_t *res = out + p.out_row;
+    int i = R - 1, j = C - 1, first = R;
+    while (i > 0 && j > 0) {
+        res[i] = j;
+        first = i;
+        const uint8_t dir = dp[skew_index(i, j, R, C)];
+        if (dir != 1) --i;
+        if (dir != 0) --j;
+    }
+    for (int r = 0; r < first; ++r) res[r] = 0;
+}
+
+int dtw_threads(int maxdiag) {
+    const int t = (maxdiag + kDtwPer - 1) / kDtwPer;
+    return std::min(kDtwMaxThreads, std::max(64, (t + 31) / 32 * 32));
+}
+
+template <typename T>
+int launch_dtw(const T *cost, const PairMeta *pairs, const PairMeta &single, int n_pairs, int maxdiag, uint8_t *dirs, T *path_cost,
+               T *dtw_full, cudaStream_t st) {
+    const size_t smem = (size_t)3 * maxdiag * sizeof(T);
+    const int threads = dtw_threads(maxdiag);
+    if (dtw_full) {
+        static size_t configured[kSmemCacheDevices] = {};
+        SVB_TRY(raise_smem_limit(dtw_kernel<T, true>, smem, configured));
+        dtw_kernel<T, true><<<n_pairs, threads, smem, st>>>(cost, pairs, single, maxdiag, dirs, path_cost, dtw_full);
+    } else {
+        static size_t configured[kSmemCacheDevices] = {};
+        SVB_TRY(raise_smem_limit(dtw_kernel<T, false>, smem, configured));
+        dtw_kernel<T, false><<<n_pairs, threads, smem, st>>>(cost, pairs, single, maxdiag, dirs, path_cost, nullptr);
+    }
+    SVB_CUDA(cudaGetLastError());
+    return SVB_OK;
+}
+
+// workspace layout of svb_sadtw_align: [seq metas | pair metas | histograms | skewed costs | direction bytes]
+struct Layout {
+    size_t off[5], total;
+    int64_t rows_src, rows_tgt, cells;
+};
+
+int sadtw_layout(int32_t n, const int32_t *src_len, const int32_t *tgt_len, Layout &L) {
+    SVB_CHECK(n > 0 && n <= kMaxPairs, SVB_ERR_INVALID, "sadtw: %d pairs (1 .. %d)", n, kMaxPairs);
+    SVB_CHECK(src_len && tgt_len, SVB_ERR_INVALID, "sadtw: null length array");
+    L.rows_src = L.rows_tgt = L.cells = 0;
+    for (int p = 0; p < n; ++p) {
+        SVB_CHECK(src_len[p] >= 2 && tgt_len[p] >= 2, SVB_ERR_INVALID,
+                  "sadtw: pair %d has %d amateur and %d professional frames (at least 2 each are needed)", p, src_len[p], tgt_len[p]);
+        SVB_CHECK(std::min(src_len[p], tgt_len[p]) <= kMaxDiag, SVB_ERR_INVALID,
+                  "sadtw: pair %d: min(%d, %d) frames exceeds the %d-cell anti-diagonal of the DTW kernel", p, src_len[p], tgt_len[p],
+                  kMaxDiag);
+        L.rows_src += src_len[p], L.rows_tgt += tgt_len[p], L.cells += (int64_t)src_len[p] * tgt_len[p];
+    }
+    L.off[0] = 0;
+    L.off[1] = align_up(L.off[0] + (size_t)2 * n * sizeof(SeqMeta));
+    L.off[2] = align_up(L.off[1] + (size_t)n * sizeof(PairMeta));
+    L.off[3] = align_up(L.off[2] + (size_t)(L.rows_src + L.rows_tgt) * kBins * sizeof(float));
+    L.off[4] = align_up(L.off[3] + (size_t)L.cells * sizeof(float));
+    L.total = align_up(L.off[4] + (size_t)L.cells);
+    return SVB_OK;
+}
+
+struct StageTimer {
+    cudaEvent_t ev[5] = {};
+    bool on;
+    explicit StageTimer(bool on_) : on(on_) {}
+    ~StageTimer() {
+        for (auto e : ev)
+            if (e) cudaEventDestroy(e);
+    }
+    int create() {
+        if (on)
+            for (auto &e : ev) SVB_CUDA(cudaEventCreate(&e));
+        return SVB_OK;
+    }
+    int mark(int k, cudaStream_t st) {
+        if (on) SVB_CUDA(cudaEventRecord(ev[k], st));
+        return SVB_OK;
+    }
+    int read(float *ms) {
+        if (!on) return SVB_OK;
+        SVB_CUDA(cudaEventSynchronize(ev[4]));
+        for (int k = 0; k < 4; ++k) SVB_CUDA(cudaEventElapsedTime(ms + k, ev[k], ev[k + 1]));
+        return SVB_OK;
+    }
+};
+
+}  // namespace
+
+extern "C" int64_t svb_sadtw_workspace_bytes(int32_t n_pairs, const int32_t *src_len_host, const int32_t *tgt_len_host,
+                                             int64_t *offsets_host) {
+    Layout L;
+    if (sadtw_layout(n_pairs, src_len_host, tgt_len_host, L) != SVB_OK) return -1;
+    if (offsets_host)
+        for (int k = 0; k < 5; ++k) offsets_host[k] = (int64_t)L.off[k];
+    return (int64_t)L.total;
+}
+
+extern "C" int svb_sadtw_align(const void *src_f0_dev, const void *tgt_f0_dev, int32_t dtype, int32_t variant, int32_t n_pairs,
+                               const int32_t *src_len_host, const int32_t *tgt_len_host, const double *tgt_scale_host,
+                               void *workspace_dev, int64_t workspace_bytes, int64_t *alignment_dev, float *path_cost_dev,
+                               float *stage_ms_host, void *stream) {
+    SVB_CHECK(src_f0_dev && tgt_f0_dev && workspace_dev && alignment_dev, SVB_ERR_INVALID, "sadtw: null argument");
+    SVB_CHECK(dtype == SVB_SADTW_F32 || dtype == SVB_SADTW_F64, SVB_ERR_INVALID, "sadtw: bad f0 dtype %d", dtype);
+    SVB_CHECK(variant == SVB_SADTW || variant == SVB_EHSADTW, SVB_ERR_INVALID, "sadtw: bad variant %d", variant);
+    Layout L;
+    SVB_TRY(sadtw_layout(n_pairs, src_len_host, tgt_len_host, L));
+    SVB_CHECK(workspace_bytes >= (int64_t)L.total, SVB_ERR_INVALID, "sadtw: workspace of %lld bytes, %lld needed",
+              (long long)workspace_bytes, (long long)L.total);
+    const int n = n_pairs;
+    std::vector<SeqMeta> seqs(2 * (size_t)n);
+    std::vector<PairMeta> pairs(n);
+    int64_t fs = 0, ft = 0, cells = 0;
+    int maxlen = 0, maxdiag = 0;
+    int64_t maxtiles = 0;
+    for (int p = 0; p < n; ++p) {
+        const int S = src_len_host[p], T = tgt_len_host[p];
+        const double scale = tgt_scale_host ? tgt_scale_host[p] : (double)T / (double)S;
+        SVB_TRY(make_seq(variant, fs, fs, S, 1.0, "amateur sequence", p, seqs[p]));
+        SVB_TRY(make_seq(variant, ft, L.rows_src + ft, T, scale, "professional sequence", p, seqs[n + p]));
+        pairs[p] = PairMeta{fs, L.rows_src + ft, cells, ft, T, S};
+        fs += S, ft += T, cells += (int64_t)S * T;
+        maxlen = std::max(maxlen, std::max(S, T));
+        maxdiag = std::max(maxdiag, std::min(S, T));
+        maxtiles = std::max(maxtiles, (int64_t)((S + kTileJ - 1) / kTileJ) * ((T + kTileI - 1) / kTileI));
+    }
+    // everything is validated: from here on, launches
+    cudaStream_t st = as_stream(stream);
+    char *ws = static_cast<char *>(workspace_dev);
+    SeqMeta *d_seqs = reinterpret_cast<SeqMeta *>(ws + L.off[0]);
+    PairMeta *d_pairs = reinterpret_cast<PairMeta *>(ws + L.off[1]);
+    float *d_hist = reinterpret_cast<float *>(ws + L.off[2]), *d_cost = reinterpret_cast<float *>(ws + L.off[3]);
+    uint8_t *d_dirs = reinterpret_cast<uint8_t *>(ws + L.off[4]);
+    SVB_CUDA(cudaMemcpyAsync(d_seqs, seqs.data(), seqs.size() * sizeof(SeqMeta), cudaMemcpyHostToDevice, st));
+    SVB_CUDA(cudaMemcpyAsync(d_pairs, pairs.data(), pairs.size() * sizeof(PairMeta), cudaMemcpyHostToDevice, st));
+    StageTimer tm(stage_ms_host != nullptr);
+    SVB_TRY(tm.create());
+    SVB_TRY(tm.mark(0, st));
+    const dim3 hgrid((maxlen + kHistThreads / 8 - 1) / (kHistThreads / 8), 2 * n);
+    if (dtype == SVB_SADTW_F32)
+        sadtw_hist_kernel<float><<<hgrid, kHistThreads, 0, st>>>(static_cast<const float *>(src_f0_dev),
+                                                                static_cast<const float *>(tgt_f0_dev), n, d_seqs, variant, d_hist,
+                                                                nullptr);
+    else
+        sadtw_hist_kernel<double><<<hgrid, kHistThreads, 0, st>>>(static_cast<const double *>(src_f0_dev),
+                                                                 static_cast<const double *>(tgt_f0_dev), n, d_seqs, variant, d_hist,
+                                                                 nullptr);
+    SVB_CUDA(cudaGetLastError());
+    SVB_TRY(tm.mark(1, st));
+    const dim3 cgrid((unsigned)maxtiles, n);
+    sadtw_cost_kernel<<<cgrid, kCostThreads, 0, st>>>(d_hist, d_pairs, d_cost);
+    SVB_CUDA(cudaGetLastError());
+    SVB_TRY(tm.mark(2, st));
+    SVB_TRY(launch_dtw<float>(d_cost, d_pairs, PairMeta{}, n, maxdiag, d_dirs, path_cost_dev, nullptr, st));
+    SVB_TRY(tm.mark(3, st));
+    backtrack_kernel<<<(n + 127) / 128, 128, 0, st>>>(d_dirs, d_pairs, PairMeta{}, n, alignment_dev);
+    SVB_CUDA(cudaGetLastError());
+    SVB_TRY(tm.mark(4, st));
+    return tm.read(stage_ms_host);
+}
+
+extern "C" int64_t svb_sadtw_histogram_workspace_bytes(int32_t n_seq) {
+    if (n_seq <= 0 || n_seq > kMaxPairs) return -1;
+    return (int64_t)align_up((size_t)n_seq * sizeof(SeqMeta));
+}
+
+extern "C" int svb_sadtw_histogram(const void *f0_dev, int32_t dtype, int32_t variant, int32_t n_seq, const int32_t *len_host,
+                                   const double *scale_host, void *workspace_dev, int64_t workspace_bytes, float *hist_dev,
+                                   int32_t *counts_dev, void *stream) {
+    SVB_CHECK(f0_dev && len_host && workspace_dev && hist_dev, SVB_ERR_INVALID, "sadtw_histogram: null argument");
+    SVB_CHECK(dtype == SVB_SADTW_F32 || dtype == SVB_SADTW_F64, SVB_ERR_INVALID, "sadtw_histogram: bad f0 dtype %d", dtype);
+    SVB_CHECK(variant == SVB_SADTW || variant == SVB_EHSADTW, SVB_ERR_INVALID, "sadtw_histogram: bad variant %d", variant);
+    const int64_t need = svb_sadtw_histogram_workspace_bytes(n_seq);
+    SVB_CHECK(need > 0, SVB_ERR_INVALID, "sadtw_histogram: %d sequences (1 .. %d)", n_seq, kMaxPairs);
+    SVB_CHECK(workspace_bytes >= need, SVB_ERR_INVALID, "sadtw_histogram: workspace of %lld bytes, %lld needed",
+              (long long)workspace_bytes, (long long)need);
+    std::vector<SeqMeta> seqs(n_seq);
+    int64_t off = 0;
+    int maxlen = 0;
+    for (int k = 0; k < n_seq; ++k) {
+        SVB_TRY(make_seq(variant, off, off, len_host[k], scale_host ? scale_host[k] : 1.0, "sequence", k, seqs[k]));
+        off += len_host[k];
+        maxlen = std::max(maxlen, (int)len_host[k]);
+    }
+    cudaStream_t st = as_stream(stream);
+    SVB_CUDA(cudaMemcpyAsync(workspace_dev, seqs.data(), seqs.size() * sizeof(SeqMeta), cudaMemcpyHostToDevice, st));
+    const SeqMeta *d_seqs = static_cast<const SeqMeta *>(workspace_dev);
+    const dim3 grid((maxlen + kHistThreads / 8 - 1) / (kHistThreads / 8), n_seq);
+    if (dtype == SVB_SADTW_F32) {
+        const float *f = static_cast<const float *>(f0_dev);
+        sadtw_hist_kernel<float><<<grid, kHistThreads, 0, st>>>(f, f, n_seq, d_seqs, variant, hist_dev, counts_dev);
+    } else {
+        const double *f = static_cast<const double *>(f0_dev);
+        sadtw_hist_kernel<double><<<grid, kHistThreads, 0, st>>>(f, f, n_seq, d_seqs, variant, hist_dev, counts_dev);
+    }
+    SVB_CUDA(cudaGetLastError());
+    return SVB_OK;
+}
+
+extern "C" int svb_sadtw_cost(const float *hist_a_dev, int32_t n_a, const float *hist_b_dev, int32_t n_b, float *dist_dev,
+                              void *stream) {
+    SVB_CHECK(hist_a_dev && hist_b_dev && dist_dev, SVB_ERR_INVALID, "sadtw_cost: null argument");
+    SVB_CHECK(n_a > 0 && n_b > 0, SVB_ERR_INVALID, "sadtw_cost: empty histogram (%d x %d rows)", n_a, n_b);
+    SVB_CHECK(((uintptr_t)hist_a_dev & 15) == 0 && ((uintptr_t)hist_b_dev & 15) == 0, SVB_ERR_INVALID,
+              "sadtw_cost: histograms must be 16-byte aligned");
+    const int64_t cells = (int64_t)n_a * n_b;
+    const unsigned grid = (unsigned)std::min<int64_t>((cells + kCostThreads - 1) / kCostThreads, 65536);
+    sadtw_dist_kernel<<<grid, kCostThreads, 0, as_stream(stream)>>>(hist_a_dev, n_a, hist_b_dev, n_b, dist_dev);
+    SVB_CUDA(cudaGetLastError());
+    return SVB_OK;
+}
+
+extern "C" int64_t svb_dtw_workspace_bytes(int32_t dtype, int32_t rows, int32_t cols) {
+    if ((dtype != SVB_SADTW_F32 && dtype != SVB_SADTW_F64) || rows <= 0 || cols <= 0 || std::min(rows, cols) > kMaxDiag) return -1;
+    const size_t cells = (size_t)rows * cols;
+    return (int64_t)(align_up(cells * (dtype == SVB_SADTW_F32 ? 4 : 8)) + align_up(cells));
+}
+
+extern "C" int svb_dtw_align(const void *cost_dev, int32_t dtype, int32_t rows, int32_t cols, void *workspace_dev,
+                             int64_t workspace_bytes, int64_t *alignment_dev, void *path_cost_dev, void *dtw_dev, void *stream) {
+    SVB_CHECK(cost_dev && workspace_dev, SVB_ERR_INVALID, "dtw_align: null argument");
+    SVB_CHECK(dtype == SVB_SADTW_F32 || dtype == SVB_SADTW_F64, SVB_ERR_INVALID, "dtw_align: bad cost dtype %d", dtype);
+    SVB_CHECK(rows > 0 && cols > 0, SVB_ERR_INVALID, "dtw_align: empty cost matrix (%d x %d)", rows, cols);
+    SVB_CHECK(std::min(rows, cols) <= kMaxDiag, SVB_ERR_INVALID,
+              "dtw_align: min(%d, %d) exceeds the %d-cell anti-diagonal of the DTW kernel", rows, cols, kMaxDiag);
+    const int64_t need = svb_dtw_workspace_bytes(dtype, rows, cols);
+    SVB_CHECK(workspace_bytes >= need, SVB_ERR_INVALID, "dtw_align: workspace of %lld bytes, %lld needed", (long long)workspace_bytes,
+              (long long)need);
+    const size_t cells = (size_t)rows * cols, esz = dtype == SVB_SADTW_F32 ? 4 : 8;
+    char *ws = static_cast<char *>(workspace_dev);
+    uint8_t *dirs = reinterpret_cast<uint8_t *>(ws + align_up(cells * esz));
+    PairMeta single{0, 0, 0, 0, rows, cols};
+    cudaStream_t st = as_stream(stream);
+    const unsigned grid = (unsigned)std::min<size_t>((cells + 255) / 256, 65536);
+    const int maxdiag = std::min(rows, cols);
+    if (dtype == SVB_SADTW_F32) {
+        skew_kernel<float><<<grid, 256, 0, st>>>(static_cast<const float *>(cost_dev), rows, cols, reinterpret_cast<float *>(ws));
+        SVB_CUDA(cudaGetLastError());
+        SVB_TRY(launch_dtw<float>(reinterpret_cast<const float *>(ws), nullptr, single, 1, maxdiag, dirs,
+                                  static_cast<float *>(path_cost_dev), static_cast<float *>(dtw_dev), st));
+    } else {
+        skew_kernel<double><<<grid, 256, 0, st>>>(static_cast<const double *>(cost_dev), rows, cols, reinterpret_cast<double *>(ws));
+        SVB_CUDA(cudaGetLastError());
+        SVB_TRY(launch_dtw<double>(reinterpret_cast<const double *>(ws), nullptr, single, 1, maxdiag, dirs,
+                                   static_cast<double *>(path_cost_dev), static_cast<double *>(dtw_dev), st));
+    }
+    if (alignment_dev) {
+        backtrack_kernel<<<1, 32, 0, st>>>(dirs, nullptr, single, 1, alignment_dev);
+        SVB_CUDA(cudaGetLastError());
+    }
+    return SVB_OK;
+}

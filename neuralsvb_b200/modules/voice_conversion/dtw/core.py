@@ -1,0 +1,251 @@
+"""Shape-aware DTW on the GPU (csrc/sadtw.cu): the batched entry points behind the drop-in ``align``, ``shape_aware_dtw`` and
+``enhance_sadtw`` modules, plus ``align_pitch`` for a binarizer and ``a2p_alignment_batch`` for ``MleSVBVAE``'s ``a2p`` way.
+
+f0 contours may be numpy arrays or torch tensors, on the host or on a CUDA device, shaped [S] or [S, 1], float32 or float64; the
+arithmetic runs in that type, like the reference's.  Host inputs are copied to the current CUDA device.  There is no CPU path.
+"""
+import ctypes
+
+import numpy as np
+import torch
+
+from neuralsvb_b200 import _native
+
+VARIANTS = {'SADTW': 0, 'EHSADTW': 1}
+DTYPES = {torch.float32: 0, torch.float64: 1}
+BINS = 48
+
+
+def _vp(t):
+    return None if t is None else ctypes.c_void_p(t.data_ptr())
+
+
+def _i32(v):
+    a = np.ascontiguousarray(v, dtype=np.int32)
+    return a, ctypes.c_void_p(a.ctypes.data)
+
+
+def _check(rc, what):
+    if rc is not None and rc < 0:
+        msg = _native.lib().svb_last_error().decode('utf-8', 'replace')
+        if rc == -1:                   # SVB_ERR_INVALID: rejected before any launch
+            raise ValueError(f'{what}: {msg}')
+        raise RuntimeError(f'libsvb_vocoder {what} failed ({rc}): {msg}')
+    return rc
+
+
+def device_of(*xs):
+    """The CUDA device of the first device tensor among xs, else the current CUDA device."""
+    for x in xs:
+        if torch.is_tensor(x) and x.is_cuda:
+            return x.device
+    if not torch.cuda.is_available():
+        raise RuntimeError('shape-aware DTW runs on CUDA: neuralsvb_b200 has no CPU fallback')
+    return torch.device('cuda', torch.cuda.current_device())
+
+
+def as_tensor(x):
+    if torch.is_tensor(x):
+        return x.detach()
+    return torch.from_numpy(np.ascontiguousarray(x))
+
+
+def f0_tensor(f, device):
+    """1-D contiguous device tensor of an f0 contour ([S] or [S, 1], float32 or float64)."""
+    t = as_tensor(f)
+    if t.dim() == 2 and t.shape[1] == 1:
+        t = t[:, 0]
+    if t.dim() != 1:
+        raise ValueError(f'an f0 contour must be [S] or [S, 1], got {tuple(t.shape)}')
+    if t.dtype not in DTYPES:
+        raise TypeError(f'an f0 contour must be float32 or float64, got {t.dtype}')
+    return t.to(device).contiguous()
+
+
+def _check_finite(t):
+    if not bool(torch.isfinite(t).all()):
+        raise ValueError('f0 contains NaN or inf (the reference exits on it)')
+
+
+def _batch_f0(fs, device, what):
+    ts = [f0_tensor(f, device) for f in fs]
+    dts = {t.dtype for t in ts}
+    if len(dts) > 1:
+        raise TypeError(f'{what} f0 contours mix float32 and float64; a batch runs in one type')
+    lens = [int(t.shape[0]) for t in ts]
+    if min(lens) < 2:
+        raise ValueError(f'{what} contour of {min(lens)} frames: at least 2 are needed (the reference divides by zero)')
+    cat = torch.cat(ts) if len(ts) > 1 else ts[0]
+    _check_finite(cat)
+    return cat, lens, ts[0].dtype
+
+
+class AlignResult:
+    """alignment: int64 device tensor [sum T] (pair p's rows after the pairs before it), offsets: its row offsets [n + 1] (host),
+    path_cost: float32 [n] DTW value at each pair's last cell, stage_ms: (histogram, cost, dtw, backtrack) CUDA-event times or None,
+    workspace / sections: the workspace and its section byte offsets when keep_workspace=True."""
+
+    def __init__(self, **kw):
+        self.__dict__.update(kw)
+
+    def split(self):
+        """One host int64 numpy array per pair."""
+        a = self.alignment.cpu().numpy()
+        return [a[self.offsets[p]:self.offsets[p + 1]] for p in range(len(self.offsets) - 1)]
+
+
+def align_batch(srcs, tgts, method='EHSADTW', scales=None, stage_ms=False, keep_workspace=False):
+    """Shape-aware DTW of n pairs in one launch sequence: srcs = amateur contours (S_p frames), tgts = professional ones (T_p
+    frames); scales: the professional histogram's scale factor per pair (default T_p / S_p, cal_shape_dist's)."""
+    if method not in VARIANTS:
+        raise ValueError(f'method must be one of {sorted(VARIANTS)}, got {method!r}')
+    if len(srcs) != len(tgts) or len(srcs) == 0:
+        raise ValueError(f'{len(srcs)} amateur and {len(tgts)} professional contours')
+    device = device_of(*srcs, *tgts)
+    src, S, dt = _batch_f0(srcs, device, 'amateur')
+    tgt, T, dt2 = _batch_f0(tgts, device, 'professional')
+    if dt != dt2:
+        raise TypeError('amateur and professional f0 must have the same type')
+    n, lib = len(S), _native.lib()
+    s_arr, s_p = _i32(S)
+    t_arr, t_p = _i32(T)
+    sec = (ctypes.c_int64 * 5)()
+    ws_bytes = _check(lib.svb_sadtw_workspace_bytes(n, s_p, t_p, sec), 'sadtw_workspace_bytes')
+    sc = None
+    if scales is not None:
+        sc = np.ascontiguousarray(scales, dtype=np.float64)
+        if sc.shape != (n,):
+            raise ValueError(f'{n} pairs but {sc.shape} scale factors')
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
+    out = torch.empty(int(t_arr.sum()), dtype=torch.int64, device=device)
+    pc = torch.empty(n, dtype=torch.float32, device=device)
+    ms = (ctypes.c_float * 4)() if stage_ms else None
+    with torch.cuda.device(device):
+        _check(lib.svb_sadtw_align(_vp(src), _vp(tgt), DTYPES[dt], VARIANTS[method], n, s_p, t_p,
+                                   None if sc is None else ctypes.c_void_p(sc.ctypes.data), _vp(ws), ws_bytes, _vp(out), _vp(pc), ms,
+                                   _native.current_stream_ptr(device)), 'sadtw_align')
+    return AlignResult(alignment=out, offsets=np.concatenate([[0], np.cumsum(T)]).astype(np.int64), path_cost=pc,
+                       stage_ms=tuple(ms) if stage_ms else None, src_len=S, tgt_len=T,
+                       workspace=ws if keep_workspace else None, sections=list(sec) if keep_workspace else None)
+
+
+def histogram(f0s, method='SADTW', scales=None, counts=False):
+    """The histogram kernel alone on n contours: float32 device [sum len, 48] (k / total) and, with counts=True, int32 k."""
+    device = device_of(*f0s)
+    f, lens, dt = _batch_f0(f0s, device, 'the')
+    n, lib = len(lens), _native.lib()
+    l_arr, l_p = _i32(lens)
+    sc = np.ascontiguousarray(np.ones(n) if scales is None else scales, dtype=np.float64)
+    ws_bytes = _check(lib.svb_sadtw_histogram_workspace_bytes(n), 'sadtw_histogram_workspace_bytes')
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
+    rows = int(l_arr.sum())
+    hist = torch.empty(rows, BINS, dtype=torch.float32, device=device)
+    cnt = torch.empty(rows, BINS, dtype=torch.int32, device=device) if counts else None
+    with torch.cuda.device(device):
+        _check(lib.svb_sadtw_histogram(_vp(f), DTYPES[dt], VARIANTS[method], n, l_p, ctypes.c_void_p(sc.ctypes.data), _vp(ws),
+                                       ws_bytes, _vp(hist), _vp(cnt), _native.current_stream_ptr(device)), 'sadtw_histogram')
+    return (hist, cnt) if counts else hist
+
+
+def hist_of_f0(input_f, method, max_window=64, normalize_hist=False, scale_factor=1.):
+    """cal_hist_of_f0: a list of T lists of 48 numbers (ints, or k / total floats with normalize_hist)."""
+    if max_window != 64:
+        raise NotImplementedError(f'max_window={max_window}: only the 64-frame windows the pitch alignment uses are implemented')
+    _, c = histogram([input_f], method, [float(scale_factor)], counts=True)
+    c = c.cpu().numpy().astype(np.int64)
+    if normalize_hist:
+        return (c.astype(np.float64) / c.sum(1, keepdims=True).astype(np.float64)).tolist()
+    return c.tolist()
+
+
+def hist_dist(hist_a, hist_b):
+    """cal_hist_dist: float32 [T1, T2] on hist_a's device."""
+    device = device_of(hist_a, hist_b)
+    a = as_tensor(hist_a).to(device=device, dtype=torch.float32).contiguous()
+    b = as_tensor(hist_b).to(device=device, dtype=torch.float32).contiguous()
+    if a.dim() != 2 or b.dim() != 2 or a.shape[1] != BINS or b.shape[1] != BINS:
+        raise ValueError(f'histograms must be [T, {BINS}], got {tuple(a.shape)} and {tuple(b.shape)}')
+    dist = torch.empty(a.shape[0], b.shape[0], dtype=torch.float32, device=device)
+    with torch.cuda.device(device):
+        _check(_native.lib().svb_sadtw_cost(_vp(a), a.shape[0], _vp(b), b.shape[0], _vp(dist), _native.current_stream_ptr(device)),
+               'sadtw_cost')
+    home = hist_a.device if torch.is_tensor(hist_a) else torch.device('cpu')
+    return dist.to(home)
+
+
+def shape_dist(src, tgt, src_len, tgt_len, method):
+    """cal_shape_dist: [1, S, T] float32 (the amateur histogram at scale 1, the professional one at tgt_len / src_len)."""
+    hs = histogram([src], method)
+    ht = histogram([tgt], method, [tgt_len / src_len])
+    d = hist_dist(hs, ht)
+    return d.unsqueeze(0).to(src.device if torch.is_tensor(src) else torch.device('cpu'))
+
+
+def dtw(costs, alignment=True, matrix=False):
+    """time_warp / align_from_distances on a [rows, cols] float32 or float64 cost: (alignment int64 [rows] or None, DTW value at
+    the last cell, DTW matrix or None), device tensors."""
+    device = device_of(costs)
+    c = as_tensor(costs)
+    if c.dim() != 2:
+        raise ValueError(f'a cost matrix is [rows, cols], got {tuple(c.shape)}')
+    if c.dtype not in DTYPES:
+        raise TypeError(f'a cost matrix must be float32 or float64, got {c.dtype}')
+    c = c.to(device).contiguous()
+    R, C = c.shape
+    lib = _native.lib()
+    ws_bytes = lib.svb_dtw_workspace_bytes(DTYPES[c.dtype], R, C)
+    if ws_bytes < 0:
+        raise ValueError(f'time_warp: unsupported cost shape {tuple(c.shape)} (min(rows, cols) <= 8192)')
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
+    al = torch.empty(R, dtype=torch.int64, device=device) if alignment else None
+    pc = torch.empty(1, dtype=c.dtype, device=device)
+    full = torch.empty_like(c) if matrix else None
+    with torch.cuda.device(device):
+        _check(lib.svb_dtw_align(_vp(c), DTYPES[c.dtype], R, C, _vp(ws), ws_bytes, _vp(al), _vp(pc), _vp(full),
+                                 _native.current_stream_ptr(device)), 'dtw_align')
+    return al, pc, full
+
+
+def align_one(src, tgt, input, method):
+    """SADTW / EHSADTW(src, tgt, input) -> (input[alignment], alignment as a list)."""
+    alignment = align_batch([src], [tgt], method).alignment.cpu().tolist()
+    return input[alignment], alignment
+
+
+def dtw_align_batch(srcs, tgts, inputs, srcs_lens, tgt_lens, method):
+    """DTW_align: every pair of the padded batch in one launch sequence, the histograms over the whole padded rows and the
+    professional scale factor tgt_len / src_len, as the reference does."""
+    B = len(srcs)
+    sl = [int(x) for x in (srcs_lens if srcs_lens is not None else [srcs[b].shape[0] for b in range(B)])]
+    tl = [int(x) for x in (tgt_lens if tgt_lens is not None else [tgts[b].shape[0] for b in range(B)])]
+    r = align_batch([srcs[b] for b in range(B)], [tgts[b] for b in range(B)], method, scales=[t / s for s, t in zip(sl, tl)])
+    return torch.stack([inputs[b][a.tolist()] for b, a in enumerate(r.split())], dim=0)
+
+
+def align_pitch(src_f0s, tgt_f0s, method='EHSADTW'):
+    """Batched pitch alignment for a binarizer: the a2p alignment of every (amateur, professional) pair, as host int64 arrays of
+    the professional lengths (what binarize_para.get_pitch_align stores per item)."""
+    return align_batch(list(src_f0s), list(tgt_f0s), method).split()
+
+
+def a2p_alignment_batch(amateur_f0, prof_f0, amateur_len, prof_len, method='EHSADTW'):
+    """The [B, T_prof] int64 device tensor MleSVBVAE.forward takes as a2p_alignment, from padded f0 batches [B, T_ama] / [B, T_prof]
+    and the true lengths: pair b aligns amateur_f0[b, :amateur_len[b]] with prof_f0[b, :prof_len[b]], then MultiSpkEmbDataset's rule
+    (alignment[:prof_len].clip(max=amateur_len - 1)) and collate_1d's zero padding up to T_prof = prof_f0.shape[1]."""
+    a, p = as_tensor(amateur_f0), as_tensor(prof_f0)
+    if a.dim() != 2 or p.dim() != 2 or a.shape[0] != p.shape[0]:
+        raise ValueError(f'amateur_f0 / prof_f0 must be [B, T], got {tuple(a.shape)} and {tuple(p.shape)}')
+    B, Tp = p.shape
+    la = [int(x) for x in as_tensor(amateur_len).reshape(-1).tolist()]
+    lp = [int(x) for x in as_tensor(prof_len).reshape(-1).tolist()]
+    if len(la) != B or len(lp) != B:
+        raise ValueError(f'{B} pairs but {len(la)} / {len(lp)} lengths')
+    if max(lp) > Tp or max(la) > a.shape[1]:
+        raise ValueError('a length exceeds the padded f0 batch')
+    device = device_of(amateur_f0, prof_f0)
+    r = align_batch([a[b, :la[b]] for b in range(B)], [p[b, :lp[b]] for b in range(B)], method)
+    lp_t = torch.tensor(lp, device=device)
+    cap = torch.repeat_interleave(torch.tensor(la, device=device) - 1, lp_t)
+    out = torch.zeros(B, Tp, dtype=torch.int64, device=device)
+    out[torch.arange(Tp, device=device)[None, :] < lp_t[:, None]] = torch.minimum(r.alignment, cap)
+    return out

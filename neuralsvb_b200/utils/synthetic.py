@@ -507,3 +507,29 @@ def make_disc_mel(B, T, pad, seed=1234, n_mel=80):
         if p:
             m[b, T - p:] = 0.0
     return torch.from_numpy(m.astype(np.float32))
+
+
+def make_f0_pair(seed, S, T, fps=172.27):
+    """(amateur [S], professional [T]) float64 f0 contours in Hz for the shape-aware DTW: one melody of held notes (note steps of
+    a few semitones), sung twice.  The professional take has 5.5 Hz vibrato; the amateur one is detuned by up to half a semitone,
+    drifts, has slower vibrato and different note timing.  Both have unvoiced gaps (f0 = 0) between some notes, like a denormed
+    pitch track.  fps: frames per second (22050 Hz / hop 128)."""
+    rs = np.random.RandomState(seed + 61)
+    n_notes = max(1, int(round(max(S, T) / fps * 2.5)))
+    notes = 57 + np.cumsum(rs.randint(-4, 5, size=n_notes)).clip(-12, 12)
+    gaps = rs.rand(n_notes) < 0.3
+    base = rs.dirichlet(np.full(n_notes, 4.0))
+
+    def take(n, jitter, vib_hz, vib_st, detune, drift):
+        w = base * np.exp(rs.randn(n_notes) * jitter)
+        edges = np.concatenate([[0], np.cumsum(w / w.sum())]) * n
+        t = np.arange(n)
+        idx = np.searchsorted(edges[1:-1], t, side='right')
+        semis = notes[idx] + detune + drift * t / max(n - 1, 1) + vib_st * np.sin(2 * np.pi * vib_hz * t / fps + rs.rand() * 6.28)
+        f0 = 440.0 * 2.0 ** ((semis - 69) / 12.0)
+        pos = (t - edges[idx]) / np.maximum(edges[idx + 1] - edges[idx], 1)
+        f0[gaps[idx] & (pos > 0.75)] = 0.0
+        return f0
+    prof = take(T, 0.05, 5.5, 0.35, 0.0, 0.0)
+    ama = take(S, 0.35, 4.5, 0.15, rs.uniform(-0.5, 0.5), rs.uniform(-0.4, 0.4))
+    return ama, prof
