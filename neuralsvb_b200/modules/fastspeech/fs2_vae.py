@@ -136,6 +136,19 @@ class _NativeStack(nn.Module):
             pass
 
 
+def check_frames(T, stride=4):
+    """The frame counts a GlobalFVAE takes (vae_models.py:96-128): a multiple of the stride, because the decoder rebuilds T from the
+    T / stride latent frames, and long enough that the encoder's three k = 3 stride-2 poolings leave at least one frame (T >= 60 at
+    stride 4).  The reference's data loader crops every clip to a multiple of ``frames_multiple`` (4).  A shorter clip would leave
+    the poolings an empty time axis, whose mean is NaN rather than an error."""
+    n = T // stride
+    for _ in range(3):
+        n = (n - 3) // 2 + 1
+    if T % stride or n < 1:
+        raise ValueError(f'{T} frames: the GlobalFVAE takes a multiple of {stride} frames, at least {15 * stride} '
+                         f'(its posterior encoder pools T / {stride} frames three times by 2)')
+
+
 def _prep_mask_g(x_mask, g, B, T, gin):
     mask = None if not torch.is_tensor(x_mask) else x_mask.float().expand(B, 1, T).reshape(B, T).contiguous()
     gc = None if g is None else g.float().expand(B, gin, T).contiguous()
@@ -438,6 +451,8 @@ class GlobalFVAE(nn.Module):
 
     def forward(self, x=None, x_mask=None, g=None, infer=False, eps=None):
         from neuralsvb_b200.modules.hifigan.discriminators import conv_nct
+        if not infer:
+            check_frames(g.shape[-1], self.strides[0])
         g_sqz = g
         for c in self.g_pre_net:                                                                        # vae_models.py:20
             g_sqz = conv_nct(g_sqz.float(), c.weight, c.bias, c.kernel_size[0], stride=c.stride[0], pad=c.padding[0])

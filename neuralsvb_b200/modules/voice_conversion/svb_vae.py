@@ -22,7 +22,7 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
-from neuralsvb_b200.modules.fastspeech.fs2_vae import GlobalFVAE
+from neuralsvb_b200.modules.fastspeech.fs2_vae import GlobalFVAE, check_frames
 from neuralsvb_b200.modules.voice_conversion.vc_modules import VCASR, _bn_affine, _conv, _Holder
 
 
@@ -55,7 +55,7 @@ class _ConvStacks(nn.Module):
         x = _conv(x.transpose(1, 2).contiguous(), self.in_proj.weight, self.in_proj.bias)
         for blk in self.conv:
             h = _conv(x, blk.conv.conv.weight, blk.conv.conv.bias, K=self.K, pad=self.K // 2)
-            x = x + torch.relu(F.group_norm(h, blk.norm.num_groups, blk.norm.weight, blk.norm.bias, blk.norm.eps))
+            x = x + torch.relu(blk.norm(h))                         # nn.GroupNorm: F.group_norm with its parameters
         return _conv(x.contiguous(), self.out_proj.weight, self.out_proj.bias).transpose(1, 2)
 
 
@@ -145,6 +145,8 @@ class MleSVBVAE(nn.Module):
             raise RuntimeError('neuralsvb_b200 MleSVBVAE is inference only: call .eval() and run under torch.no_grad()')
         if self.trainable and not amateur_mel.is_cuda:
             raise RuntimeError('neuralsvb_b200 has no CPU path: move the module and its inputs to a CUDA device')
+        for mel in (amateur_mel, prof_mel):                         # before any launch: both clips go through the GlobalFVAE
+            check_frames(mel.shape[1], self.vae_model.strides[0])
         ways = kwargs['concurrent_ways']
         ret = {}
         ac = self.prepare_condition(amateur_mel, amateur_pitch, spk_ids=amateur_spk_id)

@@ -13,13 +13,14 @@ def _sub(w, prefix):
     return {k[len(prefix):]: v for k, v in w.items() if k.startswith(prefix)}
 
 
-def conv_stacks(w, pre, x, n_layers=3):
-    """ConvStacks (modules/commons/common_layers.py:672-707) with ConvBlock norm 'gn' (:739-773), res=True.  x [B, T, H]."""
+def conv_stacks(w, pre, x, n_layers=3, relu=None):
+    """ConvStacks (modules/commons/common_layers.py:672-707) with ConvBlock norm 'gn' (:739-773), res=True.  x [B, T, H].
+    ``relu(name, x)``, when given, replaces the ReLU on the output of the GroupNorm ``name`` (see oracle/svb_vae_train.py)."""
     x = F.linear(x, w[pre + '.in_proj.weight'], w[pre + '.in_proj.bias']).transpose(1, 2)
     for i in range(n_layers):
         h = F.conv1d(x, w[f'{pre}.conv.{i}.conv.conv.weight'], w[f'{pre}.conv.{i}.conv.conv.bias'], padding=2)
         h = F.group_norm(h, h.shape[1] // 16, w[f'{pre}.conv.{i}.norm.weight'], w[f'{pre}.conv.{i}.norm.bias'], 1e-5)
-        x = x + torch.relu(h)
+        x = x + (torch.relu(h) if relu is None else relu(f'{pre}.conv.{i}.norm', h))
     return F.linear(x.transpose(1, 2), w[pre + '.out_proj.weight'], w[pre + '.out_proj.bias'])
 
 

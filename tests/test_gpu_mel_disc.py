@@ -343,11 +343,12 @@ def model_tc(request, monkeypatch):
 def test_svb_step_with_adversarial_terms_matches_float64(model_tc, phase):
     """The phase-2 generator step with {a2a,p2p}_a and the phase-3 mapping step with a2p_a: the MleSVBVAE on its native kernels
     plus the native discriminator (frozen, train mode: its Dropout2d stays active in phase 3), against float64 autograd through
-    oracle/svb_vae_train.svb_train_losses plus oracle/multi_window_disc.svb_adv_losses, on the discriminator's own leaky-relu masks.
-    Bars are the steps' own (tests/test_gpu_svb_vae_train.py): BatchNorm amplification dominates them."""
+    oracle/svb_vae_train.svb_train_losses plus oracle/multi_window_disc.svb_adv_losses, on the discriminator's own leaky-relu masks
+    and, as tests/test_gpu_svb_vae_train._tied_step does, on the native PPG, train-mode BatchNorm inputs and ReLU masks.  Bars are the steps'
+    own (tests/test_gpu_svb_vae_train.py)."""
     from neuralsvb_b200.modules.commons.mel_loss import mel_l1_ssim_loss
     from oracle import svb_vae_train as O
-    from tests.test_gpu_svb_vae_train import MAP_BARS, _compare_step, _model, _set_phase
+    from tests.test_gpu_svb_vae_train import MAP_BARS, MAP_ZERO_GRAD, _compare_step, _model, _native_relu, _recorded, _set_phase, _tie
     from tests.test_gpu_svb_vae_train import STEP_BARS as SVB_STEP_BARS
     Ta, Tp = 136, 140                                   # long enough for the 128-frame window: the adversarial terms exist
     batch = S.make_svb_batch(2, Ta, Tp, 1234)
@@ -361,7 +362,8 @@ def test_svb_step_with_adversarial_terms_matches_float64(model_tc, phase):
     snap = {k: v.detach().clone() for k, v in m.state_dict().items()}
     b = {k: v.cuda() for k, v in batch.items()}
     targets = {'a2a': b['amateur_mel'], 'p2p': b['prof_mel'], 'a2p': b['prof_mel']}
-    ret = m(**b, concurrent_ways=ways, eps=torch.zeros(2, 128, 1, device='cuda'))
+    with _recorded(m) as trace:
+        ret = m(**b, concurrent_ways=ways, eps=torch.zeros(2, 128, 1, device='cuda'))
     losses = {}
     for way in ways:
         if 'kl' in ret[way]:
@@ -379,16 +381,21 @@ def test_svb_step_with_adversarial_terms_matches_float64(model_tc, phase):
     req = {n for n, q in m.named_parameters() if q.requires_grad}
     p = {k: (v.double().clone().requires_grad_(k in req) if v.is_floating_point() else v.clone()) for k, v in snap.items()}
     b64 = {k: (v.double() if v.is_floating_point() else v) for k, v in b.items()}
-    ref, out = O.svb_train_losses(p, b64, torch.zeros(2, 128, 1, device='cuda', dtype=torch.float64), phase)
+    tie, left = _tie(trace['bn'])
+    relu, masks_left = _native_relu(trace)
+    ref, out = O.svb_train_losses(p, b64, torch.zeros(2, 128, 1, device='cuda', dtype=torch.float64), phase,
+                                  ppg=dict(zip(('amateur', 'prof'), trace['ppg'])), tie=tie, relu=relu)
+    assert not any(left.values()) and not any(masks_left.values())
     ref.update(OD.svb_adv_losses(_sd64(disc, False), 'g' if phase == 2 else 3, {w: out[w]['mel_out'] for w in adv},
                                  starts=[d[0] for d in draws], scales=[[[s.double() for s in w] for w in d[1]] for d in draws],
                                  masks=_masks(rec, len(adv))))
     assert {f'{w}_a' for w in adv} <= set(ref)
     sum(ref.values()).backward()
     bars = (SVB_STEP_BARS if phase == 2 else MAP_BARS)[model_tc]
-    # The latent map's convs.0 / convs.3 biases feed train-mode BatchNorms directly: their exact gradient is 0 (the norm removes
-    # any per-channel shift), so both sides hold only rounding.  They are checked to stay at that level instead of relatively.
-    shift_free = {'z_mapping_function.convs.0.bias', 'z_mapping_function.convs.3.bias'} if phase == 3 else set()
+    # The latent map's convs.0 / convs.3 biases feed train-mode BatchNorms directly (spk_proj.2's through convs.0): their exact
+    # gradient is 0 (the norm removes any per-channel shift), so both sides hold only rounding.  They are checked to stay at that
+    # level instead of relatively.
+    shift_free = set(MAP_ZERO_GRAD) if phase == 3 else set()
     big = max(float(m.get_parameter(k).grad.abs().max()) for k in req)
     for k in shift_free:
         got, want = float(m.get_parameter(k).grad.abs().max()), float(p[k].grad.abs().max())
