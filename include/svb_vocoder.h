@@ -495,6 +495,33 @@ int64_t svb_dtw_workspace_bytes(int32_t dtype, int32_t rows, int32_t cols);
 int svb_dtw_align(const void *cost_dev, int32_t dtype, int32_t rows, int32_t cols, void *workspace_dev, int64_t workspace_bytes,
                   int64_t *alignment_dev, void *path_cost_dev, void *dtw_dev, void *stream);
 
+/* ---- Baseline pitch alignments of the paper's comparison (csrc/sadtw.cu): LoNDTW (modules/voice_conversion/dtw/local_norm_dtw.py),
+ * NaiveDTW / ZMNaiveDTW / NNaiveDTW (naive_dtw.py) over time_warp / align_from_distances, and NInterpo (naive_interpo.py).  Batches
+ * are ragged as in svb_sadtw_align: src_dev holds the amateur rows of every pair, tgt_dev the professional ones, float32 or float64
+ * (dtype, svb_sadtw_dtype), each row feat_dim values (NaiveDTW: 1 .. 4096; every other method aligns 1-D f0: 1).  The cost is
+ * torch.cdist's in the input's type: its matrix-product form sqrt(clamp_min(((sum_k -2 x_k y_k) + |x|^2) + |y|^2, 0)) summed in order
+ * k = 0, 1, ..., or, when both sides have at most 25 frames, sqrt(sum_k (x_k - y_k)^2).  NInterpo maps professional frame i to
+ * amateur frame min(floor(float(i) * (float(S) / T)), S - 1) (F.interpolate(mode='nearest')) and runs no DTW.
+ * svb_dtw_baselines_workspace_bytes: size of the caller-owned workspace (-1 on a bad method, dtype or length).
+ * svb_dtw_baselines_align writes alignment_dev int64 [sum tgt_len] as svb_sadtw_align does; path_cost_dev (NULL = not wanted; not
+ *   written by NInterpo) [n] in the input's type = the pair's DTW value at its last cell; stage_ms_host (NULL = not wanted) receives
+ *   4 CUDA-event times (per-frame features, cost, DTW, backtrack) and makes the call synchronise.
+ * svb_dtw_baselines_cost writes the cost alone, pair p's cdist matrix [src_len[p], tgt_len[p]] row-major after those of the pairs
+ *   before it, in the input's type (NInterpo is refused).
+ * Both reject before any launch (SVB_ERR_INVALID): a null pointer, a bad dtype, method or feat_dim, a length below 2, min(S, T) >
+ * 8192 for a DTW method, or a short workspace. */
+typedef enum svb_dtw_baseline {
+    SVB_LONDTW = 0, SVB_NAIVEDTW = 1, SVB_ZMNAIVEDTW = 2, SVB_NNAIVEDTW = 3, SVB_NINTERPO = 4
+} svb_dtw_baseline;
+int64_t svb_dtw_baselines_workspace_bytes(int32_t method, int32_t dtype, int32_t n_pairs, const int32_t *src_len_host,
+                                          const int32_t *tgt_len_host);
+int svb_dtw_baselines_align(const void *src_dev, const void *tgt_dev, int32_t dtype, int32_t method, int32_t n_pairs,
+                            const int32_t *src_len_host, const int32_t *tgt_len_host, int32_t feat_dim, void *workspace_dev,
+                            int64_t workspace_bytes, int64_t *alignment_dev, void *path_cost_dev, float *stage_ms_host, void *stream);
+int svb_dtw_baselines_cost(const void *src_dev, const void *tgt_dev, int32_t dtype, int32_t method, int32_t n_pairs,
+                           const int32_t *src_len_host, const int32_t *tgt_len_host, int32_t feat_dim, void *workspace_dev,
+                           int64_t workspace_bytes, void *cost_dev, void *stream);
+
 /* Host-only view of the schedule of a merged tensor-core launch (csrc/conv_tc.cu: tc_schedule; no CUDA call, usable without a GPU):
  * `n_layers` convolutions of one shape class (taps KS[l], residual / accumulate flags) over B clips x Tq rows, tiles of 128 rows in
  * items of up to MT tiles, `col_blocks` column blocks, `grid` CTAs.  items_out receives 5 ints per item (layer, column block, clip,

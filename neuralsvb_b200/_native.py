@@ -194,6 +194,9 @@ _PROTOS = {
     'svb_sadtw_cost': (ctypes.c_int, [_P, _I32, _P, _I32, _P, _P]),
     'svb_dtw_workspace_bytes': (_I64, [_I32, _I32, _I32]),
     'svb_dtw_align': (ctypes.c_int, [_P, _I32, _I32, _I32, _P, _I64, _P, _P, _P, _P]),
+    'svb_dtw_baselines_workspace_bytes': (_I64, [_I32, _I32, _I32, _P, _P]),
+    'svb_dtw_baselines_align': (ctypes.c_int, [_P, _P, _I32, _I32, _I32, _P, _P, _I32, _P, _I64, _P, _P, _P, _P]),
+    'svb_dtw_baselines_cost': (ctypes.c_int, [_P, _P, _I32, _I32, _I32, _P, _P, _I32, _P, _I64, _P, _P]),
 }
 
 

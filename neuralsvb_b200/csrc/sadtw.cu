@@ -557,3 +557,396 @@ extern "C" int svb_dtw_align(const void *cost_dev, int32_t dtype, int32_t rows, 
     }
     return SVB_OK;
 }
+
+// =================================================================================================================================
+// Baseline pitch alignments of the paper's comparison on the same ragged batches, skewed cost layout, DTW and backtrack kernels:
+//   LoNDTW     (local_norm_dtw.py): per frame the 64-value context f[t-32 .. t+31] (zeros outside [0, len)) minus its mean;
+//   NaiveDTW   (naive_dtw.py): rows of [S, H] features as they are (H = 1 for f0, 80 for a mel);
+//   ZMNaiveDTW: f0 - mean(f0);  NNaiveDTW: (f0 - mean(f0)) / (std(f0) + 1e-8), std unbiased;
+// then cost[i, j] = torch.cdist(amateur features, professional features)[j, i].  cdist takes its matrix-product form when either
+// side has more than 25 rows: sqrt(clamp_min(((sum_k (-2 x_k) y_k) + |x|^2) + |y|^2, 0)), the sum over k in order k = 0, 1, ...
+// (BLAS's order is not known; this is the fixed one), and |x - y| = sqrt(sum_k (x_k - y_k)^2) otherwise.  On the plateaus of a sung
+// note the rounding of the product form decides the path, so it is followed operation by operation with round-to-nearest
+// intrinsics (no FMA).  Everything runs in the input's type.
+//   NInterpo   (naive_interpo.py): no DTW; professional frame i takes amateur frame min(floor(float(i) * (float(S) / T)), S - 1),
+// F.interpolate(mode='nearest')'s float32 rule.
+// =================================================================================================================================
+namespace {
+
+enum { kLoN = 0, kNaive = 1, kZMNaive = 2, kNNaive = 3, kNInterpo = 4 };
+constexpr int kCtx = 64, kCtxHalf = 32;     // LoNDTW's context: f[t - 32 .. t + 31]
+constexpr int kDirectMaxRows = 25;          // torch.cdist's matrix-product form needs more rows than this on one side
+constexpr int kBTile = 64, kBThreads = 256, kBStage = 66;   // 64 x 64 cells per CTA, 4 x 4 per thread; output stage row stride
+constexpr int kBPrepThreads = 256;
+constexpr int kMaxFeat = 4096;
+
+struct BSeq {
+    int64_t in_row;                 // first row in its input array
+    int64_t buf_row;                // first row in the per-frame buffers (amateur rows of all pairs, then the professional ones)
+    int32_t len, pad_;
+};
+
+__device__ __forceinline__ float sqrt_rn(float a) { return __fsqrt_rn(a); }
+__device__ __forceinline__ double sqrt_rn(double a) { return __dsqrt_rn(a); }
+
+// fixed-order block sum of one double per thread
+__device__ double block_sum(double v, double *red) {
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    double s = 0.0;
+    for (int w = 0; w < kBPrepThreads / 32; ++w) s += red[w];
+    return s;
+}
+
+// one CTA per sequence: ZM / NN write the normalised f0 to feat; every method writes the squared norm of a frame's features to
+// norm (|x|^2 of cdist: sequential over k); LoNDTW also writes its context mean to mean.
+template <typename T>
+__global__ void __launch_bounds__(kBPrepThreads) baseline_prep_kernel(int method, const T *__restrict__ src, const T *__restrict__ tgt,
+                                                                      int n, int H, const BSeq *__restrict__ seqs, T *__restrict__ feat,
+                                                                      T *__restrict__ norm, T *__restrict__ mean) {
+    __shared__ double red[kBPrepThreads / 32];
+    const BSeq s = seqs[blockIdx.x];
+    const int len = s.len;
+    const T *x = ((int)blockIdx.x < n ? src : tgt) + s.in_row * H;
+    if (method == kZMNaive || method == kNNaive) {
+        // torch: mean = sum / len in the input's type (the sum accumulated in double here, then rounded once), std =
+        // sqrt(sum (x - mean)^2 / (len - 1)) accumulated in double
+        double acc = 0.0;
+        for (int t = threadIdx.x; t < len; t += kBPrepThreads) acc += (double)x[t];
+        const double sum = block_sum(acc, red);
+        const T mu = div_rn((T)sum, (T)len);
+        T den = (T)1;
+        if (method == kNNaive) {
+            const double md = sum / (double)len;
+            double q = 0.0;
+            for (int t = threadIdx.x; t < len; t += kBPrepThreads) q += ((double)x[t] - md) * ((double)x[t] - md);
+            const double m2 = block_sum(q, red);
+            den = add_rn((T)sqrt(m2 / (double)(len - 1)), (T)1e-8);
+        }
+        for (int t = threadIdx.x; t < len; t += kBPrepThreads) {
+            T f = sub_rn(x[t], mu);
+            if (method == kNNaive) f = div_rn(f, den);
+            feat[s.buf_row + t] = f;
+            norm[s.buf_row + t] = mul_rn(f, f);
+        }
+    } else if (method == kLoN) {
+        for (int t = threadIdx.x; t < len; t += kBPrepThreads) {
+            T m = (T)0;
+            for (int k = 0; k < kCtx; ++k) {
+                const int u = t - kCtxHalf + k;
+                m = add_rn(m, (u >= 0 && u < len) ? x[u] : (T)0);
+            }
+            m = div_rn(m, (T)kCtx);
+            T q = (T)0;
+            for (int k = 0; k < kCtx; ++k) {
+                const int u = t - kCtxHalf + k;
+                const T d = sub_rn((u >= 0 && u < len) ? x[u] : (T)0, m);
+                q = add_rn(q, mul_rn(d, d));
+            }
+            mean[s.buf_row + t] = m;
+            norm[s.buf_row + t] = q;
+        }
+    } else {
+        for (int t = threadIdx.x; t < len; t += kBPrepThreads) {
+            T q = (T)0;
+            for (int k = 0; k < H; ++k) q = add_rn(q, mul_rn(x[(int64_t)t * H + k], x[(int64_t)t * H + k]));
+            norm[s.buf_row + t] = q;
+        }
+    }
+}
+
+// feature k of frame t of a sequence (0 past its end or past the feature count)
+template <typename T, int MODE>
+__device__ __forceinline__ T feature(const T *x, const T *feat, const T *mean, int64_t buf_row, int len, int H, int t, int k) {
+    if (t >= len) return (T)0;
+    if (MODE == kLoN) {
+        const int u = t - kCtxHalf + k;
+        return sub_rn((u >= 0 && u < len) ? x[u] : (T)0, mean[buf_row + t]);
+    } else if (MODE == kNaive) {
+        return k < H ? x[(int64_t)t * H + k] : (T)0;
+    } else {
+        return feat[buf_row + t];
+    }
+}
+
+// grid (64 x 64 tiles of the largest pair, n_pairs): a CTA computes rows [i0, i0 + 64) (professional frames) x columns
+// [j0, j0 + 64) (amateur frames) of pair blockIdx.y.  Features are staged KC at a time in shared memory, k-major (the amateur side
+// pre-multiplied by -2 in the product form, exact); thread (ty, tx) accumulates the 4 x 4 cells (i0 + ty + 16 a, j0 + tx + 16 b) in
+// registers, so each staged value is used 4 times from a register and 16 times from shared memory.  The finished tile goes back
+// through shared memory and out anti-diagonal by anti-diagonal: one contiguous run of the skewed layout per tile diagonal.
+// rowmajor: write [C, R] (cdist's [S, T]) at cell_off instead.
+template <typename T, int MODE, int KC>
+__global__ void __launch_bounds__(kBThreads) baseline_cost_kernel(const T *__restrict__ src, const T *__restrict__ tgt, int H,
+                                                                  int64_t rows_src, const PairMeta *__restrict__ pairs,
+                                                                  const T *__restrict__ feat, const T *__restrict__ norm,
+                                                                  const T *__restrict__ mean, int rowmajor, T *__restrict__ cost) {
+    constexpr int K = MODE == kLoN ? kCtx : 1;
+    __shared__ __align__(16) unsigned char smem[kBTile * kBStage * sizeof(T)];
+    T *xs = reinterpret_cast<T *>(smem), *ys = xs + KC * (kBTile + 1);     // [KC][65]: amateur (j), professional (i)
+    T *stage = reinterpret_cast<T *>(smem);
+    const PairMeta p = pairs[blockIdx.y];
+    const int R = p.R, C = p.C, tiles_j = (C + kBTile - 1) / kBTile;
+    if ((int)blockIdx.x >= tiles_j * ((R + kBTile - 1) / kBTile)) return;
+    const int i0 = (blockIdx.x / tiles_j) * kBTile, j0 = (blockIdx.x % tiles_j) * kBTile;
+    const bool direct = R <= kDirectMaxRows && C <= kDirectMaxRows;
+    const int Kn = MODE == kNaive ? H : K;
+    const int hs = MODE == kNaive ? H : 1;
+    const T *xa = src + p.src_row * hs, *xb = tgt + (p.tgt_row - rows_src) * hs;
+    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+    T acc[4][4];
+#pragma unroll
+    for (int a = 0; a < 4; ++a)
+#pragma unroll
+        for (int b = 0; b < 4; ++b) acc[a][b] = (T)0;
+    for (int k0 = 0; k0 < Kn; k0 += KC) {
+        __syncthreads();
+        for (int q = threadIdx.x; q < 2 * KC * kBTile; q += kBThreads) {
+            const bool is_b = q >= KC * kBTile;
+            const int r = (is_b ? q - KC * kBTile : q) / KC, kk = q % KC;
+            if (is_b) {
+                ys[kk * (kBTile + 1) + r] = feature<T, MODE>(xb, feat, mean, p.tgt_row, R, H, i0 + r, k0 + kk);
+            } else {
+                const T v = feature<T, MODE>(xa, feat, mean, p.src_row, C, H, j0 + r, k0 + kk);
+                xs[kk * (kBTile + 1) + r] = direct ? v : mul_rn((T)-2, v);
+            }
+        }
+        __syncthreads();
+#pragma unroll
+        for (int kk = 0; kk < KC; ++kk) {
+            T yv[4], xv[4];
+#pragma unroll
+            for (int a = 0; a < 4; ++a) yv[a] = ys[kk * (kBTile + 1) + ty + 16 * a];
+#pragma unroll
+            for (int b = 0; b < 4; ++b) xv[b] = xs[kk * (kBTile + 1) + tx + 16 * b];
+            if (direct) {
+#pragma unroll
+                for (int a = 0; a < 4; ++a)
+#pragma unroll
+                    for (int b = 0; b < 4; ++b) {
+                        const T d = sub_rn(xv[b], yv[a]);
+                        acc[a][b] = add_rn(acc[a][b], mul_rn(d, d));
+                    }
+            } else {
+#pragma unroll
+                for (int a = 0; a < 4; ++a)
+#pragma unroll
+                    for (int b = 0; b < 4; ++b) acc[a][b] = add_rn(acc[a][b], mul_rn(xv[b], yv[a]));
+            }
+        }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int a = 0; a < 4; ++a) {
+        const int il = ty + 16 * a, i = i0 + il;
+        const T yn = i < R ? norm[p.tgt_row + i] : (T)0;
+#pragma unroll
+        for (int b = 0; b < 4; ++b) {
+            const int jl = tx + 16 * b, j = j0 + jl;
+            T v = acc[a][b];
+            if (!direct) {
+                v = add_rn(add_rn(v, j < C ? norm[p.src_row + j] : (T)0), yn);
+                v = v < (T)0 ? (T)0 : v;
+            }
+            v = sqrt_rn(v);
+            if (rowmajor) {
+                if (i < R && j < C) cost[p.cell_off + (int64_t)j * R + i] = v;
+            } else {
+                stage[il * kBStage + jl] = v;
+            }
+        }
+    }
+    if (rowmajor) return;
+    __syncthreads();
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const int ri = min(kBTile, R - i0), rj = min(kBTile, C - j0);
+    for (int dl = w; dl < ri + rj - 1; dl += kBThreads / 32) {
+        const int lo = max(0, dl - rj + 1), hi = min(dl, ri - 1);
+        const int64_t base = p.cell_off + skew_index(i0 + lo, j0 + dl - lo, R, C);
+        for (int c = lane; c <= hi - lo; c += 32) cost[base + c] = stage[(lo + c) * kBStage + dl - lo - c];
+    }
+}
+
+// NInterpo: out[i] = min(floor(float(i) * (float(S) / float(T))), S - 1) for every professional frame i of every pair
+__global__ void nearest_index_kernel(const PairMeta *__restrict__ pairs, int64_t *__restrict__ out) {
+    const PairMeta p = pairs[blockIdx.y];
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= p.R) return;
+    const float scale = __fdiv_rn((float)p.C, (float)p.R);
+    const int64_t k = (int64_t)floorf(__fmul_rn((float)i, scale));
+    out[p.out_row + i] = k < p.C - 1 ? k : p.C - 1;
+}
+
+// workspace of the baseline alignments: [pair metas | seq metas | feat | norm | mean | skewed cost | direction bytes]
+struct BLayout {
+    size_t off[7], total;
+    int64_t rows_src, rows_tgt, cells;
+    int maxR, maxdiag;
+    int64_t maxtiles;
+};
+
+int baseline_layout(int32_t method, int32_t dtype, int32_t n, const int32_t *src_len, const int32_t *tgt_len, BLayout &L) {
+    SVB_CHECK(dtype == SVB_SADTW_F32 || dtype == SVB_SADTW_F64, SVB_ERR_INVALID, "dtw_baselines: bad dtype %d", dtype);
+    SVB_CHECK(method >= SVB_LONDTW && method <= SVB_NINTERPO, SVB_ERR_INVALID, "dtw_baselines: bad method %d", method);
+    SVB_CHECK(n > 0 && n <= kMaxPairs, SVB_ERR_INVALID, "dtw_baselines: %d pairs (1 .. %d)", n, kMaxPairs);
+    SVB_CHECK(src_len && tgt_len, SVB_ERR_INVALID, "dtw_baselines: null length array");
+    const bool dtw = method != SVB_NINTERPO;
+    L.rows_src = L.rows_tgt = L.cells = L.maxtiles = 0;
+    L.maxR = L.maxdiag = 0;
+    for (int p = 0; p < n; ++p) {
+        SVB_CHECK(src_len[p] >= 2 && tgt_len[p] >= 2, SVB_ERR_INVALID,
+                  "dtw_baselines: pair %d has %d amateur and %d professional frames (at least 2 each are needed)", p, src_len[p],
+                  tgt_len[p]);
+        SVB_CHECK(!dtw || std::min(src_len[p], tgt_len[p]) <= kMaxDiag, SVB_ERR_INVALID,
+                  "dtw_baselines: pair %d: min(%d, %d) frames exceeds the %d-cell anti-diagonal of the DTW kernel", p, src_len[p],
+                  tgt_len[p], kMaxDiag);
+        L.rows_src += src_len[p], L.rows_tgt += tgt_len[p];
+        if (dtw) L.cells += (int64_t)src_len[p] * tgt_len[p];
+        L.maxR = std::max(L.maxR, (int)tgt_len[p]);
+        L.maxdiag = std::max(L.maxdiag, (int)std::min(src_len[p], tgt_len[p]));
+        L.maxtiles = std::max(L.maxtiles, (int64_t)((src_len[p] + kBTile - 1) / kBTile) * ((tgt_len[p] + kBTile - 1) / kBTile));
+    }
+    const size_t esz = dtype == SVB_SADTW_F32 ? 4 : 8, rows = dtw ? (size_t)(L.rows_src + L.rows_tgt) : 0;
+    L.off[0] = 0;
+    L.off[1] = align_up((size_t)n * sizeof(PairMeta));
+    L.off[2] = align_up(L.off[1] + (dtw ? (size_t)2 * n * sizeof(BSeq) : 0));
+    L.off[3] = align_up(L.off[2] + rows * esz);
+    L.off[4] = align_up(L.off[3] + rows * esz);
+    L.off[5] = align_up(L.off[4] + rows * esz);
+    L.off[6] = align_up(L.off[5] + (size_t)L.cells * esz);
+    L.total = align_up(L.off[6] + (size_t)L.cells);
+    return SVB_OK;
+}
+
+int baseline_check(const void *src, const void *tgt, int32_t dtype, int32_t method, int32_t n, const int32_t *src_len,
+                   const int32_t *tgt_len, int32_t feat_dim, const void *ws, int64_t ws_bytes, BLayout &L) {
+    SVB_CHECK(src && tgt && ws, SVB_ERR_INVALID, "dtw_baselines: null argument");
+    SVB_TRY(baseline_layout(method, dtype, n, src_len, tgt_len, L));
+    if (method == SVB_NAIVEDTW)
+        SVB_CHECK(feat_dim >= 1 && feat_dim <= kMaxFeat, SVB_ERR_INVALID, "dtw_baselines: feat_dim %d (1 .. %d)", feat_dim, kMaxFeat);
+    else
+        SVB_CHECK(feat_dim == 1, SVB_ERR_INVALID, "dtw_baselines: feat_dim %d (method %d aligns 1-D f0)", feat_dim, method);
+    SVB_CHECK(ws_bytes >= (int64_t)L.total, SVB_ERR_INVALID, "dtw_baselines: workspace of %lld bytes, %lld needed", (long long)ws_bytes,
+              (long long)L.total);
+    return SVB_OK;
+}
+
+template <typename T>
+int launch_baseline_cost(int method, const T *src, const T *tgt, int n, int H, const BLayout &L, char *ws, int rowmajor, T *cost,
+                         StageTimer &tm, cudaStream_t st) {
+    const BSeq *d_seqs = reinterpret_cast<const BSeq *>(ws + L.off[1]);
+    const PairMeta *d_pairs = reinterpret_cast<const PairMeta *>(ws + L.off[0]);
+    T *feat = reinterpret_cast<T *>(ws + L.off[2]), *norm = reinterpret_cast<T *>(ws + L.off[3]), *mean = reinterpret_cast<T *>(ws + L.off[4]);
+    baseline_prep_kernel<T><<<2 * n, kBPrepThreads, 0, st>>>(method, src, tgt, n, H, d_seqs, feat, norm, mean);
+    SVB_CUDA(cudaGetLastError());
+    SVB_TRY(tm.mark(1, st));
+    const dim3 grid((unsigned)L.maxtiles, n);
+    if (method == kLoN)
+        baseline_cost_kernel<T, kLoN, 16><<<grid, kBThreads, 0, st>>>(src, tgt, H, L.rows_src, d_pairs, feat, norm, mean, rowmajor, cost);
+    else if (method == kNaive && H > 1)
+        baseline_cost_kernel<T, kNaive, 16><<<grid, kBThreads, 0, st>>>(src, tgt, H, L.rows_src, d_pairs, feat, norm, mean, rowmajor,
+                                                                        cost);
+    else if (method == kNaive)
+        baseline_cost_kernel<T, kNaive, 1><<<grid, kBThreads, 0, st>>>(src, tgt, H, L.rows_src, d_pairs, feat, norm, mean, rowmajor, cost);
+    else
+        baseline_cost_kernel<T, kZMNaive, 1><<<grid, kBThreads, 0, st>>>(src, tgt, H, L.rows_src, d_pairs, feat, norm, mean, rowmajor,
+                                                                         cost);
+    SVB_CUDA(cudaGetLastError());
+    return SVB_OK;
+}
+
+// pair metas (cells at cell_off; rowmajor_cells: the [S, T] matrices of the cost-only entry are packed the same way) and seq metas
+void baseline_metas(int n, const int32_t *src_len, const int32_t *tgt_len, const BLayout &L, std::vector<PairMeta> &pairs,
+                    std::vector<BSeq> &seqs) {
+    pairs.resize(n), seqs.resize(2 * (size_t)n);
+    int64_t fs = 0, ft = 0, cells = 0;
+    for (int p = 0; p < n; ++p) {
+        const int S = src_len[p], T = tgt_len[p];
+        pairs[p] = PairMeta{fs, L.rows_src + ft, cells, ft, T, S};
+        seqs[p] = BSeq{fs, fs, S, 0};
+        seqs[n + p] = BSeq{ft, L.rows_src + ft, T, 0};
+        fs += S, ft += T, cells += (int64_t)S * T;
+    }
+}
+
+}  // namespace
+
+extern "C" int64_t svb_dtw_baselines_workspace_bytes(int32_t method, int32_t dtype, int32_t n_pairs, const int32_t *src_len_host,
+                                                     const int32_t *tgt_len_host) {
+    BLayout L;
+    if (baseline_layout(method, dtype, n_pairs, src_len_host, tgt_len_host, L) != SVB_OK) return -1;
+    return (int64_t)L.total;
+}
+
+extern "C" int svb_dtw_baselines_align(const void *src_dev, const void *tgt_dev, int32_t dtype, int32_t method, int32_t n_pairs,
+                                       const int32_t *src_len_host, const int32_t *tgt_len_host, int32_t feat_dim, void *workspace_dev,
+                                       int64_t workspace_bytes, int64_t *alignment_dev, void *path_cost_dev, float *stage_ms_host,
+                                       void *stream) {
+    SVB_CHECK(alignment_dev, SVB_ERR_INVALID, "dtw_baselines: null argument");
+    BLayout L;
+    SVB_TRY(baseline_check(src_dev, tgt_dev, dtype, method, n_pairs, src_len_host, tgt_len_host, feat_dim, workspace_dev,
+                           workspace_bytes, L));
+    const int n = n_pairs;
+    std::vector<PairMeta> pairs;
+    std::vector<BSeq> seqs;
+    baseline_metas(n, src_len_host, tgt_len_host, L, pairs, seqs);
+    // everything is validated: from here on, launches
+    cudaStream_t st = as_stream(stream);
+    char *ws = static_cast<char *>(workspace_dev);
+    PairMeta *d_pairs = reinterpret_cast<PairMeta *>(ws + L.off[0]);
+    SVB_CUDA(cudaMemcpyAsync(d_pairs, pairs.data(), pairs.size() * sizeof(PairMeta), cudaMemcpyHostToDevice, st));
+    StageTimer tm(stage_ms_host != nullptr);
+    SVB_TRY(tm.create());
+    SVB_TRY(tm.mark(0, st));
+    if (method == SVB_NINTERPO) {
+        nearest_index_kernel<<<dim3((L.maxR + 255) / 256, n), 256, 0, st>>>(d_pairs, alignment_dev);
+        SVB_CUDA(cudaGetLastError());
+        for (int k = 1; k < 5; ++k) SVB_TRY(tm.mark(k, st));
+        return tm.read(stage_ms_host);
+    }
+    SVB_CUDA(cudaMemcpyAsync(ws + L.off[1], seqs.data(), seqs.size() * sizeof(BSeq), cudaMemcpyHostToDevice, st));
+    uint8_t *d_dirs = reinterpret_cast<uint8_t *>(ws + L.off[6]);
+    if (dtype == SVB_SADTW_F32) {
+        float *cost = reinterpret_cast<float *>(ws + L.off[5]);
+        SVB_TRY(launch_baseline_cost<float>(method, static_cast<const float *>(src_dev), static_cast<const float *>(tgt_dev), n, feat_dim,
+                                            L, ws, 0, cost, tm, st));
+        SVB_TRY(tm.mark(2, st));
+        SVB_TRY(launch_dtw<float>(cost, d_pairs, PairMeta{}, n, L.maxdiag, d_dirs, static_cast<float *>(path_cost_dev), nullptr, st));
+    } else {
+        double *cost = reinterpret_cast<double *>(ws + L.off[5]);
+        SVB_TRY(launch_baseline_cost<double>(method, static_cast<const double *>(src_dev), static_cast<const double *>(tgt_dev), n,
+                                             feat_dim, L, ws, 0, cost, tm, st));
+        SVB_TRY(tm.mark(2, st));
+        SVB_TRY(launch_dtw<double>(cost, d_pairs, PairMeta{}, n, L.maxdiag, d_dirs, static_cast<double *>(path_cost_dev), nullptr, st));
+    }
+    SVB_TRY(tm.mark(3, st));
+    backtrack_kernel<<<(n + 127) / 128, 128, 0, st>>>(d_dirs, d_pairs, PairMeta{}, n, alignment_dev);
+    SVB_CUDA(cudaGetLastError());
+    SVB_TRY(tm.mark(4, st));
+    return tm.read(stage_ms_host);
+}
+
+extern "C" int svb_dtw_baselines_cost(const void *src_dev, const void *tgt_dev, int32_t dtype, int32_t method, int32_t n_pairs,
+                                      const int32_t *src_len_host, const int32_t *tgt_len_host, int32_t feat_dim, void *workspace_dev,
+                                      int64_t workspace_bytes, void *cost_dev, void *stream) {
+    SVB_CHECK(cost_dev, SVB_ERR_INVALID, "dtw_baselines_cost: null argument");
+    SVB_CHECK(method != SVB_NINTERPO, SVB_ERR_INVALID, "dtw_baselines_cost: NInterpo has no cost matrix");
+    BLayout L;
+    SVB_TRY(baseline_check(src_dev, tgt_dev, dtype, method, n_pairs, src_len_host, tgt_len_host, feat_dim, workspace_dev,
+                           workspace_bytes, L));
+    const int n = n_pairs;
+    std::vector<PairMeta> pairs;
+    std::vector<BSeq> seqs;
+    baseline_metas(n, src_len_host, tgt_len_host, L, pairs, seqs);
+    cudaStream_t st = as_stream(stream);
+    char *ws = static_cast<char *>(workspace_dev);
+    StageTimer off(false);
+    SVB_CUDA(cudaMemcpyAsync(ws + L.off[0], pairs.data(), pairs.size() * sizeof(PairMeta), cudaMemcpyHostToDevice, st));
+    SVB_CUDA(cudaMemcpyAsync(ws + L.off[1], seqs.data(), seqs.size() * sizeof(BSeq), cudaMemcpyHostToDevice, st));
+    if (dtype == SVB_SADTW_F32)
+        return launch_baseline_cost<float>(method, static_cast<const float *>(src_dev), static_cast<const float *>(tgt_dev), n, feat_dim, L,
+                                           ws, 1, static_cast<float *>(cost_dev), off, st);
+    return launch_baseline_cost<double>(method, static_cast<const double *>(src_dev), static_cast<const double *>(tgt_dev), n, feat_dim,
+                                        L, ws, 1, static_cast<double *>(cost_dev), off, st);
+}

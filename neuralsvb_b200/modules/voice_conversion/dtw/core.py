@@ -1,5 +1,6 @@
-"""Shape-aware DTW on the GPU (csrc/sadtw.cu): the batched entry points behind the drop-in ``align``, ``shape_aware_dtw`` and
-``enhance_sadtw`` modules, plus ``align_pitch`` for a binarizer and ``a2p_alignment_batch`` for ``MleSVBVAE``'s ``a2p`` way.
+"""Pitch alignment on the GPU (csrc/sadtw.cu): the batched entry points behind the drop-in ``align``, ``shape_aware_dtw``,
+``enhance_sadtw``, ``local_norm_dtw``, ``naive_dtw`` and ``naive_interpo`` modules, plus ``align_pitch`` for a binarizer,
+``a2p_alignment_batch`` for ``MleSVBVAE``'s ``a2p`` way and ``alignment_accuracy`` for the paper's comparison of the six methods.
 
 f0 contours may be numpy arrays or torch tensors, on the host or on a CUDA device, shaped [S] or [S, 1], float32 or float64; the
 arithmetic runs in that type, like the reference's.  Host inputs are copied to the current CUDA device.  There is no CPU path.
@@ -12,6 +13,8 @@ import torch
 from neuralsvb_b200 import _native
 
 VARIANTS = {'SADTW': 0, 'EHSADTW': 1}
+BASELINES = {'LoNDTW': 0, 'NaiveDTW': 1, 'ZMNaiveDTW': 2, 'NNaiveDTW': 3, 'NInterpo': 4}
+METHODS = tuple(VARIANTS) + tuple(BASELINES)
 DTYPES = {torch.float32: 0, torch.float64: 1}
 BINS = 48
 
@@ -96,9 +99,12 @@ class AlignResult:
 
 def align_batch(srcs, tgts, method='EHSADTW', scales=None, stage_ms=False, keep_workspace=False):
     """Shape-aware DTW of n pairs in one launch sequence: srcs = amateur contours (S_p frames), tgts = professional ones (T_p
-    frames); scales: the professional histogram's scale factor per pair (default T_p / S_p, cal_shape_dist's)."""
+    frames); scales: the professional histogram's scale factor per pair (default T_p / S_p, cal_shape_dist's).  The baseline
+    methods (BASELINES) go to baseline_batch."""
+    if method in BASELINES:
+        return baseline_batch(srcs, tgts, method, stage_ms)
     if method not in VARIANTS:
-        raise ValueError(f'method must be one of {sorted(VARIANTS)}, got {method!r}')
+        raise ValueError(f'method must be one of {sorted(METHODS)}, got {method!r}')
     if len(srcs) != len(tgts) or len(srcs) == 0:
         raise ValueError(f'{len(srcs)} amateur and {len(tgts)} professional contours')
     device = device_of(*srcs, *tgts)
@@ -249,3 +255,123 @@ def a2p_alignment_batch(amateur_f0, prof_f0, amateur_len, prof_len, method='EHSA
     out = torch.zeros(B, Tp, dtype=torch.int64, device=device)
     out[torch.arange(Tp, device=device)[None, :] < lp_t[:, None]] = torch.minimum(r.alignment, cap)
     return out
+
+
+# ---- baseline alignments (LoNDTW, NaiveDTW, ZMNaiveDTW, NNaiveDTW, NInterpo) ---------------------------------------------------
+
+def _baseline_inputs(xs, what, method):
+    """Host-side checks of one side of a batch, before any device is looked for: 1-D f0 ([S] or [S, 1]) for every method but
+    NaiveDTW, which takes [S, H] features ([S] is [S, 1]); float32 or float64, one type, at least 2 frames."""
+    ts = []
+    for x in xs:
+        t = as_tensor(x)
+        if method == 'NaiveDTW':
+            t = t[:, None] if t.dim() == 1 else t
+            if t.dim() != 2:
+                raise ValueError(f'NaiveDTW features must be [S, H], got {tuple(t.shape)}')
+        else:
+            t = t[:, 0] if t.dim() == 2 and t.shape[1] == 1 else t
+            if t.dim() != 1:
+                raise ValueError(f'an f0 contour must be [S] or [S, 1], got {tuple(t.shape)}')
+        if t.dtype not in DTYPES:
+            raise TypeError(f'{what} input must be float32 or float64, got {t.dtype}')
+        ts.append(t)
+    if len({t.dtype for t in ts}) > 1:
+        raise TypeError(f'{what} inputs mix float32 and float64; a batch runs in one type')
+    if len({tuple(t.shape[1:]) for t in ts}) > 1:
+        raise ValueError(f'{what} features of different widths in one batch')
+    if min(t.shape[0] for t in ts) < 2:
+        raise ValueError(f'{what} sequence of {min(t.shape[0] for t in ts)} frames: at least 2 are needed')
+    return ts
+
+
+def _baseline_prepare(srcs, tgts, method):
+    if method not in BASELINES:
+        raise ValueError(f'method must be one of {sorted(BASELINES)}, got {method!r}')
+    if len(srcs) != len(tgts) or len(srcs) == 0:
+        raise ValueError(f'{len(srcs)} amateur and {len(tgts)} professional sequences')
+    a = _baseline_inputs(srcs, 'amateur', method)
+    b = _baseline_inputs(tgts, 'professional', method)
+    if a[0].dtype != b[0].dtype:
+        raise TypeError('amateur and professional inputs must have the same type')
+    if a[0].shape[1:] != b[0].shape[1:]:
+        raise ValueError(f'amateur features {tuple(a[0].shape[1:])} but professional ones {tuple(b[0].shape[1:])}')
+    device = device_of(*srcs, *tgts)
+    src = torch.cat([t.to(device) for t in a]).contiguous()
+    tgt = torch.cat([t.to(device) for t in b]).contiguous()
+    if method != 'NInterpo':
+        _check_finite(src)
+        _check_finite(tgt)
+    S, T = [int(t.shape[0]) for t in a], [int(t.shape[0]) for t in b]
+    H = int(a[0].shape[1]) if method == 'NaiveDTW' else 1
+    return src, tgt, S, T, H, device
+
+
+def baseline_batch(srcs, tgts, method, stage_ms=False):
+    """A baseline alignment of n pairs in one launch sequence: the method's cost kernel writes the skewed cost, then the DTW and
+    backtrack kernels of the shape-aware path run unchanged (NInterpo: the nearest-neighbour index map alone).  path_cost is in
+    the input's type (None for NInterpo); stage_ms: (features, cost, dtw, backtrack) CUDA-event times."""
+    src, tgt, S, T, H, device = _baseline_prepare(srcs, tgts, method)
+    n, lib, dt = len(S), _native.lib(), src.dtype
+    s_arr, s_p = _i32(S)
+    t_arr, t_p = _i32(T)
+    ws_bytes = _check(lib.svb_dtw_baselines_workspace_bytes(BASELINES[method], DTYPES[dt], n, s_p, t_p), 'dtw_baselines_workspace_bytes')
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
+    out = torch.empty(int(t_arr.sum()), dtype=torch.int64, device=device)
+    pc = torch.empty(n, dtype=dt, device=device) if method != 'NInterpo' else None
+    ms = (ctypes.c_float * 4)() if stage_ms else None
+    with torch.cuda.device(device):
+        _check(lib.svb_dtw_baselines_align(_vp(src), _vp(tgt), DTYPES[dt], BASELINES[method], n, s_p, t_p, H, _vp(ws), ws_bytes,
+                                           _vp(out), _vp(pc), ms, _native.current_stream_ptr(device)), 'dtw_baselines_align')
+    return AlignResult(alignment=out, offsets=np.concatenate([[0], np.cumsum(T)]).astype(np.int64), path_cost=pc,
+                       stage_ms=tuple(ms) if stage_ms else None, src_len=S, tgt_len=T, workspace=None, sections=None)
+
+
+def baseline_costs(srcs, tgts, method):
+    """The cost kernel alone: per pair the cdist matrix [S_p, T_p] in the input's type, device tensors (views of one buffer)."""
+    if method == 'NInterpo':
+        raise ValueError('NInterpo has no cost matrix')
+    src, tgt, S, T, H, device = _baseline_prepare(srcs, tgts, method)
+    n, lib, dt = len(S), _native.lib(), src.dtype
+    s_arr, s_p = _i32(S)
+    t_arr, t_p = _i32(T)
+    ws_bytes = _check(lib.svb_dtw_baselines_workspace_bytes(BASELINES[method], DTYPES[dt], n, s_p, t_p), 'dtw_baselines_workspace_bytes')
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
+    cells = [s * t for s, t in zip(S, T)]
+    out = torch.empty(sum(cells), dtype=dt, device=device)
+    with torch.cuda.device(device):
+        _check(lib.svb_dtw_baselines_cost(_vp(src), _vp(tgt), DTYPES[dt], BASELINES[method], n, s_p, t_p, H, _vp(ws), ws_bytes,
+                                          _vp(out), _native.current_stream_ptr(device)), 'dtw_baselines_cost')
+    return [c.view(s, t) for c, s, t in zip(torch.split(out, cells), S, T)]
+
+
+def alignment_accuracy(alignments, amateur_mel2ph, prof_mel2ph):
+    """The paper's alignment accuracy per pair, job()'s (prof_mel2ph == amateur_mel2ph[alignment]).sum() / (prof_mel2ph != 0).sum(),
+    for n pairs at once on the device: alignments (an AlignResult, or n int sequences of the professional lengths), the amateur
+    and professional mel2ph tracks (n each).  Returns a float64 numpy array [n]."""
+    if isinstance(alignments, AlignResult):
+        alignments = [alignments.alignment[alignments.offsets[p]:alignments.offsets[p + 1]] for p in range(len(alignments.offsets) - 1)]
+    n = len(alignments)
+    if n == 0 or len(amateur_mel2ph) != n or len(prof_mel2ph) != n:
+        raise ValueError(f'{n} alignments, {len(amateur_mel2ph)} amateur and {len(prof_mel2ph)} professional mel2ph tracks')
+    al = [as_tensor(a).reshape(-1) for a in alignments]
+    am = [as_tensor(m).reshape(-1) for m in amateur_mel2ph]
+    pm = [as_tensor(m).reshape(-1) for m in prof_mel2ph]
+    for p in range(n):
+        if al[p].shape[0] != pm[p].shape[0]:
+            raise ValueError(f'pair {p}: an alignment of {al[p].shape[0]} frames for {pm[p].shape[0]} professional frames')
+        if al[p].dtype.is_floating_point or al[p].dtype == torch.bool:
+            raise TypeError(f'pair {p}: alignment indices must be integers, got {al[p].dtype}')
+    device = device_of(*alignments, *amateur_mel2ph, *prof_mel2ph)
+    S = torch.tensor([m.shape[0] for m in am], device=device)
+    T = torch.tensor([m.shape[0] for m in pm], device=device)
+    pair = torch.repeat_interleave(torch.arange(n, device=device), T)
+    idx = torch.cat([a.to(device, torch.int64) for a in al])
+    if bool(((idx < 0) | (idx >= S[pair])).any()):
+        raise ValueError('an alignment index is outside its amateur track')
+    first = torch.cumsum(S, 0) - S
+    ama = torch.cat([m.to(device) for m in am])[idx + first[pair]]
+    prof = torch.cat([m.to(device) for m in pm])
+    hit = torch.zeros(n, dtype=torch.float64, device=device).index_add_(0, pair, (prof == ama).double())
+    voiced = torch.zeros(n, dtype=torch.float64, device=device).index_add_(0, pair, (prof != 0).double())
+    return (hit / voiced).cpu().numpy()

@@ -533,3 +533,19 @@ def make_f0_pair(seed, S, T, fps=172.27):
     prof = take(T, 0.05, 5.5, 0.35, 0.0, 0.0)
     ama = take(S, 0.35, 4.5, 0.15, rs.uniform(-0.5, 0.5), rs.uniform(-0.4, 0.4))
     return ama, prof
+
+
+def make_mel2ph_pair(seed, S, T):
+    """(amateur [S], professional [T]) int64 mel2ph tracks for scoring a pitch alignment: the same phoneme sequence (ids 1 ..
+    n_ph) sung with different durations, monotone runs, and a few trailing frames of zero padding per take."""
+    rs = np.random.RandomState(seed + 67)
+    n_ph = max(1, min(S, T) // 12)
+
+    def take(n):
+        pad = rs.randint(0, max(1, n // 10) + 1) if n > n_ph + 1 else 0
+        w = rs.dirichlet(np.full(n_ph, 3.0))
+        edges = np.floor(np.concatenate([[0], np.cumsum(w)]) * (n - pad)).astype(np.int64)
+        m = np.zeros(n, np.int64)
+        m[:n - pad] = np.searchsorted(edges[1:-1], np.arange(n - pad), side='right') + 1
+        return m
+    return take(S), take(T)
