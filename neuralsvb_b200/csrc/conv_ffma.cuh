@@ -30,6 +30,8 @@ struct ConvArgs {
     int accumulate;
     int cin_blk = 0;      // grouped convolution (tensor-core kernel only): input channels read by ONE column block
                           // (block nblk reads channels [nblk*cin_blk, (nblk+1)*cin_blk)); 0 = dense (all Cin)
+    int epi_stream = 1;   // tensor-core kernel: residual / running sum bulk-copied into shared memory during the MMAs where
+                          // the plan has room (conv_tc.cu); 0 = per-thread loads in the epilogue
 };
 
 int launch_conv_ffma(const ConvArgs &a, cudaStream_t st);

@@ -74,6 +74,9 @@ struct TcArgs {
     uint32_t op_bytes;          // operand slot: Rp rows x 128 B (x2 with the 3xTF32 lo plane), sized for the largest halo
     uint32_t wtile_bytes;       // one (column block, chunk, tap) weight tile (x2 with the 3xTF32 lo plane)
     uint32_t off_op, off_w, off_bias;   // byte offsets of operand slots / weight ring / bias in dynamic smem
+    int epi_slots;              // streamed epilogue: residual / running-sum pieces in flight per math warp (0: per-thread loads)
+    int l2_prefetch;            // per-thread loads: the producer prefetches each item's residual / running-sum rows into L2
+    uint32_t off_epi;           // byte offset of the piece ring [kMathWarps][epi_slots][kEpiPieceBytes]
 };
 
 constexpr int kMaxW = 8;
@@ -89,6 +92,12 @@ constexpr int kTrRows = kTransformWarps * 32 / 8;   // rows one pass of the tran
 constexpr int kBiasBytes = 4096;        // bias of the layer(s) (<= 1024 floats; wider layers take 12 KB)
 
 static_assert(512 + 2 * kTcMaxLayers * sizeof(TcLayer) <= 1024, "the layer table lives in smem bytes 512 .. 1023");
+// Streamed epilogue: one piece = the 16 rows x 32 channels one warp's accumulator fragment covers in one G32T channel
+// group, a contiguous 2 KB span of the residual or of the running sum.
+constexpr int kEpiMaxSlots = 4;
+constexpr uint32_t kEpiPieceBytes = 16 * 128;
+static_assert(256 + kMathWarps * kEpiMaxSlots * 8 <= 512, "the piece barriers live in smem bytes 256 .. 511");
+static_assert(kMaxItems * 16 + kMathWarps * 4 <= kItemBytes, "the math warps' slot parities follow the item table");
 
 // Slab of a fused item (output rows [t0, t0 + P) of a clip): c1 runs over the 256 rows from t0 - h2, so its slab starts
 // at padded row kPad + t0 - h2 - h1.  The copy stops at the clip's last padded row (in_Tp): a bulk copy never reads the
@@ -135,6 +144,22 @@ __device__ __forceinline__ void conv_tap_mma(float *d, uint32_t a_row, uint32_t 
     }
 }
 
+// v[j] of four registers by a per-lane index, as predicated selects: written as C++, the compiler turns the choice into an
+// indexed load from a local-memory copy of the accumulators
+__device__ __forceinline__ float pick4(int j, float v0, float v1, float v2, float v3) {
+    float r;
+    asm("{\n\t.reg .pred p, q;\n\t"
+        "setp.ne.s32 p, %1, 0;\n\t"
+        "setp.ne.s32 q, %1, 2;\n\t"
+        "selp.f32 %0, %3, %2, p;\n\t"       // j != 0: v1 for now
+        "selp.f32 %0, %0, %4, q;\n\t"       // j == 2: v2
+        "setp.eq.s32 p, %1, 3;\n\t"
+        "selp.f32 %0, %5, %0, p;\n\t}"      // j == 3: v3
+        : "=f"(r)
+        : "r"(j), "f"(v0), "f"(v1), "f"(v2), "f"(v3));
+    return r;
+}
+
 // Persistent kernel: one CTA per SM walks its work items (one or two 128-row tiles of one clip for one column block
 // of one layer).  Every stage is decoupled by mbarriers, so the TMA producer runs ahead into the next items and the
 // transform warps prepare operands while the warpgroups multiply the previous chunk.
@@ -157,6 +182,7 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
     uint64_t *raw_full = bars, *a_ready = bars + 4, *a_empty = bars + 8;      // up to 4 operand slots
     uint64_t *w_full = bars + 12, *w_empty = bars + 12 + kMaxW;
     int *n_items_s = reinterpret_cast<int *>(w_empty + kMaxW);
+    uint64_t *epi_full = bars + 32;                                           // [kMathWarps][kEpiMaxSlots] piece arrivals
     TcLayer *Ls = reinterpret_cast<TcLayer *>(smem + 512);                    // per-layer table (dynamic indexing)
     const int4 *items = reinterpret_cast<const int4 *>(smem + 1024);         // [kMaxItems]
     unsigned char *op0 = smem + p.off_op;                            // [nA][op_bytes]: TMA target AND MMA operand
@@ -168,6 +194,8 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
         // a_ready: one arrival per transform warp; a_empty / w_empty: one per math warp
         for (int i = 0; i < 4; ++i) mbar_init(raw_full + i, 1), mbar_init(a_ready + i, kTransformWarps), mbar_init(a_empty + i, kMathWarps);
         for (int i = 0; i < kMaxW; ++i) mbar_init(w_full + i, 1), mbar_init(w_empty + i, kMathWarps);
+        for (int i = 0; i < kMathWarps * kEpiMaxSlots; ++i) mbar_init(epi_full + i, 1);
+        for (int i = 0; i < kMathWarps; ++i) reinterpret_cast<uint32_t *>(smem + 1024 + kMaxItems * 16)[i] = 0;   // slot parities
         fence_barrier_init();
     }
     {   // constant data (not produced by the previous kernel): staged once, before the PDL wait
@@ -243,6 +271,18 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
                             w_k += p.wtile_bytes;
                             if (++sW == p.nW) sW = 0, phW ^= 1;
                         }
+                    }
+                }
+                if (p.l2_prefetch) {
+                    // the rows this item's epilogue reads with per-thread loads, issued behind its last slab: they reach L2
+                    // while the item's MMAs run, so those loads wait for L2 instead of HBM
+                    const TcLayer &Lo = Ls[FUSED ? p.n_layers + it.layer : it.layer];
+                    const int rows = min(FUSED ? p.fused_P : it.mt * kTcM, a.Tq - it.t0);
+                    const int gout = c4t_groups(a.Cout);
+                    for (int g = 0; g < N / 32 && rows > 0; ++g) {
+                        const size_t off = (((size_t)it.b * gout + it.nblk * (N / 32) + g) * a.out_Tp + kPad + it.t0) * 32;
+                        if (Lo.res) bulk_prefetch_l2(Lo.res + off, (uint32_t)rows * 128);
+                        if (Lo.accumulate) bulk_prefetch_l2(Lo.out + off, (uint32_t)rows * 128);
                     }
                 }
                 if (FUSED) {                                                      // then c2's tiles, (chunk, tap) in order
@@ -406,6 +446,111 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
                 }
             }
         };
+        // ---- streamed epilogue (p.epi_slots > 0; layers with a residual or a running sum, never an upsampler): the loads
+        // above depend on each other through the stores (out may alias res), so every one of them waits a full memory
+        // latency.  Instead, lane 0 bulk-copies this warp's pieces into its own ring of epi_slots 2 KB slots as soon as the
+        // item starts, the MMAs hide the copies, and a slot takes the piece epi_slots further on once it has been read.
+        // Pieces of an item in consumption order: block, 32-channel group, then the residual before the running sum.
+        // Only N <= 64 compiles it (tc_epi_pieces); nothing of it stays in registers across the MMAs (the slot parities
+        // live in smem).
+        constexpr bool EPI = N <= 64;
+        auto epi_bar = [&](int slot) { return epi_full + (warp - kWarpMath0) * kEpiMaxSlots + slot; };
+        auto epi_buf = [&](int slot) {
+            return smem + p.off_epi + ((uint32_t)(warp - kWarpMath0) * p.epi_slots + slot) * kEpiPieceBytes;
+        };
+        uint32_t *epi_ph_s = reinterpret_cast<uint32_t *>(smem + 1024 + kMaxItems * 16) + (warp - kWarpMath0);
+        auto piece_rows = [&](const TcItem &it, int blk) {                 // rows of this warp's piece that are written
+            const int i0 = kTcM * blk + 64 * wg + 16 * (warp & 3);
+            int rows = min(16, a.Tq - (it.t0 + i0));
+            if (FUSED) rows = min(rows, p.fused_P - i0);
+            return rows;
+        };
+        auto epi_pieces = [&](const TcItem &it, const TcLayer &L) {
+            int nb = 0;
+            for (int blk = 0; blk < it.mt; ++blk) nb += piece_rows(it, blk) > 0;
+            return nb * (N / 32) * ((L.res != nullptr) + L.accumulate);
+        };
+        auto epi_issue = [&](const TcItem &it, const TcLayer &L, int k, int slot) {      // lane 0
+            const int nsrc = (L.res != nullptr) + L.accumulate, per_blk = (N / 32) * nsrc;
+            const int blk = k / per_blk, r = k - blk * per_blk, g = r / nsrc;
+            const bool old = L.res == nullptr || r - g * nsrc == 1;
+            const uint32_t bytes = (uint32_t)piece_rows(it, blk) * 128;
+            const float *src = (old ? L.out : L.res) + (((size_t)it.b * gout + it.nblk * (N / 32) + g) * a.out_Tp + kPad + it.t0 +
+                                                        kTcM * blk + 64 * wg + 16 * (warp & 3)) * 32;
+            mbar_expect_tx(epi_bar(slot), bytes);
+            bulk_g2s(epi_buf(slot), src, bytes, epi_bar(slot));
+        };
+        auto epi_begin = [&](const TcItem &it, const TcLayer &L) {
+            // the running sum was stored by this warp's previous item (chain-ordered lists): make those generic-proxy
+            // stores visible to the bulk copies; the previous item's reads of the slots are also done (__syncwarp)
+            if (L.accumulate) fence_proxy_async_global();
+            __syncwarp();
+            if (lane == 0) {
+                fence_proxy_async();
+                const int n = min(epi_pieces(it, L), p.epi_slots);
+                for (int k = 0; k < n; ++k) epi_issue(it, L, k, k);
+            }
+        };
+        // same expression, same order and no contraction as `epilogue`: ((acc + b) + res) * out_scale (+ old)
+        auto epilogue_stream = [&](const TcItem &it, const TcLayer &L, const float *acc, int blk, int n_pieces, int &k, int &slot,
+                                   uint32_t &epi_ph) {
+            const int rows = piece_rows(it, blk);
+            if (rows <= 0) return;
+            const bool has_res = L.res != nullptr, accumulate = L.accumulate != 0;
+            const float out_scale = L.out_scale;
+            const float *bias_s = reinterpret_cast<const float *>(smem + p.off_bias) + L.bias_off;
+            const int rq = lane >> 2;
+#pragma unroll
+            for (int g = 0; g < N / 32; ++g) {
+                int s_res = 0, s_old = 0;
+                auto take = [&]() {
+                    const int s = slot;
+                    mbar_wait(epi_bar(s), (epi_ph >> s) & 1u);
+                    epi_ph ^= 1u << s;
+                    if (++slot == p.epi_slots) slot = 0;
+                    return s;
+                };
+                if (has_res) s_res = take();
+                if (accumulate) s_old = take();
+                const float *rs = reinterpret_cast<const float *>(epi_buf(s_res));
+                const float *os = reinterpret_cast<const float *>(epi_buf(s_old));
+                const int cg = it.nblk * N + 32 * g;                        // first column of the channel group
+                float *out_g = L.out + (((size_t)it.b * gout + (cg >> 5)) * a.out_Tp + kPad + it.t0 + kTcM * blk + 64 * wg +
+                                        16 * (warp & 3)) * 32;
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int r = rq + 8 * h;
+                    if (r >= rows) continue;
+#pragma unroll
+                    for (int u = 0; u < 4; ++u) {
+                        // the 8-column block rotates with the row: the 8 rows of one access cover all 32 banks
+                        const int jj = (u + rq) & 3, c = 8 * jj + c_lo, co = cg + c;
+                        const float *ap = acc + 16 * g + 2 * h;
+                        const float x0 = pick4(jj, ap[0], ap[4], ap[8], ap[12]), x1 = pick4(jj, ap[1], ap[5], ap[9], ap[13]);
+                        const float b0 = co < a.Cout ? bias_s[co] : 0.f, b1 = co + 1 < a.Cout ? bias_s[co + 1] : 0.f;
+                        float2 o = make_float2(__fadd_rn(x0, b0), __fadd_rn(x1, b1));
+                        if (has_res) {
+                            const float2 rv = *reinterpret_cast<const float2 *>(rs + r * 32 + c);
+                            o.x = __fadd_rn(o.x, rv.x), o.y = __fadd_rn(o.y, rv.y);
+                        }
+                        o.x = __fmul_rn(o.x, out_scale), o.y = __fmul_rn(o.y, out_scale);
+                        if (accumulate) {
+                            const float2 old = *reinterpret_cast<const float2 *>(os + r * 32 + c);
+                            o.x = __fadd_rn(o.x, old.x), o.y = __fadd_rn(o.y, old.y);
+                        }
+                        *reinterpret_cast<float2 *>(out_g + r * 32 + c) = o;
+                    }
+                }
+                __syncwarp();                                               // every lane has read the group's slots
+                if (lane == 0) {
+                    fence_proxy_async();
+                    const int nsrc = (int)has_res + (int)accumulate;
+                    for (int t = 0; t < nsrc; ++t)
+                        if (k + t + p.epi_slots < n_pieces) epi_issue(it, L, k + t + p.epi_slots, t == 0 && has_res ? s_res : s_old);
+                }
+                k += (int)has_res + (int)accumulate;
+            }
+        };
         // one item of one (TWO = false) or two (TWO = true) tiles; per output element the MMAs accumulate in the same
         // order either way (chunk, tap, then the split terms)
         auto run_mma_slab = [&](auto two, const TcLayer &L) {
@@ -443,11 +588,26 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
             if (TWO) wgmma_keep<N>(acc1);
             release();
         };
+        // the epilogue of the output layer L of an item, from both accumulator blocks; epi_begin(it, L) ran before the MMAs
+        auto epilogue_item = [&](auto two, const TcItem &it, const TcLayer &L) {
+            if (EPI && p.epi_slots > 0 && (L.res != nullptr || L.accumulate)) {
+                const int n_pieces = epi_pieces(it, L);
+                int k = 0, slot = 0;
+                uint32_t ph = *epi_ph_s;                                    // parity bit per slot
+                epilogue_stream(it, L, acc0, 0, n_pieces, k, slot, ph);
+                if (decltype(two)::value) epilogue_stream(it, L, acc1, 1, n_pieces, k, slot, ph);
+                __syncwarp();
+                if (lane == 0) *epi_ph_s = ph;
+            } else {
+                epilogue(it, L, acc0, 0);
+                if (decltype(two)::value) epilogue(it, L, acc1, kTcM);
+            }
+        };
         auto run_item = [&](auto two, const TcItem &it) {
             const TcLayer &L = Ls[it.layer];
+            if (EPI && p.epi_slots > 0 && (L.res != nullptr || L.accumulate)) epi_begin(it, L);
             run_mma_slab(two, L);
-            epilogue(it, L, acc0, 0);
-            if (decltype(two)::value) epilogue(it, L, acc1, kTcM);
+            epilogue_item(two, it, L);
         };
         // ---- fused items: c1's epilogue stores c2's operand for the item's rows 0 .. 255 (time tq0 + row) into the
         // intermediate, in the layout the transform warps give a slab (hi / lo split or tf32 rounding, SWIZZLE_128B)
@@ -485,6 +645,7 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
         auto run_fused = [&](const TcItem &it) {
             const TcLayer &L1 = Ls[it.layer], &L2 = Ls[p.n_layers + it.layer];
             const int h2 = (L2.KS - 1) / 2;
+            if (EPI && p.epi_slots > 0 && (L2.res != nullptr || L2.accumulate)) epi_begin(it, L2);
             run_mma_slab(std::true_type(), L1);
             // the other warpgroup's c2 wgmmas of the previous item have retired: the intermediate may be overwritten
             named_bar_sync(1, kMathWarps * 32);
@@ -516,8 +677,7 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
             wgmma_keep<N>(acc0);
             wgmma_keep<N>(acc1);
             release();
-            epilogue(it, L2, acc0, 0);
-            epilogue(it, L2, acc1, kTcM);
+            epilogue_item(std::true_type(), it, L2);
         };
         if (p.w_resident && n_items > 0) mbar_wait(w_full, 0);
         for (int n = 0; n < n_items; ++n) {
@@ -699,6 +859,46 @@ static int sm_count() {
     return n[slot];
 }
 
+// Streamed epilogue (kernel: epilogue_stream): whether the layers a[0..n) take it, and how many 2 KB pieces one math
+// warp's item needs at most.  Upsamplers interleave phases in their output rows, so their pieces are not contiguous.
+// How many sources (residual, running sum) the epilogue of the layers a[0..n) reads: 0 when none does, when SVB_EPI=0
+// asked for per-thread loads, or for upsamplers, whose output rows interleave phases and so are not contiguous.
+static int tc_epi_sources(int n, const ConvArgs *a) {
+    int nsrc = 0;
+    for (int l = 0; l < n; ++l) {
+        if (!a[l].epi_stream || a[l].ups_u != 0) return 0;
+        if ((reinterpret_cast<uintptr_t>(a[l].out) | reinterpret_cast<uintptr_t>(a[l].res)) & 15) return 0;   // bulk copies
+        nsrc = std::max(nsrc, (a[l].res != nullptr) + (a[l].accumulate != 0));
+    }
+    return nsrc;
+}
+
+// Streamed epilogue (kernel: epilogue_stream): the 2 KB pieces one math warp's item needs at most, 0 where the layers do
+// not take it.  N > 64 does not: with two blocks of N / 2 accumulators per thread it spills at the 168-register
+// ceiling, and on an H100 (700 W) the C = 256 / 128 residual launches ran 20 % slower with it.  Those launches have the
+// producer prefetch the item's residual / running-sum rows into L2 instead (TcArgs::l2_prefetch).
+static int tc_epi_pieces(int n, const ConvArgs *a, int MT, int n_tile) {
+    return n_tile > 64 ? 0 : MT * (n_tile / 32) * tc_epi_sources(n, a);
+}
+
+// The piece ring comes out of the weight ring's share of `avail` bytes: the most slots per math warp (at most one per
+// piece of an item, at least the `min_slots` pieces one channel group reads together) that leave the weight ring
+// min(nW, 4) tiles.  Returns the slots (0: none fit) and the new *nW.  SVB_TC_EPI_SLOTS caps the slots (measurement).
+static int tc_epi_fit(size_t avail, uint32_t wtile_bytes, int pieces, int min_slots, int *nW) {
+    int cap = kEpiMaxSlots;
+    if (const char *e = getenv("SVB_TC_EPI_SLOTS")) cap = std::max(0, std::min(kEpiMaxSlots, atoi(e)));
+    for (int s = std::min(cap, pieces); s >= min_slots; --s) {
+        const size_t ring = (size_t)s * kMathWarps * kEpiPieceBytes;
+        if (ring >= avail) continue;
+        const int nw = std::min((int)((avail - ring) / wtile_bytes), kMaxW);
+        if (nw >= std::min(*nW, 4)) {
+            *nW = nw;
+            return s;
+        }
+    }
+    return 0;
+}
+
 // Shape-class plan of one launch: tiles per item, operand slots, weight ring / residency and the shared-memory carve-up.
 // `a[0..n)` are layers of the same shape class (channels, rows, upsampling) that may differ in taps / dilation / pointers;
 // slots are sized for the largest halo.  `grid` > 0: the launch runs the implicit round-robin list on that many CTAs;
@@ -776,7 +976,23 @@ static int tc_plan(int n, const TcWeights *const *w, const ConvArgs *a, int prec
         two = 2 * ((g2 + grid - 1) / grid) <= (g1 + grid - 1) / grid;
     }
     if (!two) SVB_CHECK(fit(1), SVB_ERR_INVALID, "tc conv: tile does not fit shared memory (N %d)", p.n_tile);
+    // the piece ring of the streamed epilogue goes between the weights and the bias; it never changes MT or nA
+    p.epi_slots = 0, p.off_epi = 0;
+    if (const int pieces = tc_epi_pieces(n, a, p.MT, p.n_tile)) {
+        const size_t fixed = p.w_resident ? (size_t)round_up((int)res_bytes, 1024) : 0;   // resident tiles: nothing to shrink
+        int nW = p.w_resident ? 0 : p.nW;
+        const size_t avail = budget - p.off_w;
+        const int s = avail > fixed ? tc_epi_fit(avail - fixed, p.w_resident ? 1u : p.wtile_bytes, pieces, pieces / (p.MT * (p.n_tile / 32)), &nW) : 0;
+        if (s > 0) {
+            if (!p.w_resident) p.nW = nW;
+            p.epi_slots = s;
+            p.off_epi = p.off_w + (uint32_t)round_up((int)(p.w_resident ? fixed : (size_t)p.nW * p.wtile_bytes), 1024);
+            p.off_bias = p.off_epi + (uint32_t)s * kMathWarps * kEpiPieceBytes;
+            smem = (size_t)p.off_bias + bias_bytes;
+        }
+    }
     SVB_CHECK(smem <= 227 * 1024, SVB_ERR_INVALID, "tc conv: no tiling fits (N %d, %d layers)", p.n_tile, n);
+    p.l2_prefetch = p.epi_slots == 0 && tc_epi_sources(n, a) > 0;
     uint32_t res_off = 0;
     for (int l = 0; l < n; ++l) {
         TcLayer &L = p.L[l];
@@ -789,8 +1005,8 @@ static int tc_plan(int n, const TcWeights *const *w, const ConvArgs *a, int prec
     for (int l = n; l < 2 * kTcMaxLayers; ++l) p.L[l] = p.L[0];
     p.fused_P = 0, p.off_inter = 0, p.inter_bytes = 0;
     if (getenv("SVB_TC_VERBOSE"))
-        fprintf(stderr, "[tc] %d layer(s) Cin %d CoutP %d KS %d.. halo %d Tq %d | n_tile %d MT %d nA %d nW %d resident %d smem %zu\n", n,
-                a0.Cin, a0.CoutP, a0.KS, halo, a0.Tq, p.n_tile, p.MT, p.nA, p.nW, p.w_resident, smem);
+        fprintf(stderr, "[tc] %d layer(s) Cin %d CoutP %d KS %d.. halo %d Tq %d | n_tile %d MT %d nA %d nW %d resident %d smem %zu epi %d l2pf %d\n", n,
+                a0.Cin, a0.CoutP, a0.KS, halo, a0.Tq, p.n_tile, p.MT, p.nA, p.nW, p.w_resident, smem, p.epi_slots, p.l2_prefetch);
     p.groups_per_b = (tiles + p.MT - 1) / p.MT;
     p.total_groups = p.groups_per_b * a0.B * p.col_blocks;
     return SVB_OK;
@@ -833,10 +1049,22 @@ static bool tc_plan_fused(int n, const TcWeights *const *w, const ConvArgs *a, i
     p.nA = nA_pref;
     if (p.off_op + (size_t)p.nA * p.op_bytes + inter_area + 2 * (size_t)p.wtile_bytes > budget) p.nA = 2;
     if (p.off_op + (size_t)p.nA * p.op_bytes + inter_area + 2 * (size_t)p.wtile_bytes > budget) return false;
-    p.off_inter = p.off_op + (uint32_t)p.nA * p.op_bytes;
-    p.off_w = p.off_inter + (uint32_t)inter_area;
-    p.nW = std::min((int)((budget - p.off_w) / p.wtile_bytes), kMaxW);
-    p.off_bias = p.off_w + (uint32_t)round_up(p.nW * (int)p.wtile_bytes, 1024);
+    // the piece ring of the streamed epilogue (c2's residual / running sum) comes out of the weight ring; where it does not
+    // fit next to 3 slab slots (C = 64 at k 11, d 5), the plan drops to 2 slots for it
+    const int pieces = tc_epi_pieces(n, a + n, 2, p.n_tile);
+    auto layout = [&](int nA, bool ring) {
+        p.nA = nA;
+        p.off_inter = p.off_op + (uint32_t)nA * p.op_bytes;
+        p.off_w = p.off_inter + (uint32_t)inter_area;
+        p.nW = std::min((int)((budget - p.off_w) / p.wtile_bytes), kMaxW);
+        p.epi_slots = ring ? tc_epi_fit(budget - p.off_w, p.wtile_bytes, pieces, pieces / (2 * (p.n_tile / 32)), &p.nW) : 0;
+        return p.epi_slots > 0;
+    };
+    const int nA = p.nA;
+    if (!pieces || !(layout(nA, true) || (nA > 2 && layout(2, true)))) layout(nA, false);
+    p.l2_prefetch = p.epi_slots == 0 && tc_epi_sources(n, a + n) > 0;
+    p.off_epi = p.off_w + (uint32_t)round_up(p.nW * (int)p.wtile_bytes, 1024);
+    p.off_bias = p.off_epi + (uint32_t)p.epi_slots * kMathWarps * kEpiPieceBytes;
     smem = (size_t)p.off_bias + bias_bytes;
     if (smem > 227 * 1024) return false;
     for (int l = 0; l < 2 * n; ++l) {
@@ -1092,8 +1320,8 @@ int launch_conv_tc_multi(int n, const TcWeights *const *w, const ConvArgs *a, in
               "tc conv: work list was built for another plan (layers %d / %d, MT %d / %d)", wl.n_layers, n, wl.MT, p.MT);
     p.work = wl.items, p.work_off = wl.off;
     if (fused && getenv("SVB_TC_VERBOSE"))
-        fprintf(stderr, "[tc] fused %d chain(s) C %d KS %d.. dil %d.. Tq %d | P %d nA %d nW %d smem %zu\n", n, a[0].Cin, a[0].KS, a[0].dil,
-                a[0].Tq, p.fused_P, p.nA, p.nW, smem);
+        fprintf(stderr, "[tc] fused %d chain(s) C %d KS %d.. dil %d.. Tq %d | P %d nA %d nW %d smem %zu epi %d\n", n, a[0].Cin, a[0].KS,
+                a[0].dil, a[0].Tq, p.fused_P, p.nA, p.nW, smem, p.epi_slots);
     return tc_dispatch(p, precision, wl.grid, smem, st, fused);
 }
 

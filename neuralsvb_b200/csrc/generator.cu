@@ -181,6 +181,7 @@ int run_conv(svb_gen *g, const ConvLayer &L, const float *in, int in_Tp, float *
     a.in = in, a.w = L.w, a.bias = L.b, a.res = res, a.out = out;
     a.B = B, a.Cin = L.Cin, a.in_Tp = in_Tp, a.Cout = L.Cout, a.out_Tp = out_Tp, a.CoutP = L.CoutP, a.Tq = Tq;
     a.KS = L.KS, a.dil = L.dil, a.ups_u = L.ups_u, a.in_slope = in_slope, a.out_scale = scale, a.accumulate = accumulate;
+    a.epi_stream = g->epi;
     if (g->cfg.precision != SVB_PREC_FP32 && tc_supported(L.tc, a)) return launch_conv_tc(L.tc, a, g->cfg.precision, st, max_ctas);
     return launch_conv_ffma(a, st);
 }
@@ -198,6 +199,7 @@ int run_conv_multi(svb_gen *g, int stage, int nk, const ConvLayer *const *Ls, co
     for (int j = 0; j < (fused ? 2 * nk : nk); ++j) {
         const ConvLayer &L = *Ls[j];
         a[j] = resblock_args(L, in[j], out[j], res[j], scale[j], accumulate[j], B, Tq, Tp, in_slope);
+        a[j].epi_stream = g->epi;
         w[j] = &L.tc;
         bytes += 4.0 * ((double)B * Tq * L.Cin + (double)B * Tq * L.Cout * (1 + (res[j] ? 1 : 0) + (accumulate[j] ? 1 : 0)));
         flops += 2.0 * L.macs_per_row * (double)B * Tq;
@@ -475,6 +477,7 @@ extern "C" int svb_gen_create(const svb_gen_config *cfg, int device, svb_gen_t *
     if (const char *e = getenv("SVB_CHAINS")) g->chains = atoi(e);
     if (const char *e = getenv("SVB_MERGE")) g->merge = atoi(e) != 0;
     if (const char *e = getenv("SVB_FUSE")) g->fuse = atoi(e) != 0;
+    if (const char *e = getenv("SVB_EPI")) g->epi = atoi(e) != 0;
     if (const char *e = getenv("SVB_CHAIN_BIAS")) g->chain_bias = atof(e);
     *out = g;
     return SVB_OK;

@@ -143,6 +143,8 @@ struct svb_gen {
     bool merge = true;              // SVB_MERGE=0: one launch per convolution (round-1 schedule)
     bool fuse = true;               // SVB_FUSE=0: two launches per ResBlock1 step also where the fused launch fits (the
                                     // reference path of the bit-identity tests)
+    bool epi = true;                // SVB_EPI=0: the tensor-core epilogue loads residual / running sum per thread instead
+                                    // of streaming them through shared memory (the reference of its bit-identity tests)
     std::map<int, svb::TcWorkList> worklists;
 
     bool profile = false;

@@ -44,8 +44,14 @@ __device__ __forceinline__ void bulk_g2s(void *dst_smem, const void *src_gmem, u
                  "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar))
                  : "memory");
 }
+// L2 prefetch of a contiguous global span (16-byte aligned, a multiple of 16 bytes); nothing lands in shared memory
+__device__ __forceinline__ void bulk_prefetch_l2(const void *src_gmem, uint32_t bytes) {
+    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src_gmem), "r"(bytes) : "memory");
+}
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// generic-proxy global writes -> visible to later bulk copies (async proxy) that read them
+__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
 // named barrier over the first `threads` threads of the CTA (id 0 is __syncthreads)
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t threads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
