@@ -16,8 +16,8 @@ step and the phase-3 mapping step of ``SVBVAEMleTask``, tasks/singing/svb_vae_ta
 autograd node with a native backward (``_conv`` -> ``_TcConvFn`` / ``_ConvNctFn``, the GlobalFVAE through ``_WNTrainFn`` /
 ``_FVAEDecTrainFn``); the BatchNorms of ``upsample_layer`` and of the latent map use batch statistics in ``train()`` mode and update
 their running statistics as ``nn.BatchNorm1d`` does; ``vc_asr`` always runs without grad (the reference ``.detach()``es its output).
-The mel reconstruction loss is ``neuralsvb_b200.modules.commons.mel_loss.mel_l1_ssim_loss``; the DDP step (BASELINE cfg 4) is not part
-of this package."""
+The mel reconstruction loss is ``neuralsvb_b200.modules.commons.mel_loss.mel_l1_ssim_loss``; the task that drives the steps
+(single GPU or data parallel) is ``neuralsvb_b200.tasks.singing.svb_vae_task.SVBVAEMleTask``."""
 import torch
 import torch.nn.functional as F
 from torch import nn

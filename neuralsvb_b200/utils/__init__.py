@@ -1,4 +1,5 @@
 """Helpers the hot path's callers use (reference: utils/__init__.py)."""
+import sys
 import time
 
 import torch
@@ -66,6 +67,48 @@ def move_to_cpu(tensors):
     if isinstance(tensors, torch.Tensor):
         return tensors.cpu()
     return tensors
+
+
+def collate_1d(values, pad_idx=0):
+    """1-D tensors -> [B, max_len], right-padded with ``pad_idx`` (reference: utils/__init__.py:118-133)."""
+    res = values[0].new(len(values), max(v.size(0) for v in values)).fill_(pad_idx)
+    for i, v in enumerate(values):
+        res[i, :len(v)] = v
+    return res
+
+
+def collate_2d(values, pad_idx=0):
+    """[T_i, C] tensors -> [B, max T_i, C], right-padded with ``pad_idx`` (reference: utils/__init__.py:136-150)."""
+    res = values[0].new(len(values), max(v.size(0) for v in values), values[0].shape[1]).fill_(pad_idx)
+    for i, v in enumerate(values):
+        res[i, :len(v)] = v
+    return res
+
+
+def batch_by_size(indices, num_tokens_fn, max_tokens=None, max_sentences=None, required_batch_size_multiple=1):
+    """Consecutive runs of ``indices`` whose padded size (len x longest) stays within ``max_tokens`` and whose length stays within
+    ``max_sentences``; a full batch is cut to a multiple of ``required_batch_size_multiple`` and the rest carried over
+    (reference: utils/__init__.py:153-217)."""
+    max_tokens = sys.maxsize if max_tokens is None else max_tokens
+    max_sentences = sys.maxsize if max_sentences is None else max_sentences
+    bsz_mult = required_batch_size_multiple
+    sample_len, sample_lens, batch, batches = 0, [], [], []
+    for idx in indices:
+        num_tokens = num_tokens_fn(idx)
+        sample_lens.append(num_tokens)
+        sample_len = max(sample_len, num_tokens)
+        assert sample_len <= max_tokens, f'sentence at index {idx} of size {sample_len} exceeds max_tokens limit of {max_tokens}!'
+        num_tokens = (len(batch) + 1) * sample_len
+        if len(batch) > 0 and (len(batch) == max_sentences or num_tokens > max_tokens):
+            mod_len = max(bsz_mult * (len(batch) // bsz_mult), len(batch) % bsz_mult)
+            batches.append(batch[:mod_len])
+            batch = batch[mod_len:]
+            sample_lens = sample_lens[mod_len:]
+            sample_len = max(sample_lens) if len(sample_lens) > 0 else 0
+        batch.append(idx)
+    if len(batch) > 0:
+        batches.append(batch)
+    return batches
 
 
 def tensors_to_scalars(tensors):

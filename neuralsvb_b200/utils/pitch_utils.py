@@ -5,6 +5,17 @@ import numpy as np
 import torch
 
 F0_MAX = 1100.0
+F0_BIN, F0_MIN = 256, 50.0
+F0_MEL_MIN, F0_MEL_MAX = 1127 * np.log(1 + F0_MIN / 700), 1127 * np.log(1 + F0_MAX / 700)
+
+
+def f0_to_coarse(f0):
+    """Coarse pitch ids in [1, 255] from f0 in Hz (numpy): the mel-scaled f0 quantised into F0_BIN - 2 bins, unvoiced -> 1."""
+    f0_mel = 1127 * np.log(1 + np.asarray(f0) / 700)
+    f0_mel[f0_mel > 0] = (f0_mel[f0_mel > 0] - F0_MEL_MIN) * (F0_BIN - 2) / (F0_MEL_MAX - F0_MEL_MIN) + 1
+    f0_mel[f0_mel <= 1] = 1
+    f0_mel[f0_mel > F0_BIN - 1] = F0_BIN - 1
+    return np.rint(f0_mel).astype(np.int64)
 
 
 def norm_interp_f0(f0, hparams):

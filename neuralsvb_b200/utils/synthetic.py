@@ -549,3 +549,57 @@ def make_mel2ph_pair(seed, S, T):
         m[:n - pad] = np.searchsorted(edges[1:-1], np.arange(n - pad), side='right') + 1
         return m
     return take(S), take(T)
+
+
+def write_svb_binary(data_dir, n_items=8, seed=1234, n_valid=2, n_test=2, frames=(60, 256)):
+    """Write a paired-singing dataset in the layout data_gen/singing/binarize_para.py writes (``{train,valid,test}.data`` / ``.idx``,
+    ``{prefix}_lengths.npy``, ``train_f0s_mean_std.npy``, ``phone_set.json``), plus what the SVB config points at next to it:
+    ``asr/model_ckpt_steps_0.ckpt`` (a random VCASR encoder as ``state_dict.model``, the pretrain_asr_ckpt layout) and
+    ``hifigan/`` (config.yaml + a random hop-128 HiFi-GAN-NSF in the vocoder checkpoint layout).
+
+    Each item: an amateur and a professional take of independent lengths (multiples of 4 in ``frames``), log10-range mels,
+    f0 from ``make_f0_pair`` with coarse pitch ids, ``a2p_f0_alignment`` = the monotone linear map from professional to amateur
+    frames, and ``multi_spk_emb`` [5, 256].  Runs on the CPU."""
+    import json
+    import os
+
+    import yaml
+
+    from neuralsvb_b200.utils.indexed_datasets import IndexedDatasetBuilder
+    from neuralsvb_b200.utils.pitch_utils import f0_to_coarse
+    os.makedirs(data_dir, exist_ok=True)
+    rs = np.random.RandomState(seed + 71)
+    lo, hi = frames[0] // 4, frames[1] // 4
+    with open(os.path.join(data_dir, 'phone_set.json'), 'w') as f:
+        json.dump([f'ph{i}' for i in range(60)], f)
+    train_f0s = []
+    for prefix, n in (('train', n_items), ('valid', n_valid), ('test', n_test)):
+        builder = IndexedDatasetBuilder(os.path.join(data_dir, prefix))
+        lengths = []
+        for i in range(n):
+            Ta, Tp = 4 * int(rs.randint(lo, hi + 1)), 4 * int(rs.randint(lo, hi + 1))
+            f0, prof_f0 = make_f0_pair(int(rs.randint(0, 2 ** 31 - 1)), Ta, Tp)
+            mel = lambda T: (rs.randn(T, 80) * 1.2 - 2.5).clip(-6, 1.5).astype(np.float32)
+            item = {'item_name': f'{prefix}_{i:04d}#Amateur', 'mel': mel(Ta), 'prof_mel': mel(Tp), 'f0': f0, 'prof_f0': prof_f0,
+                    'pitch': f0_to_coarse(f0), 'prof_pitch': f0_to_coarse(prof_f0),
+                    'a2p_f0_alignment': np.round(np.arange(Tp) * (Ta - 1) / max(Tp - 1, 1)).astype(np.int64),
+                    'multi_spk_emb': _normal(rs, (5, 256), 0.5), 'len': Ta, 'prof_len': Tp}
+            builder.add_item(item)
+            lengths.append(max(Ta, Tp))
+            if prefix == 'train':
+                train_f0s += [f0, prof_f0]
+        builder.finalize()
+        np.save(os.path.join(data_dir, f'{prefix}_lengths.npy'), lengths)
+    f0s = np.concatenate(train_f0s)
+    f0s = f0s[f0s != 0]
+    np.save(os.path.join(data_dir, 'train_f0s_mean_std.npy'), [np.mean(f0s).item(), np.std(f0s).item()])
+    os.makedirs(os.path.join(data_dir, 'asr'), exist_ok=True)
+    torch.save({'state_dict': {'model': make_vc_asr_state_dict(seed)}, 'global_step': 0},
+               os.path.join(data_dir, 'asr', 'model_ckpt_steps_0.ckpt'))
+    voc = os.path.join(data_dir, 'hifigan')
+    os.makedirs(voc, exist_ok=True)
+    h = hifigan_config(hop=128)
+    with open(os.path.join(voc, 'config.yaml'), 'w') as f:
+        yaml.safe_dump(h, f)
+    torch.save({'state_dict': {'model_gen': make_generator_state_dict(h, seed)}, 'global_step': 0, 'epoch': 0,
+                'checkpoint_callback_best': 0.0, 'optimizer_states': []}, os.path.join(voc, 'model_ckpt_steps_0.ckpt'))
