@@ -522,6 +522,40 @@ int svb_dtw_baselines_cost(const void *src_dev, const void *tgt_dev, int32_t dty
                            const int32_t *src_len_host, const int32_t *tgt_len_host, int32_t feat_dim, void *workspace_dev,
                            int64_t workspace_bytes, void *cost_dev, void *stream);
 
+/* ---- Autocorrelation pitch tracker (csrc/pitch_ac.cu): the f0 of the binarizer's get_pitch (data_gen/tts/data_gen_utils.py:150-184),
+ * Boersma's method as Praat's "To Pitch (ac)" describes it; oracle/pitch_ac.py states every step.  A batch is ragged: n_clips
+ * float32 waveforms concatenated (clip c has lengths[c] samples, host array), each analysed on its own grid of
+ * floor((N / sr - 3 / floor) / time_step) + 1 frames, and the path's f0 placed into mel_frames[c] output frames (lpad zero frames in
+ * front, then cut, or extended with the last value), the clips' outputs back to back.  time_step must be hop / sr.
+ * svb_pitch_ac_workspace_bytes: size of the caller-owned workspace (-1 on a bad config or length); frames_out (NULL = not wanted)
+ *   receives each clip's analysis frame count.
+ * svb_pitch_ac_batch (device pointers): f0_out_dev float32 [sum mel_frames]; cand_dev (NULL = not wanted) float32 [frames, 15, 2] =
+ *   (frequency, strength) of the unvoiced candidate then the voiced ones strongest first (unused: (0, -inf)); count_dev int32 [frames];
+ *   r_dev float32 [frames, tau_max + 2] = the normalised autocorrelation r(tau); stage_ms_host (NULL = not wanted) receives 3 CUDA-event
+ *   times (clip statistics, candidates, path) and makes the call synchronise.
+ * svb_pitch_ac_batch_host: the same from host memory: one H2D copy, the three launches, one D2H copy; synchronises.
+ * All reject before any launch (SVB_ERR_INVALID): a null pointer, a bad config, a clip shorter than one window, a short workspace. */
+typedef struct svb_pitch_config {
+    int32_t sr;
+    int32_t hop;
+    double floor;                  /* Hz (80)                                 */
+    double ceiling;                /* Hz (750)                                */
+    double time_step;              /* s, hop / sr                             */
+    double voicing_threshold;      /* 0.6                                     */
+    double silence_threshold;      /* 0.03                                    */
+    double octave_cost;            /* 0.01                                    */
+    double octave_jump_cost;       /* 0.35                                    */
+    double voiced_unvoiced_cost;   /* 0.14                                    */
+    int32_t lpad;                  /* zero frames placed in front (2 pad_size) */
+    int32_t reserved;
+} svb_pitch_config;
+int64_t svb_pitch_ac_workspace_bytes(const svb_pitch_config *cfg, const int64_t *lengths, int32_t n_clips, int32_t *frames_out);
+int svb_pitch_ac_batch(const svb_pitch_config *cfg, const float *wav_concat_dev, const int64_t *lengths, int32_t n_clips,
+                       const int64_t *mel_frames, float *f0_out_dev, void *workspace_dev, int64_t workspace_bytes, float *cand_dev,
+                       int32_t *count_dev, float *r_dev, float *stage_ms_host, void *stream);
+int svb_pitch_ac_batch_host(const svb_pitch_config *cfg, const float *wav_concat_host, const int64_t *lengths, int32_t n_clips,
+                            const int64_t *mel_frames, float *f0_out_host, int device, void *stream);
+
 /* Host-only view of the schedule of a merged tensor-core launch (csrc/conv_tc.cu: tc_schedule; no CUDA call, usable without a GPU):
  * `n_layers` convolutions of one shape class (taps KS[l], residual / accumulate flags) over B clips x Tq rows, tiles of 128 rows in
  * items of up to MT tiles, `col_blocks` column blocks, `grid` CTAs.  items_out receives 5 ints per item (layer, column block, clip,

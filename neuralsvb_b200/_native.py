@@ -16,7 +16,8 @@ CSRC = os.path.join(_HERE, 'csrc')
 LIB_PATH = os.path.join(_HERE, 'libsvb_vocoder.so')
 HEADER = os.path.join(_ROOT, 'include', 'svb_vocoder.h')
 SOURCES = ['wn.cu', 'conformer.cu', 'api.cu', 'conv_ffma.cu', 'conv_tc.cu', 'nsf_source.cu', 'frontend.cu', 'generator.cu', 'layer_api.cu', 'disc_ops.cu',
-           'train_ops.cu', 'generator_bwd.cu', 'disc_bwd.cu', 'tc_layer.cu', 'wgrad_tc.cu', 'mel_loss.cu', 'mel_disc.cu', 'sadtw.cu']
+           'train_ops.cu', 'generator_bwd.cu', 'disc_bwd.cu', 'tc_layer.cu', 'wgrad_tc.cu', 'mel_loss.cu', 'mel_disc.cu', 'sadtw.cu',
+           'pitch_ac.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '-Xcompiler', '-fPIC', '-shared']
 
@@ -49,6 +50,15 @@ class StftConfig(ctypes.Structure):
         ('n_fft', ctypes.c_int32), ('hop', ctypes.c_int32), ('win', ctypes.c_int32),
         ('pad_mode', ctypes.c_int32), ('out_kind', ctypes.c_int32), ('clamp_input', ctypes.c_int32),
         ('n_mels', ctypes.c_int32), ('frames_major', ctypes.c_int32), ('eps', ctypes.c_float),
+    ]
+
+
+class PitchConfig(ctypes.Structure):
+    _fields_ = [
+        ('sr', ctypes.c_int32), ('hop', ctypes.c_int32), ('floor', ctypes.c_double), ('ceiling', ctypes.c_double),
+        ('time_step', ctypes.c_double), ('voicing_threshold', ctypes.c_double), ('silence_threshold', ctypes.c_double),
+        ('octave_cost', ctypes.c_double), ('octave_jump_cost', ctypes.c_double), ('voiced_unvoiced_cost', ctypes.c_double),
+        ('lpad', ctypes.c_int32), ('reserved', ctypes.c_int32),
     ]
 
 
@@ -197,6 +207,9 @@ _PROTOS = {
     'svb_dtw_baselines_workspace_bytes': (_I64, [_I32, _I32, _I32, _P, _P]),
     'svb_dtw_baselines_align': (ctypes.c_int, [_P, _P, _I32, _I32, _I32, _P, _P, _I32, _P, _I64, _P, _P, _P, _P]),
     'svb_dtw_baselines_cost': (ctypes.c_int, [_P, _P, _I32, _I32, _I32, _P, _P, _I32, _P, _I64, _P, _P]),
+    'svb_pitch_ac_workspace_bytes': (_I64, [ctypes.POINTER(PitchConfig), _P, _I32, _P]),
+    'svb_pitch_ac_batch': (ctypes.c_int, [ctypes.POINTER(PitchConfig), _P, _P, _I32, _P, _P, _P, _I64, _P, _P, _P, _P, _P]),
+    'svb_pitch_ac_batch_host': (ctypes.c_int, [ctypes.POINTER(PitchConfig), _P, _P, _I32, _P, _P, ctypes.c_int, _P]),
 }
 
 

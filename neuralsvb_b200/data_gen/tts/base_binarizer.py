@@ -5,7 +5,8 @@ single-threaded CPU workers (data_gen/tts/base_binarizer.py:128-178, data_gen/si
 ``OMP_NUM_THREADS=1`` at data_gen/tts/bin/binarize.py:3).  Here the files of a split are grouped into ragged batches
 and every batch is ONE device call (``HifiGAN.wav2spec_batch`` -> ``svb_wav2spec_batch_host``); the items written are
 the reference's: ``item_name, wav_fn, spk_id, mel [T, 80] (log10), wav float16 [T*hop], sec, len`` (+ ``f0`` when a
-pitch function is supplied: the reference's parselmouth extractor is third-party CPU data preparation, out of scope),
+pitch function is supplied: ``data_gen.tts.data_gen_utils.get_pitch`` is this package's GPU tracker, and the reference's
+parselmouth extractor can be passed instead),
 in the reference's IndexedDataset format plus ``{prefix}_lengths.npy``.  Text / alignment / speaker-embedding fields
 belong to the acoustic model's data preparation and are not produced."""
 import os
@@ -28,13 +29,13 @@ class VocoderBinarizer:
         os.makedirs(self.binary_data_dir, exist_ok=True)
         return {prefix: self.process_data(prefix) for prefix in ('valid', 'test', 'train') if prefix in self.items}
 
-    def _batches(self, metas):
-        """Group consecutive items up to ``batch_seconds`` of audio (arrays are measured, files are stat'ed: 2 bytes/sample)."""
+    def _batches(self, metas, wavs_of=lambda m: (m[1],)):
+        """Group consecutive items up to ``batch_seconds`` of audio (arrays are measured, files are stat'ed: 2 bytes/sample).
+        ``wavs_of(meta)``: the waveforms an item holds (its one take here; both takes of a pair in the paired binarizer)."""
         sr = hparams['audio_sample_rate']
         cur, sec = [], 0.0
         for m in metas:
-            w = m[1]
-            s = (os.path.getsize(w) / 2.0 if isinstance(w, str) else len(w)) / sr
+            s = sum((os.path.getsize(w) / 2.0 if isinstance(w, str) else len(w)) for w in wavs_of(m)) / sr
             if cur and sec + s > self.batch_seconds:
                 yield cur
                 cur, sec = [], 0.0

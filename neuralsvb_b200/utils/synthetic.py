@@ -563,8 +563,6 @@ def write_svb_binary(data_dir, n_items=8, seed=1234, n_valid=2, n_test=2, frames
     import json
     import os
 
-    import yaml
-
     from neuralsvb_b200.utils.indexed_datasets import IndexedDatasetBuilder
     from neuralsvb_b200.utils.pitch_utils import f0_to_coarse
     os.makedirs(data_dir, exist_ok=True)
@@ -593,6 +591,15 @@ def write_svb_binary(data_dir, n_items=8, seed=1234, n_valid=2, n_test=2, frames
     f0s = np.concatenate(train_f0s)
     f0s = f0s[f0s != 0]
     np.save(os.path.join(data_dir, 'train_f0s_mean_std.npy'), [np.mean(f0s).item(), np.std(f0s).item()])
+    write_svb_checkpoints(data_dir, seed)
+
+
+def write_svb_checkpoints(data_dir, seed=1234):
+    """What the SVB config points at next to a dataset: ``asr/model_ckpt_steps_0.ckpt`` (a random VCASR encoder) and ``hifigan/``
+    (config.yaml + a random hop-128 HiFi-GAN-NSF checkpoint)."""
+    import os
+
+    import yaml
     os.makedirs(os.path.join(data_dir, 'asr'), exist_ok=True)
     torch.save({'state_dict': {'model': make_vc_asr_state_dict(seed)}, 'global_step': 0},
                os.path.join(data_dir, 'asr', 'model_ckpt_steps_0.ckpt'))
@@ -603,3 +610,95 @@ def write_svb_binary(data_dir, n_items=8, seed=1234, n_valid=2, n_test=2, frames
         yaml.safe_dump(h, f)
     torch.save({'state_dict': {'model_gen': make_generator_state_dict(h, seed)}, 'global_step': 0, 'epoch': 0,
                 'checkpoint_callback_best': 0.0, 'optimizer_states': []}, os.path.join(voc, 'model_ckpt_steps_0.ckpt'))
+
+
+def make_sung_take(f0_frames, seed, sr=22050, hop=128, breath=True):
+    """(wav float32 [len(f0_frames) * hop], true f0 float64 per sample, 0 = unvoiced) of one singing-like take: a harmonic source
+    whose phase integrates the frame contour (linearly interpolated over voiced frames), with a per-take spectral tilt, a slow
+    amplitude envelope and 10 ms fades at every voicing edge, over silence or low-level breath noise in the gaps."""
+    rs = np.random.RandomState(seed + 73)
+    f0_frames = np.asarray(f0_frames, np.float64)
+    n = len(f0_frames) * hop
+    voiced_fr = f0_frames > 0
+    k = np.arange(n)
+    voiced = voiced_fr[k // hop]
+    if voiced_fr.any():
+        pos = np.nonzero(voiced_fr)[0] * hop + hop / 2.0
+        f0 = np.interp(k, pos, f0_frames[voiced_fr])
+    else:
+        f0 = np.zeros(n)
+    f0 = np.where(voiced, f0, 0.0)
+    phase = 2 * np.pi * np.cumsum(f0) / sr + rs.uniform(0, 2 * np.pi)
+    tilt = rs.uniform(0.8, 1.6)
+    src = np.zeros(n)
+    for h in range(1, 40):
+        amp = h ** -tilt * rs.uniform(0.7, 1.3)
+        src += np.where(h * f0 < 0.45 * sr, amp * np.sin(h * phase + rs.uniform(0, 2 * np.pi)), 0.0)
+    fade = int(0.01 * sr)
+    ramp = np.convolve(voiced.astype(np.float64), np.hanning(2 * fade + 1) / np.hanning(2 * fade + 1).sum(), mode='same')
+    env = (0.55 + 0.25 * np.sin(2 * np.pi * k / sr * rs.uniform(0.3, 1.2) + rs.uniform(0, 6.28))) * ramp
+    wav = 0.35 * env * src / max(1.0, np.abs(src).max() / 2.5)
+    if breath:
+        wav += (1.0 - ramp) * 0.004 * rs.standard_normal(n)
+    return np.clip(wav, -1, 1).astype(np.float32), f0
+
+
+def write_svb_raw(processed_dir, binary_data_dir=None, seed=1234, sr=22050, hop=128, seconds=(1.5, 3.0), gap_frames=None):
+    """Write a raw paired-singing set in PopBuTFy's layout, for the paired binarizer (egs/svb_binarize_synthetic.yaml):
+    ``{processed_dir}/data/{spk}#singing#{song}/{spk}#singing#{song}_{Amateur|Professional}_{k}.wav`` (16-bit WAV at sr),
+    ``{processed_dir}/spk_emb/{item_name}.npy`` (256-d, one per amateur take) and ``{processed_dir}/phone_set.json``.
+
+    Three speakers (Female1, Female2, Male1) sing two songs in two pieces each; each pair is ``make_f0_pair``'s two takes through
+    ``make_sung_take``.  Besides the regular pairs: ``Female2#singing#Song_B_Amateur_1``'s professional take is ``gap_frames`` frames
+    (default 240) longer than the amateur one; ``Male1#singing#Song_A_Amateur_1`` is digital silence; ``Female1#singing#Song_C_Amateur_0``
+    has no professional take; ``Female1#speech#Talk_Amateur_0`` is not singing.  With ``binary_data_dir``, phone_set.json and the
+    checkpoints of ``write_svb_checkpoints`` are written there too.
+
+    Returns {item_name: true f0 per sample (float64, 0 = unvoiced)} for every file written."""
+    import json
+    import os
+
+    from scipy.io import wavfile
+    rs = np.random.RandomState(seed + 79)
+    fps = sr / hop
+    gap_frames = 240 if gap_frames is None else gap_frames
+    truth = {}
+
+    def write(name, wav, f0):
+        d = os.path.join(processed_dir, 'data', name.rsplit('_', 2)[0])
+        os.makedirs(d, exist_ok=True)
+        wavfile.write(os.path.join(d, name + '.wav'), sr, np.round(np.clip(wav, -1, 1) * 32767).astype(np.int16))
+        truth[name] = f0
+
+    emb_dir = os.path.join(processed_dir, 'spk_emb')
+    os.makedirs(emb_dir, exist_ok=True)
+    spk_shift = {'Female1': 5, 'Female2': 3, 'Male1': -4}
+    for spk, shift in spk_shift.items():
+        songs = [('Song_A', 2), ('Song_B', 2)] + ([('Song_C', 1)] if spk == 'Female1' else [])
+        for song, pieces in songs:
+            for piece in range(pieces):
+                base = f'{spk}#singing#{song}'
+                ama, prof = f'{base}_Amateur_{piece}', f'{base}_Professional_{piece}'
+                S = int(rs.uniform(*seconds) * fps)
+                T = S + gap_frames if ama == 'Female2#singing#Song_B_Amateur_1' else int(S * rs.uniform(0.85, 1.15))
+                fa, fp = make_f0_pair(int(rs.randint(0, 2 ** 31 - 1)), S, T, fps)
+                fa, fp = fa * 2 ** (shift / 12), fp * 2 ** (shift / 12)
+                wa, ta = make_sung_take(fa, int(rs.randint(0, 2 ** 31 - 1)), sr, hop)
+                if ama == 'Male1#singing#Song_A_Amateur_1':
+                    wa, ta = np.zeros_like(wa), np.zeros_like(ta)
+                write(ama, wa, ta)
+                np.save(os.path.join(emb_dir, ama + '.npy'), _normal(rs, (256,), 0.5))
+                if song != 'Song_C':
+                    wp, tp = make_sung_take(fp, int(rs.randint(0, 2 ** 31 - 1)), sr, hop)
+                    write(prof, wp, tp)
+    f0, _ = make_f0_pair(int(rs.randint(0, 2 ** 31 - 1)), int(2 * fps), int(2 * fps), fps)
+    w, t = make_sung_take(f0, int(rs.randint(0, 2 ** 31 - 1)), sr, hop)
+    write('Female1#speech#Talk_Amateur_0', w, t)
+    phones = [f'ph{i}' for i in range(60)]
+    for d in [processed_dir] + ([binary_data_dir] if binary_data_dir else []):
+        os.makedirs(d, exist_ok=True)
+        with open(os.path.join(d, 'phone_set.json'), 'w') as f:
+            json.dump(phones, f)
+    if binary_data_dir:
+        write_svb_checkpoints(binary_data_dir, seed)
+    return truth
