@@ -227,7 +227,18 @@ __global__ void __launch_bounds__(32 * kFPC) pitch_cand_kernel(const float *__re
         for (int i = 0; i < R - 1; ++i) wv[i] = wv[i + 1];
         wv[R - 1] = fb[k + tau0 + R];
     }
-    const float ra0 = __shfl_sync(0xffffffffu, acc[0], 0);
+    // An exactly constant window has r_a(0) = 0 and localPeak = 0: the text's float64 mean of equal floats is exact.  The fp32 mean
+    // above need not be, and the +-1-ulp residue it leaves would normalise to r(tau) ~ 1.  Such a window leaves |x - mean| within
+    // a few ulps of |mean| (the fp32 sum of L <= 1723 equal terms is within 60 ulps), so only a window that small pays for the
+    // exact test.
+    bool flat = false;
+    if (lp <= 1e-4f * fabsf(mean)) {
+        bool same = true;
+        for (int k = lane; k < p.L; k += 32) same = same && xs[k] == xs[0];
+        flat = __all_sync(0xffffffffu, same);
+    }
+    if (flat) lp = 0.f;
+    const float ra0 = flat ? 0.f : __shfl_sync(0xffffffffu, acc[0], 0);
     float *rr = rbuf + warp * 32 * R;
     const long long fg = (long long)cl.frame_off + j;
 #pragma unroll

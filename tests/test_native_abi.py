@@ -174,3 +174,125 @@ def test_schedule_handles_an_odd_tile_count():
     tiles = items[:, 4]
     assert set(tiles.tolist()) == {1, 2}                                      # the last item of a clip has one tile
     assert int(tiles.sum()) == 2 * 3 * 5
+
+
+# ---- autocorrelation pitch tracker (csrc/pitch_ac.cu): host-side planning and refusals
+PITCH_CONFIGS = [(22050, 128, 8), (22050, 256, 4), (22880, 128, 8), (22881, 128, 8), (24000, 128, 8), (44100, 256, 4),
+                 (45920, 256, 4), (16000, 110, 0)]
+
+
+def _pitch_cfg(sr, hop, lpad):
+    from neuralsvb_b200.data_gen.tts import data_gen_utils as DG
+    return DG.pitch_config({'audio_sample_rate': sr, 'hop_size': hop}, lpad)
+
+
+def _pitch_frames(l, cfg, lengths):
+    import numpy as np
+    lens = np.ascontiguousarray(lengths, dtype=np.int64)
+    out = np.full(len(lens), -7, np.int32)
+    ws = l.svb_pitch_ac_workspace_bytes(ctypes.byref(cfg), lens.ctypes.data, len(lens), out.ctypes.data)
+    return ws, out
+
+
+@pytest.mark.parametrize('sr,hop,lpad', PITCH_CONFIGS, ids=[f'{s}-{h}-{p}' for s, h, p in PITCH_CONFIGS])
+def test_pitch_frame_counts_match_the_oracle_grid(built, sr, hop, lpad):
+    """frames_out of svb_pitch_ac_workspace_bytes equals oracle.pitch_ac.grid and data_gen_utils.pitch_frames for clips around one
+    window (L), one window plus a hop, and random lengths; a clip with no analysis frame is refused by all three."""
+    import numpy as np
+
+    from neuralsvb_b200.data_gen.tts import data_gen_utils as DG
+    from oracle import pitch_ac as P
+    l = _native.lib()
+    cfg = _pitch_cfg(sr, hop, lpad)
+    hp = {'audio_sample_rate': sr, 'hop_size': hop}
+    L = 2 * int(np.floor(3.0 / 80.0 * sr / 2.0)) + 1
+    rs = np.random.RandomState(sr + hop)
+    Ns = list(range(L - 4, L + 5)) + list(range(L + hop - 4, L + hop + 5)) + rs.randint(L, 40 * sr, 40).tolist()
+    refused = 0
+    for N in Ns:
+        try:
+            n = P.grid(N, sr, hop / sr)[0]
+        except ValueError:
+            n = 0
+        ws, out = _pitch_frames(l, cfg, [N])
+        if n == 0:
+            refused += 1
+            assert ws < 0 and b'shorter than one pitch window' in l.svb_last_error(), N
+            assert DG.pitch_frames(N, hp) < 1, N
+            continue
+        assert ws > 0 and out[0] == n == DG.pitch_frames(N, hp), (N, ws, out[0], n, DG.pitch_frames(N, hp))
+    assert 0 < refused < len(Ns)
+    # the same lengths in one ragged call
+    good = [N for N in Ns if DG.pitch_frames(N, hp) >= 1]
+    ws, out = _pitch_frames(l, cfg, good)
+    assert ws > 0 and out.tolist() == [P.grid(N, sr, hop / sr)[0] for N in good]
+
+
+def test_pitch_refuses_bad_arguments_without_gpu(built):
+    """svb_pitch_ac_workspace_bytes and svb_pitch_ac_batch refuse before any CUDA call (negative status, message set).  Host buffers
+    stand in for the device pointers: a refusal must come before one is touched."""
+    import numpy as np
+
+    from oracle import pitch_ac as P
+    l = _native.lib()
+    buf = np.zeros(1 << 16, np.float32)
+    p = ctypes.c_void_p(buf.ctypes.data)
+    ok = [22050, 30000]
+    mel = np.array([200, 240, 100], np.int64)
+
+    def refuse(c, lens, msg, n=None):
+        lens = np.ascontiguousarray(lens, dtype=np.int64)
+        n = len(lens) if n is None else n
+        frames = np.zeros(max(len(lens), 1), np.int32)
+        assert l.svb_pitch_ac_workspace_bytes(c, lens.ctypes.data, n, frames.ctypes.data) < 0, msg
+        assert msg in l.svb_last_error(), (msg, l.svb_last_error())
+        l.svb_pitch_ac_workspace_bytes(cfg(hop=0), lens.ctypes.data, n, None)    # another message in between
+        assert msg not in l.svb_last_error()
+        assert l.svb_pitch_ac_batch(c, p, lens.ctypes.data, n, mel.ctypes.data, p, p, 1 << 30, None, None, None, None, None) < 0
+        assert msg in l.svb_last_error(), (msg, l.svb_last_error())
+
+    def cfg(**kw):
+        c = _pitch_cfg(22050, 128, 8)
+        for k, v in kw.items():
+            setattr(c, k, v)
+        return ctypes.byref(c)
+
+    assert l.svb_pitch_ac_workspace_bytes(cfg(), np.array(ok, np.int64).ctypes.data, 2, None) > 0    # the refusals below are not vacuous
+    refuse(None, ok, b'null config')
+    big = _pitch_cfg(45920, 256, 4)
+    assert l.svb_pitch_ac_workspace_bytes(ctypes.byref(big), np.array(ok, np.int64).ctypes.data, 2, None) > 0   # 576 lags: the widest
+    big.sr, big.time_step = 45921, 256 / 45921                              # ceil(45921 / 80) + 2 = 577 lags
+    refuse(ctypes.byref(big), ok, b'needs 577 lags, more than 576')
+    big.sr, big.time_step = 48000, 256 / 48000
+    refuse(ctypes.byref(big), ok, b'more than 576')
+    refuse(cfg(ceiling=11025.5), ok, b'above sr / 2')
+    assert l.svb_pitch_ac_workspace_bytes(cfg(ceiling=11025.0), np.array(ok, np.int64).ctypes.data, 2, None) > 0
+    refuse(cfg(time_step=0.0058), ok, b'is not hop / sr')
+    refuse(cfg(time_step=256 / 22050), ok, b'is not hop / sr')
+    refuse(cfg(lpad=-1), ok, b'negative lpad')
+    for k in ('voicing_threshold', 'octave_cost', 'octave_jump_cost', 'voiced_unvoiced_cost'):
+        refuse(cfg(**{k: -0.01}), ok, b'negative threshold or cost')
+    refuse(cfg(silence_threshold=0.0), ok, b'negative threshold or cost')
+    refuse(cfg(), [22050, 0, 30000], b'clip 1 has 0 samples')
+    longest = next(N for N in range(900, 700, -1) if _no_frame(P, N, 22050, 128))
+    assert not _no_frame(P, longest + 1, 22050, 128)
+    refuse(cfg(), [22050, 30000, longest], b'clip 2 has %d samples' % longest)
+    refuse(cfg(), ok, b'no clips', n=0)
+    # null buffers and a short workspace: svb_pitch_ac_batch only (the planner takes no buffers)
+    lens = np.array(ok, np.int64)
+    need = l.svb_pitch_ac_workspace_bytes(cfg(), lens.ctypes.data, 2, None)
+    batch = lambda wav=p, m=mel.ctypes.data, f0=p, ws=p, nb=need: l.svb_pitch_ac_batch(cfg(), wav, lens.ctypes.data, 2, m, f0, ws, nb,
+                                                                                        None, None, None, None, None)
+    for k in ('wav', 'm', 'f0', 'ws'):
+        assert batch(**{k: None}) < 0 and b'null buffer' in l.svb_last_error(), k
+    assert batch(nb=need - 1) < 0 and b'workspace of %d bytes, %d needed' % (need - 1, need) in l.svb_last_error()
+    assert l.svb_pitch_ac_workspace_bytes(cfg(), None, 2, None) < 0 and b'null lengths' in l.svb_last_error()
+    assert (buf == 0).all()
+
+
+def _no_frame(P, N, sr, hop):
+    try:
+        P.grid(N, sr, hop / sr)
+        return False
+    except ValueError:
+        return True
