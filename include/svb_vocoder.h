@@ -556,6 +556,27 @@ int svb_pitch_ac_batch(const svb_pitch_config *cfg, const float *wav_concat_dev,
 int svb_pitch_ac_batch_host(const svb_pitch_config *cfg, const float *wav_concat_host, const int64_t *lengths, int32_t n_clips,
                             const int64_t *mel_frames, float *f0_out_host, int device, void *stream);
 
+/* ---- Resampling (csrc/resample.cu): librosa.core.load(path, sr=target)'s resampy kaiser_best resampler (reference
+ * data_gen/tts/data_gen_utils.py:111); oracle/resample.py states every step.  A batch is ragged: n_clips float32 waveforms concatenated
+ * (clip c has lengths[c] samples at src_sr[c] Hz, host arrays; rates may differ within a batch), one target rate per call.  Clip c
+ * yields out_lengths[c] = ceil(lengths[c] ratio) samples (int(lengths[c] ratio) filtered ones, then fix_length zeros), the clips'
+ * outputs back to back; a clip already at target_sr is copied.  win_host: the filter's float64 right wing (nwin taps, num_table per
+ * zero crossing: 32769 and 512 for kaiser_best), scaled and differenced here per source rate.
+ * svb_resample_plan: size of the caller-owned workspace, -1 on a bad rate, a clip that yields no sample, or a ratio below
+ *   1 / num_table; res_lengths_out / out_lengths_out (NULL = not wanted) receive each clip's lengths before and after the padding.
+ *   No CUDA call.
+ * svb_resample_batch (device pointers): out_dev float32 [sum out_lengths]; stage_ms_host (NULL = not wanted) receives 2 CUDA-event
+ *   times (time register, filter) and makes the call synchronise.
+ * svb_resample_batch_host: the same from host memory: one H2D copy of the samples, the launches, one D2H copy; synchronises.
+ * All reject before any launch (SVB_ERR_INVALID): a null pointer, a bad rate or length, a short workspace. */
+int64_t svb_resample_plan(int32_t target_sr, const int32_t *src_sr, const int64_t *lengths, int32_t n_clips, int32_t nwin,
+                          int32_t num_table, int64_t *res_lengths_out, int64_t *out_lengths_out);
+int svb_resample_batch(int32_t target_sr, const int32_t *src_sr, const int64_t *lengths, int32_t n_clips, const double *win_host,
+                       int32_t nwin, int32_t num_table, const float *wav_concat_dev, float *out_dev, void *workspace_dev,
+                       int64_t workspace_bytes, float *stage_ms_host, void *stream);
+int svb_resample_batch_host(int32_t target_sr, const int32_t *src_sr, const int64_t *lengths, int32_t n_clips, const double *win_host,
+                            int32_t nwin, int32_t num_table, const float *wav_concat_host, float *out_host, int device, void *stream);
+
 /* Host-only view of the schedule of a merged tensor-core launch (csrc/conv_tc.cu: tc_schedule; no CUDA call, usable without a GPU):
  * `n_layers` convolutions of one shape class (taps KS[l], residual / accumulate flags) over B clips x Tq rows, tiles of 128 rows in
  * items of up to MT tiles, `col_blocks` column blocks, `grid` CTAs.  items_out receives 5 ints per item (layer, column block, clip,

@@ -2,8 +2,9 @@
 ``{processed_data_dir}/data/*/*.wav``, keep the items of ``hparams['datasets']``, split them by ``test_prefixes`` and write
 ``spk_map.json``.  ``process_data`` is the subclass's (binarize_para.py).
 
-The reference reads PopBuTFy's mp3 files through librosa; here the input is WAV at ``audio_sample_rate``, converted once
-beforehand (for example ``ffmpeg -i x.mp3 -ac 1 -ar 22050 x.wav``)."""
+The reference reads PopBuTFy's mp3 files through librosa; here the input is WAV at any rate and channel count (folded to mono and
+resampled to ``audio_sample_rate`` on the GPU as ``librosa.core.load`` does), so mp3 files are decoded to WAV once beforehand (for
+example ``ffmpeg -i x.mp3 x.wav``)."""
 import glob
 import json
 import logging
@@ -44,9 +45,8 @@ class SingingBinarizer:
         for ds_id, processed_data_dir in enumerate(self.processed_data_dirs):
             wav_fns = sorted(glob.glob(f'{processed_data_dir}/data/*/*.wav'))
             if not wav_fns and glob.glob(f'{processed_data_dir}/data/*/*.mp3'):
-                raise ValueError(f'{processed_data_dir}/data holds mp3 files only: the binarizer reads WAV at audio_sample_rate '
-                                 f'({hparams["audio_sample_rate"]} Hz); convert them once, e.g. '
-                                 f'ffmpeg -i x.mp3 -ac 1 -ar {hparams["audio_sample_rate"]} x.wav')
+                raise ValueError(f'{processed_data_dir}/data holds mp3 files only: the binarizer reads WAV (any rate; it resamples '
+                                 f'to {hparams["audio_sample_rate"]} Hz itself); decode them once, e.g. ffmpeg -i x.mp3 x.wav')
             for wav_fn in wav_fns:
                 item_name = os.path.splitext(os.path.basename(wav_fn))[0]
                 if len(self.processed_data_dirs) > 1:

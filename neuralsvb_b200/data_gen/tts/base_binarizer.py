@@ -13,6 +13,7 @@ import os
 
 import numpy as np
 
+from neuralsvb_b200.utils import audio
 from neuralsvb_b200.utils.hparams import hparams
 from neuralsvb_b200.utils.indexed_datasets import IndexedDatasetBuilder
 from neuralsvb_b200.vocoders.base_vocoder import get_vocoder_cls
@@ -30,12 +31,13 @@ class VocoderBinarizer:
         return {prefix: self.process_data(prefix) for prefix in ('valid', 'test', 'train') if prefix in self.items}
 
     def _batches(self, metas, wavs_of=lambda m: (m[1],)):
-        """Group consecutive items up to ``batch_seconds`` of audio (arrays are measured, files are stat'ed: 2 bytes/sample).
-        ``wavs_of(meta)``: the waveforms an item holds (its one take here; both takes of a pair in the paired binarizer)."""
+        """Group consecutive items up to ``batch_seconds`` of audio (arrays are at audio_sample_rate; a file's duration is read
+        from its WAV header, at the file's own rate).  ``wavs_of(meta)``: the waveforms an item holds (its one take here; both takes
+        of a pair in the paired binarizer).  Every clip's output is the same in any batch, so grouping changes no item."""
         sr = hparams['audio_sample_rate']
         cur, sec = [], 0.0
         for m in metas:
-            s = sum((os.path.getsize(w) / 2.0 if isinstance(w, str) else len(w)) for w in wavs_of(m)) / sr
+            s = sum(audio.wav_seconds(w) if isinstance(w, str) else len(w) / sr for w in wavs_of(m))
             if cur and sec + s > self.batch_seconds:
                 yield cur
                 cur, sec = [], 0.0

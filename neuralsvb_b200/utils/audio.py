@@ -1,8 +1,14 @@
 """Host helpers of the wav -> mel front end (reference: utils/audio.py:57-117 and the call
 sites of librosa.filters.mel in data_gen/tts/data_gen_utils.py:130, modules/hifigan/mel_utils.py:62).
 The STFT / magnitude / mel projection / log themselves run in the fused CUDA kernel
-(csrc/frontend.cu); what stays on the host is the constant mel filterbank and index arithmetic."""
+(csrc/frontend.cu); what stays on the host is the constant mel filterbank and index arithmetic.
+
+Loading audio (``load_wav``, ``resample_batch``): the reference's ``librosa.core.load(path, sr=sr)`` for WAV files -- decode,
+fold to mono, resample with resampy's ``kaiser_best`` filter -- with the resampling in csrc/resample.cu (oracle/resample.py
+states the algorithm)."""
+import ctypes
 import functools
+import struct
 
 import numpy as np
 
@@ -76,3 +82,130 @@ def save_wav(wav, path, sr, norm=False):
     if norm:
         wav = wav / np.abs(wav).max()
     wavfile.write(path, sr, (wav * np.float32(32767)).astype(np.int16))
+
+
+KAISER_BEST = dict(num_zeros=64, precision=9, beta=14.769656459379492, rolloff=0.9475937167399596)
+
+
+@functools.lru_cache(maxsize=1)
+def kaiser_best_window():
+    """(win float64 [32769], num_table 512): resampy's ``sinc_window`` right wing for ``kaiser_best``, rebuilt from its
+    construction (resampy 0.2.2 ships it precomputed; bit agreement with that file has not been checked)."""
+    from scipy.signal.windows import kaiser
+    p = KAISER_BEST
+    num_bits = 2 ** p['precision']
+    n = num_bits * p['num_zeros']
+    sinc_win = p['rolloff'] * np.sinc(p['rolloff'] * np.linspace(0, p['num_zeros'], num=n + 1, endpoint=True))
+    win = np.ascontiguousarray(kaiser(2 * n + 1, p['beta'])[n:] * sinc_win)
+    win.setflags(write=False)
+    return win, num_bits
+
+
+def wav_info(path):
+    """(sample rate, frames, channels) from a WAV file's header, without reading its samples."""
+    with open(path, 'rb') as f:
+        riff = f.read(12)
+        if len(riff) < 12 or riff[:4] != b'RIFF' or riff[8:12] != b'WAVE':
+            raise ValueError(f'{path}: not a RIFF/WAVE file')
+        fmt = None
+        while True:
+            head = f.read(8)
+            if len(head) < 8:
+                raise ValueError(f'{path}: no data chunk')
+            cid, size = head[:4], struct.unpack('<I', head[4:])[0]
+            if cid == b'fmt ':
+                body = f.read(size + (size & 1))
+                channels, sr = struct.unpack('<HI', body[2:8])
+                block_align = struct.unpack('<H', body[12:14])[0]
+                fmt = (sr, channels, block_align)
+            elif cid == b'data':
+                if fmt is None:
+                    raise ValueError(f'{path}: data chunk before fmt chunk')
+                return fmt[0], size // fmt[2], fmt[1]
+            else:
+                f.seek(size + (size & 1), 1)
+
+
+def wav_seconds(path):
+    """Duration of a WAV file in seconds, from its header."""
+    sr, frames, _ = wav_info(path)
+    return frames / sr
+
+
+def read_wav(path):
+    """(float32 mono samples, file rate) of a WAV file, decoded as ``librosa.load`` documents: integer PCM / 2^(bits - 1) (scipy
+    returns 24-bit as left-justified int32), uint8 as (x - 128) / 128, float as is; channels averaged in float32."""
+    from scipy.io import wavfile
+    sr, data = wavfile.read(path)
+    if data.dtype.kind == 'i':
+        data = data.astype(np.float32) / float(np.iinfo(data.dtype).max + 1)
+    elif data.dtype.kind == 'u':
+        data = (data.astype(np.float32) - 128.0) / 128.0
+    data = data.astype(np.float32)
+    if data.ndim > 1:
+        data = data.mean(axis=1)
+    return data, int(sr)
+
+
+def _resample_args(orig_srs, lengths):
+    srs = np.ascontiguousarray(orig_srs, dtype=np.int32)
+    lens = np.ascontiguousarray(lengths, dtype=np.int64)
+    if srs.shape != lens.shape:
+        raise ValueError(f'{len(srs)} sample rates for {len(lens)} clips')
+    return srs, lens
+
+
+def resample_lengths(lengths, orig_srs, target_sr):
+    """(before, after) padding: int(n ratio) and ceil(n ratio) samples per clip (n itself at the target rate).  Raises ValueError for a
+    clip that yields no sample or a bad rate.  No CUDA call."""
+    from neuralsvb_b200 import _native
+    srs, lens = _resample_args(orig_srs, lengths)
+    win, num_table = kaiser_best_window()
+    res, out = np.zeros(len(lens), np.int64), np.zeros(len(lens), np.int64)
+    if _native.lib().svb_resample_plan(int(target_sr), srs.ctypes.data_as(ctypes.c_void_p), lens.ctypes.data_as(ctypes.c_void_p),
+                                       len(lens), len(win), num_table, res.ctypes.data_as(ctypes.c_void_p),
+                                       out.ctypes.data_as(ctypes.c_void_p)) < 0:
+        raise ValueError(_native.lib().svb_last_error().decode('utf-8', 'replace'))
+    return res, out
+
+
+def resample_batch(wavs, orig_srs, target_sr):
+    """Resample each float32 clip from its own rate to ``target_sr`` with resampy's kaiser_best filter, zero-padded to
+    ceil(n target_sr / sr) samples like ``librosa.resample(..., fix=True)``: ONE device call over the ragged batch
+    (svb_resample_batch_host).  A clip already at target_sr comes back unchanged.  Raises ValueError for a clip too short to
+    yield a sample or a bad rate."""
+    import torch
+
+    from neuralsvb_b200 import _native
+    wavs = [np.ascontiguousarray(w, dtype=np.float32) for w in wavs]
+    if not wavs:
+        return []
+    if any(w.ndim != 1 for w in wavs):
+        raise ValueError('resample_batch takes 1-D (mono) clips')
+    srs, lens = _resample_args(orig_srs, [len(w) for w in wavs])
+    _, out_lens = resample_lengths(lens, srs, target_sr)
+    if not torch.cuda.is_available():
+        raise RuntimeError('resample_batch runs on CUDA: neuralsvb_b200 has no CPU fallback')
+    device = torch.device('cuda', torch.cuda.current_device())
+    win, num_table = kaiser_best_window()
+    cat = np.ascontiguousarray(np.concatenate(wavs))
+    out = np.empty(max(int(out_lens.sum()), 1), np.float32)
+    lib = _native.lib()
+    with torch.cuda.device(device):
+        _native.check(lib.svb_resample_batch_host(int(target_sr), srs.ctypes.data_as(ctypes.c_void_p), lens.ctypes.data_as(ctypes.c_void_p),
+                                                  len(wavs), win.ctypes.data_as(ctypes.c_void_p), len(win), num_table,
+                                                  cat.ctypes.data_as(ctypes.c_void_p), out.ctypes.data_as(ctypes.c_void_p),
+                                                  device.index, _native.current_stream_ptr(device)), 'resample')
+    res, o = [], 0
+    for w, sr, n in zip(wavs, srs, out_lens):
+        res.append(w if int(sr) == int(target_sr) else out[o:o + int(n)].copy())
+        o += int(n)
+    return res
+
+
+def load_wav(path, sr=22050):
+    """``librosa.core.load(path, sr=sr)`` for a WAV file: (float32 mono samples at ``sr``, sr); ``sr=None`` keeps the file's rate."""
+    data, file_sr = read_wav(path)
+    if sr is None or file_sr == sr:
+        return data, file_sr
+    return resample_batch([data], [file_sr], sr)[0], sr

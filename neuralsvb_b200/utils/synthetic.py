@@ -643,9 +643,10 @@ def make_sung_take(f0_frames, seed, sr=22050, hop=128, breath=True):
     return np.clip(wav, -1, 1).astype(np.float32), f0
 
 
-def write_svb_raw(processed_dir, binary_data_dir=None, seed=1234, sr=22050, hop=128, seconds=(1.5, 3.0), gap_frames=None):
+def write_svb_raw(processed_dir, binary_data_dir=None, seed=1234, sr=22050, hop=128, seconds=(1.5, 3.0), gap_frames=None,
+                  file_sr=None, channels=1, sample_format='int16'):
     """Write a raw paired-singing set in PopBuTFy's layout, for the paired binarizer (egs/svb_binarize_synthetic.yaml):
-    ``{processed_dir}/data/{spk}#singing#{song}/{spk}#singing#{song}_{Amateur|Professional}_{k}.wav`` (16-bit WAV at sr),
+    ``{processed_dir}/data/{spk}#singing#{song}/{spk}#singing#{song}_{Amateur|Professional}_{k}.wav`` (16-bit mono WAV at sr),
     ``{processed_dir}/spk_emb/{item_name}.npy`` (256-d, one per amateur take) and ``{processed_dir}/phone_set.json``.
 
     Three speakers (Female1, Female2, Male1) sing two songs in two pieces each; each pair is ``make_f0_pair``'s two takes through
@@ -654,20 +655,32 @@ def write_svb_raw(processed_dir, binary_data_dir=None, seed=1234, sr=22050, hop=
     has no professional take; ``Female1#speech#Talk_Amateur_0`` is not singing.  With ``binary_data_dir``, phone_set.json and the
     checkpoints of ``write_svb_checkpoints`` are written there too.
 
-    Returns {item_name: true f0 per sample (float64, 0 = unvoiced)} for every file written."""
+    ``sr`` / ``hop`` are the model's rate and hop (the f0 contours have sr / hop frames per second).  The files are recorded at
+    ``file_sr`` (default sr; the takes are synthesised at that rate, round(hop file_sr / sr) samples per contour frame) with
+    ``channels`` channels (channel c is the take times 1 - 0.2 c) as ``sample_format`` 'int16' or 'float32' samples.
+
+    Returns {item_name: true f0 per sample of the file (float64, 0 = unvoiced)} for every file written."""
     import json
     import os
 
     from scipy.io import wavfile
+    if sample_format not in ('int16', 'float32') or channels < 1:
+        raise ValueError(f'write_svb_raw writes int16 or float32 samples on 1 or more channels, not {sample_format} x {channels}')
     rs = np.random.RandomState(seed + 79)
     fps = sr / hop
+    file_sr = sr if file_sr is None else int(file_sr)
+    file_hop = hop if file_sr == sr else int(round(hop * file_sr / sr))
     gap_frames = 240 if gap_frames is None else gap_frames
     truth = {}
 
     def write(name, wav, f0):
         d = os.path.join(processed_dir, 'data', name.rsplit('_', 2)[0])
         os.makedirs(d, exist_ok=True)
-        wavfile.write(os.path.join(d, name + '.wav'), sr, np.round(np.clip(wav, -1, 1) * 32767).astype(np.int16))
+        wav = np.clip(wav, -1, 1)
+        if channels > 1:
+            wav = np.stack([wav * np.float32(1 - 0.2 * c) for c in range(channels)], axis=1)
+        data = np.round(wav * 32767).astype(np.int16) if sample_format == 'int16' else wav.astype(np.float32)
+        wavfile.write(os.path.join(d, name + '.wav'), file_sr, data)
         truth[name] = f0
 
     emb_dir = os.path.join(processed_dir, 'spk_emb')
@@ -683,16 +696,16 @@ def write_svb_raw(processed_dir, binary_data_dir=None, seed=1234, sr=22050, hop=
                 T = S + gap_frames if ama == 'Female2#singing#Song_B_Amateur_1' else int(S * rs.uniform(0.85, 1.15))
                 fa, fp = make_f0_pair(int(rs.randint(0, 2 ** 31 - 1)), S, T, fps)
                 fa, fp = fa * 2 ** (shift / 12), fp * 2 ** (shift / 12)
-                wa, ta = make_sung_take(fa, int(rs.randint(0, 2 ** 31 - 1)), sr, hop)
+                wa, ta = make_sung_take(fa, int(rs.randint(0, 2 ** 31 - 1)), file_sr, file_hop)
                 if ama == 'Male1#singing#Song_A_Amateur_1':
                     wa, ta = np.zeros_like(wa), np.zeros_like(ta)
                 write(ama, wa, ta)
                 np.save(os.path.join(emb_dir, ama + '.npy'), _normal(rs, (256,), 0.5))
                 if song != 'Song_C':
-                    wp, tp = make_sung_take(fp, int(rs.randint(0, 2 ** 31 - 1)), sr, hop)
+                    wp, tp = make_sung_take(fp, int(rs.randint(0, 2 ** 31 - 1)), file_sr, file_hop)
                     write(prof, wp, tp)
     f0, _ = make_f0_pair(int(rs.randint(0, 2 ** 31 - 1)), int(2 * fps), int(2 * fps), fps)
-    w, t = make_sung_take(f0, int(rs.randint(0, 2 ** 31 - 1)), sr, hop)
+    w, t = make_sung_take(f0, int(rs.randint(0, 2 ** 31 - 1)), file_sr, file_hop)
     write('Female1#speech#Talk_Amateur_0', w, t)
     phones = [f'ph{i}' for i in range(60)]
     for d in [processed_dir] + ([binary_data_dir] if binary_data_dir else []):

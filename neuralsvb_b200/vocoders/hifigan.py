@@ -60,19 +60,26 @@ def stft_config(hp, pad_mode, out_kind, eps, frames_major=1, clamp=0):
 
 
 def _load_wav(wav_fn, sr):
-    from scipy.io import wavfile
-    file_sr, data = wavfile.read(wav_fn)
-    if data.dtype.kind == 'i':
-        data = data.astype(np.float32) / float(np.iinfo(data.dtype).max + 1)
-    elif data.dtype.kind == 'u':
-        data = (data.astype(np.float32) - 128.0) / 128.0
-    data = data.astype(np.float32)
-    if data.ndim > 1:
-        data = data.mean(axis=1)
-    if file_sr != sr:
-        raise ValueError(f'{wav_fn}: sample rate {file_sr} != audio_sample_rate {sr}; resampling '
-                         '(librosa.core.load in the reference) is data preparation, outside this path')
-    return data
+    """librosa.core.load(wav_fn, sr=sr) for a WAV file (utils/audio.load_wav): decoded, mono, resampled on the GPU when the file's
+    rate is not sr."""
+    return audio.load_wav(wav_fn, sr)[0]
+
+
+def _load_wavs(wav_fns, sr):
+    """Decode every path (arrays are taken to be at sr already), then resample all off-rate files in ONE device call."""
+    wavs, rates = [], []
+    for w in wav_fns:
+        if isinstance(w, str):
+            data, file_sr = audio.read_wav(w)
+        else:
+            data, file_sr = np.ascontiguousarray(w, dtype=np.float32), sr
+        wavs.append(data)
+        rates.append(file_sr)
+    off = [i for i, r in enumerate(rates) if r != sr]
+    if off:
+        for i, y in zip(off, audio.resample_batch([wavs[i] for i in off], [rates[i] for i in off], sr)):
+            wavs[i] = y
+    return wavs
 
 
 @register_vocoder
@@ -155,13 +162,13 @@ class HifiGAN(BaseVocoder):
         """The binarizer's per-file ``wav2spec`` loop (data_gen/tts/base_binarizer.py:168-178,
         data_gen/singing/binarize_para.py:116-217) as ONE device call over a ragged batch: list of paths / float arrays
         -> list of (wav [T*hop], mel [T, n_mel] log10), identical to ``wav2spec`` clip by clip
-        (svb_wav2spec_batch_host: one H2D, one launch over all frames of all clips, one D2H)."""
+        (svb_wav2spec_batch_host: one H2D, one launch over all frames of all clips, one D2H).  Files at another rate than
+        audio_sample_rate are first resampled together in one ``audio.resample_batch`` call."""
         hp = hparams if hp is None else hp
         device = _require_cuda()
         if hp.get('loud_norm', False):
             raise NotImplementedError('loud_norm (pyloudnorm BS.1770) is data preparation, outside this path')
-        wavs = [_load_wav(w, hp['audio_sample_rate']) if isinstance(w, str) else np.ascontiguousarray(w, dtype=np.float32)
-                for w in wav_fns]
+        wavs = _load_wavs(wav_fns, hp['audio_sample_rate'])
         if not wavs:
             return []
         lib = _native.lib()
@@ -191,7 +198,8 @@ class HifiGAN(BaseVocoder):
 
     @staticmethod
     def wav2spec(wav_fn, return_linear=False, hp=None):
-        """wav file path (same sample rate) or float array -> (wav [T*hop], mel [T, n_mel] log10)
+        """wav file path (any sample rate: resampled like librosa.core.load) or float array at audio_sample_rate ->
+        (wav [T*hop], mel [T, n_mel] log10)
         [+ normalised dB linear spectrogram [T, n_fft/2+1]]   (vocoders/pwg.py:105-122)."""
         hp = hparams if hp is None else hp
         device = _require_cuda()
