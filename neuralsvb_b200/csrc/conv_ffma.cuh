@@ -32,6 +32,8 @@ struct ConvArgs {
                           // (block nblk reads channels [nblk*cin_blk, (nblk+1)*cin_blk)); 0 = dense (all Cin)
     int epi_stream = 1;   // tensor-core kernel: residual / running sum bulk-copied into shared memory during the MMAs where
                           // the plan has room (conv_tc.cu); 0 = per-thread loads in the epilogue
+    int fused_ctas = 0;   // fused tensor-core launches of C = 32: 1 = one CTA per SM; otherwise two where the layout and the
+                          // batch allow them (conv_tc.cu: tc_fused_ctas)
 };
 
 int launch_conv_ffma(const ConvArgs &a, cudaStream_t st);

@@ -89,6 +89,10 @@ constexpr int kTcThreadsP = 384;
 constexpr int kWarpProducer = 0, kWarpTransform0 = 1, kWarpMath0 = 4;
 constexpr int kMathWarps = 8, kTransformWarps = 3;
 constexpr int kTrRows = kTransformWarps * 32 / 8;   // rows one pass of the transform warps covers (8 lanes per row)
+// CTAs per SM the kernel is compiled for.  The fused 32-column kernel runs two (80 registers per thread): its per-item
+// chain (c1 MMAs, c1 epilogue into the intermediate, two named barriers, c2 MMAs, c2 epilogue) leaves the tensor pipe
+// idle outside the MMAs, and the other CTA's MMAs fill those phases.  Every other kernel uses 113-168 registers.
+__host__ __device__ constexpr int tc_min_ctas(int n, bool fused) { return fused && n == 32 ? 2 : 1; }
 constexpr int kBiasBytes = 4096;        // bias of the layer(s) (<= 1024 floats; wider layers take 12 KB)
 
 static_assert(512 + 2 * kTcMaxLayers * sizeof(TcLayer) <= 1024, "the layer table lives in smem bytes 512 .. 1023");
@@ -107,13 +111,16 @@ __host__ __device__ inline void tc_fused_slab(int t0, int h1, int h2, int in_Tp,
     *rows = min(2 * kTcM + 2 * h1, in_Tp - *row0);
 }
 
-// a work item, as staged in shared memory: x = layer | column block << 8 | tiles << 24, y = clip, z = first row
+// a work item, as staged in shared memory: x = layer | column block << 8 | tiles << 24, y = clip, z = first row.  Fused
+// items are always two tiles of the launch's only column block (tc_plan_fused): constants, not registers.
 struct TcItem {
     int layer, nblk, mt, b, t0;
 };
+template <bool FUSED>
 __device__ __forceinline__ TcItem item_decode(const int4 v) {
     TcItem it;
-    it.layer = v.x & 0xff, it.nblk = (v.x >> 8) & 0xffff, it.mt = v.x >> 24, it.b = v.y, it.t0 = v.z;
+    it.layer = v.x & 0xff, it.b = v.y, it.t0 = v.z;
+    it.nblk = FUSED ? 0 : (v.x >> 8) & 0xffff, it.mt = FUSED ? 2 : v.x >> 24;
     return it;
 }
 
@@ -172,7 +179,7 @@ __device__ __forceinline__ float pick4(int j, float v0, float v1, float v2, floa
 // and the intermediate holds the same values c2's transform makes from c1's exact fp32 output: the results are
 // bit-identical.
 template <int MODE, int N, bool FUSED>
-__global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __grid_constant__ TcArgs p) {
+__global__ void __launch_bounds__(kTcThreadsP, tc_min_ctas(N, FUSED)) conv1d_c4_tc_kernel(const __grid_constant__ TcArgs p) {
     extern __shared__ __align__(1024) unsigned char smem[];
     constexpr bool BF = MODE == SVB_PREC_BF16X3;
     constexpr bool X3 = MODE == SVB_PREC_TF32X3;
@@ -245,7 +252,7 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
                     bulk_g2s(wring + Ls[l].w_res_off, Ls[l].w, (uint32_t)Ls[l].KS * p.wtile_bytes, w_full);
             }
             for (int n = 0; n < n_items; ++n) {
-                const TcItem it = item_decode(items[n]);
+                const TcItem it = item_decode<FUSED>(items[n]);
                 const TcLayer &L = Ls[it.layer];
                 const int halo = (L.KS - 1) / 2 * L.dil;
                 uint32_t raw_bytes = (uint32_t)(it.mt * kTcM + 2 * halo) * 128;
@@ -310,7 +317,7 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
         const float slope = a.in_slope;                         // 0 <= slope <= 1: lrelu(x) = max(x, slope * x)
         int sA = 0, phA = 0;
         for (int n = 0; n < n_items; ++n) {
-            const TcItem it = item_decode(items[n]);
+            const TcItem it = item_decode<FUSED>(items[n]);
             const int R = it.mt * kTcM + (Ls[it.layer].KS - 1) / 2 * Ls[it.layer].dil * 2;
             for (int c = 0; c < p.n_chunks; ++c) {
                 mbar_wait(raw_full + sA, phA);
@@ -396,10 +403,19 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
         const uint32_t op_base = desc_lo(smem_u32(op0)) + (uint32_t)wg * ((64 * 128) >> 4), w_base = desc_lo(smem_u32(wring));
         const uint32_t op_step = p.op_bytes >> 4, wtile_step = p.wtile_bytes >> 4;
         constexpr uint32_t tile_step = (kTcM * 128) >> 4;                  // the second tile of an item starts 128 rows on
-        const int gout = c4t_groups(a.Cout);
+        const int cout = FUSED ? N : a.Cout, gout = FUSED ? N / 32 : c4t_groups(a.Cout);     // fused launches: Cout = N
         const int r_lo = 64 * wg + 16 * (warp & 3) + (lane >> 2);           // first accumulator row of this thread
         const int c_lo = 2 * (lane & 3);                                    // first accumulator column of this thread
         float acc0[N / 2], acc1[N / 2];                                     // blocks wg and wg + 2
+        // The first MMA of an item overwrites the accumulators (scale 0), but wgmma operands are read-write, so the compiler
+        // keeps the previous item's values live through the whole epilogue.  The two-CTA kernel (80 registers) zeroes them
+        // before that MMA instead: a block's registers are free as soon as its epilogue has read them.
+        auto acc_clear = [&]() {
+            if constexpr (tc_min_ctas(N, FUSED) == 2) {
+#pragma unroll
+                for (int i = 0; i < N / 2; ++i) acc0[i] = 0.f, acc1[i] = 0.f;
+            }
+        };
         int sA = 0, phA = 0, sW = 0, phW = 0;
         int pend_w = -1, pend_a = -1;                                       // slots read by the wgmma group in flight
         auto release = [&]() {
@@ -427,10 +443,11 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
                 for (int j = 0; j < N / 8; ++j) {
                     const int cop = it.nblk * N + 8 * j + c_lo;             // a column pair never straddles an upsampler phase
                     int phi = 0, co = cop;
-                    if (a.ups_u > 0) phi = cop / a.Cout, co = cop - phi * a.Cout;
+                    const bool ups = !FUSED && a.ups_u > 0;                 // fused launches never upsample
+                    if (ups) phi = cop / a.Cout, co = cop - phi * a.Cout;
                     const size_t idx = (((size_t)it.b * gout + (co >> 5)) * a.out_Tp + kPad +
-                                        (a.ups_u > 0 ? (size_t)q * a.ups_u + phi : (size_t)q)) * 32 + (co & 31);
-                    const float b0 = co < a.Cout ? bias_s[co] : 0.f, b1 = co + 1 < a.Cout ? bias_s[co + 1] : 0.f;
+                                        (ups ? (size_t)q * a.ups_u + phi : (size_t)q)) * 32 + (co & 31);
+                    const float b0 = co < cout ? bias_s[co] : 0.f, b1 = co + 1 < cout ? bias_s[co + 1] : 0.f;
                     float2 o = make_float2(acc[4 * j + 2 * h] + b0, acc[4 * j + 2 * h + 1] + b1);
                     if (res) {
                         const float2 rv = __ldg(reinterpret_cast<const float2 *>(res + idx));
@@ -471,9 +488,10 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
             return nb * (N / 32) * ((L.res != nullptr) + L.accumulate);
         };
         auto epi_issue = [&](const TcItem &it, const TcLayer &L, int k, int slot) {      // lane 0
-            const int nsrc = (L.res != nullptr) + L.accumulate, per_blk = (N / 32) * nsrc;
-            const int blk = k / per_blk, r = k - blk * per_blk, g = r / nsrc;
-            const bool old = L.res == nullptr || r - g * nsrc == 1;
+            // 1 or 2 sources and 1 or 2 groups per block: shifts, not divisions (few registers at the refill inside the epilogue)
+            const int lg_src = L.res != nullptr && L.accumulate, lg_blk = lg_src + (N == 64);
+            const int blk = k >> lg_blk, r = k - (blk << lg_blk), g = r >> lg_src;
+            const bool old = L.res == nullptr || r - (g << lg_src) == 1;
             const uint32_t bytes = (uint32_t)piece_rows(it, blk) * 128;
             const float *src = (old ? L.out : L.res) + (((size_t)it.b * gout + it.nblk * (N / 32) + g) * a.out_Tp + kPad + it.t0 +
                                                         kTcM * blk + 64 * wg + 16 * (warp & 3)) * 32;
@@ -527,7 +545,7 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
                         const int jj = (u + rq) & 3, c = 8 * jj + c_lo, co = cg + c;
                         const float *ap = acc + 16 * g + 2 * h;
                         const float x0 = pick4(jj, ap[0], ap[4], ap[8], ap[12]), x1 = pick4(jj, ap[1], ap[5], ap[9], ap[13]);
-                        const float b0 = co < a.Cout ? bias_s[co] : 0.f, b1 = co + 1 < a.Cout ? bias_s[co + 1] : 0.f;
+                        const float b0 = co < cout ? bias_s[co] : 0.f, b1 = co + 1 < cout ? bias_s[co + 1] : 0.f;
                         float2 o = make_float2(__fadd_rn(x0, b0), __fadd_rn(x1, b1));
                         if (has_res) {
                             const float2 rv = *reinterpret_cast<const float2 *>(rs + r * 32 + c);
@@ -558,6 +576,7 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
             const int KS = L.KS;
             const uint32_t tap_step = (uint32_t)L.dil * (128 >> 4);       // a tap is a row shift of the operand
             uint32_t scale = 0;                                             // first MMA of the item overwrites
+            acc_clear();
             for (int c = 0; c < p.n_chunks; ++c) {
                 mbar_wait(a_ready + sA, phA);
                 uint32_t a_tap = op_base + sA * op_step;
@@ -656,6 +675,7 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
             const uint32_t inter_lo_plane = (X3 ? p.inter_bytes / 2 : 64u) >> 4;
             const uint32_t inter_base = desc_lo(smem_u32(inter)) + (uint32_t)wg * ((64 * 128) >> 4);
             uint32_t scale = 0;
+            acc_clear();
             for (int c = 0; c < p.n_chunks; ++c) {
                 uint32_t a_tap = inter_base + (uint32_t)c * (p.inter_bytes >> 4);
                 for (int k = 0; k < L2.KS; ++k) {
@@ -681,7 +701,7 @@ __global__ void __launch_bounds__(kTcThreadsP, 1) conv1d_c4_tc_kernel(const __gr
         };
         if (p.w_resident && n_items > 0) mbar_wait(w_full, 0);
         for (int n = 0; n < n_items; ++n) {
-            const TcItem it = item_decode(items[n]);
+            const TcItem it = item_decode<FUSED>(items[n]);
             if constexpr (FUSED) run_fused(it);
             else if (it.mt == 2) run_item(std::true_type(), it);
             else run_item(std::false_type(), it);
@@ -822,13 +842,18 @@ bool tc_supported(const TcWeights &w, const ConvArgs &a) {
            (a.ups_u == 0 || a.Cout % 32 == 0) && a.Cout <= 3072;
 }
 
+// The dynamic shared-memory limit set on each device for one kernel instantiation.  Every caller that raises it (launches,
+// the occupancy query of the fused plans) goes through this one cache, so the limit only ever rises: a launch of a larger
+// plan never finds it lowered by a query for a smaller one.
+template <int MODE, int N, bool FUSED>
+size_t tc_smem_configured[kSmemCacheDevices] = {};
+
 template <int MODE, int N, bool FUSED>
 static int launch_mode(const TcArgs &p, int grid, size_t smem, cudaStream_t st) {
     auto kern = conv1d_c4_tc_kernel<MODE, N, FUSED>;
     // function attributes are per device: one process may drive several GPUs (the reference's mp.spawn gives one each,
     // but nothing in the C ABI forbids a handle per device in one process)
-    static size_t configured[kSmemCacheDevices] = {};
-    SVB_TRY(raise_smem_limit(kern, smem, configured, 0));      // sets the exact size on first use, also below 48 KB
+    SVB_TRY(raise_smem_limit(kern, smem, tc_smem_configured<MODE, N, FUSED>, 0));   // exact size on first use, also below 48 KB
     static bool carve[kMaxDevices] = {};
     int dev = 0;
     SVB_CUDA(cudaGetDevice(&dev));
@@ -1015,8 +1040,12 @@ static int tc_plan(int n, const TcWeights *const *w, const ConvArgs *a, int prec
 // Plan of a fused launch over n ResBlock chains: a[0..n) are the c1 layers, a[n..2n) the c2 layers of the same step.
 // Every item is 256 c1 rows; the c1 slab slots, the intermediate (256 + 2 max h2 rows per 32-channel chunk), a weight
 // ring of at least 2 tiles (c1's and c2's tiles stream through it in order) and the biases of all 2n layers share the
-// shared memory.  Returns false when the shape is not one a fused launch runs or the layout does not fit.
-static bool tc_plan_fused(int n, const TcWeights *const *w, const ConvArgs *a, int precision, TcArgs &p, size_t &smem) {
+// shared memory.  ctas = 1: up to 227 KB, three slab slots.  ctas = 2 (C = 32 only, the kernel compiled for two CTAs
+// per SM): half of the SM's 228 KB less the 1 KB each CTA reserves, so one slab slot (the next item's slab is copied and
+// transformed while this item runs c1's epilogue and c2; the other CTA's MMAs cover the rest) and a bias area of just
+// the 2n layers' biases.  Returns false when the shape is not one a fused launch runs or the layout does not fit.
+constexpr size_t kSmemPerSm = 228 * 1024, kSmemReservedPerCta = 1024;
+static bool tc_plan_fused(int n, const TcWeights *const *w, const ConvArgs *a, int precision, int ctas, TcArgs &p, size_t &smem) {
     if (n < 1 || n > kTcMaxLayers) return false;
     const ConvArgs &a0 = a[0];
     for (int l = 0; l < 2 * n; ++l) {
@@ -1025,7 +1054,7 @@ static bool tc_plan_fused(int n, const TcWeights *const *w, const ConvArgs *a, i
             a[l].in_slope != a0.in_slope || !w[l]->ok || w[l]->n_tile != a0.Cin || (l >= n && a[l].dil != 1))
             return false;
     }
-    if (a0.Cin != 32 && a0.Cin != 64) return false;
+    if ((a0.Cin != 32 && a0.Cin != 64) || (ctas != 1 && ctas != tc_min_ctas(a0.Cin, true))) return false;
     const int planes = precision == SVB_PREC_TF32X3 ? 2 : 1;
     int h1 = 0, h2 = 0;
     for (int l = 0; l < n; ++l) h1 = std::max(h1, (a[l].KS - 1) / 2 * a[l].dil), h2 = std::max(h2, (a[n + l].KS - 1) / 2);
@@ -1040,14 +1069,16 @@ static bool tc_plan_fused(int n, const TcWeights *const *w, const ConvArgs *a, i
     p.fused_P = 2 * kTcM - 2 * h2;
     p.op_bytes = (uint32_t)round_up(2 * kTcM + 2 * h1, 8) * 128 * planes;
     p.inter_bytes = (uint32_t)round_up(2 * kTcM + 2 * h2, 8) * 128 * planes;
-    const size_t bias_bytes = kBiasBytes;                       // 2n x Cout <= 6 x 64 floats
-    const size_t budget = 227 * 1024 - bias_bytes;
-    int nA_pref = 3;
-    if (const char *e = getenv("SVB_TC_NA")) nA_pref = std::max(2, std::min(4, atoi(e)));
+    // 2n x Cout <= 6 x 64 floats
+    const size_t bias_bytes = ctas == 1 ? kBiasBytes : (size_t)round_up(2 * n * a0.Cout * 4, 128);
+    const size_t smem_max = ctas == 1 ? 227 * 1024 : kSmemPerSm / 2 - kSmemReservedPerCta;
+    const size_t budget = smem_max - bias_bytes;
+    int nA_pref = ctas == 1 ? 3 : 1;
+    if (const char *e = getenv("SVB_TC_NA"); e && ctas == 1) nA_pref = std::max(2, std::min(4, atoi(e)));
     p.off_op = 1024 + kItemBytes;
     const size_t inter_area = (size_t)p.n_chunks * p.inter_bytes;
     p.nA = nA_pref;
-    if (p.off_op + (size_t)p.nA * p.op_bytes + inter_area + 2 * (size_t)p.wtile_bytes > budget) p.nA = 2;
+    if (p.off_op + (size_t)p.nA * p.op_bytes + inter_area + 2 * (size_t)p.wtile_bytes > budget) p.nA = std::min(p.nA, 2);
     if (p.off_op + (size_t)p.nA * p.op_bytes + inter_area + 2 * (size_t)p.wtile_bytes > budget) return false;
     // the piece ring of the streamed epilogue (c2's residual / running sum) comes out of the weight ring; where it does not
     // fit next to 3 slab slots (C = 64 at k 11, d 5), the plan drops to 2 slots for it
@@ -1062,11 +1093,12 @@ static bool tc_plan_fused(int n, const TcWeights *const *w, const ConvArgs *a, i
     };
     const int nA = p.nA;
     if (!pieces || !(layout(nA, true) || (nA > 2 && layout(2, true)))) layout(nA, false);
+    if (const char *e = getenv("SVB_TC_NW")) p.nW = std::min(p.nW, std::max(2, atoi(e)));      // ring depth (measurement)
     p.l2_prefetch = p.epi_slots == 0 && tc_epi_sources(n, a + n) > 0;
     p.off_epi = p.off_w + (uint32_t)round_up(p.nW * (int)p.wtile_bytes, 1024);
     p.off_bias = p.off_epi + (uint32_t)p.epi_slots * kMathWarps * kEpiPieceBytes;
     smem = (size_t)p.off_bias + bias_bytes;
-    if (smem > 227 * 1024) return false;
+    if (smem > smem_max) return false;
     for (int l = 0; l < 2 * n; ++l) {
         TcLayer &L = p.L[l];
         L.in = a[l].in, L.res = a[l].res, L.out = a[l].out, L.bias = a[l].bias;
@@ -1258,23 +1290,48 @@ int tc_schedule(int n, const int *KS, const int *KS2, const int *has_res, const 
     return SVB_OK;
 }
 
-// plan of a merged (fused = false: n layers) or fused (n chains, 2n layers) launch
-static int tc_plan_multi(int n, const TcWeights *const *w, const ConvArgs *a, int precision, bool fused, TcArgs &p, size_t &smem) {
+// plan of a merged (fused = false: n layers) or fused (n chains, 2n layers, `ctas` per SM) launch
+static int tc_plan_multi(int n, const TcWeights *const *w, const ConvArgs *a, int precision, bool fused, int ctas, TcArgs &p,
+                         size_t &smem) {
     if (!fused) return tc_plan(n, w, a, precision, 0, p, smem);
-    SVB_CHECK(tc_plan_fused(n, w, a, precision, p, smem), SVB_ERR_INVALID, "tc conv: no fused layout for %d chains of C = %d", n, a[0].Cin);
+    SVB_CHECK(tc_plan_fused(n, w, a, precision, ctas, p, smem), SVB_ERR_INVALID, "tc conv: no fused layout for %d chains of C = %d",
+              n, a[0].Cin);
     return SVB_OK;
 }
 
-// Fused launches over the n chains of a step (c1 layers a[0..n), c2 layers a[n..2n)): the layout fits shared memory,
-// there are at least 4 items per CTA (fused items are never split, so fewer leave SMs idle where the two-launch path
-// balances with one-tile items), and both work lists of a stage (plain and chain-ordered) fit the per-CTA item table.
-// Bounds of the LPT schedule: a CTA's load ends at most one unit above the mean, so it holds at most
-// (mean + max cost) / min cost units.
-bool tc_fused_fits(int n, const TcWeights *const *w, const ConvArgs *a, int precision) {
+// CTAs of the fused kernel that fit one SM at `smem` bytes (the runtime's occupancy calculator: registers, threads, shared
+// memory and the per-CTA reservation of this device)
+template <int MODE, int N>
+static int tc_fused_occupancy(size_t smem) {
+    auto kern = conv1d_c4_tc_kernel<MODE, N, true>;
+    if (raise_smem_limit(kern, smem, tc_smem_configured<MODE, N, true>, 0) != SVB_OK) return 0;
+    int blocks = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, kern, kTcThreadsP, smem) != cudaSuccess) {
+        cudaGetLastError();
+        return 0;
+    }
+    return blocks;
+}
+
+// Fused launches over the n chains of a step with `ctas` CTAs per SM (c1 layers a[0..n), c2 layers a[n..2n)): the layout
+// fits shared memory and that many CTAs fit an SM, there are at least 4 items per CTA (fused items are never split, so
+// fewer leave SMs idle where the two-launch path balances with one-tile items), and both work lists of a stage (plain and
+// chain-ordered) fit the per-CTA item table.  Bounds of the LPT schedule: a CTA's load ends at most one unit above the
+// mean, so it holds at most (mean + max cost) / min cost units.
+static bool tc_fused_fits_ctas(int n, const TcWeights *const *w, const ConvArgs *a, int precision, int ctas) {
     TcArgs p;
     size_t smem = 0;
-    if (!tc_plan_fused(n, w, a, precision, p, smem)) return false;
-    const int grid = sm_count();
+    if (!tc_plan_fused(n, w, a, precision, ctas, p, smem)) return false;
+    if (ctas > 1) {
+        int fit = 0;
+        switch (precision) {
+            case SVB_PREC_TF32: fit = tc_fused_occupancy<SVB_PREC_TF32, 32>(smem); break;
+            case SVB_PREC_TF32X3: fit = tc_fused_occupancy<SVB_PREC_TF32X3, 32>(smem); break;
+            default: fit = tc_fused_occupancy<SVB_PREC_BF16X3, 32>(smem); break;
+        }
+        if (fit < ctas) return false;
+    }
+    const int grid = ctas * sm_count();
     const double units = (double)a[0].B * p.groups_per_b, beta = 160.0 / std::max(32, a[0].Cin);
     if (units * n < 4.0 * grid) return false;
     double sum = 0, mx = 0, mn = 1e30;
@@ -1286,11 +1343,25 @@ bool tc_fused_fits(int n, const TcWeights *const *w, const ConvArgs *a, int prec
     return plain <= kMaxItems && chained <= kMaxItems;
 }
 
+// CTAs per SM of a fused launch: two where the C = 32 kernel's two-CTA plan fits, else one; 0 when neither fits.
+// ConvArgs::fused_ctas = 1 (SVB_TC_FUSED_CTAS=1) keeps one CTA per SM.
+static int tc_fused_ctas(int n, const TcWeights *const *w, const ConvArgs *a, int precision) {
+    const int two = tc_min_ctas(a[0].Cin, true);
+    if (two > 1 && a[0].fused_ctas != 1 && tc_fused_fits_ctas(n, w, a, precision, two)) return two;
+    return tc_fused_fits_ctas(n, w, a, precision, 1) ? 1 : 0;
+}
+
+bool tc_fused_fits(int n, const TcWeights *const *w, const ConvArgs *a, int precision) {
+    return tc_fused_ctas(n, w, a, precision) > 0;
+}
+
 int tc_worklist_build(int n, const TcWeights *const *w, const ConvArgs *a, int precision, bool chain_ordered, TcWorkList *out, bool fused) {
     TcArgs p;
     size_t smem = 0;
-    SVB_TRY(tc_plan_multi(n, w, a, precision, fused, p, smem));
-    const int grid = sm_count();
+    const int ctas = fused ? tc_fused_ctas(n, w, a, precision) : 1;
+    SVB_CHECK(ctas > 0, SVB_ERR_INVALID, "tc conv: no fused plan for %d chains of C = %d", n, a[0].Cin);
+    SVB_TRY(tc_plan_multi(n, w, a, precision, fused, ctas, p, smem));
+    const int grid = ctas * sm_count();
     const ConvArgs *ao = fused ? a + n : a;                      // the layers whose epilogue writes the output
     int KS[kTcMaxLayers], KS2[kTcMaxLayers], has_res[kTcMaxLayers], accum[kTcMaxLayers];
     for (int l = 0; l < n; ++l) KS[l] = a[l].KS, KS2[l] = ao[l].KS, has_res[l] = ao[l].res != nullptr, accum[l] = ao[l].accumulate;
@@ -1305,7 +1376,7 @@ int tc_worklist_build(int n, const TcWeights *const *w, const ConvArgs *a, int p
     SVB_CUDA(cudaMemcpy(out->items, items.data(), items.size() * sizeof(int4), cudaMemcpyHostToDevice));
     SVB_CUDA(cudaMemcpy(out->off, off.data(), off.size() * sizeof(int), cudaMemcpyHostToDevice));
     out->grid = grid, out->n_items = (int)items.size(), out->MT = p.MT, out->n_layers = n, out->chain_ordered = chain_ordered;
-    out->fused = fused;
+    out->fused = fused, out->ctas_per_sm = ctas;
     if (getenv("SVB_TC_VERBOSE"))
         fprintf(stderr, "[tc] work list: %d layers, %zu items over %d CTAs, balance %.3f (mean / max load)\n", n, items.size(), grid, balance);
     return SVB_OK;
@@ -1315,13 +1386,16 @@ int launch_conv_tc_multi(int n, const TcWeights *const *w, const ConvArgs *a, in
     SVB_CHECK(precision >= SVB_PREC_TF32 && precision <= SVB_PREC_BF16X3, SVB_ERR_INVALID, "tc conv: bad precision %d", precision);
     TcArgs p;
     size_t smem = 0;
-    SVB_TRY(tc_plan_multi(n, w, a, precision, fused, p, smem));
-    SVB_CHECK(wl.items && wl.n_layers == n && wl.MT == p.MT && wl.fused == fused && wl.grid == sm_count(), SVB_ERR_STATE,
+    // a fused list fixes the plan (CTAs per SM); a layer set that plan no longer fits makes the list stale (the caller rebuilds)
+    if (fused) SVB_CHECK(tc_plan_fused(n, w, a, precision, wl.ctas_per_sm, p, smem), SVB_ERR_STATE,
+                         "tc conv: fused work list was built for %d CTAs per SM", wl.ctas_per_sm);
+    else SVB_TRY(tc_plan(n, w, a, precision, 0, p, smem));
+    SVB_CHECK(wl.items && wl.n_layers == n && wl.MT == p.MT && wl.fused == fused && wl.grid == wl.ctas_per_sm * sm_count(), SVB_ERR_STATE,
               "tc conv: work list was built for another plan (layers %d / %d, MT %d / %d)", wl.n_layers, n, wl.MT, p.MT);
     p.work = wl.items, p.work_off = wl.off;
     if (fused && getenv("SVB_TC_VERBOSE"))
-        fprintf(stderr, "[tc] fused %d chain(s) C %d KS %d.. dil %d.. Tq %d | P %d nA %d nW %d smem %zu epi %d\n", n, a[0].Cin, a[0].KS,
-                a[0].dil, a[0].Tq, p.fused_P, p.nA, p.nW, smem, p.epi_slots);
+        fprintf(stderr, "[tc] fused %d chain(s) C %d KS %d.. dil %d.. Tq %d | P %d nA %d nW %d smem %zu ctas/SM %d epi %d\n", n, a[0].Cin,
+                a[0].KS, a[0].dil, a[0].Tq, p.fused_P, p.nA, p.nW, smem, wl.ctas_per_sm, p.epi_slots);
     return tc_dispatch(p, precision, wl.grid, smem, st, fused);
 }
 

@@ -32,6 +32,7 @@ struct TcWorkList {
     int4 *items = nullptr;
     int *off = nullptr;
     int grid = 0, n_items = 0, MT = 0, n_layers = 0;
+    int ctas_per_sm = 1;    // fused lists: the plan the list was built for (grid = ctas_per_sm x SMs)
     bool chain_ordered = false;
     bool fused = false;
 };
@@ -43,7 +44,7 @@ void tc_worklist_free(TcWorkList *wl);
 // the per-CTA item list of a merged launch is bounded (shared memory): very long batches fall back to one launch per layer
 bool tc_merge_fits(int n, int B, int Tq, int Cout, int n_tile);
 // whether one step of n ResBlock1 chains (w / a as for fused work lists) runs as a fused launch: C = 32 or 64, and the
-// layout fits shared memory (not in tf32x3) and the item table
+// layout fits shared memory (not in tf32x3) and the item table, with two CTAs per SM (C = 32) or one
 bool tc_fused_fits(int n, const TcWeights *const *w, const ConvArgs *a, int precision);
 // one persistent launch over `n` layers that share channels / rows / upsampling (taps, dilation and pointers may differ)
 int launch_conv_tc_multi(int n, const TcWeights *const *w, const ConvArgs *a, int precision, cudaStream_t st, const TcWorkList &wl,

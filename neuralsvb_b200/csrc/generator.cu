@@ -101,6 +101,7 @@ bool stage_fused(const svb_gen *g, const Stage &s, int B, int Ti) {
         for (int j = 0; j < nk; ++j) {
             a[j] = resblock_args(s.c1[j][m], nullptr, nullptr, nullptr, 1.f, 0, B, Ti, c4t_rows(Ti), 0.1f);
             a[nk + j] = resblock_args(s.c2[j][m], nullptr, nullptr, nullptr, 1.f, 0, B, Ti, c4t_rows(Ti), 0.1f);
+            a[j].fused_ctas = a[nk + j].fused_ctas = g->fused_ctas;
             w[j] = &s.c1[j][m].tc, w[nk + j] = &s.c2[j][m].tc;
         }
         if (!tc_fused_fits(nk, w, a, g->cfg.precision)) return false;
@@ -199,7 +200,7 @@ int run_conv_multi(svb_gen *g, int stage, int nk, const ConvLayer *const *Ls, co
     for (int j = 0; j < (fused ? 2 * nk : nk); ++j) {
         const ConvLayer &L = *Ls[j];
         a[j] = resblock_args(L, in[j], out[j], res[j], scale[j], accumulate[j], B, Tq, Tp, in_slope);
-        a[j].epi_stream = g->epi;
+        a[j].epi_stream = g->epi, a[j].fused_ctas = g->fused_ctas;
         w[j] = &L.tc;
         bytes += 4.0 * ((double)B * Tq * L.Cin + (double)B * Tq * L.Cout * (1 + (res[j] ? 1 : 0) + (accumulate[j] ? 1 : 0)));
         flops += 2.0 * L.macs_per_row * (double)B * Tq;
@@ -478,6 +479,7 @@ extern "C" int svb_gen_create(const svb_gen_config *cfg, int device, svb_gen_t *
     if (const char *e = getenv("SVB_MERGE")) g->merge = atoi(e) != 0;
     if (const char *e = getenv("SVB_FUSE")) g->fuse = atoi(e) != 0;
     if (const char *e = getenv("SVB_EPI")) g->epi = atoi(e) != 0;
+    if (const char *e = getenv("SVB_TC_FUSED_CTAS")) g->fused_ctas = atoi(e);
     if (const char *e = getenv("SVB_CHAIN_BIAS")) g->chain_bias = atof(e);
     *out = g;
     return SVB_OK;

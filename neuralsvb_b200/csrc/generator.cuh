@@ -145,6 +145,8 @@ struct svb_gen {
                                     // reference path of the bit-identity tests)
     bool epi = true;                // SVB_EPI=0: the tensor-core epilogue loads residual / running sum per thread instead
                                     // of streaming them through shared memory (the reference of its bit-identity tests)
+    int fused_ctas = 0;             // SVB_TC_FUSED_CTAS=1: the fused C = 32 steps keep one CTA per SM where two fit (the
+                                    // reference of the two-CTA bit-identity tests); 2 or unset: two where they fit
     std::map<int, svb::TcWorkList> worklists;
 
     bool profile = false;
