@@ -24,7 +24,6 @@
 //   pipeline fill / drain of a persistent launch is paid once per step of the chains, not per layer.
 #include <algorithm>
 #include <cmath>
-#include <cstring>
 #include <cstdlib>
 #include <type_traits>
 #include <vector>
@@ -70,7 +69,8 @@ struct TcArgs {
     int w_resident;             // every layer's tiles stay in shared memory for the whole launch (narrow layers)
     int blk_chunk_step;         // grouped conv: first input chunk of column block nblk = nblk * blk_chunk_step (0: dense)
     uint32_t w_res_bytes;       // resident: total bytes of all layers' tiles
-    int pdl;                    // launched with programmatic stream serialization
+    int reserved;               // keeps the fields below at their offsets: ptxas allocates the kernel's registers by the
+                                // parameter layout, and moved fields cost the fused N = 64 kernel up to 5 more registers
     uint32_t op_bytes;          // operand slot: Rp rows x 128 B (x2 with the 3xTF32 lo plane), sized for the largest halo
     uint32_t wtile_bytes;       // one (column block, chunk, tap) weight tile (x2 with the 3xTF32 lo plane)
     uint32_t off_op, off_w, off_bias;   // byte offsets of operand slots / weight ring / bias in dynamic smem
@@ -112,7 +112,7 @@ __host__ __device__ inline void tc_fused_slab(int t0, int h1, int h2, int in_Tp,
 }
 
 // a work item, as staged in shared memory: x = layer | column block << 8 | tiles << 24, y = clip, z = first row.  Fused
-// items are always two tiles of the launch's only column block (tc_plan_fused): constants, not registers.
+// items are always two tiles of the launch's only column block (tc_plan): constants, not registers.
 struct TcItem {
     int layer, nblk, mt, b, t0;
 };
@@ -233,10 +233,8 @@ __global__ void __launch_bounds__(kTcThreadsP, tc_min_ctas(N, FUSED)) conv1d_c4_
     // Programmatic dependent launch: everything above (barrier init, constant staging) overlapped the
     // tail of the previous kernel in the stream; its results are needed from here on.  The next
     // kernel may begin ITS prologue as soon as every CTA of this grid has reached this point.
-    if (p.pdl) {
-        asm volatile("griddepcontrol.wait;" ::: "memory");
-        asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-    }
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
     // all ring indices / phases are kept as incrementing counters -- no runtime integer divisions in the loops
     if (warp == kWarpProducer) {
@@ -246,7 +244,16 @@ __global__ void __launch_bounds__(kTcThreadsP, tc_min_ctas(N, FUSED)) conv1d_c4_
             const int gin = c4t_groups(a.Cin);
             const size_t group_stride = (size_t)a.in_Tp * 32;                     // floats between channel groups
             int sA = 0, phA = 1, sW = 0, phW = 1;                                 // "empty" barriers start free
-            if (p.w_resident && n_items > 0) {                                    // all layers' tiles, once
+            auto stream_w = [&](const unsigned char *&w_k, int tiles) {          // the next `tiles` tiles from w_k through the ring
+                for (int k = 0; k < tiles; ++k) {
+                    mbar_wait(w_empty + sW, phW);
+                    mbar_expect_tx(w_full + sW, p.wtile_bytes);
+                    bulk_g2s(wring + sW * p.wtile_bytes, w_k, p.wtile_bytes, w_full + sW);
+                    w_k += p.wtile_bytes;
+                    if (++sW == p.nW) sW = 0, phW ^= 1;
+                }
+            };
+            if (!FUSED && p.w_resident && n_items > 0) {                          // all layers' tiles, once (never fused)
                 mbar_expect_tx(w_full, p.w_res_bytes);
                 for (int l = 0; l < p.n_layers; ++l)
                     bulk_g2s(wring + Ls[l].w_res_off, Ls[l].w, (uint32_t)Ls[l].KS * p.wtile_bytes, w_full);
@@ -270,15 +277,7 @@ __global__ void __launch_bounds__(kTcThreadsP, tc_min_ctas(N, FUSED)) conv1d_c4_
                     bulk_g2s(op0 + sA * p.op_bytes, in_c, raw_bytes, raw_full + sA);
                     in_c += group_stride;
                     if (++sA == p.nA) sA = 0, phA ^= 1;
-                    if (!p.w_resident) {
-                        for (int k = 0; k < L.KS; ++k) {
-                            mbar_wait(w_empty + sW, phW);
-                            mbar_expect_tx(w_full + sW, p.wtile_bytes);
-                            bulk_g2s(wring + sW * p.wtile_bytes, w_k, p.wtile_bytes, w_full + sW);
-                            w_k += p.wtile_bytes;
-                            if (++sW == p.nW) sW = 0, phW ^= 1;
-                        }
-                    }
+                    if (FUSED || !p.w_resident) stream_w(w_k, L.KS);
                 }
                 if (p.l2_prefetch) {
                     // the rows this item's epilogue reads with per-thread loads, issued behind its last slab: they reach L2
@@ -294,14 +293,8 @@ __global__ void __launch_bounds__(kTcThreadsP, tc_min_ctas(N, FUSED)) conv1d_c4_
                 }
                 if (FUSED) {                                                      // then c2's tiles, (chunk, tap) in order
                     const TcLayer &L2 = Ls[p.n_layers + it.layer];
-                    w_k = L2.w + (size_t)it.nblk * p.n_chunks * L2.KS * p.wtile_bytes;
-                    for (int k = 0; k < p.n_chunks * L2.KS; ++k) {
-                        mbar_wait(w_empty + sW, phW);
-                        mbar_expect_tx(w_full + sW, p.wtile_bytes);
-                        bulk_g2s(wring + sW * p.wtile_bytes, w_k, p.wtile_bytes, w_full + sW);
-                        w_k += p.wtile_bytes;
-                        if (++sW == p.nW) sW = 0, phW ^= 1;
-                    }
+                    w_k = L2.w;
+                    stream_w(w_k, p.n_chunks * L2.KS);
                 }
             }
         }
@@ -569,38 +562,47 @@ __global__ void __launch_bounds__(kTcThreadsP, tc_min_ctas(N, FUSED)) conv1d_c4_
                 k += (int)has_res + (int)accumulate;
             }
         };
-        // one item of one (TWO = false) or two (TWO = true) tiles; per output element the MMAs accumulate in the same
-        // order either way (chunk, tap, then the split terms)
-        auto run_mma_slab = [&](auto two, const TcLayer &L) {
-            constexpr bool TWO = decltype(two)::value;
+        // The MMAs of one item for layer L over one (TWO = false) or two (TWO = true) tiles; per output element they
+        // accumulate in the same order either way (chunk, tap, then the split terms).  SLAB: the A operand of chunk c is
+        // the next operand slot (waited on, released with the chunk's last tap) and a tap is a row shift of dil rows; else
+        // it is the fused intermediate, chunk c at a fixed stride, and a tap is one row on.  Fused plans stream their weights.
+        unsigned char *inter = smem + p.off_inter;
+        auto run_mma = [&](auto two, auto slab, const TcLayer &L) {
+            constexpr bool TWO = decltype(two)::value, SLAB = decltype(slab)::value;
             const int KS = L.KS;
-            const uint32_t tap_step = (uint32_t)L.dil * (128 >> 4);       // a tap is a row shift of the operand
+            const uint32_t tap_step = (SLAB ? (uint32_t)L.dil : 1u) * (128 >> 4);
+            const uint32_t lo_plane = SLAB ? a_lo_plane : (X3 ? p.inter_bytes / 2 : 64u) >> 4;
             uint32_t scale = 0;                                             // first MMA of the item overwrites
             acc_clear();
             for (int c = 0; c < p.n_chunks; ++c) {
-                mbar_wait(a_ready + sA, phA);
-                uint32_t a_tap = op_base + sA * op_step;
+                uint32_t a_tap;
+                if constexpr (SLAB) {
+                    mbar_wait(a_ready + sA, phA);
+                    a_tap = op_base + sA * op_step;
+                } else {
+                    a_tap = desc_lo(smem_u32(inter)) + (uint32_t)wg * ((64 * 128) >> 4) + (uint32_t)c * (p.inter_bytes >> 4);
+                }
                 uint32_t b_tap = w_base + (L.w_res_off >> 4);               // resident tiles (single chunk)
                 for (int k = 0; k < KS; ++k) {
-                    if (!p.w_resident) {
+                    if (FUSED || !p.w_resident) {
                         mbar_wait(w_full + sW, phW);
                         b_tap = w_base + sW * wtile_step;
                     }
                     wgmma_fence();
-                    conv_tap_mma<MODE, N>(acc0, a_tap, b_tap, a_lo_plane, b_lo_plane, hi, scale);
-                    if (TWO) conv_tap_mma<MODE, N>(acc1, a_tap + tile_step, b_tap, a_lo_plane, b_lo_plane, hi, scale);
+                    conv_tap_mma<MODE, N>(acc0, a_tap, b_tap, lo_plane, b_lo_plane, hi, scale);
+                    if (TWO) conv_tap_mma<MODE, N>(acc1, a_tap + tile_step, b_tap, lo_plane, b_lo_plane, hi, scale);
                     wgmma_commit();
                     wgmma_wait<1>();
                     release();                                              // the previous tap's group has completed
-                    if (!p.w_resident) {
+                    if (FUSED || !p.w_resident) {
                         pend_w = sW;
                         if (++sW == p.nW) sW = 0, phW ^= 1;
                     }
-                    if (k == KS - 1) pend_a = sA;
+                    if (SLAB && k == KS - 1) pend_a = sA;
                     scale = 1;
                     a_tap += tap_step, b_tap += wtile_step;
                 }
-                if (++sA == p.nA) sA = 0, phA ^= 1;
+                if (SLAB && ++sA == p.nA) sA = 0, phA ^= 1;
             }
             wgmma_wait<0>();
             wgmma_keep<N>(acc0);
@@ -625,12 +627,11 @@ __global__ void __launch_bounds__(kTcThreadsP, tc_min_ctas(N, FUSED)) conv1d_c4_
         auto run_item = [&](auto two, const TcItem &it) {
             const TcLayer &L = Ls[it.layer];
             if (EPI && p.epi_slots > 0 && (L.res != nullptr || L.accumulate)) epi_begin(it, L);
-            run_mma_slab(two, L);
+            run_mma(two, std::true_type(), L);
             epilogue_item(two, it, L);
         };
         // ---- fused items: c1's epilogue stores c2's operand for the item's rows 0 .. 255 (time tq0 + row) into the
         // intermediate, in the layout the transform warps give a slab (hi / lo split or tf32 rounding, SWIZZLE_128B)
-        unsigned char *inter = smem + p.off_inter;
         auto stage_intermediate = [&](const TcLayer &L1, const float *acc, int row0, int tq0) {
             const float *bias_s = reinterpret_cast<const float *>(smem + p.off_bias) + L1.bias_off;
             const float slope = a.in_slope;
@@ -665,41 +666,17 @@ __global__ void __launch_bounds__(kTcThreadsP, tc_min_ctas(N, FUSED)) conv1d_c4_
             const TcLayer &L1 = Ls[it.layer], &L2 = Ls[p.n_layers + it.layer];
             const int h2 = (L2.KS - 1) / 2;
             if (EPI && p.epi_slots > 0 && (L2.res != nullptr || L2.accumulate)) epi_begin(it, L2);
-            run_mma_slab(std::true_type(), L1);
+            run_mma(std::true_type(), std::true_type(), L1);
             // the other warpgroup's c2 wgmmas of the previous item have retired: the intermediate may be overwritten
             named_bar_sync(1, kMathWarps * 32);
             stage_intermediate(L1, acc0, 0, it.t0 - h2);
             stage_intermediate(L1, acc1, kTcM, it.t0 - h2);
             fence_proxy_async();                                            // generic-proxy writes -> visible to the tensor core
             named_bar_sync(1, kMathWarps * 32);                             // c2's tap shifts read rows the other warpgroup wrote
-            const uint32_t inter_lo_plane = (X3 ? p.inter_bytes / 2 : 64u) >> 4;
-            const uint32_t inter_base = desc_lo(smem_u32(inter)) + (uint32_t)wg * ((64 * 128) >> 4);
-            uint32_t scale = 0;
-            acc_clear();
-            for (int c = 0; c < p.n_chunks; ++c) {
-                uint32_t a_tap = inter_base + (uint32_t)c * (p.inter_bytes >> 4);
-                for (int k = 0; k < L2.KS; ++k) {
-                    mbar_wait(w_full + sW, phW);
-                    const uint32_t b_tap = w_base + sW * wtile_step;
-                    wgmma_fence();
-                    conv_tap_mma<MODE, N>(acc0, a_tap, b_tap, inter_lo_plane, b_lo_plane, hi, scale);
-                    conv_tap_mma<MODE, N>(acc1, a_tap + tile_step, b_tap, inter_lo_plane, b_lo_plane, hi, scale);
-                    wgmma_commit();
-                    wgmma_wait<1>();
-                    release();
-                    pend_w = sW;
-                    if (++sW == p.nW) sW = 0, phW ^= 1;
-                    scale = 1;
-                    a_tap += 128 >> 4;
-                }
-            }
-            wgmma_wait<0>();
-            wgmma_keep<N>(acc0);
-            wgmma_keep<N>(acc1);
-            release();
+            run_mma(std::true_type(), std::false_type(), L2);
             epilogue_item(std::true_type(), it, L2);
         };
-        if (p.w_resident && n_items > 0) mbar_wait(w_full, 0);
+        if (!FUSED && p.w_resident && n_items > 0) mbar_wait(w_full, 0);
         for (int n = 0; n < n_items; ++n) {
             const TcItem it = item_decode<FUSED>(items[n]);
             if constexpr (FUSED) run_fused(it);
@@ -710,30 +687,6 @@ __global__ void __launch_bounds__(kTcThreadsP, tc_min_ctas(N, FUSED)) conv1d_c4_
 }
 
 // ------------------------------------------------------------------ host side
-static float host_tf32(float x) {   // round to nearest, ties away (cvt.rna.tf32.f32)
-    uint32_t u;
-    std::memcpy(&u, &x, 4);
-    if ((u & 0x7F800000u) == 0x7F800000u) return x;
-    u += 0x1000u;
-    u &= 0xFFFFE000u;
-    float r;
-    std::memcpy(&r, &u, 4);
-    return r;
-}
-static uint16_t host_bf16(float x) {   // round to nearest even (__float2bfloat16_rn)
-    uint32_t u;
-    std::memcpy(&u, &x, 4);
-    if ((u & 0x7F800000u) == 0x7F800000u) return (uint16_t)(u >> 16);
-    u += 0x7FFFu + ((u >> 16) & 1u);
-    return (uint16_t)(u >> 16);
-}
-static float bf16_to_float(uint16_t h) {
-    const uint32_t u = (uint32_t)h << 16;
-    float r;
-    std::memcpy(&r, &u, 4);
-    return r;
-}
-
 static int pick_n_tile(int CoutP) {      // columns per CTA: a multiple of 32 (one G32T channel group per epilogue block)
     if (CoutP % 32 != 0) return 0;
     if (CoutP <= 128) return CoutP;
@@ -742,55 +695,10 @@ static int pick_n_tile(int CoutP) {      // columns per CTA: a multiple of 32 (o
     return 0;
 }
 
-// Weight tiles in K-major SWIZZLE_128B order: row n (output column) = 128 bytes holding the 32 input
-// channels of the chunk; the 16-byte chunk c of row n is stored at chunk position c ^ (n & 7).
-int tc_pack_weights(const float *packed, int KS, int Cin, int CoutP, TcWeights *out, std::vector<void *> *allocs, int force_n_tile) {
-    out->KS = KS, out->Cin = Cin, out->CoutP = CoutP, out->ok = false;
-    const int n_tile = force_n_tile > 0 ? force_n_tile : pick_n_tile(CoutP);
-    if (force_n_tile > 0 && (CoutP % force_n_tile != 0 || force_n_tile % 32 != 0 || force_n_tile > 128)) return SVB_OK;
-    if (n_tile == 0 || n_tile % 8 != 0 || Cin % 4 != 0) return SVB_OK;    // CUDA cores handle it
-    out->n_tile = n_tile;
-    // input channels are padded to whole 32-channel groups (zero weights against the zero pad channels of G32T)
-    const int n_chunks = (Cin + kTcCK - 1) / kTcCK, n_blk = CoutP / n_tile;
-    const size_t tile_b = (size_t)n_tile * 128;                    // bytes per tile plane
-    const size_t n_tiles = (size_t)n_blk * n_chunks * KS;
-    std::vector<unsigned char> tf(n_tiles * tile_b), tf3(n_tiles * tile_b * 2), bf(n_tiles * tile_b);
-    for (int nb = 0; nb < n_blk; ++nb)
-        for (int c = 0; c < n_chunks; ++c)
-            for (int k = 0; k < KS; ++k) {
-                const size_t t = ((size_t)nb * n_chunks + c) * KS + k;
-                float *t1 = reinterpret_cast<float *>(tf.data() + t * tile_b);
-                float *t3h = reinterpret_cast<float *>(tf3.data() + t * tile_b * 2);
-                float *t3l = reinterpret_cast<float *>(tf3.data() + t * tile_b * 2 + tile_b);
-                uint16_t *tb = reinterpret_cast<uint16_t *>(bf.data() + t * tile_b);
-                for (int n = 0; n < n_tile; ++n)
-                    for (int ci = 0; ci < kTcCK; ++ci) {
-                        const int cin_i = c * kTcCK + ci;
-                        const float w = cin_i < Cin ? packed[((size_t)k * Cin + cin_i) * CoutP + nb * n_tile + n] : 0.f;
-                        const float h = host_tf32(w);
-                        const int c16 = ci >> 2;                   // fp32: 4 channels per 16-byte chunk
-                        const size_t i4 = (size_t)n * 32 + ((c16 ^ (n & 7)) << 2) + (ci & 3);
-                        t1[i4] = h, t3h[i4] = h, t3l[i4] = host_tf32(w - h);
-                        const uint16_t bh = host_bf16(w), bl = host_bf16(w - bf16_to_float(bh));
-                        const int ch = ci >> 3, cl = 4 + (ci >> 3); // bf16: 8 channels per chunk; hi chunks 0-3, lo 4-7
-                        tb[(size_t)n * 64 + ((ch ^ (n & 7)) << 3) + (ci & 7)] = bh;
-                        tb[(size_t)n * 64 + ((cl ^ (n & 7)) << 3) + (ci & 7)] = bl;
-                    }
-            }
-    auto up = [&](const void *src, size_t bytes, void **dst) -> int {
-        SVB_CUDA(cudaMalloc(dst, bytes));
-        allocs->push_back(*dst);
-        SVB_CUDA(cudaMemcpy(*dst, src, bytes, cudaMemcpyHostToDevice));
-        return SVB_OK;
-    };
-    SVB_TRY(up(tf.data(), tf.size(), &out->blob[SVB_PREC_TF32]));
-    SVB_TRY(up(tf3.data(), tf3.size(), &out->blob[SVB_PREC_TF32X3]));
-    SVB_TRY(up(bf.data(), bf.size(), &out->blob[SVB_PREC_BF16X3]));
-    out->ok = true;
-    return SVB_OK;
-}
-
-// device twin of the loops in tc_pack_weights: one thread per (tile, output column n, input channel ci)
+// Weight tiles in K-major SWIZZLE_128B order: row n (output column) = 128 bytes holding the 32 input channels of the
+// chunk; the 16-byte chunk c of row n is stored at chunk position c ^ (n & 7).  One thread per (tile, output column n,
+// input channel ci); every byte of the three blobs is written (input channels past Cin are zero weights against the
+// zero pad channels of G32T).
 __global__ void tc_repack_kernel(const float *__restrict__ packed, int KS, int Cin, int CoutP, int n_tile, int n_chunks,
                                  long long total, unsigned char *__restrict__ tf, unsigned char *__restrict__ tf3,
                                  unsigned char *__restrict__ bf) {
@@ -804,7 +712,7 @@ __global__ void tc_repack_kernel(const float *__restrict__ packed, int KS, int C
     const int nb = (int)(t / ((long long)KS * n_chunks));
     const int cin_i = c * kTcCK + ci;
     const float w = cin_i < Cin ? packed[((size_t)k * Cin + cin_i) * CoutP + nb * n_tile + n] : 0.f;
-    auto tf32 = [](float x) {      // host_tf32: round half up in magnitude to 10 mantissa bits
+    auto tf32 = [](float x) {      // round half up in magnitude to 10 mantissa bits
         uint32_t u = __float_as_uint(x);
         if ((u & 0x7F800000u) == 0x7F800000u) return x;
         u += 0x1000u;
@@ -813,14 +721,14 @@ __global__ void tc_repack_kernel(const float *__restrict__ packed, int KS, int C
     };
     const size_t tile_b = (size_t)n_tile * 128;
     const float h = tf32(w);
-    const size_t i4 = (size_t)n * 32 + (((ci >> 2) ^ (n & 7)) << 2) + (ci & 3);
+    const size_t i4 = (size_t)n * 32 + (((ci >> 2) ^ (n & 7)) << 2) + (ci & 3);     // fp32: 4 channels per 16-byte chunk
     reinterpret_cast<float *>(tf + t * tile_b)[i4] = h;
     reinterpret_cast<float *>(tf3 + t * tile_b * 2)[i4] = h;
     reinterpret_cast<float *>(tf3 + t * tile_b * 2 + tile_b)[i4] = tf32(w - h);
     const __nv_bfloat16 bh = __float2bfloat16_rn(w);
     const __nv_bfloat16 bl = __float2bfloat16_rn(w - __bfloat162float(bh));
     uint16_t *tb = reinterpret_cast<uint16_t *>(bf + t * tile_b);
-    const int ch = ci >> 3, cl = 4 + (ci >> 3);
+    const int ch = ci >> 3, cl = 4 + (ci >> 3);         // bf16: 8 channels per chunk; hi chunks 0-3, lo 4-7
     tb[(size_t)n * 64 + ((ch ^ (n & 7)) << 3) + (ci & 7)] = __bfloat16_as_ushort(bh);
     tb[(size_t)n * 64 + ((cl ^ (n & 7)) << 3) + (ci & 7)] = __bfloat16_as_ushort(bl);
 }
@@ -833,6 +741,27 @@ int tc_repack_weights_dev(const float *packed_dev, const TcWeights &w, cudaStrea
         packed_dev, w.KS, w.Cin, w.CoutP, w.n_tile, n_chunks, total, reinterpret_cast<unsigned char *>(w.blob[SVB_PREC_TF32]),
         reinterpret_cast<unsigned char *>(w.blob[SVB_PREC_TF32X3]), reinterpret_cast<unsigned char *>(w.blob[SVB_PREC_BF16X3]));
     SVB_CUDA(cudaGetLastError());
+    return SVB_OK;
+}
+
+int tc_pack_weights(const float *packed_dev, int KS, int Cin, int CoutP, TcWeights *out, std::vector<void *> *allocs, cudaStream_t st,
+                    int force_n_tile) {
+    out->KS = KS, out->Cin = Cin, out->CoutP = CoutP, out->ok = false;
+    const int n_tile = force_n_tile > 0 ? force_n_tile : pick_n_tile(CoutP);
+    if (force_n_tile > 0 && (CoutP % force_n_tile != 0 || force_n_tile % 32 != 0 || force_n_tile > 128)) return SVB_OK;
+    if (n_tile == 0 || n_tile % 8 != 0 || Cin % 4 != 0) return SVB_OK;    // CUDA cores handle it
+    out->n_tile = n_tile;
+    const int n_chunks = (Cin + kTcCK - 1) / kTcCK;
+    const size_t plane = (size_t)(CoutP / n_tile) * n_chunks * KS * n_tile * 128;     // all tiles, one plane each
+    for (int prec : {SVB_PREC_TF32, SVB_PREC_TF32X3, SVB_PREC_BF16X3}) {
+        SVB_CUDA(cudaMalloc(&out->blob[prec], prec == SVB_PREC_TF32X3 ? 2 * plane : plane));
+        allocs->push_back(out->blob[prec]);
+    }
+    out->ok = true;
+    if (packed_dev) {
+        SVB_TRY(tc_repack_weights_dev(packed_dev, *out, st));
+        SVB_CUDA(cudaStreamSynchronize(st));
+    }
     return SVB_OK;
 }
 
@@ -866,7 +795,7 @@ static int launch_mode(const TcArgs &p, int grid, size_t smem, cudaStream_t st) 
     cfg.gridDim = dim3(grid), cfg.blockDim = dim3(kTcThreadsP), cfg.dynamicSmemBytes = smem, cfg.stream = st;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = p.pdl ? 1 : 0;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr, cfg.numAttrs = 1;
     SVB_CUDA(cudaLaunchKernelEx(&cfg, kern, p));
     return SVB_OK;
@@ -884,8 +813,6 @@ static int sm_count() {
     return n[slot];
 }
 
-// Streamed epilogue (kernel: epilogue_stream): whether the layers a[0..n) take it, and how many 2 KB pieces one math
-// warp's item needs at most.  Upsamplers interleave phases in their output rows, so their pieces are not contiguous.
 // How many sources (residual, running sum) the epilogue of the layers a[0..n) reads: 0 when none does, when SVB_EPI=0
 // asked for per-thread loads, or for upsamplers, whose output rows interleave phases and so are not contiguous.
 static int tc_epi_sources(int n, const ConvArgs *a) {
@@ -924,102 +851,149 @@ static int tc_epi_fit(size_t avail, uint32_t wtile_bytes, int pieces, int min_sl
     return 0;
 }
 
-// Shape-class plan of one launch: tiles per item, operand slots, weight ring / residency and the shared-memory carve-up.
-// `a[0..n)` are layers of the same shape class (channels, rows, upsampling) that may differ in taps / dilation / pointers;
-// slots are sized for the largest halo.  `grid` > 0: the launch runs the implicit round-robin list on that many CTAs;
-// 0: a host-built work list (tc_schedule balances it).
-static int tc_plan(int n, const TcWeights *const *w, const ConvArgs *a, int precision, int grid, TcArgs &p, size_t &smem) {
-    SVB_CHECK(n >= 1 && n <= kTcMaxLayers, SVB_ERR_INVALID, "tc conv: %d layers in one launch", n);
+// Dynamic shared memory of one launch (p.MT, p.op_bytes and p.wtile_bytes set): header and item table, nA operand slots,
+// `inter_bytes` of intermediate (fused launches), the weights, the piece ring of the streamed epilogue and `bias_bytes` of
+// bias, within `budget` bytes before the bias.
+// * Operand slots double as TMA targets: nA_pref of them (3 keep two slab copies in flight behind the MMAs), 2 when
+//   nA_pref does not fit next to two weight tiles.
+// * Weights: resident (res_bytes > 0: every layer's tiles, one chunk and one column block) with nA_pref or 2 slots where
+//   they fit; else a ring of up to kMaxW tiles, at least one per tile of an item.
+// * The piece ring (`pieces` per math warp at most) comes out of the weight ring.  ring_takes_slot: where it does not fit
+//   next to nA > 2 slots (C = 64 at k 11, d 5 in fused launches), the layout drops to 2 slots for it; else it never changes
+//   nA, and goes without the ring where it does not fit.
+// Returns false when no layout fits.
+static bool tc_layout(TcArgs &p, size_t &smem, size_t budget, size_t bias_bytes, int nA_pref, size_t inter_bytes, size_t res_bytes,
+                      int pieces, bool ring_takes_slot) {
+    p.off_op = 1024 + kItemBytes;
+    auto slots_end = [&](int nA) { return p.off_op + (size_t)nA * p.op_bytes + inter_bytes; };
+    p.w_resident = 0;
+    for (int nA : {nA_pref, 2}) {
+        if (res_bytes > 0 && slots_end(nA) + res_bytes <= budget) {
+            p.nA = nA, p.w_resident = 1;
+            break;
+        }
+    }
+    if (!p.w_resident) {
+        p.nA = slots_end(nA_pref) + 2 * (size_t)p.wtile_bytes > budget ? std::min(nA_pref, 2) : nA_pref;
+        if (slots_end(p.nA) + (size_t)p.MT * p.wtile_bytes > budget) return false;
+    }
+    const size_t res_area = (size_t)round_up((int)res_bytes, 1024);
+    const int min_slots = pieces / (p.MT * (p.n_tile / 32));
+    auto place = [&](int nA, bool ring) {
+        p.nA = nA;
+        p.off_w = (uint32_t)slots_end(nA);
+        const size_t avail = budget - p.off_w;
+        p.nW = p.w_resident ? 1 : std::min((int)(avail / p.wtile_bytes), kMaxW);
+        p.epi_slots = 0;
+        if (ring && p.w_resident) {
+            int nw = 0;
+            p.epi_slots = avail > res_area ? tc_epi_fit(avail - res_area, 1u, pieces, min_slots, &nw) : 0;
+        } else if (ring) {
+            p.epi_slots = tc_epi_fit(avail, p.wtile_bytes, pieces, min_slots, &p.nW);
+        }
+        return p.epi_slots > 0;
+    };
+    const int nA = p.nA;
+    if (!pieces || !(place(nA, true) || (ring_takes_slot && nA > 2 && place(2, true)))) place(nA, false);
+    p.w_res_bytes = p.w_resident ? (uint32_t)res_bytes : 0;
+    p.off_epi = p.off_w + (uint32_t)(p.w_resident ? res_area : round_up(p.nW * (int)p.wtile_bytes, 1024));
+    p.off_bias = p.off_epi + (uint32_t)p.epi_slots * kMathWarps * kEpiPieceBytes;
+    smem = (size_t)p.off_bias + bias_bytes;
+    return smem <= budget + bias_bytes;
+}
+
+// Plan of one launch: tiles per item, the shared-memory layout (tc_layout) and the layer table.
+// ctas = 0: one layer or a merged launch.  a[0..n) are layers of the same shape class (channels, rows, upsampling) that
+//   may differ in taps / dilation / pointers; slots are sized for the largest halo.  `grid` > 0: the launch runs the
+//   implicit round-robin list on that many CTAs; 0: a host-built work list (tc_schedule balances it).
+// ctas > 0: a fused launch over n ResBlock chains with `ctas` CTAs per SM: a[0..n) are the c1 layers, a[n..2n) the c2
+//   layers of the same step.  Every item is 256 c1 rows; the c1 slab slots, the intermediate (256 + 2 max h2 rows per
+//   32-channel chunk), a weight ring of at least 2 tiles (c1's and c2's tiles stream through it in order) and the biases
+//   of all 2n layers share the shared memory.  ctas = 1: up to 227 KB, three slab slots.  ctas = 2 (C = 32 only, the
+//   kernel compiled for two CTAs per SM): half of the SM's 228 KB less the 1 KB each CTA reserves, so one slab slot (the
+//   next item's slab is copied and transformed while this item runs c1's epilogue and c2; the other CTA's MMAs cover the
+//   rest) and a bias area of just the 2n layers' biases.  A shape that no fused launch runs, or whose layout does not
+//   fit, returns SVB_ERR_INVALID without setting the error message: callers probe for fused plans.
+constexpr size_t kSmemPerSm = 228 * 1024, kSmemReservedPerCta = 1024;
+static int tc_plan(int n, const TcWeights *const *w, const ConvArgs *a, int precision, int ctas, int grid, TcArgs &p, size_t &smem) {
+    const bool fused = ctas > 0;
     const ConvArgs &a0 = a[0];
-    for (int l = 1; l < n; ++l)
-        SVB_CHECK(a[l].B == a0.B && a[l].Cin == a0.Cin && a[l].Cout == a0.Cout && a[l].CoutP == a0.CoutP && a[l].Tq == a0.Tq &&
-                      a[l].in_Tp == a0.in_Tp && a[l].out_Tp == a0.out_Tp && a[l].ups_u == a0.ups_u && a[l].in_slope == a0.in_slope &&
-                      a[l].cin_blk == a0.cin_blk && w[l]->n_tile == w[0]->n_tile,
-                  SVB_ERR_INVALID, "tc conv: layers of one launch must share the shape class");
-    SVB_CHECK(w[0]->n_tile == 32 || w[0]->n_tile == 64 || w[0]->n_tile == 96 || w[0]->n_tile == 128, SVB_ERR_INVALID,
-              "tc conv: %d columns per tile", w[0]->n_tile);
+    const int planes = precision == SVB_PREC_TF32X3 ? 2 : 1;
+    int halo = 0;                   // one layer or a merged launch: the largest halo
+    if (fused) {
+        if (n < 1 || n > kTcMaxLayers) return SVB_ERR_INVALID;
+        for (int l = 0; l < 2 * n; ++l) {
+            if (a[l].B != a0.B || a[l].Cin != a0.Cin || a[l].Cout != a0.Cin || a[l].CoutP != a0.Cin || a[l].Tq != a0.Tq ||
+                a[l].in_Tp != a0.in_Tp || a[l].out_Tp != a0.in_Tp || a[l].ups_u != 0 || a[l].cin_blk != 0 ||
+                a[l].in_slope != a0.in_slope || !w[l]->ok || w[l]->n_tile != a0.Cin || (l >= n && a[l].dil != 1))
+                return SVB_ERR_INVALID;
+        }
+        if ((a0.Cin != 32 && a0.Cin != 64) || (ctas != 1 && ctas != tc_min_ctas(a0.Cin, true))) return SVB_ERR_INVALID;
+        int h1 = 0, h2 = 0;
+        for (int l = 0; l < n; ++l) h1 = std::max(h1, (a[l].KS - 1) / 2 * a[l].dil), h2 = std::max(h2, (a[n + l].KS - 1) / 2);
+        if (h1 + h2 > kPad || 2 * h2 >= kTcM) return SVB_ERR_INVALID;     // the shifted slab starts inside the zero padding
+        p.n_tile = a0.Cin, p.n_chunks = a0.Cin / kTcCK, p.blk_chunk_step = 0, p.col_blocks = 1;
+        p.MT = 2;
+        p.wtile_bytes = (uint32_t)p.n_tile * 128 * planes;
+        p.fused_P = 2 * kTcM - 2 * h2;
+        p.op_bytes = (uint32_t)round_up(2 * kTcM + 2 * h1, 8) * 128 * planes;
+        p.inter_bytes = (uint32_t)round_up(2 * kTcM + 2 * h2, 8) * 128 * planes;
+        // 2n x Cout <= 6 x 64 floats
+        const size_t bias_bytes = ctas == 1 ? kBiasBytes : (size_t)round_up(2 * n * a0.Cout * 4, 128);
+        const size_t smem_max = ctas == 1 ? 227 * 1024 : kSmemPerSm / 2 - kSmemReservedPerCta;
+        if (!tc_layout(p, smem, smem_max - bias_bytes, bias_bytes, ctas == 1 ? 3 : 1, (size_t)p.n_chunks * p.inter_bytes, 0,
+                       tc_epi_pieces(n, a + n, 2, p.n_tile), true))
+            return SVB_ERR_INVALID;
+        p.off_inter = p.off_op + (uint32_t)p.nA * p.op_bytes;
+        p.groups_per_b = (a0.Tq + p.fused_P - 1) / p.fused_P;
+        p.total_groups = p.groups_per_b * a0.B;
+    } else {
+        SVB_CHECK(n >= 1 && n <= kTcMaxLayers, SVB_ERR_INVALID, "tc conv: %d layers in one launch", n);
+        for (int l = 1; l < n; ++l)
+            SVB_CHECK(a[l].B == a0.B && a[l].Cin == a0.Cin && a[l].Cout == a0.Cout && a[l].CoutP == a0.CoutP && a[l].Tq == a0.Tq &&
+                          a[l].in_Tp == a0.in_Tp && a[l].out_Tp == a0.out_Tp && a[l].ups_u == a0.ups_u && a[l].in_slope == a0.in_slope &&
+                          a[l].cin_blk == a0.cin_blk && w[l]->n_tile == w[0]->n_tile,
+                      SVB_ERR_INVALID, "tc conv: layers of one launch must share the shape class");
+        SVB_CHECK(w[0]->n_tile == 32 || w[0]->n_tile == 64 || w[0]->n_tile == 96 || w[0]->n_tile == 128, SVB_ERR_INVALID,
+                  "tc conv: %d columns per tile", w[0]->n_tile);
+        const int cin_eff = a0.cin_blk > 0 ? a0.cin_blk : a0.Cin;     // input channels one column block contracts over
+        p.n_tile = w[0]->n_tile, p.n_chunks = (cin_eff + kTcCK - 1) / kTcCK;
+        p.blk_chunk_step = a0.cin_blk > 0 ? p.n_chunks : 0;
+        int ks_sum = 0;
+        for (int l = 0; l < n; ++l) halo = std::max(halo, (a[l].KS - 1) / 2 * a[l].dil), ks_sum += a[l].KS;
+        const int tiles = (a0.Tq + kTcM - 1) / kTcM;              // 128-row tiles per clip
+        p.col_blocks = a0.CoutP / p.n_tile;
+        p.wtile_bytes = (uint32_t)p.n_tile * 128 * planes;
+        const size_t bias_bytes = (size_t)n * a0.Cout <= 1024 ? kBiasBytes : 3 * kBiasBytes;
+        SVB_CHECK((size_t)n * a0.Cout * 4 <= bias_bytes, SVB_ERR_INVALID, "tc conv: %d layers x %d biases exceed the shared-memory bias area", n, a0.Cout);
+        // narrow layers (one chunk, one column block) keep every layer's tiles resident
+        const size_t res_bytes = p.n_chunks == 1 && p.col_blocks == 1 ? (size_t)ks_sum * p.wtile_bytes : 0;
+        // ---- items of MT tiles: MT = 2 (each weight tile feeds 256 rows; the two math warpgroups hold two m64 blocks each)
+        // when a clip has 2 tiles and the 256-row slabs fit shared memory next to a weight ring of 2 tiles (or the resident
+        // weights), else MT = 1.  Work lists may still carry one-tile items (odd tile counts, balance splits).
+        auto fit = [&](int mt) {
+            p.MT = mt;
+            p.op_bytes = (uint32_t)round_up(mt * kTcM + 2 * halo, 8) * 128 * planes;
+            return tc_layout(p, smem, 227 * 1024 - bias_bytes, bias_bytes, 3, 0, res_bytes, tc_epi_pieces(n, a, mt, p.n_tile), false);
+        };
+        bool two = tiles >= 2 && fit(2);
+        if (two && grid > 0) {
+            // implicit round-robin list over `grid` CTAs: keep MT = 2 only if its makespan (in tiles) is no longer
+            const long long per = (long long)a0.B * (a0.CoutP / p.n_tile);
+            const long long g1 = per * tiles, g2 = per * ((tiles + 1) / 2);
+            two = 2 * ((g2 + grid - 1) / grid) <= (g1 + grid - 1) / grid;
+        }
+        if (!two) SVB_CHECK(fit(1), SVB_ERR_INVALID, "tc conv: tile does not fit shared memory (N %d)", p.n_tile);
+        p.fused_P = 0, p.off_inter = 0, p.inter_bytes = 0;
+        p.groups_per_b = (tiles + p.MT - 1) / p.MT;
+        p.total_groups = p.groups_per_b * a0.B * p.col_blocks;
+    }
     p.a = a0, p.n_layers = n;
     p.work = nullptr, p.work_off = nullptr;
-    const int cin_eff = a0.cin_blk > 0 ? a0.cin_blk : a0.Cin;     // input channels one column block contracts over
-    p.n_tile = w[0]->n_tile, p.n_chunks = (cin_eff + kTcCK - 1) / kTcCK;
-    p.blk_chunk_step = a0.cin_blk > 0 ? p.n_chunks : 0;
-    int halo = 0, ks_sum = 0;
-    for (int l = 0; l < n; ++l) halo = std::max(halo, (a[l].KS - 1) / 2 * a[l].dil), ks_sum += a[l].KS;
-    const int tiles = (a0.Tq + kTcM - 1) / kTcM;              // 128-row tiles per clip
-    p.col_blocks = a0.CoutP / p.n_tile;
-    const int planes = precision == SVB_PREC_TF32X3 ? 2 : 1;
-    p.wtile_bytes = (uint32_t)p.n_tile * 128 * planes;
-    p.pdl = 1;
-    if (const char *e = getenv("SVB_TC_PDL")) p.pdl = atoi(e) != 0;
-    // ---- items of MT tiles: MT = 2 (each weight tile feeds 256 rows; the two math warpgroups hold two m64 blocks each)
-    // when a clip has 2 tiles and the 256-row slabs fit shared memory next to a weight ring of 2 tiles (or the resident
-    // weights), else MT = 1.  Work lists may still carry one-tile items (odd tile counts, balance splits).
-    smem = 0;
-    const size_t bias_bytes = (size_t)n * a0.Cout <= 1024 ? kBiasBytes : 3 * kBiasBytes;
-    SVB_CHECK((size_t)n * a0.Cout * 4 <= bias_bytes, SVB_ERR_INVALID, "tc conv: %d layers x %d biases exceed the shared-memory bias area", n, a0.Cout);
-    const size_t budget = 227 * 1024 - bias_bytes;
-    // operand slots double as TMA targets: 3 of them keep two slab copies in flight behind the MMAs
-    int nA_pref = 3;
-    if (const char *e = getenv("SVB_TC_NA")) nA_pref = std::max(2, std::min(4, atoi(e)));
-    // narrow layers (one chunk, one column block): every layer's tiles stay resident
-    const size_t res_bytes = (size_t)ks_sum * p.wtile_bytes;
-    const bool can_res = p.n_chunks == 1 && p.col_blocks == 1;
-    auto fit = [&](int mt) {
-        p.MT = mt;
-        p.op_bytes = (uint32_t)round_up(mt * kTcM + 2 * halo, 8) * 128 * planes;
-        p.off_op = 1024 + kItemBytes;
-        p.w_resident = 0;
-        for (int nA : {nA_pref, 2}) {
-            if (can_res && p.off_op + (size_t)nA * p.op_bytes + res_bytes <= budget) {
-                p.nA = nA, p.w_resident = 1;
-                break;
-            }
-        }
-        if (!p.w_resident) {
-            p.nA = nA_pref;
-            if (p.off_op + (size_t)p.nA * p.op_bytes + 2 * (size_t)p.wtile_bytes > budget) p.nA = 2;
-            if (p.off_op + (size_t)p.nA * p.op_bytes + (size_t)(mt == 2 ? 2 : 1) * p.wtile_bytes > budget) return false;
-        }
-        p.off_w = p.off_op + (uint32_t)p.nA * p.op_bytes;
-        const size_t avail = budget - p.off_w;
-        size_t w_area;
-        if (p.w_resident) {
-            p.nW = 1, p.w_res_bytes = (uint32_t)res_bytes, w_area = res_bytes;
-        } else {
-            p.nW = std::max(1, std::min((int)(avail / p.wtile_bytes), kMaxW));
-            p.w_res_bytes = 0, w_area = (size_t)p.nW * p.wtile_bytes;
-        }
-        p.off_bias = p.off_w + (uint32_t)round_up((int)w_area, 1024);
-        smem = (size_t)p.off_bias + bias_bytes;
-        return true;
-    };
-    bool two = tiles >= 2 && fit(2);
-    if (two && grid > 0) {
-        // implicit round-robin list over `grid` CTAs: keep MT = 2 only if its makespan (in tiles) is no longer
-        const long long per = (long long)a0.B * (a0.CoutP / p.n_tile);
-        const long long g1 = per * tiles, g2 = per * ((tiles + 1) / 2);
-        two = 2 * ((g2 + grid - 1) / grid) <= (g1 + grid - 1) / grid;
-    }
-    if (!two) SVB_CHECK(fit(1), SVB_ERR_INVALID, "tc conv: tile does not fit shared memory (N %d)", p.n_tile);
-    // the piece ring of the streamed epilogue goes between the weights and the bias; it never changes MT or nA
-    p.epi_slots = 0, p.off_epi = 0;
-    if (const int pieces = tc_epi_pieces(n, a, p.MT, p.n_tile)) {
-        const size_t fixed = p.w_resident ? (size_t)round_up((int)res_bytes, 1024) : 0;   // resident tiles: nothing to shrink
-        int nW = p.w_resident ? 0 : p.nW;
-        const size_t avail = budget - p.off_w;
-        const int s = avail > fixed ? tc_epi_fit(avail - fixed, p.w_resident ? 1u : p.wtile_bytes, pieces, pieces / (p.MT * (p.n_tile / 32)), &nW) : 0;
-        if (s > 0) {
-            if (!p.w_resident) p.nW = nW;
-            p.epi_slots = s;
-            p.off_epi = p.off_w + (uint32_t)round_up((int)(p.w_resident ? fixed : (size_t)p.nW * p.wtile_bytes), 1024);
-            p.off_bias = p.off_epi + (uint32_t)s * kMathWarps * kEpiPieceBytes;
-            smem = (size_t)p.off_bias + bias_bytes;
-        }
-    }
-    SVB_CHECK(smem <= 227 * 1024, SVB_ERR_INVALID, "tc conv: no tiling fits (N %d, %d layers)", p.n_tile, n);
-    p.l2_prefetch = p.epi_slots == 0 && tc_epi_sources(n, a) > 0;
+    p.l2_prefetch = p.epi_slots == 0 && tc_epi_sources(n, fused ? a + n : a) > 0;
+    const int n_tab = fused ? 2 * n : n;
     uint32_t res_off = 0;
-    for (int l = 0; l < n; ++l) {
+    for (int l = 0; l < n_tab; ++l) {
         TcLayer &L = p.L[l];
         L.in = a[l].in, L.res = a[l].res, L.out = a[l].out, L.bias = a[l].bias;
         L.w = reinterpret_cast<const unsigned char *>(w[l]->blob[precision]);
@@ -1027,89 +1001,12 @@ static int tc_plan(int n, const TcWeights *const *w, const ConvArgs *a, int prec
         L.bias_off = l * a0.Cout, L.w_res_off = res_off;
         res_off += (uint32_t)a[l].KS * p.wtile_bytes;
     }
-    for (int l = n; l < 2 * kTcMaxLayers; ++l) p.L[l] = p.L[0];
-    p.fused_P = 0, p.off_inter = 0, p.inter_bytes = 0;
-    if (getenv("SVB_TC_VERBOSE"))
+    for (int l = n_tab; l < 2 * kTcMaxLayers; ++l) p.L[l] = p.L[0];
+    if (!fused && getenv("SVB_TC_VERBOSE"))
         fprintf(stderr, "[tc] %d layer(s) Cin %d CoutP %d KS %d.. halo %d Tq %d | n_tile %d MT %d nA %d nW %d resident %d smem %zu epi %d l2pf %d\n", n,
-                a0.Cin, a0.CoutP, a0.KS, halo, a0.Tq, p.n_tile, p.MT, p.nA, p.nW, p.w_resident, smem, p.epi_slots, p.l2_prefetch);
-    p.groups_per_b = (tiles + p.MT - 1) / p.MT;
-    p.total_groups = p.groups_per_b * a0.B * p.col_blocks;
+                a0.Cin, a0.CoutP, a0.KS, halo, a0.Tq, p.n_tile, p.MT, p.nA, p.nW, p.w_resident, smem,
+                p.epi_slots, p.l2_prefetch);
     return SVB_OK;
-}
-
-// Plan of a fused launch over n ResBlock chains: a[0..n) are the c1 layers, a[n..2n) the c2 layers of the same step.
-// Every item is 256 c1 rows; the c1 slab slots, the intermediate (256 + 2 max h2 rows per 32-channel chunk), a weight
-// ring of at least 2 tiles (c1's and c2's tiles stream through it in order) and the biases of all 2n layers share the
-// shared memory.  ctas = 1: up to 227 KB, three slab slots.  ctas = 2 (C = 32 only, the kernel compiled for two CTAs
-// per SM): half of the SM's 228 KB less the 1 KB each CTA reserves, so one slab slot (the next item's slab is copied and
-// transformed while this item runs c1's epilogue and c2; the other CTA's MMAs cover the rest) and a bias area of just
-// the 2n layers' biases.  Returns false when the shape is not one a fused launch runs or the layout does not fit.
-constexpr size_t kSmemPerSm = 228 * 1024, kSmemReservedPerCta = 1024;
-static bool tc_plan_fused(int n, const TcWeights *const *w, const ConvArgs *a, int precision, int ctas, TcArgs &p, size_t &smem) {
-    if (n < 1 || n > kTcMaxLayers) return false;
-    const ConvArgs &a0 = a[0];
-    for (int l = 0; l < 2 * n; ++l) {
-        if (a[l].B != a0.B || a[l].Cin != a0.Cin || a[l].Cout != a0.Cin || a[l].CoutP != a0.Cin || a[l].Tq != a0.Tq ||
-            a[l].in_Tp != a0.in_Tp || a[l].out_Tp != a0.in_Tp || a[l].ups_u != 0 || a[l].cin_blk != 0 ||
-            a[l].in_slope != a0.in_slope || !w[l]->ok || w[l]->n_tile != a0.Cin || (l >= n && a[l].dil != 1))
-            return false;
-    }
-    if ((a0.Cin != 32 && a0.Cin != 64) || (ctas != 1 && ctas != tc_min_ctas(a0.Cin, true))) return false;
-    const int planes = precision == SVB_PREC_TF32X3 ? 2 : 1;
-    int h1 = 0, h2 = 0;
-    for (int l = 0; l < n; ++l) h1 = std::max(h1, (a[l].KS - 1) / 2 * a[l].dil), h2 = std::max(h2, (a[n + l].KS - 1) / 2);
-    if (h1 + h2 > kPad || 2 * h2 >= kTcM) return false;           // the shifted slab starts inside the zero padding
-    p.a = a0, p.n_layers = n;
-    p.work = nullptr, p.work_off = nullptr;
-    p.n_tile = a0.Cin, p.n_chunks = a0.Cin / kTcCK, p.blk_chunk_step = 0, p.col_blocks = 1;
-    p.MT = 2, p.w_resident = 0, p.w_res_bytes = 0;
-    p.wtile_bytes = (uint32_t)p.n_tile * 128 * planes;
-    p.pdl = 1;
-    if (const char *e = getenv("SVB_TC_PDL")) p.pdl = atoi(e) != 0;
-    p.fused_P = 2 * kTcM - 2 * h2;
-    p.op_bytes = (uint32_t)round_up(2 * kTcM + 2 * h1, 8) * 128 * planes;
-    p.inter_bytes = (uint32_t)round_up(2 * kTcM + 2 * h2, 8) * 128 * planes;
-    // 2n x Cout <= 6 x 64 floats
-    const size_t bias_bytes = ctas == 1 ? kBiasBytes : (size_t)round_up(2 * n * a0.Cout * 4, 128);
-    const size_t smem_max = ctas == 1 ? 227 * 1024 : kSmemPerSm / 2 - kSmemReservedPerCta;
-    const size_t budget = smem_max - bias_bytes;
-    int nA_pref = ctas == 1 ? 3 : 1;
-    if (const char *e = getenv("SVB_TC_NA"); e && ctas == 1) nA_pref = std::max(2, std::min(4, atoi(e)));
-    p.off_op = 1024 + kItemBytes;
-    const size_t inter_area = (size_t)p.n_chunks * p.inter_bytes;
-    p.nA = nA_pref;
-    if (p.off_op + (size_t)p.nA * p.op_bytes + inter_area + 2 * (size_t)p.wtile_bytes > budget) p.nA = std::min(p.nA, 2);
-    if (p.off_op + (size_t)p.nA * p.op_bytes + inter_area + 2 * (size_t)p.wtile_bytes > budget) return false;
-    // the piece ring of the streamed epilogue (c2's residual / running sum) comes out of the weight ring; where it does not
-    // fit next to 3 slab slots (C = 64 at k 11, d 5), the plan drops to 2 slots for it
-    const int pieces = tc_epi_pieces(n, a + n, 2, p.n_tile);
-    auto layout = [&](int nA, bool ring) {
-        p.nA = nA;
-        p.off_inter = p.off_op + (uint32_t)nA * p.op_bytes;
-        p.off_w = p.off_inter + (uint32_t)inter_area;
-        p.nW = std::min((int)((budget - p.off_w) / p.wtile_bytes), kMaxW);
-        p.epi_slots = ring ? tc_epi_fit(budget - p.off_w, p.wtile_bytes, pieces, pieces / (2 * (p.n_tile / 32)), &p.nW) : 0;
-        return p.epi_slots > 0;
-    };
-    const int nA = p.nA;
-    if (!pieces || !(layout(nA, true) || (nA > 2 && layout(2, true)))) layout(nA, false);
-    if (const char *e = getenv("SVB_TC_NW")) p.nW = std::min(p.nW, std::max(2, atoi(e)));      // ring depth (measurement)
-    p.l2_prefetch = p.epi_slots == 0 && tc_epi_sources(n, a + n) > 0;
-    p.off_epi = p.off_w + (uint32_t)round_up(p.nW * (int)p.wtile_bytes, 1024);
-    p.off_bias = p.off_epi + (uint32_t)p.epi_slots * kMathWarps * kEpiPieceBytes;
-    smem = (size_t)p.off_bias + bias_bytes;
-    if (smem > smem_max) return false;
-    for (int l = 0; l < 2 * n; ++l) {
-        TcLayer &L = p.L[l];
-        L.in = a[l].in, L.res = a[l].res, L.out = a[l].out, L.bias = a[l].bias;
-        L.w = reinterpret_cast<const unsigned char *>(w[l]->blob[precision]);
-        L.KS = a[l].KS, L.dil = a[l].dil, L.out_scale = a[l].out_scale, L.accumulate = a[l].accumulate;
-        L.bias_off = l * a0.Cout, L.w_res_off = 0;
-    }
-    for (int l = 2 * n; l < 2 * kTcMaxLayers; ++l) p.L[l] = p.L[0];
-    p.groups_per_b = (a0.Tq + p.fused_P - 1) / p.fused_P;
-    p.total_groups = p.groups_per_b * a0.B;
-    return true;
 }
 
 template <int MODE>
@@ -1134,14 +1031,14 @@ static int tc_dispatch(TcArgs &p, int precision, int grid, size_t smem, cudaStre
     }
 }
 
-int launch_conv_tc(const TcWeights &w, const ConvArgs &a, int precision, cudaStream_t st, int max_ctas) {
+int launch_conv_tc(const TcWeights &w, const ConvArgs &a, int precision, cudaStream_t st) {
     SVB_CHECK(precision >= SVB_PREC_TF32 && precision <= SVB_PREC_BF16X3, SVB_ERR_INVALID, "tc conv: bad precision %d",
               precision);
     TcArgs p;
     size_t smem = 0;
     const TcWeights *wp = &w;
-    const int ctas = max_ctas > 0 ? std::min(max_ctas, sm_count()) : sm_count();
-    SVB_TRY(tc_plan(1, &wp, &a, precision, ctas, p, smem));
+    const int ctas = sm_count();
+    SVB_TRY(tc_plan(1, &wp, &a, precision, 0, ctas, p, smem));
     const int grid = std::min(p.total_groups, ctas);
     if ((p.total_groups + grid - 1) / grid > kMaxItems) {
         // more items per CTA than the shared-memory list holds: run the batch in slices of clips
@@ -1154,7 +1051,7 @@ int launch_conv_tc(const TcWeights &w, const ConvArgs &a, int precision, cudaStr
             s.in = a.in + (size_t)b0 * c4t_groups(a.Cin) * a.in_Tp * 32;
             s.out = a.out + (size_t)b0 * c4t_groups(a.Cout) * a.out_Tp * 32;
             if (a.res) s.res = a.res + (size_t)b0 * c4t_groups(a.Cout) * a.out_Tp * 32;
-            SVB_TRY(launch_conv_tc(w, s, precision, st, max_ctas));
+            SVB_TRY(launch_conv_tc(w, s, precision, st));
         }
         return SVB_OK;
     }
@@ -1256,8 +1153,7 @@ int tc_schedule(int n, const int *KS, const int *KS2, const int *has_res, const 
             if (X.b != Y.b) return X.b < Y.b;
             return X.t0 < Y.t0;
         });
-        const char *il = getenv("SVB_TC_INTERLEAVE");
-        if (!chain_ordered && n > 1 && !(il && atoi(il) == 0)) {
+        if (!chain_ordered && n > 1) {
             // alternate the layers inside a CTA (long and short items interleaved) instead of layer after layer: the slab
             // prefetch of a short-kernel item hides behind the MMAs of a long one
             std::vector<std::vector<int>> by(n);
@@ -1290,15 +1186,6 @@ int tc_schedule(int n, const int *KS, const int *KS2, const int *has_res, const 
     return SVB_OK;
 }
 
-// plan of a merged (fused = false: n layers) or fused (n chains, 2n layers, `ctas` per SM) launch
-static int tc_plan_multi(int n, const TcWeights *const *w, const ConvArgs *a, int precision, bool fused, int ctas, TcArgs &p,
-                         size_t &smem) {
-    if (!fused) return tc_plan(n, w, a, precision, 0, p, smem);
-    SVB_CHECK(tc_plan_fused(n, w, a, precision, ctas, p, smem), SVB_ERR_INVALID, "tc conv: no fused layout for %d chains of C = %d",
-              n, a[0].Cin);
-    return SVB_OK;
-}
-
 // CTAs of the fused kernel that fit one SM at `smem` bytes (the runtime's occupancy calculator: registers, threads, shared
 // memory and the per-CTA reservation of this device)
 template <int MODE, int N>
@@ -1321,7 +1208,7 @@ static int tc_fused_occupancy(size_t smem) {
 static bool tc_fused_fits_ctas(int n, const TcWeights *const *w, const ConvArgs *a, int precision, int ctas) {
     TcArgs p;
     size_t smem = 0;
-    if (!tc_plan_fused(n, w, a, precision, ctas, p, smem)) return false;
+    if (tc_plan(n, w, a, precision, ctas, 0, p, smem) != SVB_OK) return false;
     if (ctas > 1) {
         int fit = 0;
         switch (precision) {
@@ -1360,7 +1247,7 @@ int tc_worklist_build(int n, const TcWeights *const *w, const ConvArgs *a, int p
     size_t smem = 0;
     const int ctas = fused ? tc_fused_ctas(n, w, a, precision) : 1;
     SVB_CHECK(ctas > 0, SVB_ERR_INVALID, "tc conv: no fused plan for %d chains of C = %d", n, a[0].Cin);
-    SVB_TRY(tc_plan_multi(n, w, a, precision, fused, ctas, p, smem));
+    SVB_TRY(tc_plan(n, w, a, precision, fused ? ctas : 0, 0, p, smem));
     const int grid = ctas * sm_count();
     const ConvArgs *ao = fused ? a + n : a;                      // the layers whose epilogue writes the output
     int KS[kTcMaxLayers], KS2[kTcMaxLayers], has_res[kTcMaxLayers], accum[kTcMaxLayers];
@@ -1387,9 +1274,9 @@ int launch_conv_tc_multi(int n, const TcWeights *const *w, const ConvArgs *a, in
     TcArgs p;
     size_t smem = 0;
     // a fused list fixes the plan (CTAs per SM); a layer set that plan no longer fits makes the list stale (the caller rebuilds)
-    if (fused) SVB_CHECK(tc_plan_fused(n, w, a, precision, wl.ctas_per_sm, p, smem), SVB_ERR_STATE,
-                         "tc conv: fused work list was built for %d CTAs per SM", wl.ctas_per_sm);
-    else SVB_TRY(tc_plan(n, w, a, precision, 0, p, smem));
+    const int rc = tc_plan(n, w, a, precision, fused ? wl.ctas_per_sm : 0, 0, p, smem);
+    SVB_CHECK(rc == SVB_OK || !fused, SVB_ERR_STATE, "tc conv: fused work list was built for %d CTAs per SM", wl.ctas_per_sm);
+    SVB_TRY(rc);
     SVB_CHECK(wl.items && wl.n_layers == n && wl.MT == p.MT && wl.fused == fused && wl.grid == wl.ctas_per_sm * sm_count(), SVB_ERR_STATE,
               "tc conv: work list was built for another plan (layers %d / %d, MT %d / %d)", wl.n_layers, n, wl.MT, p.MT);
     p.work = wl.items, p.work_off = wl.off;

@@ -13,12 +13,14 @@ struct TcWeights {
     bool ok = false;
 };
 
-// packed_ffma: [KS][Cin][CoutP] fp32 (the FFMA packing).  Allocations are appended to `allocs`.
-// force_n_tile > 0: GEMM columns per CTA fixed by the caller (grouped layers: one tile = whole conv groups; `Cin` is then
-// the number of input channels ONE column block contracts over and packed_ffma is [KS][Cin][CoutP])
-int tc_pack_weights(const float *packed_ffma, int KS, int Cin, int CoutP, TcWeights *out, std::vector<void *> *allocs,
-                    int force_n_tile = 0);
-// same packing on the device, from a device copy of the FFMA packing into the blobs tc_pack_weights allocated
+// Picks the tiling and allocates the three blobs (appended to `allocs`); out->ok = false when the layer has no tensor-core
+// tiling.  packed_ffma_dev: device [KS][Cin][CoutP] fp32 (the FFMA packing), written on stream `st`: the blobs are filled
+// from it on that stream, which is synchronized before the call returns.  nullptr: the blobs are only allocated, for a
+// later tc_repack_weights_dev.  force_n_tile > 0: GEMM columns per CTA fixed by the caller (grouped layers: one tile =
+// whole conv groups; `Cin` is then the number of input channels ONE column block contracts over)
+int tc_pack_weights(const float *packed_ffma_dev, int KS, int Cin, int CoutP, TcWeights *out, std::vector<void *> *allocs,
+                    cudaStream_t st, int force_n_tile = 0);
+// fills the blobs tc_pack_weights allocated from a device copy of the FFMA packing, asynchronously on `st`
 // (training: the weights change after every optimizer step)
 int tc_repack_weights_dev(const float *packed_ffma_dev, const TcWeights &w, cudaStream_t st);
 bool tc_supported(const TcWeights &w, const ConvArgs &a);
@@ -49,7 +51,8 @@ bool tc_fused_fits(int n, const TcWeights *const *w, const ConvArgs *a, int prec
 // one persistent launch over `n` layers that share channels / rows / upsampling (taps, dilation and pointers may differ)
 int launch_conv_tc_multi(int n, const TcWeights *const *w, const ConvArgs *a, int precision, cudaStream_t st, const TcWorkList &wl,
                          bool fused = false);
-// max_ctas > 0 caps the persistent grid (used to run independent ResBlock chains side by side on SM subsets)
-int launch_conv_tc(const TcWeights &w, const ConvArgs &a, int precision, cudaStream_t st, int max_ctas = 0);
+// one persistent launch over one layer, one CTA per SM on the implicit round-robin list (batches whose items overflow the
+// per-CTA item table run in slices of clips)
+int launch_conv_tc(const TcWeights &w, const ConvArgs &a, int precision, cudaStream_t st);
 
 }  // namespace svb

@@ -50,7 +50,7 @@ int pack_conv(svb_gen *g, const std::string &prefix, int Cin, int Cout, int K, i
     L->macs_per_row = (double)Cin * Cout * K;
     SVB_TRY(gen_upload(g, p, &L->w));
     SVB_TRY(gen_upload(g, b->data, &L->b));
-    SVB_TRY(tc_pack_weights(p.data(), K, Cin, Cout, &L->tc, &g->dev_allocs));
+    SVB_TRY(tc_pack_weights(L->w, K, Cin, Cout, &L->tc, &g->dev_allocs, 0));
     return SVB_OK;
 }
 
@@ -65,7 +65,7 @@ int pack_convT(svb_gen *g, const std::string &prefix, int Cin, int Cout, int K, 
     L->macs_per_row = (double)Cin * Cout * K;    // per input row: u outputs x K/u taps
     SVB_TRY(gen_upload(g, p, &L->w));
     SVB_TRY(gen_upload(g, b->data, &L->b));
-    SVB_TRY(tc_pack_weights(p.data(), KS, Cin, u * Cout, &L->tc, &g->dev_allocs));
+    SVB_TRY(tc_pack_weights(L->w, KS, Cin, u * Cout, &L->tc, &g->dev_allocs, 0));
     return SVB_OK;
 }
 
@@ -92,7 +92,7 @@ ConvArgs resblock_args(const ConvLayer &L, const float *in, float *out, const fl
 // fits.  Training keeps two launches per step: its tape needs every c1 input in HBM.
 bool stage_fused(const svb_gen *g, const Stage &s, int B, int Ti) {
     const int nk = g->cfg.n_resblock_kernels, nd = g->cfg.n_dilations;
-    if (!g->fuse || !g->merge || g->chains > 1 || g->training || g->cfg.resblock != 1 || g->cfg.precision == SVB_PREC_FP32 || s.C > 64 ||
+    if (!g->fuse || !g->merge || g->training || g->cfg.resblock != 1 || g->cfg.precision == SVB_PREC_FP32 || s.C > 64 ||
         nk > kTcMaxLayers)
         return false;
     for (int m = 0; m < nd; ++m) {
@@ -169,7 +169,7 @@ struct ProfScope {
 };
 
 int run_conv(svb_gen *g, const ConvLayer &L, const float *in, int in_Tp, float *out, int out_Tp, const float *res,
-             int B, int Tq, float in_slope, float scale, int accumulate, cudaStream_t st, int max_ctas = 0) {
+             int B, int Tq, float in_slope, float scale, int accumulate, cudaStream_t st) {
     g->last_launches += 1;
     g->last_flops += 2.0 * L.macs_per_row * (double)B * Tq;
     const bool tc = g->cfg.precision != SVB_PREC_FP32 && L.tc.ok;
@@ -183,7 +183,7 @@ int run_conv(svb_gen *g, const ConvLayer &L, const float *in, int in_Tp, float *
     a.B = B, a.Cin = L.Cin, a.in_Tp = in_Tp, a.Cout = L.Cout, a.out_Tp = out_Tp, a.CoutP = L.CoutP, a.Tq = Tq;
     a.KS = L.KS, a.dil = L.dil, a.ups_u = L.ups_u, a.in_slope = in_slope, a.out_scale = scale, a.accumulate = accumulate;
     a.epi_stream = g->epi;
-    if (g->cfg.precision != SVB_PREC_FP32 && tc_supported(L.tc, a)) return launch_conv_tc(L.tc, a, g->cfg.precision, st, max_ctas);
+    if (g->cfg.precision != SVB_PREC_FP32 && tc_supported(L.tc, a)) return launch_conv_tc(L.tc, a, g->cfg.precision, st);
     return launch_conv_ffma(a, st);
 }
 
@@ -269,7 +269,7 @@ int forward_impl(svb_gen *g, const float *mel, bool mel_frame_major, const float
         // so it overlaps conv_pre and the first upsampler.
         har = F(bf.har);
         har_on_side = !g->profile;
-        cudaStream_t ns = har_on_side ? g->side[0] : st;
+        cudaStream_t ns = har_on_side ? g->side : st;
         if (har_on_side) {
             SVB_CUDA(cudaEventRecord(g->ev_fork, st));
             SVB_CUDA(cudaStreamWaitEvent(ns, g->ev_fork, 0));
@@ -280,7 +280,7 @@ int forward_impl(svb_gen *g, const float *mel, bool mel_frame_major, const float
             SVB_TRY(launch_nsf_source(f0, rand_ini, noise, seed, B, T, g->hop, (float)g->cfg.audio_sample_rate, g->lin_w,
                                       g->lin_b_dev, g->ws + bf.nsf, har, g->training ? F(bf.sines) : nullptr, ns, &l));
         }
-        if (har_on_side) SVB_CUDA(cudaEventRecord(g->ev_chain[0], ns));
+        if (har_on_side) SVB_CUDA(cudaEventRecord(g->ev_side, ns));
         g->last_launches += l;
         g->taps["har_source"] = Tap{har, 1, Tw, 0, true};
     }
@@ -298,7 +298,7 @@ int forward_impl(svb_gen *g, const float *mel, bool mel_frame_major, const float
         // x = ups[i](leaky_relu(x, 0.1))            hifigan.py:153-154
         SVB_TRY(run_conv(g, s.up, x_in, Tin_p, X, Tip, nullptr, B, Tin, 0.1f, 1.f, 0, st));
         if (f0) {                                   // x = x + noise_convs[i](har_source)   :155-157
-            if (har_on_side && i == 0) SVB_CUDA(cudaStreamWaitEvent(st, g->ev_chain[0], 0));
+            if (har_on_side && i == 0) SVB_CUDA(cudaStreamWaitEvent(st, g->ev_side, 0));
             ProfScope ps(g, st, "noise_conv_add", 4.0 * B * (2.0 * Ti * s.C + Tw), 2.0 * B * (double)Ti * s.C * s.noise.K);
             SVB_TRY(launch_noise_conv_add(X, B, s.C, Ti, Tip, har, Tw, s.noise.w, s.noise.b, s.noise.K, s.noise.stride,
                                           s.noise.pad, st));
@@ -307,12 +307,6 @@ int forward_impl(svb_gen *g, const float *mel, bool mel_frame_major, const float
         }
         g->taps["ups" + std::to_string(i)] = Tap{X, s.C, Ti, Tip, false};
         // xs = sum_j resblocks[i*nk + j](x) ; x = xs / nk      :158-164
-        // The nk ResBlocks only share their input: each chain runs on its own stream and SM subset, which
-        // amortises the per-launch fill/drain of the persistent kernels; the final convs (which add
-        // into S) are ordered by events.
-        const bool par = g->chains > 1 && nk > 1 && nk <= 3 && g->cfg.precision != SVB_PREC_FP32 && !g->profile;
-        int sms = 0;
-        SVB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, g->device));
         const bool fused = stage_fused(g, s, B, Ti);
         if (fused) {
             for (int m = 0; m < nd; ++m) {
@@ -333,7 +327,7 @@ int forward_impl(svb_gen *g, const float *mel, bool mel_frame_major, const float
             }
         }
         // merged schedule: step m of all nk chains in ONE persistent launch (the chains only share their input)
-        bool merged = !fused && g->merge && !par && nk > 1 && nk <= kTcMaxLayers && g->cfg.precision != SVB_PREC_FP32 &&
+        bool merged = !fused && g->merge && nk > 1 && nk <= kTcMaxLayers && g->cfg.precision != SVB_PREC_FP32 &&
                       s.c1[0][0].tc.ok && tc_merge_fits(nk, B, Ti, s.C, s.c1[0][0].tc.n_tile);
         for (int j = 0; merged && j < nk; ++j)
             for (int m = 0; m < nd; ++m) {
@@ -372,22 +366,7 @@ int forward_impl(svb_gen *g, const float *mel, bool mel_frame_major, const float
                 }
             }
         }
-        if (par) SVB_CUDA(cudaEventRecord(g->ev_fork, st));
         for (int j = 0; j < nk && !merged && !fused; ++j) {
-            cudaStream_t cs = par ? g->side[j] : st;
-            // SM share of a chain ~ its cost: kernel size plus a constant for the memory-bound part
-            int cap = 0;
-            if (par) {
-                double wsum = 0, wj = 0;
-                for (int jj = 0; jj < nk; ++jj) {
-                    const double wv = g->cfg.resblock_kernel_sizes[jj] + g->chain_bias;
-                    wsum += wv;
-                    if (jj == j) wj = wv;
-                }
-                cap = std::max(8, (int)(sms * wj / wsum + 0.5));
-                if (g->chains == 2) cap = 0;    // full grids on every stream: the block scheduler interleaves the chains' CTAs
-            }
-            if (par) SVB_CUDA(cudaStreamWaitEvent(cs, g->ev_fork, 0));
             for (int m = 0; m < nd; ++m) {
                 float *A = F(bf.A[i][j][m]);
                 const float *xin = m == 0 ? X : F(bf.R[i][j][m - 1]);
@@ -396,19 +375,15 @@ int forward_impl(svb_gen *g, const float *mel, bool mel_frame_major, const float
                 const float scale = last ? 1.f / nk : 1.f;
                 const int accum = (last && j > 0) ? 1 : 0;
                 if (g->cfg.resblock == 1) {         // ResBlock1.forward :54-61
-                    SVB_TRY(run_conv(g, s.c1[j][m], xin, Tip, A, Tip, nullptr, B, Ti, 0.1f, 1.f, 0, cs, cap));
-                    if (par && last && j > 0) SVB_CUDA(cudaStreamWaitEvent(cs, g->ev_chain[j - 1], 0));
-                    SVB_TRY(run_conv(g, s.c2[j][m], A, Tip, dst, Tip, xin, B, Ti, 0.1f, scale, accum, cs, cap));
+                    SVB_TRY(run_conv(g, s.c1[j][m], xin, Tip, A, Tip, nullptr, B, Ti, 0.1f, 1.f, 0, st));
+                    SVB_TRY(run_conv(g, s.c2[j][m], A, Tip, dst, Tip, xin, B, Ti, 0.1f, scale, accum, st));
                 } else {                            // ResBlock2.forward :81-86 (never in place: ping-pong A / R)
                     const float *xin2 = m == 0 ? X : (m % 2 ? F(bf.R[i][j][m - 1]) : F(bf.A[i][j][m - 1]));
                     float *dst2 = last ? S : (m % 2 ? F(bf.A[i][j][m]) : F(bf.R[i][j][m]));
-                    if (par && last && j > 0) SVB_CUDA(cudaStreamWaitEvent(cs, g->ev_chain[j - 1], 0));
-                    SVB_TRY(run_conv(g, s.c1[j][m], xin2, Tip, dst2, Tip, xin2, B, Ti, 0.1f, scale, accum, cs, cap));
+                    SVB_TRY(run_conv(g, s.c1[j][m], xin2, Tip, dst2, Tip, xin2, B, Ti, 0.1f, scale, accum, st));
                 }
             }
-            if (par) SVB_CUDA(cudaEventRecord(g->ev_chain[j], cs));
         }
-        if (par) SVB_CUDA(cudaStreamWaitEvent(st, g->ev_chain[nk - 1], 0));
         g->taps["stage" + std::to_string(i)] = Tap{S, s.C, Ti, Tip, false};
         // The tape as taps: every leaky-relu input of the ResBlocks, x{m} (input of step m; x0 is ups{i}) and, for ResBlock1,
         // t{m} (c1's output).  Only training keeps one buffer per step; inference reuses A / R across the steps.
@@ -471,16 +446,12 @@ extern "C" int svb_gen_create(const svb_gen_config *cfg, int device, svb_gen_t *
     SVB_CUDA(cudaEventCreate(&g->ev0));
     SVB_CUDA(cudaEventCreate(&g->ev1));
     SVB_CUDA(cudaEventCreateWithFlags(&g->ev_fork, cudaEventDisableTiming));
-    for (int i = 0; i < 3; ++i) {
-        SVB_CUDA(cudaStreamCreateWithFlags(&g->side[i], cudaStreamNonBlocking));
-        SVB_CUDA(cudaEventCreateWithFlags(&g->ev_chain[i], cudaEventDisableTiming));
-    }
-    if (const char *e = getenv("SVB_CHAINS")) g->chains = atoi(e);
+    SVB_CUDA(cudaStreamCreateWithFlags(&g->side, cudaStreamNonBlocking));
+    SVB_CUDA(cudaEventCreateWithFlags(&g->ev_side, cudaEventDisableTiming));
     if (const char *e = getenv("SVB_MERGE")) g->merge = atoi(e) != 0;
     if (const char *e = getenv("SVB_FUSE")) g->fuse = atoi(e) != 0;
     if (const char *e = getenv("SVB_EPI")) g->epi = atoi(e) != 0;
     if (const char *e = getenv("SVB_TC_FUSED_CTAS")) g->fused_ctas = atoi(e);
-    if (const char *e = getenv("SVB_CHAIN_BIAS")) g->chain_bias = atof(e);
     *out = g;
     return SVB_OK;
 }
@@ -501,10 +472,8 @@ extern "C" void svb_gen_destroy(svb_gen_t *g) {
     if (g->dev_out) cudaFree(g->dev_out);
     if (g->dev_i16) cudaFree(g->dev_i16);
     for (cudaEvent_t e : g->ev_pool) cudaEventDestroy(e);
-    for (int i = 0; i < 3; ++i) {
-        if (g->side[i]) cudaStreamDestroy(g->side[i]);
-        if (g->ev_chain[i]) cudaEventDestroy(g->ev_chain[i]);
-    }
+    if (g->side) cudaStreamDestroy(g->side);
+    if (g->ev_side) cudaEventDestroy(g->ev_side);
     if (g->ev_fork) cudaEventDestroy(g->ev_fork);
     if (g->ev0) cudaEventDestroy(g->ev0);
     if (g->ev1) cudaEventDestroy(g->ev1);

@@ -132,11 +132,9 @@ struct svb_gen {
         cudaEvent_t e0, e1;
         double bytes, flops;
     };
-    // independent ResBlock chains of a stage run side by side (SM subsets) on these streams
-    cudaStream_t side[3] = {nullptr, nullptr, nullptr};
-    cudaEvent_t ev_fork = nullptr, ev_chain[3] = {nullptr, nullptr, nullptr};
-    int chains = 1;     // side-by-side chains on SM subsets (experiment; the merged schedule is the default)
-    double chain_bias = 4.0;
+    // the NSF source runs on this stream, overlapping conv_pre and the first upsampler
+    cudaStream_t side = nullptr;
+    cudaEvent_t ev_fork = nullptr, ev_side = nullptr;
 
     // merged launches: the ResBlock chains of a stage step together in one persistent launch (conv_tc.cuh: TcWorkList).
     // Lists depend on the stage, the batch / length and the plan's MT; cached per (stage, chain_ordered, MT).

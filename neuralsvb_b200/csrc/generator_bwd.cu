@@ -25,7 +25,7 @@ int pack_dgrad(svb_gen *g, const HostTensor &w, int C, int K, int dil, ConvLayer
     L->macs_per_row = (double)C * C * K;
     SVB_TRY(gen_upload(g, p, &L->w));
     L->b = g->zero_bias;
-    SVB_TRY(tc_pack_weights(p.data(), K, C, C, &L->tc, &g->dev_allocs));
+    SVB_TRY(tc_pack_weights(L->w, K, C, C, &L->tc, &g->dev_allocs, 0));
     return SVB_OK;
 }
 

@@ -100,7 +100,7 @@ extern "C" int svb_conv1d_run(const float *x_nct_dev, const float *w_host, const
     cudaMemsetAsync(d_x, 0, nx * 4, st);
     cudaMemsetAsync(d_y, 0, ny * 4, st);
     TcWeights tcw;
-    rc = tc_pack_weights(packed.data(), KS, Cin, CoutP, &tcw, &allocs);
+    rc = tc_pack_weights(d_w, KS, Cin, CoutP, &tcw, &allocs, st);
     if (rc == SVB_OK) rc = launch_nct_to_c4t(x_nct_dev, d_x, B, Cin, T, Tp_in, st);
     if (rc == SVB_OK && res_nct_dev) {
         cudaMemsetAsync(d_r, 0, ny * 4, st);
@@ -190,7 +190,7 @@ extern "C" int svb_conv1d_backward_run(const float *x_nct_dev, const float *w_ho
     } else {
         // as a ResBlock conv: weight / bias gradient, the data-gradient conv, then the mask
         TcWeights tcw;
-        if (rc == SVB_OK) rc = tc_pack_weights(packed.data(), K, Cout, Cin, &tcw, &allocs);
+        if (rc == SVB_OK) rc = tc_pack_weights(d_w, K, Cout, Cin, &tcw, &allocs, st);
         if (rc == SVB_OK)
             rc = launch_wgrad(conv_wgrad_args(d_x, d_dy, dw_dev, B, Cin, Cout, Tp_x, T, K, dil, in_slope, precision != SVB_PREC_FP32), st);
         if (rc == SVB_OK) rc = launch_colsum(d_dy, B, Cout, T, Tp_x, db_dev, st);

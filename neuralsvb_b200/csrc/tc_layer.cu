@@ -269,8 +269,7 @@ extern "C" int svb_tc_layer_create(int32_t Cin, int32_t Cout, int32_t K, int32_t
         const std::vector<int> idx = to_idx(pk);
         SVB_TRY(dev_alloc((void **)map, idx.size() * sizeof(int)));
         SVB_CUDA(cudaMemcpy(*map, idx.data(), idx.size() * sizeof(int), cudaMemcpyHostToDevice));
-        std::vector<float> zeros(pk.size(), 0.f);
-        SVB_TRY(tc_pack_weights(zeros.data(), KS, ci, co, &cl.tc, &L->allocs));     // allocates the tile blobs
+        SVB_TRY(tc_pack_weights(nullptr, KS, ci, co, &cl.tc, &L->allocs, 0));     // allocates the tile blobs
         SVB_CHECK(cl.tc.ok, SVB_ERR_INVALID, "tc_layer_create: no tensor-core tiling for %d -> %d", ci, co);
         return SVB_OK;
     };
@@ -358,8 +357,7 @@ extern "C" int svb_tc_layer_create_grouped(int32_t Cin, int32_t Cout, int32_t K,
         const std::vector<int> idx = to_idx(pk);
         SVB_TRY(dev_alloc((void **)map, idx.size() * sizeof(int)));
         SVB_CUDA(cudaMemcpy(*map, idx.data(), idx.size() * sizeof(int), cudaMemcpyHostToDevice));
-        std::vector<float> zeros(pk.size(), 0.f);
-        SVB_TRY(tc_pack_weights(zeros.data(), KSp, cin_blk, co, &cl.tc, &L->allocs, n_tile));
+        SVB_TRY(tc_pack_weights(nullptr, KSp, cin_blk, co, &cl.tc, &L->allocs, 0, n_tile));
         SVB_CHECK(cl.tc.ok, SVB_ERR_INVALID, "tc_layer_create_grouped: no tensor-core tiling (%d channels per block, %d columns)", cin_blk, n_tile);
         return SVB_OK;
     };

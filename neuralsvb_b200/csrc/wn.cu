@@ -191,7 +191,7 @@ int wn_pack(svb_wn *w, const std::string &prefix, int Cin, int Cout, int K, int 
     SVB_CUDA(cudaMalloc((void **)&c->b, (size_t)Cout * 4));
     w->allocs.push_back(c->b);
     SVB_CUDA(cudaMemcpy(c->b, bt->data.data(), (size_t)Cout * 4, cudaMemcpyHostToDevice));
-    SVB_TRY(tc_pack_weights(p.data(), K, Cin, Cout, &c->tc, &w->allocs));
+    SVB_TRY(tc_pack_weights(c->w, K, Cin, Cout, &c->tc, &w->allocs, 0));
     return SVB_OK;
 }
 
@@ -279,7 +279,7 @@ extern "C" int svb_wn_finalize(svb_wn_t *w) {
         SVB_CUDA(cudaMalloc((void **)&c.b, (size_t)w->H * 4));
         w->allocs.push_back(c.b);
         SVB_CUDA(cudaMemcpy(c.b, bt->data.data(), (size_t)w->H * 4, cudaMemcpyHostToDevice));
-        SVB_TRY(tc_pack_weights(p.data(), KS, w->latent, w->stride * w->H, &c.tc, &w->allocs));
+        SVB_TRY(tc_pack_weights(c.w, KS, w->latent, w->stride * w->H, &c.tc, &w->allocs, 0));
         SVB_TRY(wn_pack(w, "out_proj", w->H, w->out_ch, 1, 1, &w->post));
     }
     w->finalized = true;
@@ -470,7 +470,7 @@ int wn_add_conv_jobs(svb_wn *w, const std::string &prefix, WnConv *c) {
     const std::vector<float> p = pack_dgrad_weights(ht.data.data(), c->Cout, c->Cin, c->K);
     SVB_TRY(wn_train_alloc(w, p.size() * 4, &c->dw));
     SVB_CUDA(cudaMemcpy(c->dw, p.data(), p.size() * 4, cudaMemcpyHostToDevice));
-    SVB_TRY(tc_pack_weights(p.data(), c->K, c->Cout, c->Cin, &c->dtc, &w->train_allocs));
+    SVB_TRY(tc_pack_weights(c->dw, c->K, c->Cout, c->Cin, &c->dtc, &w->train_allocs, 0));
     const std::vector<float> id = iota1(ht.data.size());
     PackJob f, d, b;
     f.src = d.src = prefix + ".weight", b.src = prefix + ".bias";

@@ -1,4 +1,4 @@
-"""-m gpu: the fused C = 32 ResBlock1 steps at two CTAs per SM (conv_tc.cu: tc_plan_fused with ctas = 2) against the same
+"""-m gpu: the fused C = 32 ResBlock1 steps at two CTAs per SM (conv_tc.cu: tc_plan with ctas = 2) against the same
 generator held at one CTA per SM (SVB_TC_FUSED_CTAS=1, read when the handle is created).  Every item still runs in one CTA
 in the same order, so the waveform and the stage outputs must be the same bits (torch.equal)."""
 import contextlib

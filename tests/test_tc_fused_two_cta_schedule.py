@@ -1,4 +1,4 @@
-"""Host logic of the fused C = 32 ResBlock1 launches at two CTAs per SM (csrc/conv_tc.cu: tc_plan_fused with ctas = 2,
+"""Host logic of the fused C = 32 ResBlock1 launches at two CTAs per SM (csrc/conv_tc.cu: tc_plan with ctas = 2,
 tc_worklist_build): the work lists are built over 2 x 132 = 264 CTAs of an H100.  No GPU needed."""
 import numpy as np
 import pytest
