@@ -69,14 +69,17 @@ struct TcArgs {
     int w_resident;             // every layer's tiles stay in shared memory for the whole launch (narrow layers)
     int blk_chunk_step;         // grouped conv: first input chunk of column block nblk = nblk * blk_chunk_step (0: dense)
     uint32_t w_res_bytes;       // resident: total bytes of all layers' tiles
-    int reserved;               // keeps the fields below at their offsets: ptxas allocates the kernel's registers by the
-                                // parameter layout, and moved fields cost the fused N = 64 kernel up to 5 more registers
+    int epi_ahead;              // every layer's residual is its output or lies outside it, so the staged epilogue (N > 64)
+                                // may load a piece's residual before the previous pieces are stored.  The field keeps the
+                                // ones below at their offsets: ptxas allocates the kernel's registers by the parameter
+                                // layout, and moved fields cost the fused N = 64 kernel up to 5 more registers
     uint32_t op_bytes;          // operand slot: Rp rows x 128 B (x2 with the 3xTF32 lo plane), sized for the largest halo
     uint32_t wtile_bytes;       // one (column block, chunk, tap) weight tile (x2 with the 3xTF32 lo plane)
     uint32_t off_op, off_w, off_bias;   // byte offsets of operand slots / weight ring / bias in dynamic smem
-    int epi_slots;              // streamed epilogue: residual / running-sum pieces in flight per math warp (0: per-thread loads)
-    int l2_prefetch;            // per-thread loads: the producer prefetches each item's residual / running-sum rows into L2
-    uint32_t off_epi;           // byte offset of the piece ring [kMathWarps][epi_slots][kEpiPieceBytes]
+    int epi_slots;              // piece slots per math warp (0: per-thread loads).  N <= 64: the streamed epilogue's ring of
+                                // residual / running-sum pieces in flight; N > 64: the staged epilogue's kStageSlots slots
+    int l2_prefetch;            // the producer prefetches each item's residual / running-sum rows into L2
+    uint32_t off_epi;           // byte offset of the piece slots [kMathWarps][epi_slots][tc_epi_slot_bytes(N)]
 };
 
 constexpr int kMaxW = 8;
@@ -100,6 +103,14 @@ static_assert(512 + 2 * kTcMaxLayers * sizeof(TcLayer) <= 1024, "the layer table
 // group, a contiguous 2 KB span of the residual or of the running sum.
 constexpr int kEpiMaxSlots = 4;
 constexpr uint32_t kEpiPieceBytes = 16 * 128;
+// Staged epilogue (N > 64): kStageSlots accumulator pieces in shared memory per math warp, rows padded to 144 bytes so
+// that row r, 16-byte chunk c sits at 16-byte unit 9 r + c.  The 8 rows of one fragment store and the 8 chunks of one
+// row read then fall in 8 different bank groups, and every lane's addresses differ by constants only.
+// tf32x3 does not compile it: its 32 KB weight tiles leave no room for the slots next to min(nW, 4) tiles (tc_layout).
+constexpr int kStageSlots = 2;
+constexpr uint32_t kStageRowFloats = 36, kStageSlotBytes = 16 * kStageRowFloats * 4;
+__host__ __device__ constexpr bool tc_staged(int mode, int n_tile) { return n_tile > 64 && mode != SVB_PREC_TF32X3; }
+__host__ __device__ constexpr uint32_t tc_epi_slot_bytes(int n_tile) { return n_tile > 64 ? kStageSlotBytes : kEpiPieceBytes; }
 static_assert(256 + kMathWarps * kEpiMaxSlots * 8 <= 512, "the piece barriers live in smem bytes 256 .. 511");
 static_assert(kMaxItems * 16 + kMathWarps * 4 <= kItemBytes, "the math warps' slot parities follow the item table");
 
@@ -401,10 +412,10 @@ __global__ void __launch_bounds__(kTcThreadsP, tc_min_ctas(N, FUSED)) conv1d_c4_
         const int c_lo = 2 * (lane & 3);                                    // first accumulator column of this thread
         float acc0[N / 2], acc1[N / 2];                                     // blocks wg and wg + 2
         // The first MMA of an item overwrites the accumulators (scale 0), but wgmma operands are read-write, so the compiler
-        // keeps the previous item's values live through the whole epilogue.  The two-CTA kernel (80 registers) zeroes them
-        // before that MMA instead: a block's registers are free as soon as its epilogue has read them.
+        // keeps the previous item's values live through the whole epilogue.  The two-CTA kernel (80 registers) and the staged
+        // epilogue (N > 64) zero them before that MMA instead: a block's registers are free as soon as its epilogue has read them.
         auto acc_clear = [&]() {
-            if constexpr (tc_min_ctas(N, FUSED) == 2) {
+            if constexpr (tc_min_ctas(N, FUSED) == 2 || tc_staged(MODE, N)) {
 #pragma unroll
                 for (int i = 0; i < N / 2; ++i) acc0[i] = 0.f, acc1[i] = 0.f;
             }
@@ -461,7 +472,7 @@ __global__ void __launch_bounds__(kTcThreadsP, tc_min_ctas(N, FUSED)) conv1d_c4_
         // latency.  Instead, lane 0 bulk-copies this warp's pieces into its own ring of epi_slots 2 KB slots as soon as the
         // item starts, the MMAs hide the copies, and a slot takes the piece epi_slots further on once it has been read.
         // Pieces of an item in consumption order: block, 32-channel group, then the residual before the running sum.
-        // Only N <= 64 compiles it (tc_epi_pieces); nothing of it stays in registers across the MMAs (the slot parities
+        // Only N <= 64 compiles it (tc_epi_slots); nothing of it stays in registers across the MMAs (the slot parities
         // live in smem).
         constexpr bool EPI = N <= 64;
         auto epi_bar = [&](int slot) { return epi_full + (warp - kWarpMath0) * kEpiMaxSlots + slot; };
@@ -562,6 +573,90 @@ __global__ void __launch_bounds__(kTcThreadsP, tc_min_ctas(N, FUSED)) conv1d_c4_
                 k += (int)has_res + (int)accumulate;
             }
         };
+        // ---- staged epilogue (N > 64, p.epi_slots = kStageSlots and p.epi_ahead; layers with a residual or a running sum,
+        // never an upsampler).  With two blocks of N / 2 accumulators a thread has no registers to spare for loads in flight,
+        // so a warp frees them piece by piece: it writes a piece's acc + bias into one of its kStageSlots slots, and the
+        // piece's 16 accumulator registers then hold residual / running-sum data in flight instead.  Those are loaded
+        // row-major, 4 coalesced float4 per lane and source, and each lane combines and stores the same float4s.  In flight
+        // they never take more registers than the pieces staged so far free: 32 per piece with both sources against 16 per
+        // staged piece, so two pieces are staged before the first loads, and the loads run two pieces ahead from the third
+        // piece on.  A piece's loads pass the stores of earlier pieces, which p.epi_ahead allows.  Same expression, same
+        // order and no contraction as `epilogue`: ((acc + b) + res) * out_scale (+ old); rows >= Tq are not stored.
+        auto epilogue_staged = [&](auto two, const TcItem &it, const TcLayer &L) {
+            constexpr int G = N / 32, P = (decltype(two)::value ? 2 : 1) * G;     // pieces of the item: block, then group
+            const bool has_res = L.res != nullptr, accumulate = L.accumulate != 0;
+            const float out_scale = L.out_scale;
+            const float *bias_s = reinterpret_cast<const float *>(smem + p.off_bias) + L.bias_off;
+            float *slots = reinterpret_cast<float *>(smem + p.off_epi) + (warp - kWarpMath0) * kStageSlots * (kStageSlotBytes / 4);
+            const int rq = lane >> 2, rr = lane >> 3;
+            const int rows0 = piece_rows(it, 0) - rr, rows1 = decltype(two)::value ? piece_rows(it, 1) - rr : 0;
+            // this lane's first float4 of the warp's 16 x 32 span in res / out (G32T) for piece 0, and piece k's offset from it
+            const size_t at0 = (((size_t)it.b * gout + it.nblk * G) * a.out_Tp + kPad + it.t0 + 64 * wg + 16 * (warp & 3)) * 32 + 4 * lane;
+            const float *res0 = L.res + at0;
+            float *out0 = L.out + at0;
+            const int g_stride = a.out_Tp * 32;
+            auto piece_at = [&](int k) { return (k % G) * g_stride + (k / G) * (kTcM * 32); };
+            // acc + b of piece k into slot k % 2
+            auto stage = [&](int k) {
+                const float *acc = k < G ? acc0 : acc1;
+                float *s = slots + (k % kStageSlots) * (kStageSlotBytes / 4) + rq * kStageRowFloats + c_lo;
+                __syncwarp();                                               // every lane has read the slot's previous piece
+#pragma unroll
+                for (int jj = 0; jj < 4; ++jj) {
+                    const int co = it.nblk * N + 32 * (k % G) + 8 * jj + c_lo;
+                    const float b0 = co < cout ? bias_s[co] : 0.f, b1 = co + 1 < cout ? bias_s[co + 1] : 0.f;
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const float *ap = acc + 16 * (k % G) + 4 * jj + 2 * h;
+                        *reinterpret_cast<float2 *>(s + 8 * h * kStageRowFloats + 8 * jj) = make_float2(__fadd_rn(ap[0], b0), __fadd_rn(ap[1], b1));
+                    }
+                }
+                __syncwarp();
+            };
+            float4 rv[P][4], ov[P][4];
+            auto load = [&](int k) {
+                const int rows = k < G ? rows0 : rows1, at = piece_at(k);
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const bool live = 4 * i < rows;
+                    rv[k][i] = ov[k][i] = make_float4(0.f, 0.f, 0.f, 0.f);
+                    if (has_res && live) rv[k][i] = __ldg(reinterpret_cast<const float4 *>(res0 + at + 128 * i));
+                    if (accumulate && live) ov[k][i] = *reinterpret_cast<const float4 *>(out0 + at + 128 * i);
+                }
+            };
+            auto store = [&](int k) {
+                const int rows = k < G ? rows0 : rows1;
+                const float *s = slots + (k % kStageSlots) * (kStageSlotBytes / 4) + rr * kStageRowFloats + 4 * (lane & 7);
+                float *o_p = out0 + piece_at(k);
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    if (4 * i >= rows) continue;
+                    float4 o = *reinterpret_cast<const float4 *>(s + 4 * kStageRowFloats * i);
+                    if (has_res) {
+                        const float4 r = rv[k][i];
+                        o.x = __fadd_rn(o.x, r.x), o.y = __fadd_rn(o.y, r.y), o.z = __fadd_rn(o.z, r.z), o.w = __fadd_rn(o.w, r.w);
+                    }
+                    o.x = __fmul_rn(o.x, out_scale), o.y = __fmul_rn(o.y, out_scale);
+                    o.z = __fmul_rn(o.z, out_scale), o.w = __fmul_rn(o.w, out_scale);
+                    if (accumulate) {
+                        const float4 r = ov[k][i];
+                        o.x = __fadd_rn(o.x, r.x), o.y = __fadd_rn(o.y, r.y), o.z = __fadd_rn(o.z, r.z), o.w = __fadd_rn(o.w, r.w);
+                    }
+                    *reinterpret_cast<float4 *>(o_p + 128 * i) = o;
+                }
+            };
+            stage(0);
+            if (P > 1) stage(1);
+            load(0);
+#pragma unroll
+            for (int k = 0; k < P; ++k) {
+                store(k);
+                if (k + 2 < P) stage(k + 2);
+                // loads through piece 1 after piece 0, through piece 3 after piece 1, then piece k + 2 after piece k
+#pragma unroll
+                for (int j = k < 2 ? k + 1 : k + 2; j <= (k == 0 ? 1 : k + 2) && j < P; ++j) load(j);
+            }
+        };
         // The MMAs of one item for layer L over one (TWO = false) or two (TWO = true) tiles; per output element they
         // accumulate in the same order either way (chunk, tap, then the split terms).  SLAB: the A operand of chunk c is
         // the next operand slot (waited on, released with the chunk's last tap) and a tap is a row shift of dil rows; else
@@ -619,6 +714,8 @@ __global__ void __launch_bounds__(kTcThreadsP, tc_min_ctas(N, FUSED)) conv1d_c4_
                 if (decltype(two)::value) epilogue_stream(it, L, acc1, 1, n_pieces, k, slot, ph);
                 __syncwarp();
                 if (lane == 0) *epi_ph_s = ph;
+            } else if (tc_staged(MODE, N) && p.epi_slots > 0 && p.epi_ahead && (L.res != nullptr || L.accumulate)) {
+                epilogue_staged(two, it, L);
             } else {
                 epilogue(it, L, acc0, 0);
                 if (decltype(two)::value) epilogue(it, L, acc1, kTcM);
@@ -825,22 +922,42 @@ static int tc_epi_sources(int n, const ConvArgs *a) {
     return nsrc;
 }
 
-// Streamed epilogue (kernel: epilogue_stream): the 2 KB pieces one math warp's item needs at most, 0 where the layers do
-// not take it.  N > 64 does not: with two blocks of N / 2 accumulators per thread it spills at the 168-register
-// ceiling, and on an H100 (700 W) the C = 256 / 128 residual launches ran 20 % slower with it.  Those launches have the
-// producer prefetch the item's residual / running-sum rows into L2 instead (TcArgs::l2_prefetch).
-static int tc_epi_pieces(int n, const ConvArgs *a, int MT, int n_tile) {
-    return n_tile > 64 ? 0 : MT * (n_tile / 32) * tc_epi_sources(n, a);
+// Whether every layer's residual either is its output (in place: the inference generator's middle ResBlock step, where
+// each element is read by the lane that then writes it) or does not overlap it (G32T extents), so the staged epilogue may
+// load a piece's residual before the previous pieces of the item are stored (TcArgs::epi_ahead)
+static bool tc_epi_ahead(int n, const ConvArgs *a) {
+    for (int l = 0; l < n; ++l) {
+        if (!a[l].res || a[l].res == a[l].out) continue;
+        const size_t len = (size_t)a[l].B * c4t_groups(a[l].Cout) * a[l].out_Tp * 32;
+        if (a[l].res < a[l].out + len && a[l].out < a[l].res + len) return false;
+    }
+    return true;
 }
 
-// The piece ring comes out of the weight ring's share of `avail` bytes: the most slots per math warp (at most one per
-// piece of an item, at least the `min_slots` pieces one channel group reads together) that leave the weight ring
-// min(nW, 4) tiles.  Returns the slots (0: none fit) and the new *nW.  SVB_TC_EPI_SLOTS caps the slots (measurement).
-static int tc_epi_fit(size_t avail, uint32_t wtile_bytes, int pieces, int min_slots, int *nW) {
+// Slots per math warp of the epilogue's piece area, at most the return value and at least *min_slots (0: the layers do
+// not take it).
+// * N <= 64, streamed epilogue (kernel: epilogue_stream): one per 2 KB piece of an item, at least the sources one channel
+//   group reads together.
+// * N > 64, staged epilogue (kernel: epilogue_staged): kStageSlots, where tc_epi_ahead holds (never tf32x3, whose kernel
+//   does not compile it).  The streamed epilogue does not fit there: next to two blocks of N / 2 accumulators per thread
+//   it spilled at the 168-register ceiling, and on an H100 (700 W) the C = 256 / 128 residual launches ran 20 % slower
+//   with it.  The staged epilogue keeps nothing beside the accumulators it has not yet written to its slots, and on an
+//   H100 (700 W) it took stage 1's c2 launches from 0.47 to 0.08 ms more than its c1 launches.
+static int tc_epi_slots(int n, const ConvArgs *a, int precision, int MT, int n_tile, int *min_slots) {
+    const int nsrc = tc_epi_sources(n, a);
+    if (n_tile <= 64) return *min_slots = nsrc, MT * (n_tile / 32) * nsrc;
+    *min_slots = kStageSlots;
+    return nsrc > 0 && tc_staged(precision, n_tile) && tc_epi_ahead(n, a) ? kStageSlots : 0;
+}
+
+// The piece slots come out of the weight ring's share of `avail` bytes: the most slots per math warp (max_slots .. min_slots)
+// that leave the weight ring min(nW, 4) tiles.  Returns the slots (0: none fit) and the new *nW.  SVB_TC_EPI_SLOTS caps
+// the slots (measurement).
+static int tc_epi_fit(size_t avail, uint32_t wtile_bytes, uint32_t slot_bytes, int max_slots, int min_slots, int *nW) {
     int cap = kEpiMaxSlots;
     if (const char *e = getenv("SVB_TC_EPI_SLOTS")) cap = std::max(0, std::min(kEpiMaxSlots, atoi(e)));
-    for (int s = std::min(cap, pieces); s >= min_slots; --s) {
-        const size_t ring = (size_t)s * kMathWarps * kEpiPieceBytes;
+    for (int s = std::min(cap, max_slots); s >= min_slots; --s) {
+        const size_t ring = (size_t)s * kMathWarps * slot_bytes;
         if (ring >= avail) continue;
         const int nw = std::min((int)((avail - ring) / wtile_bytes), kMaxW);
         if (nw >= std::min(*nW, 4)) {
@@ -858,12 +975,12 @@ static int tc_epi_fit(size_t avail, uint32_t wtile_bytes, int pieces, int min_sl
 //   nA_pref does not fit next to two weight tiles.
 // * Weights: resident (res_bytes > 0: every layer's tiles, one chunk and one column block) with nA_pref or 2 slots where
 //   they fit; else a ring of up to kMaxW tiles, at least one per tile of an item.
-// * The piece ring (`pieces` per math warp at most) comes out of the weight ring.  ring_takes_slot: where it does not fit
-//   next to nA > 2 slots (C = 64 at k 11, d 5 in fused launches), the layout drops to 2 slots for it; else it never changes
-//   nA, and goes without the ring where it does not fit.
+// * The epilogue's piece slots (max_slots .. min_slots per math warp, tc_epi_slots) come out of the weight ring.
+//   ring_takes_slot: where they do not fit next to nA > 2 slots (C = 64 at k 11, d 5 in fused launches), the layout drops
+//   to 2 slots for them; else they never change nA, and the layout goes without them where they do not fit.
 // Returns false when no layout fits.
 static bool tc_layout(TcArgs &p, size_t &smem, size_t budget, size_t bias_bytes, int nA_pref, size_t inter_bytes, size_t res_bytes,
-                      int pieces, bool ring_takes_slot) {
+                      int max_slots, int min_slots, bool ring_takes_slot) {
     p.off_op = 1024 + kItemBytes;
     auto slots_end = [&](int nA) { return p.off_op + (size_t)nA * p.op_bytes + inter_bytes; };
     p.w_resident = 0;
@@ -878,7 +995,7 @@ static bool tc_layout(TcArgs &p, size_t &smem, size_t budget, size_t bias_bytes,
         if (slots_end(p.nA) + (size_t)p.MT * p.wtile_bytes > budget) return false;
     }
     const size_t res_area = (size_t)round_up((int)res_bytes, 1024);
-    const int min_slots = pieces / (p.MT * (p.n_tile / 32));
+    const uint32_t slot_bytes = tc_epi_slot_bytes(p.n_tile);
     auto place = [&](int nA, bool ring) {
         p.nA = nA;
         p.off_w = (uint32_t)slots_end(nA);
@@ -887,17 +1004,17 @@ static bool tc_layout(TcArgs &p, size_t &smem, size_t budget, size_t bias_bytes,
         p.epi_slots = 0;
         if (ring && p.w_resident) {
             int nw = 0;
-            p.epi_slots = avail > res_area ? tc_epi_fit(avail - res_area, 1u, pieces, min_slots, &nw) : 0;
+            p.epi_slots = avail > res_area ? tc_epi_fit(avail - res_area, 1u, slot_bytes, max_slots, min_slots, &nw) : 0;
         } else if (ring) {
-            p.epi_slots = tc_epi_fit(avail, p.wtile_bytes, pieces, min_slots, &p.nW);
+            p.epi_slots = tc_epi_fit(avail, p.wtile_bytes, slot_bytes, max_slots, min_slots, &p.nW);
         }
         return p.epi_slots > 0;
     };
     const int nA = p.nA;
-    if (!pieces || !(place(nA, true) || (ring_takes_slot && nA > 2 && place(2, true)))) place(nA, false);
+    if (!max_slots || !(place(nA, true) || (ring_takes_slot && nA > 2 && place(2, true)))) place(nA, false);
     p.w_res_bytes = p.w_resident ? (uint32_t)res_bytes : 0;
     p.off_epi = p.off_w + (uint32_t)(p.w_resident ? res_area : round_up(p.nW * (int)p.wtile_bytes, 1024));
-    p.off_bias = p.off_epi + (uint32_t)p.epi_slots * kMathWarps * kEpiPieceBytes;
+    p.off_bias = p.off_epi + (uint32_t)p.epi_slots * kMathWarps * slot_bytes;
     smem = (size_t)p.off_bias + bias_bytes;
     return smem <= budget + bias_bytes;
 }
@@ -941,8 +1058,10 @@ static int tc_plan(int n, const TcWeights *const *w, const ConvArgs *a, int prec
         // 2n x Cout <= 6 x 64 floats
         const size_t bias_bytes = ctas == 1 ? kBiasBytes : (size_t)round_up(2 * n * a0.Cout * 4, 128);
         const size_t smem_max = ctas == 1 ? 227 * 1024 : kSmemPerSm / 2 - kSmemReservedPerCta;
+        int min_slots = 0;
+        const int max_slots = tc_epi_slots(n, a + n, precision, 2, p.n_tile, &min_slots);
         if (!tc_layout(p, smem, smem_max - bias_bytes, bias_bytes, ctas == 1 ? 3 : 1, (size_t)p.n_chunks * p.inter_bytes, 0,
-                       tc_epi_pieces(n, a + n, 2, p.n_tile), true))
+                       max_slots, min_slots, true))
             return SVB_ERR_INVALID;
         p.off_inter = p.off_op + (uint32_t)p.nA * p.op_bytes;
         p.groups_per_b = (a0.Tq + p.fused_P - 1) / p.fused_P;
@@ -974,7 +1093,9 @@ static int tc_plan(int n, const TcWeights *const *w, const ConvArgs *a, int prec
         auto fit = [&](int mt) {
             p.MT = mt;
             p.op_bytes = (uint32_t)round_up(mt * kTcM + 2 * halo, 8) * 128 * planes;
-            return tc_layout(p, smem, 227 * 1024 - bias_bytes, bias_bytes, 3, 0, res_bytes, tc_epi_pieces(n, a, mt, p.n_tile), false);
+            int min_slots = 0;
+            const int max_slots = tc_epi_slots(n, a, precision, mt, p.n_tile, &min_slots);
+            return tc_layout(p, smem, 227 * 1024 - bias_bytes, bias_bytes, 3, 0, res_bytes, max_slots, min_slots, false);
         };
         bool two = tiles >= 2 && fit(2);
         if (two && grid > 0) {
@@ -990,7 +1111,9 @@ static int tc_plan(int n, const TcWeights *const *w, const ConvArgs *a, int prec
     }
     p.a = a0, p.n_layers = n;
     p.work = nullptr, p.work_off = nullptr;
-    p.l2_prefetch = p.epi_slots == 0 && tc_epi_sources(n, fused ? a + n : a) > 0;
+    // the staged epilogue's first loads of an item find its rows in L2 too
+    p.l2_prefetch = (p.epi_slots == 0 || p.n_tile > 64) && tc_epi_sources(n, fused ? a + n : a) > 0;
+    p.epi_ahead = tc_epi_ahead(n, fused ? a + n : a);
     const int n_tab = fused ? 2 * n : n;
     uint32_t res_off = 0;
     for (int l = 0; l < n_tab; ++l) {
@@ -1003,9 +1126,9 @@ static int tc_plan(int n, const TcWeights *const *w, const ConvArgs *a, int prec
     }
     for (int l = n_tab; l < 2 * kTcMaxLayers; ++l) p.L[l] = p.L[0];
     if (!fused && getenv("SVB_TC_VERBOSE"))
-        fprintf(stderr, "[tc] %d layer(s) Cin %d CoutP %d KS %d.. halo %d Tq %d | n_tile %d MT %d nA %d nW %d resident %d smem %zu epi %d l2pf %d\n", n,
-                a0.Cin, a0.CoutP, a0.KS, halo, a0.Tq, p.n_tile, p.MT, p.nA, p.nW, p.w_resident, smem,
-                p.epi_slots, p.l2_prefetch);
+        fprintf(stderr, "[tc] %d layer(s) Cin %d CoutP %d KS %d.. halo %d Tq %d | n_tile %d MT %d nA %d nW %d resident %d smem %zu epi %d l2pf %d stage %d\n",
+                n, a0.Cin, a0.CoutP, a0.KS, halo, a0.Tq, p.n_tile, p.MT, p.nA, p.nW, p.w_resident, smem,
+                p.n_tile > 64 ? 0 : p.epi_slots, p.l2_prefetch, p.n_tile > 64 ? p.epi_slots : 0);
     return SVB_OK;
 }
 
