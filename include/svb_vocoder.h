@@ -125,7 +125,8 @@ int svb_gen_spec2wav_host_i16(svb_gen_t *g, const float *mel_host, const float *
 int svb_wav_to_int16(const float *wav_dev, int32_t B, int64_t n, int32_t norm, int16_t *out_dev, void *stream);
 
 /* Intermediate tap for layer-level parity tests: copies a named activation of the LAST forward
- * ("har_source" [B,T*hop]; "conv_pre", "ups{i}", "stage{i}" as [B,C,T_i]) to out_dev. */
+ * ("har_source" [B,T*hop]; "conv_pre", "ups{i}", "stage{i}" as [B,C,T_i]) to out_dev.  shape3 receives its shape;
+ * out_dev = NULL with capacity_floats = 0 only queries that shape. */
 int svb_gen_get_tap(svb_gen_t *g, const char *name, float *out_dev, int64_t capacity_floats,
                     int64_t *shape3, void *stream);
 int64_t svb_gen_hop(const svb_gen_t *g);

@@ -712,12 +712,13 @@ extern "C" int svb_gen_spec2wav_host_i16(svb_gen_t *g, const float *mel_host, co
 
 extern "C" int svb_gen_get_tap(svb_gen_t *g, const char *name, float *out_dev, int64_t capacity_floats, int64_t *shape3,
                                void *stream) {
-    SVB_CHECK(g && name && out_dev && shape3, SVB_ERR_INVALID, "get_tap: null argument");
+    SVB_CHECK(g && name && (out_dev || capacity_floats == 0) && shape3, SVB_ERR_INVALID, "get_tap: null argument");
     auto it = g->taps.find(name);
     SVB_CHECK(it != g->taps.end(), SVB_ERR_INVALID, "get_tap: no activation named '%s' in the last forward", name);
     const Tap &t = it->second;
     const int B = g->last_B;
     shape3[0] = B, shape3[1] = t.C, shape3[2] = t.T;
+    if (!out_dev) return SVB_OK;    // size query: shape only
     SVB_CHECK((int64_t)B * t.C * t.T <= capacity_floats, SVB_ERR_INVALID, "get_tap: buffer too small");
     cudaStream_t st = as_stream(stream);
     if (t.plain) SVB_CUDA(cudaMemcpyAsync(out_dev, t.p, (size_t)B * t.T * 4, cudaMemcpyDeviceToDevice, st));

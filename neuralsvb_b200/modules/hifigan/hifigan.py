@@ -398,14 +398,13 @@ class HifiGanGenerator(nn.Module):
         lib = _native.lib()
         g = self._handle
         dev = torch.device('cuda', self._handle_key)
-        cap = 1 << 28
         shape = (ctypes.c_int64 * 3)()
-        # query size first with a generous scratch buffer sized from the output
-        buf = torch.empty(cap // 4, device=dev, dtype=torch.float32)
-        _native.check(lib.svb_gen_get_tap(g, name.encode(), _native.ptr(buf), buf.numel(), shape,
-                                          _native.current_stream_ptr(dev)), f'get_tap({name})')
-        B, C, T = shape[0], shape[1], shape[2]
-        return buf[:B * C * T].view(B, C, T).clone()
+        st = _native.current_stream_ptr(dev)
+        # a null buffer of capacity 0 queries the shape; then the copy goes into a tensor of exactly that size
+        _native.check(lib.svb_gen_get_tap(g, name.encode(), None, 0, shape, st), f'get_tap({name})')
+        out = torch.empty(shape[0], shape[1], shape[2], device=dev, dtype=torch.float32)
+        _native.check(lib.svb_gen_get_tap(g, name.encode(), _native.ptr(out), out.numel(), shape, st), f'get_tap({name})')
+        return out
 
     def __del__(self):
         try:

@@ -111,6 +111,40 @@ def resblock2(x, w, prefix, k, dil, act=_leaky_relu):
     return x
 
 
+def upsample_forward(w, h, i, x, har=None, act=_leaky_relu):
+    """Upsampler ``i`` (hifigan.py:153-157): leaky relu of ``x`` (``conv_pre`` or ``stage{i-1}``), ``ups.{i}``, plus
+    ``noise_convs.{i}(har)`` when ``har`` [B,1,T*hop] is given.  Returns the ``ups{i}`` tap."""
+    rates, u, k = h['upsample_rates'], h['upsample_rates'][i], h['upsample_kernel_sizes'][i]
+    x = act('conv_pre' if i == 0 else f'stage{i - 1}', x, LRELU_SLOPE)
+    x = F.conv_transpose1d(x, w[f'ups.{i}.weight'], w[f'ups.{i}.bias'], stride=u, padding=(k - u) // 2)
+    if har is not None:
+        if i + 1 < len(rates):
+            s = int(np.prod(rates[i + 1:]))
+            x = x + F.conv1d(har, w[f'noise_convs.{i}.weight'], w[f'noise_convs.{i}.bias'], stride=s, padding=s // 2)
+        else:
+            x = x + F.conv1d(har, w[f'noise_convs.{i}.weight'], w[f'noise_convs.{i}.bias'])
+    return x
+
+
+def stage_forward(w, h, i, x, act=_leaky_relu):
+    """The ResBlocks of stage ``i`` on ``x`` (the ``ups{i}`` tap), summed and divided by their number
+    (hifigan.py:158-164).  Returns the ``stage{i}`` tap."""
+    nk = len(h['resblock_kernel_sizes'])
+    fn = resblock1 if h['resblock'] == '1' else resblock2
+    xs = None
+    for j, (rk, dil) in enumerate(zip(h['resblock_kernel_sizes'], h['resblock_dilation_sizes'])):
+        r = fn(x, w, f'resblocks.{i * nk + j}', rk, dil, act)
+        xs = r if xs is None else xs + r
+    return xs / nk
+
+
+def post_forward(w, h, x, act=_leaky_relu):
+    """tanh(conv_post(leaky_relu(x, 0.01))) of the last stage's output (hifigan.py:165-167)."""
+    x = act(f'stage{len(h["upsample_rates"]) - 1}', x, 0.01)   # F.leaky_relu's default slope (SURVEY D9)
+    x = F.conv1d(x, w['conv_post.weight'], w['conv_post.bias'], padding=3)
+    return torch.tanh(x)
+
+
 def generator_forward(w, h, mel, f0=None, rand_ini=None, noise=None, taps=None, act=_leaky_relu):
     """HifiGanGenerator.forward (hifigan.py:144-169) on FOLDED weights ``w``
     (see fold_weight_norm).  mel [B,80,T]; f0 [B,T] Hz or None.  ``taps``: an
@@ -120,8 +154,6 @@ def generator_forward(w, h, mel, f0=None, rand_ini=None, noise=None, taps=None, 
     last stage's at slope 0.01 before conv_post) and the ResBlock sites of
     resblock1 / resblock2."""
     rates = h['upsample_rates']
-    ksz = h['upsample_kernel_sizes']
-    nk = len(h['resblock_kernel_sizes'])
     har = None
     if f0 is not None:
         scale = int(np.prod(rates))
@@ -133,29 +165,14 @@ def generator_forward(w, h, mel, f0=None, rand_ini=None, noise=None, taps=None, 
     x = F.conv1d(mel, w['conv_pre.weight'], w['conv_pre.bias'], padding=3)
     if taps is not None:
         taps['conv_pre'] = x
-    for i, (u, k) in enumerate(zip(rates, ksz)):
-        x = act('conv_pre' if i == 0 else f'stage{i - 1}', x, LRELU_SLOPE)
-        x = F.conv_transpose1d(x, w[f'ups.{i}.weight'], w[f'ups.{i}.bias'], stride=u, padding=(k - u) // 2)
-        if har is not None:
-            if i + 1 < len(rates):
-                s = int(np.prod(rates[i + 1:]))
-                x = x + F.conv1d(har, w[f'noise_convs.{i}.weight'], w[f'noise_convs.{i}.bias'],
-                                 stride=s, padding=s // 2)
-            else:
-                x = x + F.conv1d(har, w[f'noise_convs.{i}.weight'], w[f'noise_convs.{i}.bias'])
+    for i in range(len(rates)):
+        x = upsample_forward(w, h, i, x, har, act)
         if taps is not None:
             taps[f'ups{i}'] = x
-        xs = None
-        for j, (rk, dil) in enumerate(zip(h['resblock_kernel_sizes'], h['resblock_dilation_sizes'])):
-            fn = resblock1 if h['resblock'] == '1' else resblock2
-            r = fn(x, w, f'resblocks.{i * nk + j}', rk, dil, act)
-            xs = r if xs is None else xs + r
-        x = xs / nk
+        x = stage_forward(w, h, i, x, act)
         if taps is not None:
             taps[f'stage{i}'] = x
-    x = act(f'stage{len(rates) - 1}', x, 0.01)   # F.leaky_relu's default slope (hifigan.py:165, SURVEY D9)
-    x = F.conv1d(x, w['conv_post.weight'], w['conv_post.bias'], padding=3)
-    return torch.tanh(x)
+    return post_forward(w, h, x, act)
 
 
 # ------------------------------------------------------------------ discriminators

@@ -150,3 +150,33 @@ def test_masked_generator_reference_with_its_own_masks_is_autograd():
     assert set(g_m) == set(p)
     for k, t in p.items():
         assert _rel(g_m[k], t.grad) < 1e-12, k
+
+
+def test_generator_launch_group_references_chain_to_the_oracle_taps():
+    """test_gpu_generator_forward's per-launch-group references (O.upsample_forward, O.stage_forward, O.post_forward)
+    fed the float32 oracle's own taps give back each next tap and the waveform: ``ups{i}`` is the upsampler of
+    ``conv_pre`` / ``stage{i-1}`` with the noise conv of ``har_source`` added, ``stage{i}`` the ResBlock mean of
+    ``ups{i}``."""
+    for h, T in ((S.small_config(True), 24), (S.hifigan_config(True), 3), (S.hifigan_config(False), 3)):
+        hop = int(np.prod(h['upsample_rates']))
+        B = 2
+        w = O.fold_weight_norm(S.make_generator_state_dict(h, 1234))
+        mel, f0 = S.make_mel_f0(B, T, 1234)
+        ri, nz = S.make_nsf_noise(B, T * hop, 1234)
+        nsf = h['use_pitch_embed']
+        taps = {}
+        with torch.no_grad():
+            y = O.generator_forward(w, h, mel, f0 if nsf else None, ri, nz, taps)
+            har = taps.get('har_source')
+            assert (har is not None) == nsf
+            n = len(h['upsample_rates'])
+            assert set(taps) == {'conv_pre', *(f'ups{i}' for i in range(n)), *(f'stage{i}' for i in range(n))} | (
+                {'har_source'} if nsf else set())
+            for i in range(n):
+                x = taps['conv_pre' if i == 0 else f'stage{i - 1}']
+                assert torch.equal(O.upsample_forward(w, h, i, x, har), taps[f'ups{i}']), (h['hop_size'], i)
+                assert torch.equal(O.stage_forward(w, h, i, taps[f'ups{i}']), taps[f'stage{i}']), (h['hop_size'], i)
+                if nsf:     # the noise conv is part of ups{i}: without it the tap is not reproduced
+                    assert not torch.allclose(O.upsample_forward(w, h, i, x, None), taps[f'ups{i}'])
+            assert torch.equal(O.post_forward(w, h, taps[f'stage{n - 1}']), y)
+            assert y.shape == (B, 1, T * hop)
