@@ -124,6 +124,26 @@ int svb_gen_spec2wav_host_i16(svb_gen_t *g, const float *mel_host, const float *
 /* the conversion alone on device buffers: wav_dev fp32 [B, n] -> out_dev int16 [B, n] (stream-ordered). */
 int svb_wav_to_int16(const float *wav_dev, int32_t B, int64_t n, int32_t norm, int16_t *out_dev, void *stream);
 
+/* Ragged batches (inference only): HifiGanGenerator.forward (hifigan.py:144-169) run on each clip alone, as the reference's
+ * spec2wav (vocoders/hifigan.py:55-69) vocodes clips of different lengths one at a time, in one call.  Clip b has
+ * lengths_host[b] frames, 1 <= lengths_host[b] <= T_max; the buffers are laid out as svb_gen_forward's with T = T_max, and mel /
+ * f0 frames at or past a clip's length are never read (they may hold anything).  wav_dev[b, t] = 0 for t >= lengths_host[b] * hop.
+ * Clip b is bit-identical to a B = 1 svb_gen_forward of that clip alone given the same draws (rand_ini row b, noise[b, :len*hop]);
+ * the Philox draws stay keyed by (seed, b, t).  Lengths are checked on the host before anything touches the GPU; a training
+ * handle returns SVB_ERR_STATE. */
+int svb_gen_forward_ragged(svb_gen_t *g, const float *mel_dev, const float *f0_dev, const float *rand_ini_dev,
+                           const float *noise_dev, uint64_t seed, int32_t B, int32_t T_max, const int32_t *lengths_host,
+                           float *wav_dev, void *stream);
+/* spec2wav over a ragged batch from HOST memory (vocoders/hifigan.py:55-69, clip by clip): mel_host holds the clips' [T_b, n_mel]
+ * mels back to back ([sum T_b, n_mel], as svb_wav2spec_batch_host returns them), f0_host their [T_b] f0 back to back or NULL;
+ * wav_host receives sum(T_b) * hop samples, clip after clip.  One H2D copy, one forward, one D2H copy, one synchronisation. */
+int svb_gen_spec2wav_ragged_host(svb_gen_t *g, const float *mel_host, const float *f0_host, uint64_t seed, int32_t B,
+                                 const int32_t *lengths_host, float *wav_host, void *stream);
+/* the same followed by save_wav's int16 conversion on the device (svb_gen_spec2wav_host_i16); `norm` divides each clip by the
+ * peak of its own samples.  wav_host int16 [sum T_b * hop]. */
+int svb_gen_spec2wav_ragged_host_i16(svb_gen_t *g, const float *mel_host, const float *f0_host, uint64_t seed, int32_t B,
+                                     const int32_t *lengths_host, int32_t norm, int16_t *wav_host, void *stream);
+
 /* Intermediate tap for layer-level parity tests: copies a named activation of the LAST forward
  * ("har_source" [B,T*hop]; "conv_pre", "ups{i}", "stage{i}" as [B,C,T_i]) to out_dev.  shape3 receives its shape;
  * out_dev = NULL with capacity_floats = 0 only queries that shape. */
@@ -593,6 +613,13 @@ int64_t svb_tc_schedule_probe(int32_t n_layers, const int32_t *KS, const int32_t
 int64_t svb_tc_fused_schedule_probe(int32_t n_layers, const int32_t *KS1, const int32_t *dil1, const int32_t *KS2, const int32_t *accumulate,
                                     int32_t Cin, int32_t B, int32_t Tq, int32_t chain_ordered, int32_t grid, int32_t *items_out,
                                     int64_t items_capacity, int32_t *off_out, int32_t *P_out, double *balance_out);
+/* The same for a ragged batch: clip b has lengths[b] >= 1 rows.  KS2 = NULL: the items of svb_tc_schedule_probe (taps KS, MT,
+ * col_blocks); else the fused items of svb_tc_fused_schedule_probe (c1 taps KS, c2 taps KS2, MT = 2, col_blocks = 1; P_out receives
+ * P, else 0).  items_out receives 6 ints per item: the 5 of svb_tc_schedule_probe, then the row bound the item carries. */
+int64_t svb_tc_ragged_schedule_probe(int32_t n_layers, const int32_t *KS, const int32_t *KS2, const int32_t *has_res, const int32_t *accumulate,
+                                     int32_t Cin, int32_t B, const int32_t *lengths, int32_t MT, int32_t col_blocks, int32_t chain_ordered,
+                                     int32_t grid, int32_t *items_out, int64_t items_capacity, int32_t *off_out, int32_t *P_out,
+                                     double *balance_out);
 
 #ifdef __cplusplus
 }

@@ -163,6 +163,9 @@ _PROTOS = {
     'svb_wav2spec_batch_host': (_I64, [ctypes.POINTER(StftConfig), _P, _P, _I32, _P, _P, _P, ctypes.c_int, _P]),
     'svb_gen_spec2wav_host_i16': (ctypes.c_int, [_P, _P, _P, _U64, _I32, _I32, _I32, _P, _P]),
     'svb_wav_to_int16': (ctypes.c_int, [_P, _I32, _I64, _I32, _P, _P]),
+    'svb_gen_forward_ragged': (ctypes.c_int, [_P, _P, _P, _P, _P, _U64, _I32, _I32, _P, _P, _P]),
+    'svb_gen_spec2wav_ragged_host': (ctypes.c_int, [_P, _P, _P, _U64, _I32, _P, _P, _P]),
+    'svb_gen_spec2wav_ragged_host_i16': (ctypes.c_int, [_P, _P, _P, _U64, _I32, _P, _I32, _P, _P]),
     'svb_wn_create': (ctypes.c_int, [_I32, _I32, _I32, _I32, _I32, _I32, _I32, ctypes.POINTER(_P)]),
     'svb_wn_destroy': (None, [_P]),
     'svb_wn_set_weight': (ctypes.c_int, [_P, ctypes.c_char_p, _P, ctypes.POINTER(_I64), _I32]),
@@ -182,6 +185,8 @@ _PROTOS = {
     'svb_wn_set_weight_dev': (ctypes.c_int, [_P, ctypes.c_char_p, _P, _I64, _P]),
     'svb_wn_update_weights_dev': (ctypes.c_int, [_P, _P]),
     'svb_tc_schedule_probe': (_I64, [_I32, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P, _I64, _P, ctypes.POINTER(ctypes.c_double)]),
+    'svb_tc_ragged_schedule_probe': (_I64, [_I32, _P, _P, _P, _P, _I32, _I32, _P, _I32, _I32, _I32, _I32, _P, _I64, _P, _P,
+                                             ctypes.POINTER(ctypes.c_double)]),
     'svb_tc_fused_schedule_probe': (_I64, [_I32, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _P, _I64, _P, _P,
                                            ctypes.POINTER(ctypes.c_double)]),
     'svb_layer_norm_nct': (ctypes.c_int, [_P, _P, _P, _I32, _I32, _I32, ctypes.c_float, _P, _P]),

@@ -28,6 +28,8 @@ __global__ void __launch_bounds__(256) conv1d_c4_ffma_kernel(ConvArgs a) {
     const int co_tile0 = blockIdx.y * CO_TILE;
     const int co0 = co_tile0 + warp * CPT;                     // first GEMM column of this warp
     const bool active = co0 < a.CoutP;
+    const int Tq = a.len ? a.len[b] * a.len_mul : a.Tq;       // valid rows of this clip
+    if (t0 >= Tq) return;                                      // a tile past the clip's end (ragged batches)
     const int cin_q = a.Cin >> 2;
 
     float acc[kRowsPerThread][CPT];
@@ -104,7 +106,7 @@ __global__ void __launch_bounds__(256) conv1d_c4_ffma_kernel(ConvArgs a) {
 #pragma unroll
         for (int r = 0; r < kRowsPerThread; ++r) {
             const int q = t0 + lane + 32 * r;
-            if (q >= a.Tq) continue;
+            if (q >= Tq) continue;
             const size_t row = act_q4(b, a.Cout, a.out_Tp, co >> 2, kPad + (a.ups_u > 0 ? q * a.ups_u + phi : q));
             float4 v = make_float4(acc[r][4 * c4 + 0] + bv.x, acc[r][4 * c4 + 1] + bv.y,
                                    acc[r][4 * c4 + 2] + bv.z, acc[r][4 * c4 + 3] + bv.w);
@@ -186,6 +188,30 @@ __global__ void btc_to_c4t_kernel(const float4 *__restrict__ btc, float4 *__rest
     c4t[act_q4(b, C, Tp, cq, kPad + t)] = btc[((size_t)b * T + t) * (C >> 2) + cq];
 }
 
+// ragged batches: frames at or past len[b] are written as zeros without reading the input
+__global__ void nct_to_c4t_ragged_kernel(const float *__restrict__ nct, float4 *__restrict__ c4t, int C, int T, int Tp,
+                                         const int *__restrict__ len) {
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    const int cq = blockIdx.y, b = blockIdx.z;
+    if (t >= T) return;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (t < len[b]) {
+        const float *p = nct + ((size_t)b * C + cq * 4) * T + t;
+        v = make_float4(p[0], p[T], p[2 * (size_t)T], p[3 * (size_t)T]);
+    }
+    c4t[act_q4(b, C, Tp, cq, kPad + t)] = v;
+}
+
+__global__ void btc_to_c4t_ragged_kernel(const float4 *__restrict__ btc, float4 *__restrict__ c4t, int C, int T, int Tp,
+                                         const int *__restrict__ len, const int *__restrict__ off) {
+    const int cq = blockIdx.x * blockDim.x + threadIdx.x;
+    const int t = blockIdx.y, b = blockIdx.z;
+    if (cq >= (C >> 2)) return;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (t < len[b]) v = btc[((off ? (size_t)off[b] : (size_t)b * T) + t) * (C >> 2) + cq];
+    c4t[act_q4(b, C, Tp, cq, kPad + t)] = v;
+}
+
 int launch_nct_to_c4t(const float *nct, float *c4t, int B, int C, int T, int Tp, cudaStream_t st) {
     dim3 grid((T + 127) / 128, C / 4, B);
     nct_to_c4t_kernel<<<grid, 128, 0, st>>>(nct, reinterpret_cast<float4 *>(c4t), C, T, Tp);
@@ -205,20 +231,35 @@ int launch_btc_to_c4t(const float *btc, float *c4t, int B, int C, int T, int Tp,
     SVB_CUDA(cudaGetLastError());
     return SVB_OK;
 }
+int launch_nct_to_c4t_ragged(const float *nct, float *c4t, int B, int C, int T, int Tp, const int *len, cudaStream_t st) {
+    dim3 grid((T + 127) / 128, C / 4, B);
+    nct_to_c4t_ragged_kernel<<<grid, 128, 0, st>>>(nct, reinterpret_cast<float4 *>(c4t), C, T, Tp, len);
+    SVB_CUDA(cudaGetLastError());
+    return SVB_OK;
+}
+int launch_btc_to_c4t_ragged(const float *btc, float *c4t, int B, int C, int T, int Tp, const int *len, const int *off,
+                             cudaStream_t st) {
+    dim3 grid((C / 4 + 31) / 32, T, B);
+    btc_to_c4t_ragged_kernel<<<grid, 32, 0, st>>>(reinterpret_cast<const float4 *>(btc), reinterpret_cast<float4 *>(c4t), C,
+                                                  T, Tp, len, off);
+    SVB_CUDA(cudaGetLastError());
+    return SVB_OK;
+}
 
 // ------------------------------------------------------------------------------ NSF injection
 // one thread per (row n, channel quad): the 8 quads of a 32-channel group are 8 consecutive lanes, so
 // a warp touches 4 whole 128-byte rows; har[] is a broadcast within a row; nw is packed [K][C].
 __global__ void noise_conv_add_kernel(float4 *__restrict__ x, int C, int T, int Tp, const float *__restrict__ har,
                                       int Thar, const float *__restrict__ nw, const float *__restrict__ nb, int K,
-                                      int stride, int pad) {
+                                      int stride, int pad, const int *__restrict__ len, int mul, int har_mul) {
     const int cq_n = c4t_groups(C) * 8;                       // quads per row incl. zero padding channels
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const int b = blockIdx.y;
+    const float *h = har + (size_t)b * Thar;                  // har rows are Thar samples apart
+    if (len) T = len[b] * mul, Thar = len[b] * har_mul;       // this clip's rows and har samples
     if (idx >= (long long)T * cq_n) return;
     const int n = (int)(idx / cq_n), cq = (int)(idx - (long long)n * cq_n);
     if (cq * 4 >= C) return;
-    const float *h = har + (size_t)b * Thar;
     float4 acc = __ldg(reinterpret_cast<const float4 *>(nb) + cq);
     const int base = n * stride - pad;
     for (int j = 0; j < K; ++j) {
@@ -235,10 +276,11 @@ __global__ void noise_conv_add_kernel(float4 *__restrict__ x, int C, int T, int 
 }
 
 int launch_noise_conv_add(float *x, int B, int C, int T, int Tp, const float *har, int Thar, const float *nw,
-                          const float *nb, int K, int stride, int pad, cudaStream_t st) {
+                          const float *nb, int K, int stride, int pad, cudaStream_t st, const int *len, int mul, int har_mul) {
     const long long total = (long long)T * c4t_groups(C) * 8;
     dim3 grid((unsigned)((total + 255) / 256), B);
-    noise_conv_add_kernel<<<grid, 256, 0, st>>>(reinterpret_cast<float4 *>(x), C, T, Tp, har, Thar, nw, nb, K, stride, pad);
+    noise_conv_add_kernel<<<grid, 256, 0, st>>>(reinterpret_cast<float4 *>(x), C, T, Tp, har, Thar, nw, nb, K, stride, pad, len,
+                                                mul, har_mul);
     SVB_CUDA(cudaGetLastError());
     return SVB_OK;
 }
@@ -246,12 +288,18 @@ int launch_noise_conv_add(float *x, int B, int C, int T, int Tp, const float *ha
 // ------------------------------------------------------------------------------ conv_post + tanh
 __global__ void __launch_bounds__(256) conv_post_tanh_kernel(const float4 *__restrict__ x, int C, int T, int Tp,
                                                              const float4 *__restrict__ wq, const float *__restrict__ bias, int K,
-                                                             float slope, float *__restrict__ wav) {
+                                                             float slope, float *__restrict__ wav, const int *__restrict__ len,
+                                                             int mul) {
     extern __shared__ float4 sm4[];
     const int cq_n = C >> 2, halo = (K - 1) / 2, rows = 256 + 2 * halo;
     float4 *xs = sm4;               // [cq_n][rows]
     float4 *ws = sm4 + cq_n * rows; // [cq_n][K]
     const int b = blockIdx.y, t0 = blockIdx.x * 256, tid = threadIdx.x;
+    const int Tb = len ? len[b] * mul : T;                  // this clip's samples; the rest of its row is 0
+    if (t0 >= Tb) {
+        if (t0 + tid < T) wav[(size_t)b * T + t0 + tid] = 0.f;
+        return;
+    }
     for (int idx = tid; idx < cq_n * rows; idx += 256) {
         const int r = idx / cq_n, cq = idx - r * cq_n;      // quads of a row are contiguous in G32T
         xs[cq * rows + r] = lrelu4(__ldg(x + act_q4(b, C, Tp, cq, kPad + t0 - halo + r)), slope);
@@ -260,6 +308,10 @@ __global__ void __launch_bounds__(256) conv_post_tanh_kernel(const float4 *__res
     __syncthreads();
     const int t = t0 + tid;
     if (t >= T) return;
+    if (t >= Tb) {
+        wav[(size_t)b * T + t] = 0.f;
+        return;
+    }
     float acc = __ldg(bias);
     for (int cq = 0; cq < cq_n; ++cq)
         for (int k = 0; k < K; ++k) {
@@ -271,7 +323,7 @@ __global__ void __launch_bounds__(256) conv_post_tanh_kernel(const float4 *__res
 }
 
 int launch_conv_post_tanh(const float *x, int B, int C, int T, int Tp, const float *wq, const float *bias, int K, float slope,
-                          float *wav, cudaStream_t st) {
+                          float *wav, cudaStream_t st, const int *len, int mul) {
     const int rows = 256 + (K - 1);
     const size_t smem = (size_t)(C / 4) * (rows + K) * 16;
     SVB_CHECK(smem <= 200 * 1024, SVB_ERR_INVALID, "conv_post: %d channels do not fit shared memory", C);
@@ -279,7 +331,7 @@ int launch_conv_post_tanh(const float *x, int B, int C, int T, int Tp, const flo
     SVB_TRY(raise_smem_limit(conv_post_tanh_kernel, smem, configured));
     dim3 grid((T + 255) / 256, B);
     conv_post_tanh_kernel<<<grid, 256, smem, st>>>(reinterpret_cast<const float4 *>(x), C, T, Tp,
-                                                   reinterpret_cast<const float4 *>(wq), bias, K, slope, wav);
+                                                   reinterpret_cast<const float4 *>(wq), bias, K, slope, wav, len, mul);
     SVB_CUDA(cudaGetLastError());
     return SVB_OK;
 }

@@ -13,7 +13,7 @@ namespace svb {
 //   out_scale  : * s, accumulate: out += ...                        (sum of ResBlocks / num_kernels, :158-164)
 //   ups_u > 0  : transposed-conv polyphase: the GEMM column co' = phi*Cout + co is stored to row
 //                q*ups_u + phi, channel co of `out`                 (ConvTranspose1d, :122-125,154)
-struct ConvArgs {
+struct ConvShape {
     const float *in;
     const float *w;       // packed [KS][Cin][CoutP]
     const float *bias;    // [Cout]
@@ -35,6 +35,19 @@ struct ConvArgs {
     int fused_ctas = 0;   // fused tensor-core launches of C = 32: 1 = one CTA per SM; otherwise two where the layout and the
                           // batch allow them (conv_tc.cu: tc_fused_ctas)
 };
+// The tensor-core kernel's parameters hold a ConvShape; the ragged fields follow at the end of them (TcArgs), so the
+// parameter layout ptxas allocates the kernels' registers by stays as it is.
+struct ConvArgs : ConvShape {
+    // Ragged batches (inference): clip b has len[b] * len_mul valid GEMM rows (len = frames, len_mul = rows per frame at this
+    // layer) instead of Tq, which is then the longest clip's.  Rows at or past a clip's bound are never written and never
+    // reach a valid row except through the conv's zero padding, so the caller keeps them zero.  len: device copy (read by
+    // the kernels), len_host: the same on the host (read by the planners).  nullptr: every clip has Tq rows.
+    const int *len = nullptr;
+    const int *len_host = nullptr;
+    int len_mul = 1;
+};
+// valid GEMM rows of clip b (host side)
+inline int clip_rows(const ConvArgs &a, int b) { return a.len_host ? a.len_host[b] * a.len_mul : a.Tq; }
 
 int launch_conv_ffma(const ConvArgs &a, cudaStream_t st);
 
@@ -43,14 +56,24 @@ int launch_nct_to_c4t(const float *nct, float *c4t, int B, int C, int T, int Tp,
 int launch_c4t_to_nct(const float *c4t, float *nct, int B, int C, int T, int Tp, cudaStream_t st);
 // [B][T][C] (frame-major, the reference's [T, 80] mel) -> C4T
 int launch_btc_to_c4t(const float *btc, float *c4t, int B, int C, int T, int Tp, cudaStream_t st);
+// Ragged batches: `len` (device, frames per clip) bounds clip b; its frames at or past len[b] are written as zeros and
+// never read.  nct: [B][C][T]; btc: clip b's frames start at frame off[b] of a [sum len][C] array (back to back), or at
+// b * T when off is nullptr.
+int launch_nct_to_c4t_ragged(const float *nct, float *c4t, int B, int C, int T, int Tp, const int *len, cudaStream_t st);
+int launch_btc_to_c4t_ragged(const float *btc, float *c4t, int B, int C, int T, int Tp, const int *len, const int *off,
+                             cudaStream_t st);
 
 // x[b][n][c] += nb[c] + sum_j nw[c][j] * har[b][n*stride - pad + j]     (noise_convs, hifigan.py:127-132,156-157)
+// len (device frames, or nullptr): clip b has len[b] * mul rows and len[b] * har_mul samples of har; its other rows are
+// left alone, and har past its samples is the conv's zero padding.
 int launch_noise_conv_add(float *x, int B, int C, int T, int Tp, const float *har, int Thar, const float *nw,
-                          const float *nb, int K, int stride, int pad, cudaStream_t st);
+                          const float *nb, int K, int stride, int pad, cudaStream_t st, const int *len = nullptr, int mul = 1,
+                          int har_mul = 1);
 
 // wav[b][t] = tanh(bias + sum_{ci,k} w[ci][k] * lrelu(x[b][t+k-3][ci], slope))   (hifigan.py:165-167)
+// len (device frames, or nullptr): clip b has len[b] * mul samples; the samples after them are written as 0.
 int launch_conv_post_tanh(const float *x, int B, int C, int T, int Tp, const float *wq, const float *bias_dev, int K,
-                          float slope, float *wav, cudaStream_t st);
+                          float slope, float *wav, cudaStream_t st, const int *len = nullptr, int mul = 1);
 
 // host-side weight packing (layer_api.cu)
 std::vector<float> pack_conv_weights(const float *w, int Cout, int Cin, int K);

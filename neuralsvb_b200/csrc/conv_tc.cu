@@ -57,7 +57,7 @@ struct TcLayer {                // what differs between the layers of one launch
 };
 
 struct TcArgs {
-    ConvArgs a;                 // the shape class (B, channels, rows, in_slope, ups_u ...); per-layer fields live in L[]
+    ConvShape a;                // the shape class (B, channels, rows, in_slope, ups_u ...); per-layer fields live in L[]
     TcLayer L[2 * kTcMaxLayers];    // fused launches: L[j] = c1 and L[n_layers + j] = c2 of ResBlock chain j
     int n_layers;
     int fused_P;                // fused launches: output rows per item (the same for every layer of the launch)
@@ -80,6 +80,8 @@ struct TcArgs {
                                 // residual / running-sum pieces in flight; N > 64: the staged epilogue's kStageSlots slots
     int l2_prefetch;            // the producer prefetches each item's residual / running-sum rows into L2
     uint32_t off_epi;           // byte offset of the piece slots [kMathWarps][epi_slots][tc_epi_slot_bytes(N)]
+    const int *len;             // ragged batches (ConvArgs::len / len_mul): the implicit list's clip bounds, or nullptr
+    int len_mul;
 };
 
 constexpr int kMaxW = 8;
@@ -122,17 +124,26 @@ __host__ __device__ inline void tc_fused_slab(int t0, int h1, int h2, int in_Tp,
     *rows = min(2 * kTcM + 2 * h1, in_Tp - *row0);
 }
 
-// a work item, as staged in shared memory: x = layer | column block << 8 | tiles << 24, y = clip, z = first row.  Fused
-// items are always two tiles of the launch's only column block (tc_plan): constants, not registers.
+// a work item, as staged in shared memory: x = layer | column block << 8 | tiles << 24, y = clip, z = first row, w = the
+// clip's valid rows (Tq, or its own bound in a ragged batch: rows at or past it are neither stored nor, for c2 of a fused
+// item, fed by anything but zeros).  Fused items are always two tiles of the launch's only column block (tc_plan):
+// constants, not registers.  The row bound is not decoded: it is loaded from the table where it is used (item_rows), so it
+// holds no register through the MMAs (idx is the loop counter of the item walk).
 struct TcItem {
-    int layer, nblk, mt, b, t0;
+    int layer, nblk, mt, b, t0, idx;
 };
 template <bool FUSED>
-__device__ __forceinline__ TcItem item_decode(const int4 v) {
+__device__ __forceinline__ TcItem item_decode(const int4 *items, int n) {
+    const int4 v = items[n];
     TcItem it;
-    it.layer = v.x & 0xff, it.b = v.y, it.t0 = v.z;
+    it.layer = v.x & 0xff, it.b = v.y, it.t0 = v.z, it.idx = n;
     it.nblk = FUSED ? 0 : (v.x >> 8) & 0xffff, it.mt = FUSED ? 2 : v.x >> 24;
     return it;
+}
+__device__ __forceinline__ int item_rows(const int4 *items, const TcItem &it) {
+    int v;
+    asm volatile("ld.shared.s32 %0, [%1];" : "=r"(v) : "r"(smem_u32(&items[it.idx].w)));
+    return v;
 }
 
 // one tap of one 64-row warpgroup tile: all 32 input channels of the chunk (the split cross terms first, hi*hi last)
@@ -194,7 +205,7 @@ __global__ void __launch_bounds__(kTcThreadsP, tc_min_ctas(N, FUSED)) conv1d_c4_
     extern __shared__ __align__(1024) unsigned char smem[];
     constexpr bool BF = MODE == SVB_PREC_BF16X3;
     constexpr bool X3 = MODE == SVB_PREC_TF32X3;
-    const ConvArgs &a = p.a;
+    const ConvShape &a = p.a;
     // ---- shared memory carve-up (operand slots and weight ring are 1024-byte aligned: swizzle atoms)
     uint64_t *bars = reinterpret_cast<uint64_t *>(smem);
     uint64_t *raw_full = bars, *a_ready = bars + 4, *a_empty = bars + 8;      // up to 4 operand slots
@@ -232,9 +243,21 @@ __global__ void __launch_bounds__(kTcThreadsP, tc_min_ctas(N, FUSED)) conv1d_c4_
             const int tiles = (a.Tq + kTcM - 1) / kTcM;
             for (int i = threadIdx.x; i < n; i += kTcThreadsP) {
                 const int g = blockIdx.x + i * gridDim.x;
+                if (p.len) {                                         // ragged: only the live groups, (column block, clip, group)
+                    const int live = p.total_groups / p.col_blocks;
+                    int rem = g % live, b = 0, tq = 0, tb = 0;
+                    for (;; ++b) {
+                        tq = p.len[b] * p.len_mul, tb = (tq + kTcM - 1) / kTcM;
+                        const int gb = (tb + p.MT - 1) / p.MT;
+                        if (rem < gb) break;
+                        rem -= gb;
+                    }
+                    it_w[i] = make_int4(((g / live) << 8) | (min(p.MT, tb - rem * p.MT) << 24), b, rem * (kTcM * p.MT), tq);
+                    continue;
+                }
                 const int tg = g % p.groups_per_b, r = g / p.groups_per_b;
                 const int mt = min(p.MT, tiles - tg * p.MT);          // the last group of a clip with an odd tile count has one
-                it_w[i] = make_int4(((r / a.B) << 8) | (mt << 24), r % a.B, tg * (kTcM * p.MT), 0);
+                it_w[i] = make_int4(((r / a.B) << 8) | (mt << 24), r % a.B, tg * (kTcM * p.MT), a.Tq);
             }
             if (threadIdx.x == 0) *n_items_s = n;
         }
@@ -270,7 +293,7 @@ __global__ void __launch_bounds__(kTcThreadsP, tc_min_ctas(N, FUSED)) conv1d_c4_
                     bulk_g2s(wring + Ls[l].w_res_off, Ls[l].w, (uint32_t)Ls[l].KS * p.wtile_bytes, w_full);
             }
             for (int n = 0; n < n_items; ++n) {
-                const TcItem it = item_decode<FUSED>(items[n]);
+                const TcItem it = item_decode<FUSED>(items, n);
                 const TcLayer &L = Ls[it.layer];
                 const int halo = (L.KS - 1) / 2 * L.dil;
                 uint32_t raw_bytes = (uint32_t)(it.mt * kTcM + 2 * halo) * 128;
@@ -294,7 +317,7 @@ __global__ void __launch_bounds__(kTcThreadsP, tc_min_ctas(N, FUSED)) conv1d_c4_
                     // the rows this item's epilogue reads with per-thread loads, issued behind its last slab: they reach L2
                     // while the item's MMAs run, so those loads wait for L2 instead of HBM
                     const TcLayer &Lo = Ls[FUSED ? p.n_layers + it.layer : it.layer];
-                    const int rows = min(FUSED ? p.fused_P : it.mt * kTcM, a.Tq - it.t0);
+                    const int rows = min(FUSED ? p.fused_P : it.mt * kTcM, item_rows(items, it) - it.t0);
                     const int gout = c4t_groups(a.Cout);
                     for (int g = 0; g < N / 32 && rows > 0; ++g) {
                         const size_t off = (((size_t)it.b * gout + it.nblk * (N / 32) + g) * a.out_Tp + kPad + it.t0) * 32;
@@ -321,7 +344,7 @@ __global__ void __launch_bounds__(kTcThreadsP, tc_min_ctas(N, FUSED)) conv1d_c4_
         const float slope = a.in_slope;                         // 0 <= slope <= 1: lrelu(x) = max(x, slope * x)
         int sA = 0, phA = 0;
         for (int n = 0; n < n_items; ++n) {
-            const TcItem it = item_decode<FUSED>(items[n]);
+            const TcItem it = item_decode<FUSED>(items, n);
             const int R = it.mt * kTcM + (Ls[it.layer].KS - 1) / 2 * Ls[it.layer].dil * 2;
             for (int c = 0; c < p.n_chunks; ++c) {
                 mbar_wait(raw_full + sA, phA);
@@ -440,7 +463,7 @@ __global__ void __launch_bounds__(kTcThreadsP, tc_min_ctas(N, FUSED)) conv1d_c4_
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int q = it.t0 + row0 + r_lo + 8 * h;                  // GEMM row = output time step (before upsampling)
-                if (q >= a.Tq) continue;
+                if (q >= item_rows(items, it)) continue;
                 if (FUSED && row0 + r_lo + 8 * h >= p.fused_P) continue;    // the next item's rows
 
 #pragma unroll
@@ -482,7 +505,7 @@ __global__ void __launch_bounds__(kTcThreadsP, tc_min_ctas(N, FUSED)) conv1d_c4_
         uint32_t *epi_ph_s = reinterpret_cast<uint32_t *>(smem + 1024 + kMaxItems * 16) + (warp - kWarpMath0);
         auto piece_rows = [&](const TcItem &it, int blk) {                 // rows of this warp's piece that are written
             const int i0 = kTcM * blk + 64 * wg + 16 * (warp & 3);
-            int rows = min(16, a.Tq - (it.t0 + i0));
+            int rows = min(16, item_rows(items, it) - (it.t0 + i0));
             if (FUSED) rows = min(rows, p.fused_P - i0);
             return rows;
         };
@@ -729,13 +752,13 @@ __global__ void __launch_bounds__(kTcThreadsP, tc_min_ctas(N, FUSED)) conv1d_c4_
         };
         // ---- fused items: c1's epilogue stores c2's operand for the item's rows 0 .. 255 (time tq0 + row) into the
         // intermediate, in the layout the transform warps give a slab (hi / lo split or tf32 rounding, SWIZZLE_128B)
-        auto stage_intermediate = [&](const TcLayer &L1, const float *acc, int row0, int tq0) {
+        auto stage_intermediate = [&](const TcLayer &L1, const float *acc, int row0, int tq0, int Tq) {
             const float *bias_s = reinterpret_cast<const float *>(smem + p.off_bias) + L1.bias_off;
             const float slope = a.in_slope;
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int i = row0 + r_lo + 8 * h, q = tq0 + i;
-                const bool live = q >= 0 && q < a.Tq;                       // else c2's zero padding
+                const bool live = q >= 0 && q < Tq;                         // else c2's zero padding
                 const int sw = i & 7;
 #pragma unroll
                 for (int j = 0; j < N / 8; ++j) {
@@ -766,8 +789,8 @@ __global__ void __launch_bounds__(kTcThreadsP, tc_min_ctas(N, FUSED)) conv1d_c4_
             run_mma(std::true_type(), std::true_type(), L1);
             // the other warpgroup's c2 wgmmas of the previous item have retired: the intermediate may be overwritten
             named_bar_sync(1, kMathWarps * 32);
-            stage_intermediate(L1, acc0, 0, it.t0 - h2);
-            stage_intermediate(L1, acc1, kTcM, it.t0 - h2);
+            stage_intermediate(L1, acc0, 0, it.t0 - h2, item_rows(items, it));
+            stage_intermediate(L1, acc1, kTcM, it.t0 - h2, item_rows(items, it));
             fence_proxy_async();                                            // generic-proxy writes -> visible to the tensor core
             named_bar_sync(1, kMathWarps * 32);                             // c2's tap shifts read rows the other warpgroup wrote
             run_mma(std::true_type(), std::false_type(), L2);
@@ -775,7 +798,7 @@ __global__ void __launch_bounds__(kTcThreadsP, tc_min_ctas(N, FUSED)) conv1d_c4_
         };
         if (!FUSED && p.w_resident && n_items > 0) mbar_wait(w_full, 0);
         for (int n = 0; n < n_items; ++n) {
-            const TcItem it = item_decode<FUSED>(items[n]);
+            const TcItem it = item_decode<FUSED>(items, n);
             if constexpr (FUSED) run_fused(it);
             else if (it.mt == 2) run_item(std::true_type(), it);
             else run_item(std::false_type(), it);
@@ -1032,6 +1055,13 @@ static bool tc_layout(TcArgs &p, size_t &smem, size_t budget, size_t bias_bytes,
 //   rest) and a bias area of just the 2n layers' biases.  A shape that no fused launch runs, or whose layout does not
 //   fit, returns SVB_ERR_INVALID without setting the error message: callers probe for fused plans.
 constexpr size_t kSmemPerSm = 228 * 1024, kSmemReservedPerCta = 1024;
+// Units of `unit` rows (rounded up per clip) over the clips of a launch, each clip counted to its own bound in a ragged batch;
+// `per` > 1 groups that many units (rounded up per clip).  No unit starts at or past its clip's end.
+static long long tc_live_units(const ConvArgs &a, int unit, int per = 1) {
+    long long n = 0;
+    for (int b = 0; b < a.B; ++b) n += ((clip_rows(a, b) + unit - 1) / unit + per - 1) / per;
+    return n;
+}
 static int tc_plan(int n, const TcWeights *const *w, const ConvArgs *a, int precision, int ctas, int grid, TcArgs &p, size_t &smem) {
     const bool fused = ctas > 0;
     const ConvArgs &a0 = a[0];
@@ -1065,7 +1095,7 @@ static int tc_plan(int n, const TcWeights *const *w, const ConvArgs *a, int prec
             return SVB_ERR_INVALID;
         p.off_inter = p.off_op + (uint32_t)p.nA * p.op_bytes;
         p.groups_per_b = (a0.Tq + p.fused_P - 1) / p.fused_P;
-        p.total_groups = p.groups_per_b * a0.B;
+        p.total_groups = (int)tc_live_units(a0, p.fused_P);
     } else {
         SVB_CHECK(n >= 1 && n <= kTcMaxLayers, SVB_ERR_INVALID, "tc conv: %d layers in one launch", n);
         for (int l = 1; l < n; ++l)
@@ -1100,16 +1130,17 @@ static int tc_plan(int n, const TcWeights *const *w, const ConvArgs *a, int prec
         bool two = tiles >= 2 && fit(2);
         if (two && grid > 0) {
             // implicit round-robin list over `grid` CTAs: keep MT = 2 only if its makespan (in tiles) is no longer
-            const long long per = (long long)a0.B * (a0.CoutP / p.n_tile);
-            const long long g1 = per * tiles, g2 = per * ((tiles + 1) / 2);
+            const long long per = a0.CoutP / p.n_tile;
+            const long long g1 = per * tc_live_units(a0, kTcM), g2 = per * tc_live_units(a0, kTcM, 2);
             two = 2 * ((g2 + grid - 1) / grid) <= (g1 + grid - 1) / grid;
         }
         if (!two) SVB_CHECK(fit(1), SVB_ERR_INVALID, "tc conv: tile does not fit shared memory (N %d)", p.n_tile);
         p.fused_P = 0, p.off_inter = 0, p.inter_bytes = 0;
         p.groups_per_b = (tiles + p.MT - 1) / p.MT;
-        p.total_groups = p.groups_per_b * a0.B * p.col_blocks;
+        p.total_groups = (int)tc_live_units(a0, kTcM, p.MT) * p.col_blocks;
     }
     p.a = a0, p.n_layers = n;
+    p.len = a0.len, p.len_mul = a0.len_mul;
     p.work = nullptr, p.work_off = nullptr;
     // the staged epilogue's first loads of an item find its rows in L2 too
     p.l2_prefetch = (p.epi_slots == 0 || p.n_tile > 64) && tc_epi_sources(n, fused ? a + n : a) > 0;
@@ -1174,6 +1205,7 @@ int launch_conv_tc(const TcWeights &w, const ConvArgs &a, int precision, cudaStr
             s.in = a.in + (size_t)b0 * c4t_groups(a.Cin) * a.in_Tp * 32;
             s.out = a.out + (size_t)b0 * c4t_groups(a.Cout) * a.out_Tp * 32;
             if (a.res) s.res = a.res + (size_t)b0 * c4t_groups(a.Cout) * a.out_Tp * 32;
+            if (a.len) s.len = a.len + b0, s.len_host = a.len_host + b0;
             SVB_TRY(launch_conv_tc(w, s, precision, st));
         }
         return SVB_OK;
@@ -1183,9 +1215,11 @@ int launch_conv_tc(const TcWeights &w, const ConvArgs &a, int precision, cudaStr
 
 // whether `n` layers of this shape class fit one merged launch: the per-CTA item list lives in shared memory.  Counted
 // in one-tile items: the plan may pick MT = 1, and tc_schedule may split two-tile units back into one-tile items.
-bool tc_merge_fits(int n, int B, int Tq, int Cout, int n_tile) {
-    const int tiles = (Tq + kTcM - 1) / kTcM, groups = tiles * B * std::max(1, Cout / std::max(1, n_tile));
-    return (long long)groups * n <= (long long)(kMaxItems * 8 / 10) * sm_count();
+bool tc_merge_fits(int n, int B, int Tq, int Cout, int n_tile, const int *len_host, int len_mul) {
+    long long tiles = 0;
+    for (int b = 0; b < B; ++b) tiles += ((len_host ? len_host[b] * len_mul : Tq) + kTcM - 1) / kTcM;
+    const long long groups = tiles * std::max(1, Cout / std::max(1, n_tile));
+    return groups * n <= (long long)(kMaxItems * 8 / 10) * sm_count();
 }
 
 // ---- merged launches: several layers of one shape class, host-built balanced work list
@@ -1197,15 +1231,18 @@ void tc_worklist_free(TcWorkList *wl) {
 
 // The schedule itself is plain host code (no CUDA call): exposed for the CPU tests through svb_tc_schedule_probe.
 // fused_P > 0: fused items (KS2 = c2's taps per layer) of fused_P output rows each, always 256 c1 rows, never split.
+// rows: nullptr, or the valid rows of each clip (ragged batches; Tq is then unused): a clip's items stop at its last live
+// tile, and each item carries its clip's row bound.
 int tc_schedule(int n, const int *KS, const int *KS2, const int *has_res, const int *accum, int Cin, int B, int Tq, int MT, int fused_P,
-                int col_blocks, bool chain_ordered, int grid, std::vector<int4> *items_out, std::vector<int> *off_out, double *balance_out) {
-    const int tiles = (Tq + kTcM - 1) / kTcM;
+                int col_blocks, bool chain_ordered, int grid, std::vector<int4> *items_out, std::vector<int> *off_out, double *balance_out,
+                const int *rows = nullptr) {
     const bool fused = fused_P > 0;
     // cost of an item in "taps of one tile": the MMA work plus a constant for the memory-bound part (slab, epilogue)
     const double beta = 160.0 / std::max(32, Cin);
     struct Unit {
         double cost;
         int nblk, b, t0, mt, layer;     // layer < 0: all layers in order (chain-ordered unit)
+        int Tq;                         // the clip's valid rows
     };
     auto unit_cost = [&](int layer, int mt) {
         auto taps = [&](int l) { return KS[l] + (fused ? KS2[l] : 0); };
@@ -1216,15 +1253,17 @@ int tc_schedule(int n, const int *KS, const int *KS2, const int *has_res, const 
     };
     std::vector<Unit> units;
     for (int nblk = 0; nblk < col_blocks; ++nblk)
-        for (int b = 0; b < B; ++b)
-            for (int t0 = 0; t0 < (fused ? Tq : tiles * kTcM); t0 += (fused ? fused_P : MT * kTcM)) {
+        for (int b = 0; b < B; ++b) {
+            const int Tb = rows ? rows[b] : Tq, tiles = (Tb + kTcM - 1) / kTcM;
+            for (int t0 = 0; t0 < (fused ? Tb : tiles * kTcM); t0 += (fused ? fused_P : MT * kTcM)) {
                 const int mt = fused ? 2 : std::min(MT, tiles - t0 / kTcM);
                 if (chain_ordered) {
-                    units.push_back({unit_cost(-1, mt), nblk, b, t0, mt, -1});
+                    units.push_back({unit_cost(-1, mt), nblk, b, t0, mt, -1, Tb});
                 } else {
-                    for (int l = 0; l < n; ++l) units.push_back({unit_cost(l, mt), nblk, b, t0, mt, l});
+                    for (int l = 0; l < n; ++l) units.push_back({unit_cost(l, mt), nblk, b, t0, mt, l, Tb});
                 }
             }
+        }
     // longest processing time first onto the least-loaded CTA.  When the units are too coarse for the SMs (balance below
     // 0.95, e.g. a few two-tile units per CTA), split the cheapest two-tile units into one-tile halves and redo the
     // schedule; a split is kept only if it improves the balance.
@@ -1300,7 +1339,7 @@ int tc_schedule(int n, const int *KS, const int *KS2, const int *has_res, const 
         for (int u : mine[c]) {
             const Unit &U = units[u];
             for (int l = (U.layer < 0 ? 0 : U.layer); l < (U.layer < 0 ? n : U.layer + 1); ++l)
-                items.push_back(make_int4(l | (U.nblk << 8) | (U.mt << 24), U.b, U.t0, 0));
+                items.push_back(make_int4(l | (U.nblk << 8) | (U.mt << 24), U.b, U.t0, U.Tq));
         }
         off[c + 1] = (int)items.size();
         SVB_CHECK(off[c + 1] - off[c] <= kMaxItems, SVB_ERR_INVALID, "tc conv: %d work items on one CTA (limit %d)", off[c + 1] - off[c], kMaxItems);
@@ -1342,7 +1381,7 @@ static bool tc_fused_fits_ctas(int n, const TcWeights *const *w, const ConvArgs 
         if (fit < ctas) return false;
     }
     const int grid = ctas * sm_count();
-    const double units = (double)a[0].B * p.groups_per_b, beta = 160.0 / std::max(32, a[0].Cin);
+    const double units = (double)p.total_groups, beta = 160.0 / std::max(32, a[0].Cin);
     if (units * n < 4.0 * grid) return false;
     double sum = 0, mx = 0, mn = 1e30;
     for (int l = 0; l < n; ++l) {
@@ -1377,9 +1416,11 @@ int tc_worklist_build(int n, const TcWeights *const *w, const ConvArgs *a, int p
     for (int l = 0; l < n; ++l) KS[l] = a[l].KS, KS2[l] = ao[l].KS, has_res[l] = ao[l].res != nullptr, accum[l] = ao[l].accumulate;
     std::vector<int4> items;
     std::vector<int> off;
+    std::vector<int> rows;
+    for (int b = 0; b < a[0].B && a[0].len_host; ++b) rows.push_back(clip_rows(a[0], b));
     double balance = 0;
     SVB_TRY(tc_schedule(n, KS, fused ? KS2 : nullptr, has_res, accum, a[0].Cin, a[0].B, a[0].Tq, p.MT, p.fused_P, p.col_blocks,
-                        chain_ordered, grid, &items, &off, &balance));
+                        chain_ordered, grid, &items, &off, &balance, rows.empty() ? nullptr : rows.data()));
     tc_worklist_free(out);
     SVB_CUDA(cudaMalloc((void **)&out->items, std::max<size_t>(items.size(), 1) * sizeof(int4)));
     SVB_CUDA(cudaMalloc((void **)&out->off, off.size() * sizeof(int)));
@@ -1461,6 +1502,45 @@ extern "C" int64_t svb_tc_fused_schedule_probe(int32_t n_layers, const int32_t *
         const int l = items[i].x & 0xff;
         o[0] = l, o[1] = (items[i].x >> 8) & 0xffff, o[2] = items[i].y, o[3] = items[i].z, o[4] = items[i].x >> 24;
         svb::tc_fused_slab(items[i].z, (ks1[l] - 1) / 2 * dil1[l], (ks2[l] - 1) / 2, svb::c4t_rows(Tq), &o[5], &o[6]);
+    }
+    for (int c = 0; c <= grid; ++c) off_out[c] = off[c];
+    *P_out = P;
+    return (int64_t)items.size();
+}
+
+// Host-only view of a ragged batch's schedule: clip b has lengths[b] valid rows.  KS2 = NULL: single-conv items as
+// svb_tc_schedule_probe gives them (MT 1 or 2, col_blocks column blocks); else fused items as svb_tc_fused_schedule_probe
+// gives them (MT 2, one column block, P = 256 - 2 max((KS2 - 1) / 2) output rows per item, to *P_out).  items_out receives 6
+// int32 per item: layer, column block, clip, first row, tiles, and the row bound the item carries (its clip's length).
+extern "C" int64_t svb_tc_ragged_schedule_probe(int32_t n_layers, const int32_t *KS, const int32_t *KS2, const int32_t *has_res,
+                                                const int32_t *accumulate, int32_t Cin, int32_t B, const int32_t *lengths, int32_t MT,
+                                                int32_t col_blocks, int32_t chain_ordered, int32_t grid, int32_t *items_out,
+                                                int64_t items_capacity, int32_t *off_out, int32_t *P_out, double *balance_out) {
+    SVB_CHECK(n_layers >= 1 && n_layers <= svb::kTcMaxLayers && KS && has_res && accumulate && B > 0 && lengths && grid >= 1 &&
+                  items_out && off_out && P_out && balance_out && (KS2 ? MT == 2 && col_blocks == 1 : (MT == 1 || MT == 2) && col_blocks >= 1),
+              SVB_ERR_INVALID, "tc_ragged_schedule_probe: bad argument");
+    int ks[svb::kTcMaxLayers], ks2[svb::kTcMaxLayers], hr[svb::kTcMaxLayers], ac[svb::kTcMaxLayers], h2 = 0, Tq = 0;
+    for (int l = 0; l < n_layers; ++l) {
+        ks[l] = KS[l], hr[l] = has_res[l], ac[l] = accumulate[l], ks2[l] = KS2 ? KS2[l] : 0;
+        SVB_CHECK(!KS2 || (KS2[l] >= 1 && KS2[l] < svb::kTcM), SVB_ERR_INVALID, "tc_ragged_schedule_probe: layer %d: c2 taps %d", l, ks2[l]);
+        h2 = std::max(h2, (ks2[l] - 1) / 2);
+    }
+    std::vector<int> rows(lengths, lengths + B);
+    for (int b = 0; b < B; ++b) {
+        SVB_CHECK(rows[b] >= 1, SVB_ERR_INVALID, "tc_ragged_schedule_probe: clip %d has %d rows", b, rows[b]);
+        Tq = std::max(Tq, rows[b]);
+    }
+    const int P = KS2 ? 2 * svb::kTcM - 2 * h2 : 0;
+    std::vector<int4> items;
+    std::vector<int> off;
+    SVB_TRY(svb::tc_schedule(n_layers, ks, KS2 ? ks2 : nullptr, hr, ac, Cin, B, Tq, MT, P, col_blocks, chain_ordered != 0, grid, &items,
+                             &off, balance_out, rows.data()));
+    SVB_CHECK((int64_t)items.size() <= items_capacity, SVB_ERR_INVALID, "tc_ragged_schedule_probe: %zu items, capacity %lld", items.size(),
+              (long long)items_capacity);
+    for (size_t i = 0; i < items.size(); ++i) {
+        int32_t *o = items_out + 6 * i;
+        o[0] = items[i].x & 0xff, o[1] = (items[i].x >> 8) & 0xffff, o[2] = items[i].y, o[3] = items[i].z, o[4] = items[i].x >> 24;
+        o[5] = items[i].w;
     }
     for (int c = 0; c <= grid; ++c) off_out[c] = off[c];
     *P_out = P;

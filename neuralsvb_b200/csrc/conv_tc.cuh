@@ -43,8 +43,9 @@ struct TcWorkList {
 int tc_worklist_build(int n, const TcWeights *const *w, const ConvArgs *a, int precision, bool chain_ordered, TcWorkList *out,
                       bool fused = false);
 void tc_worklist_free(TcWorkList *wl);
-// the per-CTA item list of a merged launch is bounded (shared memory): very long batches fall back to one launch per layer
-bool tc_merge_fits(int n, int B, int Tq, int Cout, int n_tile);
+// the per-CTA item list of a merged launch is bounded (shared memory): very long batches fall back to one launch per layer.
+// len_host (ragged batches, ConvArgs::len_host / len_mul): only each clip's live tiles count.
+bool tc_merge_fits(int n, int B, int Tq, int Cout, int n_tile, const int *len_host = nullptr, int len_mul = 1);
 // whether one step of n ResBlock1 chains (w / a as for fused work lists) runs as a fused launch: C = 32 or 64, and the
 // layout fits shared memory (not in tf32x3) and the item table, with two CTAs per SM (C = 32) or one
 bool tc_fused_fits(int n, const TcWeights *const *w, const ConvArgs *a, int precision);

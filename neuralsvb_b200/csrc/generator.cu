@@ -78,6 +78,19 @@ struct Plan {
     }
 };
 
+// Ragged forward: every launch bounds clip b to its own rows, len[b] x (rows per frame of the layer)
+void set_ragged(const svb_gen *g, ConvArgs &a) {
+    if (g->rg_len.empty()) return;
+    a.len = g->rg_dev, a.len_host = g->rg_len.data(), a.len_mul = a.Tq / g->cur_T;
+}
+// GEMM rows the clips of a launch of Tq rows per clip compute: their own rows in a ragged forward (last_flops, profile bytes)
+double live_rows(const svb_gen *g, int B, int Tq) {
+    if (g->rg_len.empty()) return (double)B * Tq;
+    double n = 0;
+    for (int l : g->rg_len) n += l;
+    return n * (Tq / g->cur_T);
+}
+
 ConvArgs resblock_args(const ConvLayer &L, const float *in, float *out, const float *res, float scale, int accumulate, int B, int Tq,
                        int Tp, float in_slope) {
     ConvArgs a;
@@ -102,6 +115,7 @@ bool stage_fused(const svb_gen *g, const Stage &s, int B, int Ti) {
             a[j] = resblock_args(s.c1[j][m], nullptr, nullptr, nullptr, 1.f, 0, B, Ti, c4t_rows(Ti), 0.1f);
             a[nk + j] = resblock_args(s.c2[j][m], nullptr, nullptr, nullptr, 1.f, 0, B, Ti, c4t_rows(Ti), 0.1f);
             a[j].fused_ctas = a[nk + j].fused_ctas = g->fused_ctas;
+            set_ragged(g, a[j]), set_ragged(g, a[nk + j]);
             w[j] = &s.c1[j][m].tc, w[nk + j] = &s.c2[j][m].tc;
         }
         if (!tc_fused_fits(nk, w, a, g->cfg.precision)) return false;
@@ -123,6 +137,7 @@ Buffers plan_workspace(const svb_gen *g, int B, int T, size_t *total) {
         b.X.push_back(p.take(n)), b.S.push_back(p.take(n));
         b.A.emplace_back(), b.R.emplace_back();
         const bool fused = stage_fused(g, s, B, Ti);
+        b.fused.push_back(fused);
         for (int j = 0; j < g->cfg.n_resblock_kernels; ++j) {
             // inference: one A / R buffer per chain, reused by every dilation; training: every conv input is kept (the tape).
             // Fused steps have no A, and their x ping-pongs between two R buffers: an item reads its input rows plus a halo
@@ -139,6 +154,7 @@ Buffers plan_workspace(const svb_gen *g, int B, int T, size_t *total) {
         b.sines = p.take((size_t)B * T * g->hop * 9 * 4);
         b.wav = p.take((size_t)B * T * g->hop * 4);
     }
+    b.f0 = p.take((size_t)B * T * 4);
     *total = p.total;
     return b;
 }
@@ -170,19 +186,21 @@ struct ProfScope {
 
 int run_conv(svb_gen *g, const ConvLayer &L, const float *in, int in_Tp, float *out, int out_Tp, const float *res,
              int B, int Tq, float in_slope, float scale, int accumulate, cudaStream_t st) {
+    const double rows = live_rows(g, B, Tq);
     g->last_launches += 1;
-    g->last_flops += 2.0 * L.macs_per_row * (double)B * Tq;
+    g->last_flops += 2.0 * L.macs_per_row * rows;
     const bool tc = g->cfg.precision != SVB_PREC_FP32 && L.tc.ok;
-    const double rows_out = (double)B * Tq * (L.ups_u > 0 ? L.ups_u : 1);
+    const double rows_out = rows * (L.ups_u > 0 ? L.ups_u : 1);
     // layer-streaming bytes (SURVEY 8(d)): input once, output once, residual / accumulated sum once more each
-    const double bytes = 4.0 * ((double)B * Tq * L.Cin + rows_out * L.Cout * (1 + (res ? 1 : 0) + (accumulate ? 1 : 0)));
+    const double bytes = 4.0 * (rows * L.Cin + rows_out * L.Cout * (1 + (res ? 1 : 0) + (accumulate ? 1 : 0)));
     ProfScope ps(g, st, tc ? (L.ups_u ? "conv1d_c4_tc (upsampler)" : "conv1d_c4_tc (resblock)") : "conv1d_c4_ffma", bytes,
-                 2.0 * L.macs_per_row * (double)B * Tq);
+                 2.0 * L.macs_per_row * rows);
     ConvArgs a;
     a.in = in, a.w = L.w, a.bias = L.b, a.res = res, a.out = out;
     a.B = B, a.Cin = L.Cin, a.in_Tp = in_Tp, a.Cout = L.Cout, a.out_Tp = out_Tp, a.CoutP = L.CoutP, a.Tq = Tq;
     a.KS = L.KS, a.dil = L.dil, a.ups_u = L.ups_u, a.in_slope = in_slope, a.out_scale = scale, a.accumulate = accumulate;
     a.epi_stream = g->epi;
+    set_ragged(g, a);
     if (g->cfg.precision != SVB_PREC_FP32 && tc_supported(L.tc, a)) return launch_conv_tc(L.tc, a, g->cfg.precision, st);
     return launch_conv_ffma(a, st);
 }
@@ -197,13 +215,15 @@ int run_conv_multi(svb_gen *g, int stage, int nk, const ConvLayer *const *Ls, co
     ConvArgs a[2 * kTcMaxLayers];
     const TcWeights *w[2 * kTcMaxLayers];
     double bytes = 0, flops = 0;
+    const double rows = live_rows(g, B, Tq);
     for (int j = 0; j < (fused ? 2 * nk : nk); ++j) {
         const ConvLayer &L = *Ls[j];
         a[j] = resblock_args(L, in[j], out[j], res[j], scale[j], accumulate[j], B, Tq, Tp, in_slope);
         a[j].epi_stream = g->epi, a[j].fused_ctas = g->fused_ctas;
+        set_ragged(g, a[j]);
         w[j] = &L.tc;
-        bytes += 4.0 * ((double)B * Tq * L.Cin + (double)B * Tq * L.Cout * (1 + (res[j] ? 1 : 0) + (accumulate[j] ? 1 : 0)));
-        flops += 2.0 * L.macs_per_row * (double)B * Tq;
+        bytes += 4.0 * (rows * L.Cin + rows * L.Cout * (1 + (res[j] ? 1 : 0) + (accumulate[j] ? 1 : 0)));
+        flops += 2.0 * L.macs_per_row * rows;
     }
     g->last_launches += 1;
     g->last_flops += flops;
@@ -220,15 +240,94 @@ int run_conv_multi(svb_gen *g, int stage, int nk, const ConvLayer *const *Ls, co
     return SVB_ERR_STATE;
 }
 
+// ---- ragged batches
+// The device table of a ragged forward, 4 B ints: [length | zero from | zero to | first frame].  Clip b's rows from its length up
+// to `zero to` frames may hold what an earlier, longer call on this workspace wrote (ws_live), and are zeroed before the
+// forward.  `first frame`: where the clip starts in back-to-back inputs (the host calls).
+void ragged_table(const svb_gen *g, int B, int T, const int *len, int *tab) {
+    const bool same = g->ws_B == B && g->ws_T == T && (int)g->ws_live.size() == B;     // else the workspace is zeroed anyway
+    int off = 0;
+    for (int b = 0; b < B; ++b) {
+        tab[b] = len[b], tab[B + b] = len[b];
+        tab[2 * B + b] = same ? std::max(len[b], g->ws_live[b]) : len[b];
+        tab[3 * B + b] = off, off += len[b];
+    }
+}
+
+int check_lengths(const svb_gen *g, int B, int T, const int32_t *len) {
+    SVB_CHECK(g && g->finalized, SVB_ERR_STATE, "generator: forward before finalize");
+    SVB_CHECK(!g->training, SVB_ERR_STATE, "generator: a training handle takes no lengths (ragged batches are inference only)");
+    SVB_CHECK(len && B > 0 && T > 0, SVB_ERR_INVALID, "generator: null lengths or empty batch (B %d T %d)", B, T);
+    for (int b = 0; b < B; ++b)
+        SVB_CHECK(len[b] >= 1 && len[b] <= T, SVB_ERR_INVALID, "generator: clip %d has %d frames (1 .. %d)", b, len[b], T);
+    return SVB_OK;
+}
+
+constexpr int kMaxTailBufs = 128;
+struct TailList {           // the G32T activation buffers of a forward, for zero_tails_kernel
+    int n;
+    struct {
+        unsigned long long off;     // bytes into the workspace
+        int groups, Tp, mul;        // channel groups, padded rows per group, rows per frame
+    } buf[kMaxTailBufs];
+};
+
+// rows [from, to) x mul of clip b in every buffer (from / to: frames, the ragged table's second and third parts)
+__global__ void zero_tails_kernel(const __grid_constant__ TailList L, char *ws, const int *__restrict__ tab, int B) {
+    const int b = blockIdx.z;
+    const int groups = L.buf[blockIdx.y].groups, Tp = L.buf[blockIdx.y].Tp, mul = L.buf[blockIdx.y].mul;
+    const int r0 = tab[B + b] * mul, r1 = tab[2 * B + b] * mul;
+    if (r1 <= r0) return;
+    const long long per = (long long)(r1 - r0) * 8;                 // float4 per channel group
+    float4 *base = reinterpret_cast<float4 *>(ws + L.buf[blockIdx.y].off) + ((size_t)b * groups * Tp + kPad + r0) * 8;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < per * groups; i += (long long)gridDim.x * blockDim.x) {
+        const long long grp = i / per;
+        base[grp * Tp * 8 + (i - grp * per)] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+}
+
+// f0 of back-to-back clips -> [B][T], 0 past each clip
+__global__ void unpack_f0_kernel(const float *__restrict__ cat, const int *__restrict__ tab, int B, int T, float *__restrict__ out) {
+    const int t = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
+    if (t < T) out[(size_t)b * T + t] = t < tab[b] ? cat[tab[3 * B + b] + t] : 0.f;
+}
+
+// ragged: lens = frames per clip (host), nullptr for a uniform batch.  packed_tab = nullptr: mel [B][n_mel][T] / f0 [B][T] as
+// svb_gen_forward takes them, and the ragged table is built and uploaded here; else the host call's device copy of
+// ragged_table, and mel / f0 hold the clips back to back (mel frame-major).
 int forward_impl(svb_gen *g, const float *mel, bool mel_frame_major, const float *f0, const float *rand_ini,
-                 const float *noise, uint64_t seed, int B, int T, float *wav, cudaStream_t st) {
+                 const float *noise, uint64_t seed, int B, int T, float *wav, cudaStream_t st, const int *lens = nullptr,
+                 const int *packed_tab = nullptr) {
     SVB_CHECK(g && g->finalized, SVB_ERR_STATE, "generator: forward before finalize");
     SVB_CHECK(!g->dirty, SVB_ERR_STATE, "generator: weights were set after finalize; call svb_gen_update_weights first");
     SVB_CHECK(mel && wav && B > 0 && T > 0, SVB_ERR_INVALID, "generator: null buffer or empty batch (B %d T %d)", B, T);
     SVB_CHECK(!f0 || g->cfg.use_pitch_embed, SVB_ERR_INVALID, "generator: f0 given but use_pitch_embed is off");
     SVB_CHECK((rand_ini == nullptr) == (noise == nullptr), SVB_ERR_INVALID,
               "generator: rand_ini and noise must be given together");
+    if (lens) SVB_TRY(check_lengths(g, B, T, lens));
     SVB_CUDA(cudaSetDevice(g->device));
+    const bool ragged = lens != nullptr;
+    std::vector<int> tab;
+    g->cur_T = T;
+    g->rg_dev = packed_tab;
+    if (ragged) {
+        g->rg_len.assign(lens, lens + B);
+        tab.resize(4 * (size_t)B);
+        ragged_table(g, B, T, lens, tab.data());
+        if (!packed_tab) {
+            if (tab.size() > g->rg_cap) {
+                if (g->rg_buf) SVB_CUDA(cudaFree(g->rg_buf));
+                g->rg_buf = nullptr, g->rg_cap = 0;
+                SVB_CUDA(cudaMalloc((void **)&g->rg_buf, tab.size() * sizeof(int)));
+                g->rg_cap = tab.size();
+            }
+            // pageable source: staged before the call returns, so `tab` may go out of scope
+            SVB_CUDA(cudaMemcpyAsync(g->rg_buf, tab.data(), tab.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+            g->rg_dev = g->rg_buf;
+        }
+    } else {
+        g->rg_len.clear();
+    }
     size_t need = 0;
     Buffers bf = plan_workspace(g, B, T, &need);
     if (need > g->ws_cap) {
@@ -237,29 +336,79 @@ int forward_impl(svb_gen *g, const float *mel, bool mel_frame_major, const float
         SVB_CUDA(cudaMalloc((void **)&g->ws, need));
         g->ws_cap = need, g->ws_B = 0;
     }
-    if (g->ws_B != B || g->ws_T != T) {
+    if (g->ws_B != B || g->ws_T != T || g->wl_len != g->rg_len) {     // work lists depend on the clips' lengths too
         for (auto &kv : g->worklists) tc_worklist_free(&kv.second);
         g->worklists.clear();
+        g->wl_len = g->rg_len;
     }
-    if (g->ws_B != B || g->ws_T != T || g->ws_training != g->training) {   // new layout: rebuild the zero padding of every buffer
+    // new layout (shape, mode, or which stages run fused: their buffers move): rebuild the zero padding of every buffer
+    if (g->ws_B != B || g->ws_T != T || g->ws_training != g->training || g->ws_fused != bf.fused) {
         SVB_CUDA(cudaMemsetAsync(g->ws, 0, need, st));
-        g->ws_B = B, g->ws_T = T, g->ws_training = g->training;
+        g->ws_B = B, g->ws_T = T, g->ws_training = g->training, g->ws_fused = bf.fused;
+        g->ws_live.assign(B, 0);
     }
     g->bf = bf, g->last_T = T, g->last_nsf = f0 != nullptr;
     g->last_launches = 0, g->last_flops = 0, g->last_B = B;
     g->taps.clear();
     g->recs.clear(), g->ev_used = 0;
     if (g->timing) SVB_CUDA(cudaEventRecord(g->ev0, st));
+    // Zeroing policy of ragged calls: every row at or past a clip's length must be zero in every activation buffer (the halo
+    // of the next conv reads it as the clip's zero padding), and no kernel writes such rows.  A full memset happens only when
+    // the layout changes; otherwise only the rows an earlier call left live past this call's lengths (ws_live) are zeroed,
+    // in one launch over all buffers.  Uniform calls write every row below T and leave all clips live to T.
+    if (ragged) {
+        bool any = false;
+        for (int b = 0; b < B; ++b) any = any || tab[2 * B + b] > tab[B + b];
+        if (any) {
+            TailList L;
+            L.n = 0;
+            auto add = [&](size_t off, int C, int Ti) {
+                for (int i = 0; i < L.n; ++i)
+                    if (L.buf[i].off == off) return;
+                L.buf[L.n].off = off, L.buf[L.n].groups = c4t_groups(C), L.buf[L.n].Tp = c4t_rows(Ti), L.buf[L.n].mul = Ti / T;
+                ++L.n;
+            };
+            add(bf.pre, g->cfg.upsample_initial_channel, T);
+            int Ti = T;
+            for (size_t i = 0; i < g->stages.size(); ++i) {
+                Ti *= g->stages[i].u;
+                const int C = g->stages[i].C;
+                add(bf.X[i], C, Ti), add(bf.S[i], C, Ti);
+                for (auto &v : bf.A[i])
+                    for (size_t o : v) add(o, C, Ti);
+                for (auto &v : bf.R[i])
+                    for (size_t o : v) add(o, C, Ti);
+                SVB_CHECK(L.n <= kMaxTailBufs - 10, SVB_ERR_INVALID, "generator: %d activation buffers", L.n);
+            }
+            ProfScope ps(g, st, "zero tails", 0, 0);
+            zero_tails_kernel<<<dim3(32, L.n, B), 256, 0, st>>>(L, g->ws, g->rg_dev, B);
+            SVB_CUDA(cudaGetLastError());
+            g->last_launches += 1;
+        }
+        for (int b = 0; b < B; ++b) g->ws_live[b] = lens[b];
+    } else {
+        g->ws_live.assign(B, T);
+    }
 
     auto F = [&](size_t off) { return reinterpret_cast<float *>(g->ws + off); };
     const int n_mel = g->cfg.n_mel, C0 = g->cfg.upsample_initial_channel;
     const int Tp0 = c4t_rows(T);
     {
         ProfScope ps(g, st, "mel layout", 8.0 * B * n_mel * T, 0);
-        if (mel_frame_major) SVB_TRY(launch_btc_to_c4t(mel, F(bf.mel), B, n_mel, T, Tp0, st));
+        if (ragged && mel_frame_major) SVB_TRY(launch_btc_to_c4t_ragged(mel, F(bf.mel), B, n_mel, T, Tp0, g->rg_dev,
+                                                                        packed_tab ? packed_tab + 3 * B : nullptr, st));
+        else if (ragged) SVB_TRY(launch_nct_to_c4t_ragged(mel, F(bf.mel), B, n_mel, T, Tp0, g->rg_dev, st));
+        else if (mel_frame_major) SVB_TRY(launch_btc_to_c4t(mel, F(bf.mel), B, n_mel, T, Tp0, st));
         else SVB_TRY(launch_nct_to_c4t(mel, F(bf.mel), B, n_mel, T, Tp0, st));
     }
     g->last_launches += 1;
+    if (f0 && packed_tab) {                         // back-to-back f0 -> [B][T]
+        unpack_f0_kernel<<<dim3((T + 255) / 256, B), 256, 0, st>>>(f0, packed_tab, B, T, F(bf.f0));
+        SVB_CUDA(cudaGetLastError());
+        g->last_launches += 1;
+        f0 = F(bf.f0);
+    }
+    const int *len_dev = ragged ? g->rg_dev : nullptr;
 
     const int Tw = T * g->hop;
     float *har = nullptr;
@@ -278,7 +427,7 @@ int forward_impl(svb_gen *g, const float *mel, bool mel_frame_major, const float
         {
             ProfScope ps(g, ns, "nsf source (4 kernels)", 4.0 * B * (T + (double)Tw * (noise ? 10 : 1)), 60.0 * B * Tw * 9);
             SVB_TRY(launch_nsf_source(f0, rand_ini, noise, seed, B, T, g->hop, (float)g->cfg.audio_sample_rate, g->lin_w,
-                                      g->lin_b_dev, g->ws + bf.nsf, har, g->training ? F(bf.sines) : nullptr, ns, &l));
+                                      g->lin_b_dev, g->ws + bf.nsf, har, g->training ? F(bf.sines) : nullptr, ns, &l, len_dev));
         }
         if (har_on_side) SVB_CUDA(cudaEventRecord(g->ev_side, ns));
         g->last_launches += l;
@@ -301,9 +450,9 @@ int forward_impl(svb_gen *g, const float *mel, bool mel_frame_major, const float
             if (har_on_side && i == 0) SVB_CUDA(cudaStreamWaitEvent(st, g->ev_side, 0));
             ProfScope ps(g, st, "noise_conv_add", 4.0 * B * (2.0 * Ti * s.C + Tw), 2.0 * B * (double)Ti * s.C * s.noise.K);
             SVB_TRY(launch_noise_conv_add(X, B, s.C, Ti, Tip, har, Tw, s.noise.w, s.noise.b, s.noise.K, s.noise.stride,
-                                          s.noise.pad, st));
+                                          s.noise.pad, st, len_dev, Ti / T, g->hop));
             g->last_launches += 1;
-            g->last_flops += 2.0 * B * (double)Ti * s.C * s.noise.K;
+            g->last_flops += 2.0 * live_rows(g, B, Ti) * s.C * s.noise.K;
         }
         g->taps["ups" + std::to_string(i)] = Tap{X, s.C, Ti, Tip, false};
         // xs = sum_j resblocks[i*nk + j](x) ; x = xs / nk      :158-164
@@ -328,7 +477,8 @@ int forward_impl(svb_gen *g, const float *mel, bool mel_frame_major, const float
         }
         // merged schedule: step m of all nk chains in ONE persistent launch (the chains only share their input)
         bool merged = !fused && g->merge && nk > 1 && nk <= kTcMaxLayers && g->cfg.precision != SVB_PREC_FP32 &&
-                      s.c1[0][0].tc.ok && tc_merge_fits(nk, B, Ti, s.C, s.c1[0][0].tc.n_tile);
+                      s.c1[0][0].tc.ok &&
+                      tc_merge_fits(nk, B, Ti, s.C, s.c1[0][0].tc.n_tile, ragged ? g->rg_len.data() : nullptr, Ti / T);
         for (int j = 0; merged && j < nk; ++j)
             for (int m = 0; m < nd; ++m) {
                 ConvArgs probe;
@@ -400,10 +550,11 @@ int forward_impl(svb_gen *g, const float *mel, bool mel_frame_major, const float
     // x = tanh(conv_post(leaky_relu(x)))   default slope 0.01   :165-167
     {
         ProfScope ps(g, st, "conv_post_tanh", 4.0 * B * Tin * (g->post_C + 1.0), 2.0 * B * (double)Tin * g->post_C * g->post_K);
-        SVB_TRY(launch_conv_post_tanh(x_in, B, g->post_C, Tin, Tin_p, g->post_wq, g->post_b_dev, g->post_K, 0.01f, wav, st));
+        SVB_TRY(launch_conv_post_tanh(x_in, B, g->post_C, Tin, Tin_p, g->post_wq, g->post_b_dev, g->post_K, 0.01f, wav, st,
+                                      len_dev, Tin / T));
     }
     g->last_launches += 1;
-    g->last_flops += 2.0 * B * (double)Tin * g->post_C * g->post_K;
+    g->last_flops += 2.0 * live_rows(g, B, Tin) * g->post_C * g->post_K;
     if (g->training) SVB_CUDA(cudaMemcpyAsync(F(bf.wav), wav, (size_t)B * Tw * 4, cudaMemcpyDeviceToDevice, st));
     if (g->timing) SVB_CUDA(cudaEventRecord(g->ev1, st));
     return SVB_OK;
@@ -471,6 +622,8 @@ extern "C" void svb_gen_destroy(svb_gen_t *g) {
     if (g->dev_in) cudaFree(g->dev_in);
     if (g->dev_out) cudaFree(g->dev_out);
     if (g->dev_i16) cudaFree(g->dev_i16);
+    if (g->dev_pack) cudaFree(g->dev_pack);
+    if (g->rg_buf) cudaFree(g->rg_buf);
     for (cudaEvent_t e : g->ev_pool) cudaEventDestroy(e);
     if (g->side) cudaStreamDestroy(g->side);
     if (g->ev_side) cudaEventDestroy(g->ev_side);
@@ -587,14 +740,9 @@ extern "C" int svb_gen_forward(svb_gen_t *g, const float *mel_dev, const float *
     return forward_impl(g, mel_dev, false, f0_dev, rand_ini_dev, noise_dev, seed, B, T, wav_dev, as_stream(stream));
 }
 
-extern "C" int svb_gen_spec2wav_host(svb_gen_t *g, const float *mel_host, const float *f0_host, uint64_t seed, int32_t B,
-                                     int32_t T, float *wav_host, void *stream) {
-    SVB_CHECK(g && g->finalized, SVB_ERR_STATE, "spec2wav: generator not finalized");
-    SVB_CHECK(mel_host && wav_host && B > 0 && T > 0, SVB_ERR_INVALID, "spec2wav: null buffer or empty input");
-    SVB_CUDA(cudaSetDevice(g->device));
-    cudaStream_t st = as_stream(stream);
-    const size_t n_mel = (size_t)B * T * g->cfg.n_mel, n_f0 = f0_host ? (size_t)B * T : 0;
-    const size_t n_in = n_mel + n_f0, n_out = (size_t)B * T * g->hop;
+// Host staging of the spec2wav calls: n_in floats of pinned input and its device copy, n_out floats of device output and
+// of pinned output (the D2H target, also of int16 samples).  i16: the device int16 samples of n_out floats and 4096 peaks.
+static int ensure_staging(svb_gen *g, size_t n_in, size_t n_out, bool i16) {
     if (n_in > g->pin_in_cap) {
         if (g->pin_in) cudaFreeHost(g->pin_in);
         if (g->dev_in) cudaFree(g->dev_in);
@@ -611,6 +759,24 @@ extern "C" int svb_gen_spec2wav_host(svb_gen_t *g, const float *mel_host, const 
         SVB_CUDA(cudaMalloc((void **)&g->dev_out, n_out * 4));
         g->pin_out_cap = n_out;
     }
+    if (i16 && n_out > g->i16_cap) {
+        if (g->dev_i16) cudaFree(g->dev_i16);
+        g->dev_i16 = nullptr, g->i16_cap = 0;
+        SVB_CUDA(cudaMalloc((void **)&g->dev_i16, n_out * 2 + (size_t)4096 * sizeof(unsigned)));
+        g->i16_cap = n_out;
+    }
+    return SVB_OK;
+}
+
+extern "C" int svb_gen_spec2wav_host(svb_gen_t *g, const float *mel_host, const float *f0_host, uint64_t seed, int32_t B,
+                                     int32_t T, float *wav_host, void *stream) {
+    SVB_CHECK(g && g->finalized, SVB_ERR_STATE, "spec2wav: generator not finalized");
+    SVB_CHECK(mel_host && wav_host && B > 0 && T > 0, SVB_ERR_INVALID, "spec2wav: null buffer or empty input");
+    SVB_CUDA(cudaSetDevice(g->device));
+    cudaStream_t st = as_stream(stream);
+    const size_t n_mel = (size_t)B * T * g->cfg.n_mel, n_f0 = f0_host ? (size_t)B * T : 0;
+    const size_t n_in = n_mel + n_f0, n_out = (size_t)B * T * g->hop;
+    SVB_TRY(ensure_staging(g, n_in, n_out, false));
     memcpy(g->pin_in, mel_host, n_mel * 4);
     if (f0_host) memcpy(g->pin_in + n_mel, f0_host, n_f0 * 4);
     SVB_CUDA(cudaMemcpyAsync(g->dev_in, g->pin_in, n_in * 4, cudaMemcpyHostToDevice, st));
@@ -634,22 +800,36 @@ __global__ void clip_absmax_kernel(const float *__restrict__ x, long long n, uns
     for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
     if ((threadIdx.x & 31) == 0) atomicMax(mx + b, __float_as_uint(m));      // non-negative floats order like their bit patterns
 }
-__global__ void to_int16_kernel(const float *__restrict__ x, long long n, const unsigned *__restrict__ mx, int16_t *__restrict__ y) {
+// tab (a ragged host call's table, generator.cu: ragged_table) or nullptr: clip b's len * hop samples go to sample first * hop
+// of y, back to back; the zeros past a clip (ragged forwards write them) neither move nor raise its peak
+__global__ void to_int16_kernel(const float *__restrict__ x, long long n, const unsigned *__restrict__ mx, int16_t *__restrict__ y,
+                                const int *__restrict__ tab, int hop) {
     const int b = blockIdx.y;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const long long nb = tab ? (long long)tab[b] * hop : n;
+    int16_t *yb = y + (tab ? (long long)tab[3 * gridDim.y + b] * hop : (long long)b * n);
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nb; i += (long long)gridDim.x * blockDim.x) {
         float v = x[(size_t)b * n + i];
         if (mx) v = __fdiv_rn(v, __uint_as_float(mx[b]));
         v = __fmul_rn(v, 32767.f);
-        y[(size_t)b * n + i] = (int16_t)__float2int_rz(v);
+        yb[i] = (int16_t)__float2int_rz(v);
     }
 }
-int wav_to_int16(const float *wav_dev, int B, long long n, int norm, int16_t *out_dev, unsigned *mx_dev, cudaStream_t st) {
+// the same packing for the float samples
+__global__ void pack_clips_kernel(const float *__restrict__ x, long long n, const int *__restrict__ tab, int hop, float *__restrict__ y) {
+    const int b = blockIdx.y;
+    const long long nb = (long long)tab[b] * hop;
+    float *yb = y + (long long)tab[3 * gridDim.y + b] * hop;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nb; i += (long long)gridDim.x * blockDim.x)
+        yb[i] = x[(size_t)b * n + i];
+}
+int wav_to_int16(const float *wav_dev, int B, long long n, int norm, int16_t *out_dev, unsigned *mx_dev, cudaStream_t st,
+                 const int *tab = nullptr, int hop = 1) {
     const dim3 grid((unsigned)std::min<long long>((n + 255) / 256, 132 * 4), (unsigned)B);
     if (norm) {
         SVB_CUDA(cudaMemsetAsync(mx_dev, 0, (size_t)B * sizeof(unsigned), st));
         clip_absmax_kernel<<<grid, 256, 0, st>>>(wav_dev, n, mx_dev);
     }
-    to_int16_kernel<<<grid, 256, 0, st>>>(wav_dev, n, norm ? mx_dev : nullptr, out_dev);
+    to_int16_kernel<<<grid, 256, 0, st>>>(wav_dev, n, norm ? mx_dev : nullptr, out_dev, tab, hop);
     SVB_CUDA(cudaGetLastError());
     return SVB_OK;
 }
@@ -673,28 +853,7 @@ extern "C" int svb_gen_spec2wav_host_i16(svb_gen_t *g, const float *mel_host, co
     cudaStream_t st = as_stream(stream);
     const size_t n_mel = (size_t)B * T * g->cfg.n_mel, n_f0 = f0_host ? (size_t)B * T : 0;
     const size_t n_in = n_mel + n_f0, n_out = (size_t)B * T * g->hop;
-    if (n_in > g->pin_in_cap) {
-        if (g->pin_in) cudaFreeHost(g->pin_in);
-        if (g->dev_in) cudaFree(g->dev_in);
-        g->pin_in = nullptr, g->dev_in = nullptr, g->pin_in_cap = 0;
-        SVB_CUDA(cudaMallocHost((void **)&g->pin_in, n_in * 4));
-        SVB_CUDA(cudaMalloc((void **)&g->dev_in, n_in * 4));
-        g->pin_in_cap = n_in;
-    }
-    if (n_out > g->pin_out_cap) {
-        if (g->pin_out) cudaFreeHost(g->pin_out);
-        if (g->dev_out) cudaFree(g->dev_out);
-        g->pin_out = nullptr, g->dev_out = nullptr, g->pin_out_cap = 0;
-        SVB_CUDA(cudaMallocHost((void **)&g->pin_out, n_out * 4));
-        SVB_CUDA(cudaMalloc((void **)&g->dev_out, n_out * 4));
-        g->pin_out_cap = n_out;
-    }
-    if (n_out > g->i16_cap) {
-        if (g->dev_i16) cudaFree(g->dev_i16);
-        g->dev_i16 = nullptr, g->i16_cap = 0;
-        SVB_CUDA(cudaMalloc((void **)&g->dev_i16, n_out * 2 + (size_t)4096 * sizeof(unsigned)));
-        g->i16_cap = n_out;
-    }
+    SVB_TRY(ensure_staging(g, n_in, n_out, true));
     SVB_CHECK(B <= 4096, SVB_ERR_INVALID, "spec2wav_i16: batch %d > 4096", B);
     memcpy(g->pin_in, mel_host, n_mel * 4);
     if (f0_host) memcpy(g->pin_in + n_mel, f0_host, n_f0 * 4);
@@ -753,4 +912,66 @@ extern "C" float svb_gen_last_ms(svb_gen_t *g) {
     if (cudaEventSynchronize(g->ev1) != cudaSuccess) return -1.f;
     if (cudaEventElapsedTime(&ms, g->ev0, g->ev1) != cudaSuccess) return -1.f;
     return ms;
+}
+
+extern "C" int svb_gen_forward_ragged(svb_gen_t *g, const float *mel_dev, const float *f0_dev, const float *rand_ini_dev,
+                                      const float *noise_dev, uint64_t seed, int32_t B, int32_t T_max, const int32_t *lengths_host,
+                                      float *wav_dev, void *stream) {
+    SVB_TRY(check_lengths(g, B, T_max, lengths_host));
+    return forward_impl(g, mel_dev, false, f0_dev, rand_ini_dev, noise_dev, seed, B, T_max, wav_dev, as_stream(stream), lengths_host);
+}
+
+// the ragged host calls: [mel | f0 | ragged table] in one H2D copy, one forward over [B, T_max], the clips packed back to back
+// on the device (as floats, or converted to int16), one D2H copy
+static int spec2wav_ragged_host(svb_gen *g, const float *mel_host, const float *f0_host, uint64_t seed, int B, const int32_t *len,
+                                bool i16, int norm, void *wav_host, void *stream) {
+    SVB_CHECK(mel_host && wav_host, SVB_ERR_INVALID, "spec2wav_ragged: null buffer");
+    int T = 0;
+    size_t frames = 0;
+    for (int b = 0; b < B && len; ++b) T = std::max(T, (int)len[b]), frames += len[b] > 0 ? len[b] : 0;
+    SVB_TRY(check_lengths(g, B, std::max(T, 1), len));
+    SVB_CHECK(B <= 4096, SVB_ERR_INVALID, "spec2wav_ragged: batch %d > 4096", B);
+    SVB_CUDA(cudaSetDevice(g->device));
+    cudaStream_t st = as_stream(stream);
+    const size_t n_mel = frames * g->cfg.n_mel, n_f0 = f0_host ? frames : 0, n_tab = 4 * (size_t)B;
+    const size_t n_in = n_mel + n_f0 + n_tab, n_pad = (size_t)B * T * g->hop, n_out = frames * g->hop;
+    SVB_TRY(ensure_staging(g, n_in, n_pad, i16));
+    if (!i16 && n_out > g->pack_cap) {
+        if (g->dev_pack) cudaFree(g->dev_pack);
+        g->dev_pack = nullptr, g->pack_cap = 0;
+        SVB_CUDA(cudaMalloc((void **)&g->dev_pack, n_out * 4));
+        g->pack_cap = n_out;
+    }
+    memcpy(g->pin_in, mel_host, n_mel * 4);
+    if (f0_host) memcpy(g->pin_in + n_mel, f0_host, n_f0 * 4);
+    int *tab = reinterpret_cast<int *>(g->pin_in + n_mel + n_f0);
+    ragged_table(g, B, T, len, tab);
+    SVB_CUDA(cudaMemcpyAsync(g->dev_in, g->pin_in, n_in * 4, cudaMemcpyHostToDevice, st));
+    const int *tab_dev = reinterpret_cast<const int *>(g->dev_in + n_mel + n_f0);
+    SVB_TRY(forward_impl(g, g->dev_in, true, f0_host ? g->dev_in + n_mel : nullptr, nullptr, nullptr, seed, B, T, g->dev_out, st, len,
+                         tab_dev));
+    const long long n = (long long)T * g->hop;
+    const dim3 grid((unsigned)std::min<long long>((n + 255) / 256, 132 * 4), (unsigned)B);
+    if (i16) {
+        unsigned *mx = reinterpret_cast<unsigned *>(reinterpret_cast<char *>(g->dev_i16) + (g->i16_cap * 2 + 3) / 4 * 4);
+        SVB_TRY(wav_to_int16(g->dev_out, B, n, norm, g->dev_i16, mx, st, tab_dev, g->hop));
+        SVB_CUDA(cudaMemcpyAsync(g->pin_out, g->dev_i16, n_out * 2, cudaMemcpyDeviceToHost, st));
+    } else {
+        pack_clips_kernel<<<grid, 256, 0, st>>>(g->dev_out, n, tab_dev, g->hop, g->dev_pack);
+        SVB_CUDA(cudaGetLastError());
+        SVB_CUDA(cudaMemcpyAsync(g->pin_out, g->dev_pack, n_out * 4, cudaMemcpyDeviceToHost, st));
+    }
+    SVB_CUDA(cudaStreamSynchronize(st));
+    memcpy(wav_host, g->pin_out, n_out * (i16 ? 2 : 4));
+    return SVB_OK;
+}
+
+extern "C" int svb_gen_spec2wav_ragged_host(svb_gen_t *g, const float *mel_host, const float *f0_host, uint64_t seed, int32_t B,
+                                            const int32_t *lengths_host, float *wav_host, void *stream) {
+    return spec2wav_ragged_host(g, mel_host, f0_host, seed, B, lengths_host, false, 0, wav_host, stream);
+}
+
+extern "C" int svb_gen_spec2wav_ragged_host_i16(svb_gen_t *g, const float *mel_host, const float *f0_host, uint64_t seed, int32_t B,
+                                                const int32_t *lengths_host, int32_t norm, int16_t *wav_host, void *stream) {
+    return spec2wav_ragged_host(g, mel_host, f0_host, seed, B, lengths_host, true, norm, wav_host, stream);
 }

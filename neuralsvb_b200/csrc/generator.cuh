@@ -46,6 +46,8 @@ struct Tap {
 // byte offsets into the workspace of one forward (in training mode this is also the tape of the backward)
 struct Buffers {
     size_t mel = 0, pre = 0, har = 0, nsf = 0, sines = 0, wav = 0;
+    size_t f0 = 0;                                           // [B][T] f0 of a ragged host call (clips unpacked)
+    std::vector<char> fused;                                 // per stage: its ResBlock steps run fused (no A buffers)
     std::vector<size_t> X, S;
     std::vector<std::vector<std::vector<size_t>>> A, R;      // [stage][ResBlock chain][dilation]
 };
@@ -115,9 +117,23 @@ struct svb_gen {
     std::vector<void *> job_allocs;
     bool dev_dirty = false;
 
+    // Ragged batches (svb_gen_forward_ragged).  rg_len: frames per clip of the current forward (empty: every clip has T);
+    // rg_dev: its device copy [len | zero from | zero to | first frame] (4 B ints).  Rows at or past a clip's end must be zero
+    // in every activation buffer (the conv's zero padding), and kernels never write them, but an earlier, longer call may
+    // have: ws_live[b] = the frames of clip b's rows that may be nonzero since the last full memset, and a ragged forward
+    // first zeroes each clip's rows between its length and ws_live (zero_tails in generator.cu).
+    std::vector<int> rg_len, ws_live, wl_len;   // wl_len: the lengths the cached work lists were built for
+    std::vector<char> ws_fused;                 // per stage: the fused layout the workspace was zeroed for
+    const int *rg_dev = nullptr;                // the current forward's copy (in rg_buf or in the host call's staging)
+    int *rg_buf = nullptr;
+    size_t rg_cap = 0;
+    int cur_T = 0;                              // frames of the current forward (T, or T_max of a ragged one)
+
     // host staging (spec2wav_host)
     float *pin_in = nullptr, *pin_out = nullptr, *dev_in = nullptr, *dev_out = nullptr;
     size_t pin_in_cap = 0, pin_out_cap = 0;
+    float *dev_pack = nullptr;      // the clips of a ragged host call back to back (svb_gen_spec2wav_ragged_host)
+    size_t pack_cap = 0;
     int16_t *dev_i16 = nullptr;      // int16 samples + per-clip peak (svb_gen_spec2wav_host_i16)
     size_t i16_cap = 0;
 

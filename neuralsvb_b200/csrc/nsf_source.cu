@@ -51,6 +51,8 @@ struct NsfDims {
     int T;              // F * U samples
     int nchunk;         // ceil(T / 32)
     float sr;
+    const int *len;     // frames of each clip (ragged batches) or nullptr: F
+    __device__ int frames(int b) const { return len ? len[b] : F; }
 };
 
 // initial phase: rand_ini[b][k] (k = 0 forced to 0, :54) or Philox uniform
@@ -76,16 +78,17 @@ __global__ void nsf_frame_prefix_kernel(NsfDims d, const float *__restrict__ f0,
     const float rad0 = rad_of(f0b[0], k, d.sr);
     const float r0p = rad0 + rand_ini_of(rand_ini, seed, b, k);   // fp32 add (:56)
     double carry = (double)r0p - (double)rad0;
-    for (int f0i = 0; f0i < d.F; f0i += 32) {
+    const int Fb = d.frames(b);
+    for (int f0i = 0; f0i < Fb; f0i += 32) {
         const int f = f0i + lane;
-        double v = (f < d.F) ? (double)d.U * (double)rad_of(f0b[f], k, d.sr) : 0.0;
+        double v = (f < Fb) ? (double)d.U * (double)rad_of(f0b[f], k, d.sr) : 0.0;
         double incl = v;
 #pragma unroll
         for (int o = 1; o < 32; o <<= 1) {
             const double n = __shfl_up_sync(0xffffffffu, incl, o);
             if (lane >= o) incl += n;
         }
-        if (f < d.F) out[f] = carry + (incl - v);
+        if (f < Fb) out[f] = carry + (incl - v);
         carry += __shfl_sync(0xffffffffu, incl, 31);
     }
 }
@@ -116,7 +119,7 @@ __global__ void nsf_chunk_sum_kernel(NsfDims d, const float *__restrict__ f0, co
     const float *f0b = f0 + (size_t)b * d.F;
     const float r0p = rad_of(f0b[0], k, d.sr) + rand_ini_of(rand_ini, seed, b, k);
     const int t = chunk * 32 + lane;
-    double v = (t < d.T) ? nsf_v(d, f0b, base1 + (size_t)bk * d.F, k, t, r0p) : 0.0;
+    double v = (t < d.frames(b) * d.U) ? nsf_v(d, f0b, base1 + (size_t)bk * d.F, k, t, r0p) : 0.0;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     if (lane == 0) csum[wid] = v;
@@ -153,7 +156,7 @@ __global__ void nsf_synth_kernel(NsfDims d, const float *__restrict__ f0, const 
     const int chunk = (int)(wid % d.nchunk), b = (int)(wid / d.nchunk);
     const float *f0b = f0 + (size_t)b * d.F;
     const int t = chunk * 32 + lane;
-    const bool valid = t < d.T;
+    const bool valid = t < d.frames(b) * d.U;                                 // this clip's samples; har is 0 after them
     const float f0t = valid ? f0b[t / d.U] : 0.f;
     const float uv = f0t > 0.f ? 1.f : 0.f;                                   // _f02uv (:38-42), threshold 0
     const float noise_amp = uv * 0.003f + (1.f - uv) * 0.1f / 3.f;            // (:131)
@@ -193,6 +196,7 @@ __global__ void nsf_synth_kernel(NsfDims d, const float *__restrict__ f0, const 
         if (sines && valid) sines[((size_t)b * d.T + t) * kH + k] = x;         // kept for the l_linear gradient (training)
     }
     if (valid) har[(size_t)b * d.T + t] = tanhf(merged);                       // l_tanh (:394)
+    else if (t < d.T) har[(size_t)b * d.T + t] = 0.f;
 }
 
 size_t nsf_workspace_bytes(int B, int F, int U) {
@@ -202,9 +206,9 @@ size_t nsf_workspace_bytes(int B, int F, int U) {
 
 int launch_nsf_source(const float *f0, const float *rand_ini, const float *noise, uint64_t seed, int B, int F, int U,
                       float sr, const float *lin_w_dev, const float *lin_b_dev, void *workspace, float *har, float *sines,
-                      cudaStream_t st, int *launches) {
+                      cudaStream_t st, int *launches, const int *len) {
     NsfDims d;
-    d.B = B, d.F = F, d.U = U, d.T = F * U, d.nchunk = (d.T + 31) / 32, d.sr = sr;
+    d.B = B, d.F = F, d.U = U, d.T = F * U, d.nchunk = (d.T + 31) / 32, d.sr = sr, d.len = len;
     double *base1 = reinterpret_cast<double *>(workspace);
     double *csum = base1 + (size_t)B * kH * F;
     const int tpb = 128;

@@ -174,10 +174,14 @@ class HifiGanGenerator(nn.Module):
         self._drop_handle()
         return r
 
-    def forward(self, x, f0=None, rand_ini=None, noise=None, seed=None):
+    def forward(self, x, f0=None, rand_ini=None, noise=None, seed=None, lengths=None):
         """x [B, n_mel, T] fp32 on a CUDA device, f0 [B, T] Hz or None -> [B, 1, T*hop].
         ``rand_ini`` [B,9] / ``noise`` [B,T*hop,9] inject the NSF source's random draws
         (parity testing); otherwise they are drawn in-kernel from ``seed``.
+
+        ``lengths`` (host sequence of B ints, 1 <= lengths[b] <= T): a ragged batch, inference only.  Clip b is vocoded as
+        if it were run alone on its first lengths[b] frames (svb_gen_forward_ragged); its frames past that are never read and
+        its samples from lengths[b] * hop on are 0.
 
         In ``train()`` mode with grad enabled the result carries a grad_fn: ``backward`` runs
         ``svb_gen_backward`` (native data / weight gradients) and hands every parameter its gradient
@@ -186,19 +190,28 @@ class HifiGanGenerator(nn.Module):
             raise RuntimeError('HifiGanGenerator.forward needs CUDA tensors: there is no CPU fallback '
                                '(the reference CPU path lives in the oracle, for tests only)')
         train = self.training and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())
+        if lengths is not None and train:
+            raise RuntimeError('HifiGanGenerator.forward: lengths (ragged batches) are inference only; '
+                               'call it under torch.no_grad() or in eval()')
         if seed is None:
             self.seed += 1
             seed = self.seed
+        if lengths is not None:
+            return self._run_forward(x, f0, rand_ini, noise, seed, train=False, lengths=lengths)
         if train:
             entries = self._param_entries()
             return _GenTrainFn.apply(self, x, f0, rand_ini, noise, seed, *[p for e in entries for p in e[2]])
         return self._run_forward(x, f0, rand_ini, noise, seed, train=False)
 
-    def _run_forward(self, x, f0, rand_ini, noise, seed, train):
+    def _run_forward(self, x, f0, rand_ini, noise, seed, train, lengths=None):
         lib = _native.lib()
+        B, C, T = x.shape
+        if lengths is not None:
+            lengths = np.ascontiguousarray([int(v) for v in lengths], dtype=np.int32)
+            if lengths.shape != (B,) or (lengths < 1).any() or (lengths > T).any():
+                raise ValueError(f'lengths must be {B} frame counts in [1, {T}], got {lengths.tolist()}')
         g = self._ensure_handle(x.device)
         g = self._sync_weights(g, train)
-        B, C, T = x.shape
         if C != self.n_mel:
             raise ValueError(f'expected {self.n_mel} mel bins, got {C}')
         x = x.contiguous().float()
@@ -209,8 +222,13 @@ class HifiGanGenerator(nn.Module):
         nz = None if noise is None else noise.contiguous().float().to(x.device)
         with torch.cuda.device(x.device):
             st = _native.current_stream_ptr(x.device)
-            _native.check(lib.svb_gen_forward(g, _native.ptr(x), _native.ptr(f0), _native.ptr(ri), _native.ptr(nz),
-                                              ctypes.c_uint64(seed), B, T, _native.ptr(y), st), 'gen_forward')
+            if lengths is not None:
+                _native.check(lib.svb_gen_forward_ragged(g, _native.ptr(x), _native.ptr(f0), _native.ptr(ri), _native.ptr(nz),
+                                                         ctypes.c_uint64(seed), B, T, lengths.ctypes.data_as(ctypes.c_void_p),
+                                                         _native.ptr(y), st), 'gen_forward_ragged')
+            else:
+                _native.check(lib.svb_gen_forward(g, _native.ptr(x), _native.ptr(f0), _native.ptr(ri), _native.ptr(nz),
+                                                  ctypes.c_uint64(seed), B, T, _native.ptr(y), st), 'gen_forward')
         return y
 
     # ------------------------------------------------------------------ training

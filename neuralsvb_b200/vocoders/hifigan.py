@@ -121,7 +121,13 @@ class HifiGAN(BaseVocoder):
         One call = pinned staging + H2D + generator + D2H + stream sync (svb_gen_spec2wav_host).
         ``int16=True``: save_wav's sample conversion (utils/audio.py:11-16; ``norm`` = its peak normalisation) runs on
         the device and np.int16 [B, T*hop] comes back -- half the D2H bytes, nothing left for the CPU writer pool to do
-        but ``wavfile.write`` (svb_gen_spec2wav_host_i16; the denoise post-filter needs the float path)."""
+        but ``wavfile.write`` (svb_gen_spec2wav_host_i16; the denoise post-filter needs the float path).
+
+        A list of [T_b, n_mel] mels (f0s: a list of [T_b] or None) is a ragged batch: one call vocodes every clip as
+        ``spec2wav`` would vocode it alone (svb_gen_spec2wav_ragged_host), and a list of 1-D arrays of T_b*hop samples comes
+        back; ``int16`` / ``norm`` / ``vocoder_denoise_c`` act per clip."""
+        if isinstance(mels, (list, tuple)):
+            return self._spec2wav_ragged(mels, f0s, seed, int16, norm)
         mels = np.ascontiguousarray(mels, dtype=np.float32)
         B, T, C = mels.shape
         if f0s is not None:
@@ -156,6 +162,49 @@ class HifiGAN(BaseVocoder):
             from neuralsvb_b200.vocoders.vocoder_utils import denoise
             out = np.stack([denoise(o, v=hparams['vocoder_denoise_c']) for o in out])
         return out
+
+    def _spec2wav_ragged(self, mels, f0s, seed, int16, norm):
+        mels = [np.asarray(m, dtype=np.float32) for m in mels]
+        if not mels:
+            return []
+        C = mels[0].shape[1] if mels[0].ndim == 2 else -1
+        if any(m.ndim != 2 or m.shape[1] != C or m.shape[0] < 1 for m in mels):
+            raise ValueError(f'spec2wav_batch: every mel must be [T_b >= 1, {C}], got {[m.shape for m in mels]}')
+        lengths = np.array([m.shape[0] for m in mels], np.int32)
+        mel_cat = np.ascontiguousarray(np.concatenate(mels))
+        f0_cat = None
+        if f0s is not None:
+            f0s = [np.asarray(f, dtype=np.float32).reshape(-1) for f in f0s]
+            if len(f0s) != len(mels) or any(len(f) != n for f, n in zip(f0s, lengths)):
+                raise ValueError('spec2wav_batch: one f0 of T_b frames per mel')
+            f0_cat = np.ascontiguousarray(np.concatenate(f0s))
+        lib = _native.lib()
+        g = self.model.native_handle(self.device)
+        hop = int(lib.svb_gen_hop(g))
+        if int16 and hparams.get('vocoder_denoise_c', 0.0) > 0:
+            raise ValueError('int16 output and vocoder_denoise_c > 0 are exclusive (the post-filter works on floats)')
+        out = np.empty(int(lengths.sum()) * hop, np.int16 if int16 else np.float32)
+        if seed is None:
+            self.model.seed += 1
+            seed = self.model.seed
+        f0p = None if f0_cat is None else f0_cat.ctypes.data_as(ctypes.c_void_p)
+        with torch.no_grad(), torch.cuda.device(self.device):
+            with utils.Timer('hifigan', enable=hparams.get('profile_infer', False)):
+                st = _native.current_stream_ptr(self.device)
+                if int16:
+                    _native.check(lib.svb_gen_spec2wav_ragged_host_i16(
+                        g, mel_cat.ctypes.data_as(ctypes.c_void_p), f0p, ctypes.c_uint64(seed), len(mels),
+                        lengths.ctypes.data_as(ctypes.c_void_p), int(bool(norm)), out.ctypes.data_as(ctypes.c_void_p), st),
+                        'spec2wav_ragged_i16')
+                else:
+                    _native.check(lib.svb_gen_spec2wav_ragged_host(
+                        g, mel_cat.ctypes.data_as(ctypes.c_void_p), f0p, ctypes.c_uint64(seed), len(mels),
+                        lengths.ctypes.data_as(ctypes.c_void_p), out.ctypes.data_as(ctypes.c_void_p), st), 'spec2wav_ragged')
+        outs = np.split(out, np.cumsum(lengths.astype(np.int64) * hop)[:-1])
+        if not int16 and hparams.get('vocoder_denoise_c', 0.0) > 0:      # vocoders/hifigan.py:66-69, clip by clip
+            from neuralsvb_b200.vocoders.vocoder_utils import denoise
+            outs = [denoise(o, v=hparams['vocoder_denoise_c']) for o in outs]
+        return outs
 
     @staticmethod
     def wav2spec_batch(wav_fns, hp=None):
