@@ -91,20 +91,24 @@ double live_rows(const svb_gen *g, int B, int Tq) {
     return n * (Tq / g->cur_T);
 }
 
-ConvArgs resblock_args(const ConvLayer &L, const float *in, float *out, const float *res, float scale, int accumulate, int B, int Tq,
-                       int Tp, float in_slope) {
+// every generator conv's ConvArgs: the handle's epilogue and fused-CTA settings, a ragged forward's per-clip rows
+ConvArgs conv_args(const svb_gen *g, const ConvLayer &L, const float *in, int in_Tp, float *out, int out_Tp, const float *res,
+                   int B, int Tq, float in_slope, float scale = 1.f, int accumulate = 0) {
     ConvArgs a;
     a.in = in, a.w = L.w, a.bias = L.b, a.res = res, a.out = out;
-    a.B = B, a.Cin = L.Cin, a.in_Tp = Tp, a.Cout = L.Cout, a.out_Tp = Tp, a.CoutP = L.CoutP, a.Tq = Tq;
-    a.KS = L.KS, a.dil = L.dil, a.ups_u = 0, a.in_slope = in_slope, a.out_scale = scale, a.accumulate = accumulate;
+    a.B = B, a.Cin = L.Cin, a.in_Tp = in_Tp, a.Cout = L.Cout, a.out_Tp = out_Tp, a.CoutP = L.CoutP, a.Tq = Tq;
+    a.KS = L.KS, a.dil = L.dil, a.ups_u = L.ups_u, a.in_slope = in_slope, a.out_scale = scale, a.accumulate = accumulate;
+    a.epi_stream = g->epi, a.fused_ctas = g->fused_ctas;
+    set_ragged(g, a);
     return a;
 }
 
 // Inference runs every ResBlock1 step x <- x + c2(lrelu(c1(lrelu(x)))) of a C <= 64 stage as ONE launch over its chains
 // (conv_tc.cu: fused items; c1's output stays in shared memory instead of a round trip through HBM) when the fused layout
-// fits.  Training keeps two launches per step: its tape needs every c1 input in HBM.
+// fits (checked without buffers, residuals or running sums).  Training keeps two launches per step: its tape needs every
+// c1 input in HBM.
 bool stage_fused(const svb_gen *g, const Stage &s, int B, int Ti) {
-    const int nk = g->cfg.n_resblock_kernels, nd = g->cfg.n_dilations;
+    const int nk = g->cfg.n_resblock_kernels, nd = g->cfg.n_dilations, Tip = c4t_rows(Ti);
     if (!g->fuse || !g->merge || g->training || g->cfg.resblock != 1 || g->cfg.precision == SVB_PREC_FP32 || s.C > 64 ||
         nk > kTcMaxLayers)
         return false;
@@ -112,10 +116,8 @@ bool stage_fused(const svb_gen *g, const Stage &s, int B, int Ti) {
         ConvArgs a[2 * kTcMaxLayers];
         const TcWeights *w[2 * kTcMaxLayers];
         for (int j = 0; j < nk; ++j) {
-            a[j] = resblock_args(s.c1[j][m], nullptr, nullptr, nullptr, 1.f, 0, B, Ti, c4t_rows(Ti), 0.1f);
-            a[nk + j] = resblock_args(s.c2[j][m], nullptr, nullptr, nullptr, 1.f, 0, B, Ti, c4t_rows(Ti), 0.1f);
-            a[j].fused_ctas = a[nk + j].fused_ctas = g->fused_ctas;
-            set_ragged(g, a[j]), set_ragged(g, a[nk + j]);
+            a[j] = conv_args(g, s.c1[j][m], nullptr, Tip, nullptr, Tip, nullptr, B, Ti, 0.1f);
+            a[nk + j] = conv_args(g, s.c2[j][m], nullptr, Tip, nullptr, Tip, nullptr, B, Ti, 0.1f);
             w[j] = &s.c1[j][m].tc, w[nk + j] = &s.c2[j][m].tc;
         }
         if (!tc_fused_fits(nk, w, a, g->cfg.precision)) return false;
@@ -123,6 +125,24 @@ bool stage_fused(const svb_gen *g, const Stage &s, int B, int Ti) {
     return true;
 }
 
+// Else step m of the nk chains (they only share their input) runs as ONE launch per conv of the step where all have a
+// tensor-core tiling of one width and the work lists fit the item table; else (e.g. very long batches) one launch per conv.
+bool stage_merged(const svb_gen *g, const Stage &s, int B, int Ti) {
+    const int nk = g->cfg.n_resblock_kernels, n_tile = s.c1[0][0].tc.n_tile;
+    if (!g->merge || nk < 2 || nk > kTcMaxLayers || g->cfg.precision == SVB_PREC_FP32 || !s.c1[0][0].tc.ok ||
+        !tc_merge_fits(nk, B, Ti, s.C, n_tile, g->rg_len.empty() ? nullptr : g->rg_len.data(), Ti / g->cur_T))
+        return false;
+    for (int j = 0; j < nk; ++j)
+        for (int m = 0; m < g->cfg.n_dilations; ++m) {
+            const ConvLayer &c1 = s.c1[j][m], &c2 = s.c2[j][m];
+            if (!tc_supported(c1.tc, conv_args(g, c1, nullptr, 0, nullptr, 0, nullptr, B, Ti, 0.1f)) || c1.tc.n_tile != n_tile)
+                return false;
+            if (g->cfg.resblock == 1 && (!c2.tc.ok || c2.tc.n_tile != n_tile)) return false;
+        }
+    return true;
+}
+
+// the buffers of a forward over [B, T] and each stage's schedule (a fused stage lays out its buffers differently)
 Buffers plan_workspace(const svb_gen *g, int B, int T, size_t *total) {
     Plan p;
     Buffers b;
@@ -137,7 +157,7 @@ Buffers plan_workspace(const svb_gen *g, int B, int T, size_t *total) {
         b.X.push_back(p.take(n)), b.S.push_back(p.take(n));
         b.A.emplace_back(), b.R.emplace_back();
         const bool fused = stage_fused(g, s, B, Ti);
-        b.fused.push_back(fused);
+        b.sched.push_back(fused ? Schedule::Fused : stage_merged(g, s, B, Ti) ? Schedule::Merged : Schedule::PerConv);
         for (int j = 0; j < g->cfg.n_resblock_kernels; ++j) {
             // inference: one A / R buffer per chain, reused by every dilation; training: every conv input is kept (the tape).
             // Fused steps have no A, and their x ping-pongs between two R buffers: an item reads its input rows plus a halo
@@ -158,6 +178,28 @@ Buffers plan_workspace(const svb_gen *g, int B, int T, size_t *total) {
     *total = p.total;
     return b;
 }
+
+float *ws_at(const svb_gen *g, size_t off) { return reinterpret_cast<float *>(g->ws + off); }
+
+}  // namespace
+
+StepBufs svb::step_bufs(const svb_gen *g, int i, int j, int m) {
+    const Buffers &b = g->bf;
+    const int nk = g->cfg.n_resblock_kernels, nd = g->cfg.n_dilations;
+    // the result of step k; ResBlock2 never runs in place (hifigan.py:81-86): its steps ping-pong between R and A
+    auto result = [&](int k) {
+        return ws_at(g, k == nd - 1 ? b.S[i] : (g->cfg.resblock == 2 && k % 2) ? b.A[i][j][k] : b.R[i][j][k]);
+    };
+    StepBufs s;
+    s.x = m == 0 ? ws_at(g, b.X[i]) : result(m - 1);
+    s.t = g->cfg.resblock == 1 && b.sched[i] != Schedule::Fused ? ws_at(g, b.A[i][j][m]) : nullptr;
+    s.dst = result(m);
+    s.scale = m == nd - 1 ? 1.f / nk : 1.f;
+    s.accumulate = m == nd - 1 && j > 0;
+    return s;
+}
+
+namespace {
 
 cudaEvent_t prof_event(svb_gen *g) {
     if (g->ev_used == g->ev_pool.size()) {
@@ -184,49 +226,41 @@ struct ProfScope {
     }
 };
 
-int run_conv(svb_gen *g, const ConvLayer &L, const float *in, int in_Tp, float *out, int out_Tp, const float *res,
-             int B, int Tq, float in_slope, float scale, int accumulate, cudaStream_t st) {
-    const double rows = live_rows(g, B, Tq);
-    g->last_launches += 1;
-    g->last_flops += 2.0 * L.macs_per_row * rows;
-    const bool tc = g->cfg.precision != SVB_PREC_FP32 && L.tc.ok;
-    const double rows_out = rows * (L.ups_u > 0 ? L.ups_u : 1);
-    // layer-streaming bytes (SURVEY 8(d)): input once, output once, residual / accumulated sum once more each
-    const double bytes = 4.0 * (rows * L.Cin + rows_out * L.Cout * (1 + (res ? 1 : 0) + (accumulate ? 1 : 0)));
-    ProfScope ps(g, st, tc ? (L.ups_u ? "conv1d_c4_tc (upsampler)" : "conv1d_c4_tc (resblock)") : "conv1d_c4_ffma", bytes,
-                 2.0 * L.macs_per_row * rows);
-    ConvArgs a;
-    a.in = in, a.w = L.w, a.bias = L.b, a.res = res, a.out = out;
-    a.B = B, a.Cin = L.Cin, a.in_Tp = in_Tp, a.Cout = L.Cout, a.out_Tp = out_Tp, a.CoutP = L.CoutP, a.Tq = Tq;
-    a.KS = L.KS, a.dil = L.dil, a.ups_u = L.ups_u, a.in_slope = in_slope, a.out_scale = scale, a.accumulate = accumulate;
-    a.epi_stream = g->epi;
-    set_ragged(g, a);
-    if (g->cfg.precision != SVB_PREC_FP32 && tc_supported(L.tc, a)) return launch_conv_tc(L.tc, a, g->cfg.precision, st);
-    return launch_conv_ffma(a, st);
-}
-
-// One merged launch over the nk layers `Ls` (same shape class): layer j reads in[j], writes out[j], adds res[j].
-// chain_ordered: later layers accumulate into the output of earlier ones (the ResBlock sum), see TcWorkList.
-// fused: the 2 nk entries are the c1 layers of nk chains, then their c2 layers (conv_tc.cuh: tc_worklist_build); the launch
-// is profiled with the bytes and FLOPs of the 2 nk convolutions it replaces, so the byte model stays the same across paths.
-int run_conv_multi(svb_gen *g, int stage, int nk, const ConvLayer *const *Ls, const float *const *in, float *const *out,
-                   const float *const *res, const float *scale, const int *accumulate, bool chain_ordered, int B, int Tq, int Tp,
-                   float in_slope, cudaStream_t st, bool fused = false) {
-    ConvArgs a[2 * kTcMaxLayers];
-    const TcWeights *w[2 * kTcMaxLayers];
-    double bytes = 0, flops = 0;
-    const double rows = live_rows(g, B, Tq);
-    for (int j = 0; j < (fused ? 2 * nk : nk); ++j) {
+// Counts one launch over the convs Ls[j] on a[j], j < n; returns its FLOPs and in *bytes its layer-streaming bytes (SURVEY
+// 8(d)): input once, output once, residual / running sum once more each.  Fused launches count both convs of each chain.
+double count_launch(svb_gen *g, int n, const ConvLayer *const *Ls, const ConvArgs *a, double *bytes) {
+    double flops = 0;
+    *bytes = 0;
+    for (int j = 0; j < n; ++j) {
         const ConvLayer &L = *Ls[j];
-        a[j] = resblock_args(L, in[j], out[j], res[j], scale[j], accumulate[j], B, Tq, Tp, in_slope);
-        a[j].epi_stream = g->epi, a[j].fused_ctas = g->fused_ctas;
-        set_ragged(g, a[j]);
-        w[j] = &L.tc;
-        bytes += 4.0 * (rows * L.Cin + rows * L.Cout * (1 + (res[j] ? 1 : 0) + (accumulate[j] ? 1 : 0)));
+        const double rows = live_rows(g, a[j].B, a[j].Tq), rows_out = rows * (L.ups_u > 0 ? L.ups_u : 1);
+        *bytes += 4.0 * (rows * L.Cin + rows_out * L.Cout * (1 + (a[j].res ? 1 : 0) + (a[j].accumulate ? 1 : 0)));
         flops += 2.0 * L.macs_per_row * rows;
     }
     g->last_launches += 1;
     g->last_flops += flops;
+    return flops;
+}
+
+int run_conv(svb_gen *g, const ConvLayer &L, const ConvArgs &a, cudaStream_t st) {
+    const ConvLayer *Ls = &L;
+    double bytes;
+    const double flops = count_launch(g, 1, &Ls, &a, &bytes);
+    const bool tc = g->cfg.precision != SVB_PREC_FP32 && L.tc.ok;
+    ProfScope ps(g, st, tc ? (L.ups_u ? "conv1d_c4_tc (upsampler)" : "conv1d_c4_tc (resblock)") : "conv1d_c4_ffma", bytes, flops);
+    if (g->cfg.precision != SVB_PREC_FP32 && tc_supported(L.tc, a)) return launch_conv_tc(L.tc, a, g->cfg.precision, st);
+    return launch_conv_ffma(a, st);
+}
+
+// One merged launch over the nk layers Ls[j] on a[j] (same shape class).
+// chain_ordered: later layers accumulate into the output of earlier ones (the ResBlock sum), see TcWorkList.
+// fused: the 2 nk entries are the c1 layers of nk chains, then their c2 layers (conv_tc.cuh: tc_worklist_build).
+int run_conv_multi(svb_gen *g, int stage, int nk, const ConvLayer *const *Ls, const ConvArgs *a, bool chain_ordered,
+                   cudaStream_t st, bool fused = false) {
+    const TcWeights *w[2 * kTcMaxLayers];
+    for (int j = 0; j < (fused ? 2 * nk : nk); ++j) w[j] = &Ls[j]->tc;
+    double bytes;
+    const double flops = count_launch(g, fused ? 2 * nk : nk, Ls, a, &bytes);
     ProfScope ps(g, st, "conv1d_c4_tc (resblock)", bytes, flops);
     // the list depends on the plan (MT) of this layer set: try the cached one, rebuild on a plan mismatch
     for (int attempt = 0; attempt < 2; ++attempt) {
@@ -292,20 +326,11 @@ __global__ void unpack_f0_kernel(const float *__restrict__ cat, const int *__res
     if (t < T) out[(size_t)b * T + t] = t < tab[b] ? cat[tab[3 * B + b] + t] : 0.f;
 }
 
-// ragged: lens = frames per clip (host), nullptr for a uniform batch.  packed_tab = nullptr: mel [B][n_mel][T] / f0 [B][T] as
-// svb_gen_forward takes them, and the ragged table is built and uploaded here; else the host call's device copy of
-// ragged_table, and mel / f0 hold the clips back to back (mel frame-major).
-int forward_impl(svb_gen *g, const float *mel, bool mel_frame_major, const float *f0, const float *rand_ini,
-                 const float *noise, uint64_t seed, int B, int T, float *wav, cudaStream_t st, const int *lens = nullptr,
-                 const int *packed_tab = nullptr) {
-    SVB_CHECK(g && g->finalized, SVB_ERR_STATE, "generator: forward before finalize");
-    SVB_CHECK(!g->dirty, SVB_ERR_STATE, "generator: weights were set after finalize; call svb_gen_update_weights first");
-    SVB_CHECK(mel && wav && B > 0 && T > 0, SVB_ERR_INVALID, "generator: null buffer or empty batch (B %d T %d)", B, T);
-    SVB_CHECK(!f0 || g->cfg.use_pitch_embed, SVB_ERR_INVALID, "generator: f0 given but use_pitch_embed is off");
-    SVB_CHECK((rand_ini == nullptr) == (noise == nullptr), SVB_ERR_INVALID,
-              "generator: rand_ini and noise must be given together");
-    if (lens) SVB_TRY(check_lengths(g, B, T, lens));
-    SVB_CUDA(cudaSetDevice(g->device));
+// ---- the forward, phase by phase as HifiGanGenerator.forward (hifigan.py:144-169)
+
+// Before the first kernel: the ragged table (lens, packed_tab: see forward_impl), the workspace and the stages' schedules,
+// the work-list cache, the zero padding, and the counters of the last forward.
+int prepare(svb_gen *g, int B, int T, const int *lens, const int *packed_tab, cudaStream_t st) {
     const bool ragged = lens != nullptr;
     std::vector<int> tab;
     g->cur_T = T;
@@ -341,13 +366,16 @@ int forward_impl(svb_gen *g, const float *mel, bool mel_frame_major, const float
         g->worklists.clear();
         g->wl_len = g->rg_len;
     }
-    // new layout (shape, mode, or which stages run fused: their buffers move): rebuild the zero padding of every buffer
-    if (g->ws_B != B || g->ws_T != T || g->ws_training != g->training || g->ws_fused != bf.fused) {
+    // new layout (shape, mode, or which stages run fused: their buffers move): rebuild the zero padding of every buffer.
+    // A stage that switches between merged and per-conv launches keeps its buffers.
+    std::vector<char> fused;
+    for (Schedule s : bf.sched) fused.push_back(s == Schedule::Fused);
+    if (g->ws_B != B || g->ws_T != T || g->ws_training != g->training || g->ws_fused != fused) {
         SVB_CUDA(cudaMemsetAsync(g->ws, 0, need, st));
-        g->ws_B = B, g->ws_T = T, g->ws_training = g->training, g->ws_fused = bf.fused;
+        g->ws_B = B, g->ws_T = T, g->ws_training = g->training, g->ws_fused = fused;
         g->ws_live.assign(B, 0);
     }
-    g->bf = bf, g->last_T = T, g->last_nsf = f0 != nullptr;
+    g->bf = bf, g->last_T = T;
     g->last_launches = 0, g->last_flops = 0, g->last_B = B;
     g->taps.clear();
     g->recs.clear(), g->ev_used = 0;
@@ -355,71 +383,67 @@ int forward_impl(svb_gen *g, const float *mel, bool mel_frame_major, const float
     // Zeroing policy of ragged calls: every row at or past a clip's length must be zero in every activation buffer (the halo
     // of the next conv reads it as the clip's zero padding), and no kernel writes such rows.  A full memset happens only when
     // the layout changes; otherwise only the rows an earlier call left live past this call's lengths (ws_live) are zeroed,
-    // in one launch over all buffers.  Uniform calls write every row below T and leave all clips live to T.
-    if (ragged) {
-        bool any = false;
-        for (int b = 0; b < B; ++b) any = any || tab[2 * B + b] > tab[B + b];
-        if (any) {
-            TailList L;
-            L.n = 0;
-            auto add = [&](size_t off, int C, int Ti) {
-                for (int i = 0; i < L.n; ++i)
-                    if (L.buf[i].off == off) return;
-                L.buf[L.n].off = off, L.buf[L.n].groups = c4t_groups(C), L.buf[L.n].Tp = c4t_rows(Ti), L.buf[L.n].mul = Ti / T;
-                ++L.n;
-            };
-            add(bf.pre, g->cfg.upsample_initial_channel, T);
-            int Ti = T;
-            for (size_t i = 0; i < g->stages.size(); ++i) {
-                Ti *= g->stages[i].u;
-                const int C = g->stages[i].C;
-                add(bf.X[i], C, Ti), add(bf.S[i], C, Ti);
-                for (auto &v : bf.A[i])
-                    for (size_t o : v) add(o, C, Ti);
-                for (auto &v : bf.R[i])
-                    for (size_t o : v) add(o, C, Ti);
-                SVB_CHECK(L.n <= kMaxTailBufs - 10, SVB_ERR_INVALID, "generator: %d activation buffers", L.n);
-            }
-            ProfScope ps(g, st, "zero tails", 0, 0);
-            zero_tails_kernel<<<dim3(32, L.n, B), 256, 0, st>>>(L, g->ws, g->rg_dev, B);
-            SVB_CUDA(cudaGetLastError());
-            g->last_launches += 1;
+    // in one launch over all buffers.
+    bool any = false;
+    for (int b = 0; b < B && ragged; ++b) any = any || tab[2 * B + b] > tab[B + b];
+    if (any) {
+        TailList L;
+        L.n = 0;
+        auto add = [&](size_t off, int C, int Ti) {
+            for (int i = 0; i < L.n; ++i)
+                if (L.buf[i].off == off) return;
+            L.buf[L.n].off = off, L.buf[L.n].groups = c4t_groups(C), L.buf[L.n].Tp = c4t_rows(Ti), L.buf[L.n].mul = Ti / T;
+            ++L.n;
+        };
+        add(bf.pre, g->cfg.upsample_initial_channel, T);
+        int Ti = T;
+        for (size_t i = 0; i < g->stages.size(); ++i) {
+            Ti *= g->stages[i].u;
+            const int C = g->stages[i].C;
+            add(bf.X[i], C, Ti), add(bf.S[i], C, Ti);
+            for (auto &v : bf.A[i])
+                for (size_t o : v) add(o, C, Ti);
+            for (auto &v : bf.R[i])
+                for (size_t o : v) add(o, C, Ti);
+            SVB_CHECK(L.n <= kMaxTailBufs - 10, SVB_ERR_INVALID, "generator: %d activation buffers", L.n);
         }
-        for (int b = 0; b < B; ++b) g->ws_live[b] = lens[b];
-    } else {
-        g->ws_live.assign(B, T);
+        ProfScope ps(g, st, "zero tails", 0, 0);
+        zero_tails_kernel<<<dim3(32, L.n, B), 256, 0, st>>>(L, g->ws, g->rg_dev, B);
+        SVB_CUDA(cudaGetLastError());
+        g->last_launches += 1;
     }
+    if (ragged) g->ws_live.assign(lens, lens + B);
+    else g->ws_live.assign(B, T);                   // uniform calls write every row below T
+    return SVB_OK;
+}
 
-    auto F = [&](size_t off) { return reinterpret_cast<float *>(g->ws + off); };
-    const int n_mel = g->cfg.n_mel, C0 = g->cfg.upsample_initial_channel;
-    const int Tp0 = c4t_rows(T);
+// mel -> G32T (and a host call's f0 unpacked); har_source = m_source(f0)   hifigan.py:145-149; x = conv_pre(x)   :151
+int front_end(svb_gen *g, const float *mel, bool mel_frame_major, const float *f0, const float *rand_ini, const float *noise,
+              uint64_t seed, int B, int T, const int *packed_tab, cudaStream_t st) {
+    const Buffers &bf = g->bf;
+    const bool ragged = !g->rg_len.empty();
+    const int n_mel = g->cfg.n_mel, Tp0 = c4t_rows(T), Tw = T * g->hop;
     {
         ProfScope ps(g, st, "mel layout", 8.0 * B * n_mel * T, 0);
-        if (ragged && mel_frame_major) SVB_TRY(launch_btc_to_c4t_ragged(mel, F(bf.mel), B, n_mel, T, Tp0, g->rg_dev,
+        if (ragged && mel_frame_major) SVB_TRY(launch_btc_to_c4t_ragged(mel, ws_at(g, bf.mel), B, n_mel, T, Tp0, g->rg_dev,
                                                                         packed_tab ? packed_tab + 3 * B : nullptr, st));
-        else if (ragged) SVB_TRY(launch_nct_to_c4t_ragged(mel, F(bf.mel), B, n_mel, T, Tp0, g->rg_dev, st));
-        else if (mel_frame_major) SVB_TRY(launch_btc_to_c4t(mel, F(bf.mel), B, n_mel, T, Tp0, st));
-        else SVB_TRY(launch_nct_to_c4t(mel, F(bf.mel), B, n_mel, T, Tp0, st));
+        else if (ragged) SVB_TRY(launch_nct_to_c4t_ragged(mel, ws_at(g, bf.mel), B, n_mel, T, Tp0, g->rg_dev, st));
+        else if (mel_frame_major) SVB_TRY(launch_btc_to_c4t(mel, ws_at(g, bf.mel), B, n_mel, T, Tp0, st));
+        else SVB_TRY(launch_nct_to_c4t(mel, ws_at(g, bf.mel), B, n_mel, T, Tp0, st));
     }
     g->last_launches += 1;
     if (f0 && packed_tab) {                         // back-to-back f0 -> [B][T]
-        unpack_f0_kernel<<<dim3((T + 255) / 256, B), 256, 0, st>>>(f0, packed_tab, B, T, F(bf.f0));
+        unpack_f0_kernel<<<dim3((T + 255) / 256, B), 256, 0, st>>>(f0, packed_tab, B, T, ws_at(g, bf.f0));
         SVB_CUDA(cudaGetLastError());
         g->last_launches += 1;
-        f0 = F(bf.f0);
+        f0 = ws_at(g, bf.f0);
     }
-    const int *len_dev = ragged ? g->rg_dev : nullptr;
-
-    const int Tw = T * g->hop;
-    float *har = nullptr;
-    bool har_on_side = false;
     if (f0) {
         // The NSF source only meets the main chain at the first noise_conv_add: run it on a side stream
         // so it overlaps conv_pre and the first upsampler.
-        har = F(bf.har);
-        har_on_side = !g->profile;
-        cudaStream_t ns = har_on_side ? g->side : st;
-        if (har_on_side) {
+        const bool side = !g->profile;
+        cudaStream_t ns = side ? g->side : st;
+        if (side) {
             SVB_CUDA(cudaEventRecord(g->ev_fork, st));
             SVB_CUDA(cudaStreamWaitEvent(ns, g->ev_fork, 0));
         }
@@ -427,135 +451,126 @@ int forward_impl(svb_gen *g, const float *mel, bool mel_frame_major, const float
         {
             ProfScope ps(g, ns, "nsf source (4 kernels)", 4.0 * B * (T + (double)Tw * (noise ? 10 : 1)), 60.0 * B * Tw * 9);
             SVB_TRY(launch_nsf_source(f0, rand_ini, noise, seed, B, T, g->hop, (float)g->cfg.audio_sample_rate, g->lin_w,
-                                      g->lin_b_dev, g->ws + bf.nsf, har, g->training ? F(bf.sines) : nullptr, ns, &l, len_dev));
+                                      g->lin_b_dev, g->ws + bf.nsf, ws_at(g, bf.har), g->training ? ws_at(g, bf.sines) : nullptr, ns,
+                                      &l, g->rg_dev));
         }
-        if (har_on_side) SVB_CUDA(cudaEventRecord(g->ev_side, ns));
+        if (side) SVB_CUDA(cudaEventRecord(g->ev_side, ns));
         g->last_launches += l;
-        g->taps["har_source"] = Tap{har, 1, Tw, 0, true};
+        g->taps["har_source"] = Tap{ws_at(g, bf.har), 1, Tw, 0, true};
     }
+    SVB_TRY(run_conv(g, g->conv_pre, conv_args(g, g->conv_pre, ws_at(g, bf.mel), Tp0, ws_at(g, bf.pre), Tp0, nullptr, B, T, 1.f), st));
+    g->taps["conv_pre"] = Tap{ws_at(g, bf.pre), g->cfg.upsample_initial_channel, T, Tp0, false};
+    return SVB_OK;
+}
 
-    SVB_TRY(run_conv(g, g->conv_pre, F(bf.mel), Tp0, F(bf.pre), Tp0, nullptr, B, T, 1.f, 1.f, 0, st));
-    g->taps["conv_pre"] = Tap{F(bf.pre), C0, T, Tp0, false};
+// xs = sum_j resblocks[i*nk + j](x) ; x = xs / nk   :158-164, on stage i's schedule (see Schedule for the loop orders)
+int resblocks(svb_gen *g, int i, int B, int Ti, cudaStream_t st) {
+    const Stage &s = g->stages[i];
+    const int nk = g->cfg.n_resblock_kernels, nd = g->cfg.n_dilations, Tip = c4t_rows(Ti);
+    const bool rb1 = g->cfg.resblock == 1;
+    const Schedule sched = g->bf.sched[i];
+    // c1 and c2 of step m of chain j (ResBlock2: c1 only, its residual is its input)
+    auto step = [&](int j, int m, ConvArgs *c1, ConvArgs *c2) {
+        const StepBufs b = step_bufs(g, i, j, m);
+        if (rb1) {                                  // ResBlock1.forward :54-61
+            *c1 = conv_args(g, s.c1[j][m], b.x, Tip, b.t, Tip, nullptr, B, Ti, 0.1f);
+            *c2 = conv_args(g, s.c2[j][m], b.t, Tip, b.dst, Tip, b.x, B, Ti, 0.1f, b.scale, b.accumulate);
+        } else {                                    // ResBlock2.forward :81-86
+            *c1 = conv_args(g, s.c1[j][m], b.x, Tip, b.dst, Tip, b.x, B, Ti, 0.1f, b.scale, b.accumulate);
+        }
+    };
+    if (sched == Schedule::PerConv) {
+        for (int j = 0; j < nk; ++j)
+            for (int m = 0; m < nd; ++m) {
+                ConvArgs c1, c2;
+                step(j, m, &c1, &c2);
+                SVB_TRY(run_conv(g, s.c1[j][m], c1, st));
+                if (rb1) SVB_TRY(run_conv(g, s.c2[j][m], c2, st));
+            }
+        return SVB_OK;
+    }
+    for (int m = 0; m < nd; ++m) {
+        const bool last = m == nd - 1;              // the chains add into S: chain-ordered work lists
+        const ConvLayer *L[2 * kTcMaxLayers];       // c1 of every chain, then c2
+        ConvArgs a[2 * kTcMaxLayers];
+        for (int j = 0; j < nk; ++j) {
+            L[j] = &s.c1[j][m], L[nk + j] = rb1 ? &s.c2[j][m] : nullptr;
+            step(j, m, &a[j], &a[nk + j]);
+        }
+        if (sched == Schedule::Fused) SVB_TRY(run_conv_multi(g, i, nk, L, a, last, st, true));
+        else if (!rb1) SVB_TRY(run_conv_multi(g, i, nk, L, a, last, st));
+        else {
+            SVB_TRY(run_conv_multi(g, i, nk, L, a, false, st));
+            SVB_TRY(run_conv_multi(g, i, nk, L + nk, a + nk, last, st));
+        }
+    }
+    return SVB_OK;
+}
 
-    const float *x_in = F(bf.pre);
-    int Tin = T, Tin_p = Tp0;
-    const int nk = g->cfg.n_resblock_kernels, nd = g->cfg.n_dilations;
-    for (size_t i = 0; i < g->stages.size(); ++i) {
-        Stage &s = g->stages[i];
-        const int Ti = Tin * s.u, Tip = c4t_rows(Ti);
-        float *X = F(bf.X[i]), *S = F(bf.S[i]);
-        // x = ups[i](leaky_relu(x, 0.1))            hifigan.py:153-154
-        SVB_TRY(run_conv(g, s.up, x_in, Tin_p, X, Tip, nullptr, B, Tin, 0.1f, 1.f, 0, st));
-        if (f0) {                                   // x = x + noise_convs[i](har_source)   :155-157
-            if (har_on_side && i == 0) SVB_CUDA(cudaStreamWaitEvent(st, g->ev_side, 0));
-            ProfScope ps(g, st, "noise_conv_add", 4.0 * B * (2.0 * Ti * s.C + Tw), 2.0 * B * (double)Ti * s.C * s.noise.K);
-            SVB_TRY(launch_noise_conv_add(X, B, s.C, Ti, Tip, har, Tw, s.noise.w, s.noise.b, s.noise.K, s.noise.stride,
-                                          s.noise.pad, st, len_dev, Ti / T, g->hop));
-            g->last_launches += 1;
-            g->last_flops += 2.0 * live_rows(g, B, Ti) * s.C * s.noise.K;
+// x = ups[i](leaky_relu(x, 0.1)) (+ noise_convs[i](har_source)), then the ResBlocks   :153-164; Tin: the input's rows
+int run_stage(svb_gen *g, int i, int B, int Tin, cudaStream_t st) {
+    const Stage &s = g->stages[i];
+    const int nk = g->cfg.n_resblock_kernels, nd = g->cfg.n_dilations, T = g->cur_T;
+    const int Ti = Tin * s.u, Tip = c4t_rows(Ti);
+    float *X = ws_at(g, g->bf.X[i]);
+    const float *x_in = ws_at(g, i == 0 ? g->bf.pre : g->bf.S[i - 1]);
+    SVB_TRY(run_conv(g, s.up, conv_args(g, s.up, x_in, c4t_rows(Tin), X, Tip, nullptr, B, Tin, 0.1f), st));
+    if (g->last_nsf) {                              // x = x + noise_convs[i](har_source)   :155-157
+        if (i == 0 && !g->profile) SVB_CUDA(cudaStreamWaitEvent(st, g->ev_side, 0));    // the NSF source's side stream
+        const int Tw = T * g->hop;
+        ProfScope ps(g, st, "noise_conv_add", 4.0 * B * (2.0 * Ti * s.C + Tw), 2.0 * B * (double)Ti * s.C * s.noise.K);
+        SVB_TRY(launch_noise_conv_add(X, B, s.C, Ti, Tip, ws_at(g, g->bf.har), Tw, s.noise.w, s.noise.b, s.noise.K, s.noise.stride,
+                                      s.noise.pad, st, g->rg_dev, Ti / T, g->hop));
+        g->last_launches += 1;
+        g->last_flops += 2.0 * live_rows(g, B, Ti) * s.C * s.noise.K;
+    }
+    g->taps["ups" + std::to_string(i)] = Tap{X, s.C, Ti, Tip, false};
+    SVB_TRY(resblocks(g, i, B, Ti, st));
+    g->taps["stage" + std::to_string(i)] = Tap{ws_at(g, g->bf.S[i]), s.C, Ti, Tip, false};
+    // The tape as taps: every leaky-relu input of the ResBlocks, x{m} (input of step m; x0 is ups{i}) and, for ResBlock1,
+    // t{m} (c1's output).  Only training keeps one buffer per step; inference reuses A / R across the steps.
+    for (int j = 0; j < nk && g->training; ++j) {
+        const std::string rb = "resblocks." + std::to_string(i * nk + j);
+        for (int m = 0; m < nd; ++m) {
+            const StepBufs b = step_bufs(g, i, j, m);
+            g->taps[rb + ".x" + std::to_string(m)] = Tap{b.x, s.C, Ti, Tip, false};
+            if (b.t) g->taps[rb + ".t" + std::to_string(m)] = Tap{b.t, s.C, Ti, Tip, false};
         }
-        g->taps["ups" + std::to_string(i)] = Tap{X, s.C, Ti, Tip, false};
-        // xs = sum_j resblocks[i*nk + j](x) ; x = xs / nk      :158-164
-        const bool fused = stage_fused(g, s, B, Ti);
-        if (fused) {
-            for (int m = 0; m < nd; ++m) {
-                const bool last = m == nd - 1;
-                const ConvLayer *L[2 * kTcMaxLayers];
-                const float *xin[2 * kTcMaxLayers], *res[2 * kTcMaxLayers];
-                float *dst[2 * kTcMaxLayers], scl[2 * kTcMaxLayers];
-                int acc[2 * kTcMaxLayers];
-                for (int j = 0; j < nk; ++j) {
-                    L[j] = &s.c1[j][m], L[nk + j] = &s.c2[j][m];
-                    xin[j] = m == 0 ? X : F(bf.R[i][j][m - 1]), xin[nk + j] = nullptr;
-                    res[j] = nullptr, res[nk + j] = xin[j];
-                    dst[j] = nullptr, dst[nk + j] = last ? S : F(bf.R[i][j][m]);
-                    scl[j] = 1.f, scl[nk + j] = last ? 1.f / nk : 1.f;
-                    acc[j] = 0, acc[nk + j] = (last && j > 0) ? 1 : 0;
-                }
-                SVB_TRY(run_conv_multi(g, (int)i, nk, L, xin, dst, res, scl, acc, last, B, Ti, Tip, 0.1f, st, true));
-            }
-        }
-        // merged schedule: step m of all nk chains in ONE persistent launch (the chains only share their input)
-        bool merged = !fused && g->merge && nk > 1 && nk <= kTcMaxLayers && g->cfg.precision != SVB_PREC_FP32 &&
-                      s.c1[0][0].tc.ok &&
-                      tc_merge_fits(nk, B, Ti, s.C, s.c1[0][0].tc.n_tile, ragged ? g->rg_len.data() : nullptr, Ti / T);
-        for (int j = 0; merged && j < nk; ++j)
-            for (int m = 0; m < nd; ++m) {
-                ConvArgs probe;
-                probe.Cin = s.C, probe.Cout = s.C, probe.CoutP = s.C, probe.KS = s.c1[j][m].KS, probe.dil = s.c1[j][m].dil, probe.ups_u = 0;
-                probe.bias = s.c1[j][m].b, probe.cin_blk = 0;
-                merged = merged && tc_supported(s.c1[j][m].tc, probe) && s.c1[j][m].tc.n_tile == s.c1[0][0].tc.n_tile;
-                if (g->cfg.resblock == 1) merged = merged && s.c2[j][m].tc.ok && s.c2[j][m].tc.n_tile == s.c1[0][0].tc.n_tile;
-            }
-        if (merged) {
-            for (int m = 0; m < nd; ++m) {
-                const bool last = m == nd - 1;
-                const ConvLayer *L1[kTcMaxLayers], *L2[kTcMaxLayers];
-                const float *xin[kTcMaxLayers], *ain[kTcMaxLayers], *none[kTcMaxLayers];
-                float *aout[kTcMaxLayers], *dst[kTcMaxLayers];
-                float one[kTcMaxLayers], scl[kTcMaxLayers];
-                int zero[kTcMaxLayers], acc[kTcMaxLayers];
-                for (int j = 0; j < nk; ++j) {
-                    L1[j] = &s.c1[j][m], none[j] = nullptr, one[j] = 1.f, zero[j] = 0;
-                    scl[j] = last ? 1.f / nk : 1.f, acc[j] = (last && j > 0) ? 1 : 0;
-                    if (g->cfg.resblock == 1) {                 // ResBlock1.forward :54-61
-                        L2[j] = &s.c2[j][m];
-                        xin[j] = m == 0 ? X : F(bf.R[i][j][m - 1]);
-                        aout[j] = F(bf.A[i][j][m]), ain[j] = aout[j];
-                        dst[j] = last ? S : F(bf.R[i][j][m]);
-                    } else {                                    // ResBlock2.forward :81-86 (never in place: ping-pong A / R)
-                        xin[j] = m == 0 ? X : (m % 2 ? F(bf.R[i][j][m - 1]) : F(bf.A[i][j][m - 1]));
-                        dst[j] = last ? S : (m % 2 ? F(bf.A[i][j][m]) : F(bf.R[i][j][m]));
-                    }
-                }
-                if (g->cfg.resblock == 1) {
-                    SVB_TRY(run_conv_multi(g, (int)i, nk, L1, xin, aout, none, one, zero, false, B, Ti, Tip, 0.1f, st));
-                    SVB_TRY(run_conv_multi(g, (int)i, nk, L2, ain, dst, xin, scl, acc, last, B, Ti, Tip, 0.1f, st));
-                } else {
-                    SVB_TRY(run_conv_multi(g, (int)i, nk, L1, xin, dst, xin, scl, acc, last, B, Ti, Tip, 0.1f, st));
-                }
-            }
-        }
-        for (int j = 0; j < nk && !merged && !fused; ++j) {
-            for (int m = 0; m < nd; ++m) {
-                float *A = F(bf.A[i][j][m]);
-                const float *xin = m == 0 ? X : F(bf.R[i][j][m - 1]);
-                const bool last = m == nd - 1;
-                float *dst = last ? S : F(bf.R[i][j][m]);
-                const float scale = last ? 1.f / nk : 1.f;
-                const int accum = (last && j > 0) ? 1 : 0;
-                if (g->cfg.resblock == 1) {         // ResBlock1.forward :54-61
-                    SVB_TRY(run_conv(g, s.c1[j][m], xin, Tip, A, Tip, nullptr, B, Ti, 0.1f, 1.f, 0, st));
-                    SVB_TRY(run_conv(g, s.c2[j][m], A, Tip, dst, Tip, xin, B, Ti, 0.1f, scale, accum, st));
-                } else {                            // ResBlock2.forward :81-86 (never in place: ping-pong A / R)
-                    const float *xin2 = m == 0 ? X : (m % 2 ? F(bf.R[i][j][m - 1]) : F(bf.A[i][j][m - 1]));
-                    float *dst2 = last ? S : (m % 2 ? F(bf.A[i][j][m]) : F(bf.R[i][j][m]));
-                    SVB_TRY(run_conv(g, s.c1[j][m], xin2, Tip, dst2, Tip, xin2, B, Ti, 0.1f, scale, accum, st));
-                }
-            }
-        }
-        g->taps["stage" + std::to_string(i)] = Tap{S, s.C, Ti, Tip, false};
-        // The tape as taps: every leaky-relu input of the ResBlocks, x{m} (input of step m; x0 is ups{i}) and, for ResBlock1,
-        // t{m} (c1's output).  Only training keeps one buffer per step; inference reuses A / R across the steps.
-        for (int j = 0; j < nk && g->training; ++j) {
-            const std::string rb = "resblocks." + std::to_string(i * nk + j);
-            for (int m = 0; m < nd; ++m) {
-                const size_t xm = m == 0 ? bf.X[i] : (g->cfg.resblock == 1 || m % 2) ? bf.R[i][j][m - 1] : bf.A[i][j][m - 1];
-                g->taps[rb + ".x" + std::to_string(m)] = Tap{F(xm), s.C, Ti, Tip, false};
-                if (g->cfg.resblock == 1) g->taps[rb + ".t" + std::to_string(m)] = Tap{F(bf.A[i][j][m]), s.C, Ti, Tip, false};
-            }
-        }
-        x_in = S, Tin = Ti, Tin_p = Tip;
+    }
+    return SVB_OK;
+}
+
+// ragged: lens = frames per clip (host), nullptr for a uniform batch.  packed_tab = nullptr: mel [B][n_mel][T] / f0 [B][T] as
+// svb_gen_forward takes them, and the ragged table is built and uploaded here; else the host call's device copy of
+// ragged_table, and mel / f0 hold the clips back to back (mel frame-major).
+int forward_impl(svb_gen *g, const float *mel, bool mel_frame_major, const float *f0, const float *rand_ini,
+                 const float *noise, uint64_t seed, int B, int T, float *wav, cudaStream_t st, const int *lens = nullptr,
+                 const int *packed_tab = nullptr) {
+    SVB_CHECK(g && g->finalized, SVB_ERR_STATE, "generator: forward before finalize");
+    SVB_CHECK(!g->dirty, SVB_ERR_STATE, "generator: weights were set after finalize; call svb_gen_update_weights first");
+    SVB_CHECK(mel && wav && B > 0 && T > 0, SVB_ERR_INVALID, "generator: null buffer or empty batch (B %d T %d)", B, T);
+    SVB_CHECK(!f0 || g->cfg.use_pitch_embed, SVB_ERR_INVALID, "generator: f0 given but use_pitch_embed is off");
+    SVB_CHECK((rand_ini == nullptr) == (noise == nullptr), SVB_ERR_INVALID,
+              "generator: rand_ini and noise must be given together");
+    if (lens) SVB_TRY(check_lengths(g, B, T, lens));
+    SVB_CUDA(cudaSetDevice(g->device));
+    SVB_TRY(prepare(g, B, T, lens, packed_tab, st));
+    g->last_nsf = f0 != nullptr;
+    SVB_TRY(front_end(g, mel, mel_frame_major, f0, rand_ini, noise, seed, B, T, packed_tab, st));
+    int Ti = T;
+    for (int i = 0; i < (int)g->stages.size(); ++i) {
+        SVB_TRY(run_stage(g, i, B, Ti, st));
+        Ti *= g->stages[i].u;
     }
     // x = tanh(conv_post(leaky_relu(x)))   default slope 0.01   :165-167
     {
-        ProfScope ps(g, st, "conv_post_tanh", 4.0 * B * Tin * (g->post_C + 1.0), 2.0 * B * (double)Tin * g->post_C * g->post_K);
-        SVB_TRY(launch_conv_post_tanh(x_in, B, g->post_C, Tin, Tin_p, g->post_wq, g->post_b_dev, g->post_K, 0.01f, wav, st,
-                                      len_dev, Tin / T));
+        ProfScope ps(g, st, "conv_post_tanh", 4.0 * B * Ti * (g->post_C + 1.0), 2.0 * B * (double)Ti * g->post_C * g->post_K);
+        SVB_TRY(launch_conv_post_tanh(ws_at(g, g->bf.S.back()), B, g->post_C, Ti, c4t_rows(Ti), g->post_wq, g->post_b_dev,
+                                      g->post_K, 0.01f, wav, st, g->rg_dev, Ti / T));
     }
     g->last_launches += 1;
-    g->last_flops += 2.0 * live_rows(g, B, Tin) * g->post_C * g->post_K;
-    if (g->training) SVB_CUDA(cudaMemcpyAsync(F(bf.wav), wav, (size_t)B * Tw * 4, cudaMemcpyDeviceToDevice, st));
+    g->last_flops += 2.0 * live_rows(g, B, Ti) * g->post_C * g->post_K;
+    if (g->training) SVB_CUDA(cudaMemcpyAsync(ws_at(g, g->bf.wav), wav, (size_t)B * T * g->hop * 4, cudaMemcpyDeviceToDevice, st));
     if (g->timing) SVB_CUDA(cudaEventRecord(g->ev1, st));
     return SVB_OK;
 }
@@ -768,26 +783,6 @@ static int ensure_staging(svb_gen *g, size_t n_in, size_t n_out, bool i16) {
     return SVB_OK;
 }
 
-extern "C" int svb_gen_spec2wav_host(svb_gen_t *g, const float *mel_host, const float *f0_host, uint64_t seed, int32_t B,
-                                     int32_t T, float *wav_host, void *stream) {
-    SVB_CHECK(g && g->finalized, SVB_ERR_STATE, "spec2wav: generator not finalized");
-    SVB_CHECK(mel_host && wav_host && B > 0 && T > 0, SVB_ERR_INVALID, "spec2wav: null buffer or empty input");
-    SVB_CUDA(cudaSetDevice(g->device));
-    cudaStream_t st = as_stream(stream);
-    const size_t n_mel = (size_t)B * T * g->cfg.n_mel, n_f0 = f0_host ? (size_t)B * T : 0;
-    const size_t n_in = n_mel + n_f0, n_out = (size_t)B * T * g->hop;
-    SVB_TRY(ensure_staging(g, n_in, n_out, false));
-    memcpy(g->pin_in, mel_host, n_mel * 4);
-    if (f0_host) memcpy(g->pin_in + n_mel, f0_host, n_f0 * 4);
-    SVB_CUDA(cudaMemcpyAsync(g->dev_in, g->pin_in, n_in * 4, cudaMemcpyHostToDevice, st));
-    SVB_TRY(forward_impl(g, g->dev_in, true, f0_host ? g->dev_in + n_mel : nullptr, nullptr, nullptr, seed, B, T,
-                         g->dev_out, st));
-    SVB_CUDA(cudaMemcpyAsync(g->pin_out, g->dev_out, n_out * 4, cudaMemcpyDeviceToHost, st));
-    SVB_CUDA(cudaStreamSynchronize(st));
-    memcpy(wav_host, g->pin_out, n_out * 4);
-    return SVB_OK;
-}
-
 // ---- save_wav's sample conversion on the device (utils/audio.py:11-16): [norm: wav / max|wav| per clip,] wav * 32767,
 // numpy's float -> int16 cast (truncation toward zero).  Done before the D2H copy, the transfer is 2 bytes per sample.
 namespace {
@@ -845,28 +840,75 @@ extern "C" int svb_wav_to_int16(const float *wav_dev, int32_t B, int64_t n, int3
     return rc;
 }
 
-extern "C" int svb_gen_spec2wav_host_i16(svb_gen_t *g, const float *mel_host, const float *f0_host, uint64_t seed, int32_t B,
-                                         int32_t T, int32_t norm, int16_t *wav_host, void *stream) {
-    SVB_CHECK(g && g->finalized, SVB_ERR_STATE, "spec2wav_i16: generator not finalized");
-    SVB_CHECK(mel_host && wav_host && B > 0 && T > 0, SVB_ERR_INVALID, "spec2wav_i16: null buffer or empty input");
+// The host calls: [mel | f0 (| ragged table)] in one H2D copy, one forward, [int16 conversion,] one D2H copy.  len: frames
+// per clip (T: the longest), clips packed back to back; nullptr: B clips of T frames, straight from the forward's output.
+static int spec2wav_host(svb_gen *g, const float *mel_host, const float *f0_host, uint64_t seed, int B, int T, const int32_t *len,
+                         bool i16, int norm, void *wav_host, void *stream) {
+    size_t frames = (size_t)B * T;
+    if (len) {
+        T = 0, frames = 0;
+        for (int b = 0; b < B; ++b) T = std::max(T, (int)len[b]), frames += len[b] > 0 ? len[b] : 0;
+        SVB_TRY(check_lengths(g, B, std::max(T, 1), len));
+    }
+    SVB_CHECK(g && g->finalized, SVB_ERR_STATE, "spec2wav: generator not finalized");
+    SVB_CHECK(mel_host && wav_host && B > 0 && T > 0, SVB_ERR_INVALID, "spec2wav: null buffer or empty input");
+    SVB_CHECK(B <= 4096 || !(i16 || len), SVB_ERR_INVALID, "spec2wav: batch %d > 4096", B);
     SVB_CUDA(cudaSetDevice(g->device));
     cudaStream_t st = as_stream(stream);
-    const size_t n_mel = (size_t)B * T * g->cfg.n_mel, n_f0 = f0_host ? (size_t)B * T : 0;
-    const size_t n_in = n_mel + n_f0, n_out = (size_t)B * T * g->hop;
-    SVB_TRY(ensure_staging(g, n_in, n_out, true));
-    SVB_CHECK(B <= 4096, SVB_ERR_INVALID, "spec2wav_i16: batch %d > 4096", B);
+    const size_t n_mel = frames * g->cfg.n_mel, n_f0 = f0_host ? frames : 0, n_tab = len ? 4 * (size_t)B : 0;
+    const size_t n_in = n_mel + n_f0 + n_tab, n_out = frames * g->hop;
+    SVB_TRY(ensure_staging(g, n_in, (size_t)B * T * g->hop, i16));
+    if (len && !i16 && n_out > g->pack_cap) {
+        if (g->dev_pack) cudaFree(g->dev_pack);
+        g->dev_pack = nullptr, g->pack_cap = 0;
+        SVB_CUDA(cudaMalloc((void **)&g->dev_pack, n_out * 4));
+        g->pack_cap = n_out;
+    }
     memcpy(g->pin_in, mel_host, n_mel * 4);
     if (f0_host) memcpy(g->pin_in + n_mel, f0_host, n_f0 * 4);
+    if (len) ragged_table(g, B, T, len, reinterpret_cast<int *>(g->pin_in + n_mel + n_f0));
     SVB_CUDA(cudaMemcpyAsync(g->dev_in, g->pin_in, n_in * 4, cudaMemcpyHostToDevice, st));
-    SVB_TRY(forward_impl(g, g->dev_in, true, f0_host ? g->dev_in + n_mel : nullptr, nullptr, nullptr, seed, B, T, g->dev_out, st));
-    unsigned *mx;
-    mx = reinterpret_cast<unsigned *>(reinterpret_cast<char *>(g->dev_i16) + (g->i16_cap * 2 + 3) / 4 * 4);
-    SVB_TRY(wav_to_int16(g->dev_out, B, (long long)T * g->hop, norm, g->dev_i16, mx, st));
+    const int *tab_dev = len ? reinterpret_cast<const int *>(g->dev_in + n_mel + n_f0) : nullptr;
+    SVB_TRY(forward_impl(g, g->dev_in, true, f0_host ? g->dev_in + n_mel : nullptr, nullptr, nullptr, seed, B, T, g->dev_out, st, len,
+                         tab_dev));
+    const long long n = (long long)T * g->hop;
+    const void *out = g->dev_out;
+    if (i16) {
+        unsigned *mx = reinterpret_cast<unsigned *>(reinterpret_cast<char *>(g->dev_i16) + (g->i16_cap * 2 + 3) / 4 * 4);
+        SVB_TRY(wav_to_int16(g->dev_out, B, n, norm, g->dev_i16, mx, st, tab_dev, g->hop));
+        out = g->dev_i16;
+    } else if (len) {
+        const dim3 grid((unsigned)std::min<long long>((n + 255) / 256, 132 * 4), (unsigned)B);
+        pack_clips_kernel<<<grid, 256, 0, st>>>(g->dev_out, n, tab_dev, g->hop, g->dev_pack);
+        SVB_CUDA(cudaGetLastError());
+        out = g->dev_pack;
+    }
     // the pinned float staging buffer is large enough for the 2-byte samples
-    SVB_CUDA(cudaMemcpyAsync(g->pin_out, g->dev_i16, n_out * 2, cudaMemcpyDeviceToHost, st));
+    const size_t bytes = n_out * (i16 ? 2 : 4);
+    SVB_CUDA(cudaMemcpyAsync(g->pin_out, out, bytes, cudaMemcpyDeviceToHost, st));
     SVB_CUDA(cudaStreamSynchronize(st));
-    memcpy(wav_host, g->pin_out, n_out * 2);
+    memcpy(wav_host, g->pin_out, bytes);
     return SVB_OK;
+}
+
+extern "C" int svb_gen_spec2wav_host(svb_gen_t *g, const float *mel_host, const float *f0_host, uint64_t seed, int32_t B,
+                                     int32_t T, float *wav_host, void *stream) {
+    return spec2wav_host(g, mel_host, f0_host, seed, B, T, nullptr, false, 0, wav_host, stream);
+}
+
+extern "C" int svb_gen_spec2wav_host_i16(svb_gen_t *g, const float *mel_host, const float *f0_host, uint64_t seed, int32_t B,
+                                         int32_t T, int32_t norm, int16_t *wav_host, void *stream) {
+    return spec2wav_host(g, mel_host, f0_host, seed, B, T, nullptr, true, norm, wav_host, stream);
+}
+
+extern "C" int svb_gen_spec2wav_ragged_host(svb_gen_t *g, const float *mel_host, const float *f0_host, uint64_t seed, int32_t B,
+                                            const int32_t *lengths_host, float *wav_host, void *stream) {
+    return spec2wav_host(g, mel_host, f0_host, seed, B, 0, lengths_host, false, 0, wav_host, stream);
+}
+
+extern "C" int svb_gen_spec2wav_ragged_host_i16(svb_gen_t *g, const float *mel_host, const float *f0_host, uint64_t seed, int32_t B,
+                                                const int32_t *lengths_host, int32_t norm, int16_t *wav_host, void *stream) {
+    return spec2wav_host(g, mel_host, f0_host, seed, B, 0, lengths_host, true, norm, wav_host, stream);
 }
 
 extern "C" int svb_gen_get_tap(svb_gen_t *g, const char *name, float *out_dev, int64_t capacity_floats, int64_t *shape3,
@@ -919,59 +961,4 @@ extern "C" int svb_gen_forward_ragged(svb_gen_t *g, const float *mel_dev, const 
                                       float *wav_dev, void *stream) {
     SVB_TRY(check_lengths(g, B, T_max, lengths_host));
     return forward_impl(g, mel_dev, false, f0_dev, rand_ini_dev, noise_dev, seed, B, T_max, wav_dev, as_stream(stream), lengths_host);
-}
-
-// the ragged host calls: [mel | f0 | ragged table] in one H2D copy, one forward over [B, T_max], the clips packed back to back
-// on the device (as floats, or converted to int16), one D2H copy
-static int spec2wav_ragged_host(svb_gen *g, const float *mel_host, const float *f0_host, uint64_t seed, int B, const int32_t *len,
-                                bool i16, int norm, void *wav_host, void *stream) {
-    SVB_CHECK(mel_host && wav_host, SVB_ERR_INVALID, "spec2wav_ragged: null buffer");
-    int T = 0;
-    size_t frames = 0;
-    for (int b = 0; b < B && len; ++b) T = std::max(T, (int)len[b]), frames += len[b] > 0 ? len[b] : 0;
-    SVB_TRY(check_lengths(g, B, std::max(T, 1), len));
-    SVB_CHECK(B <= 4096, SVB_ERR_INVALID, "spec2wav_ragged: batch %d > 4096", B);
-    SVB_CUDA(cudaSetDevice(g->device));
-    cudaStream_t st = as_stream(stream);
-    const size_t n_mel = frames * g->cfg.n_mel, n_f0 = f0_host ? frames : 0, n_tab = 4 * (size_t)B;
-    const size_t n_in = n_mel + n_f0 + n_tab, n_pad = (size_t)B * T * g->hop, n_out = frames * g->hop;
-    SVB_TRY(ensure_staging(g, n_in, n_pad, i16));
-    if (!i16 && n_out > g->pack_cap) {
-        if (g->dev_pack) cudaFree(g->dev_pack);
-        g->dev_pack = nullptr, g->pack_cap = 0;
-        SVB_CUDA(cudaMalloc((void **)&g->dev_pack, n_out * 4));
-        g->pack_cap = n_out;
-    }
-    memcpy(g->pin_in, mel_host, n_mel * 4);
-    if (f0_host) memcpy(g->pin_in + n_mel, f0_host, n_f0 * 4);
-    int *tab = reinterpret_cast<int *>(g->pin_in + n_mel + n_f0);
-    ragged_table(g, B, T, len, tab);
-    SVB_CUDA(cudaMemcpyAsync(g->dev_in, g->pin_in, n_in * 4, cudaMemcpyHostToDevice, st));
-    const int *tab_dev = reinterpret_cast<const int *>(g->dev_in + n_mel + n_f0);
-    SVB_TRY(forward_impl(g, g->dev_in, true, f0_host ? g->dev_in + n_mel : nullptr, nullptr, nullptr, seed, B, T, g->dev_out, st, len,
-                         tab_dev));
-    const long long n = (long long)T * g->hop;
-    const dim3 grid((unsigned)std::min<long long>((n + 255) / 256, 132 * 4), (unsigned)B);
-    if (i16) {
-        unsigned *mx = reinterpret_cast<unsigned *>(reinterpret_cast<char *>(g->dev_i16) + (g->i16_cap * 2 + 3) / 4 * 4);
-        SVB_TRY(wav_to_int16(g->dev_out, B, n, norm, g->dev_i16, mx, st, tab_dev, g->hop));
-        SVB_CUDA(cudaMemcpyAsync(g->pin_out, g->dev_i16, n_out * 2, cudaMemcpyDeviceToHost, st));
-    } else {
-        pack_clips_kernel<<<grid, 256, 0, st>>>(g->dev_out, n, tab_dev, g->hop, g->dev_pack);
-        SVB_CUDA(cudaGetLastError());
-        SVB_CUDA(cudaMemcpyAsync(g->pin_out, g->dev_pack, n_out * 4, cudaMemcpyDeviceToHost, st));
-    }
-    SVB_CUDA(cudaStreamSynchronize(st));
-    memcpy(wav_host, g->pin_out, n_out * (i16 ? 2 : 4));
-    return SVB_OK;
-}
-
-extern "C" int svb_gen_spec2wav_ragged_host(svb_gen_t *g, const float *mel_host, const float *f0_host, uint64_t seed, int32_t B,
-                                            const int32_t *lengths_host, float *wav_host, void *stream) {
-    return spec2wav_ragged_host(g, mel_host, f0_host, seed, B, lengths_host, false, 0, wav_host, stream);
-}
-
-extern "C" int svb_gen_spec2wav_ragged_host_i16(svb_gen_t *g, const float *mel_host, const float *f0_host, uint64_t seed, int32_t B,
-                                                const int32_t *lengths_host, int32_t norm, int16_t *wav_host, void *stream) {
-    return spec2wav_ragged_host(g, mel_host, f0_host, seed, B, lengths_host, true, norm, wav_host, stream);
 }

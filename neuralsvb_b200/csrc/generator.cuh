@@ -43,13 +43,26 @@ struct Tap {
     bool plain = false;     // [B][T] instead of C4T
 };
 
+// How a stage runs its ResBlock steps (decided per forward by plan_workspace): one launch per conv, chain by chain; or step
+// by step, one launch over all chains' c1 and one over their c2 (merged), or one over both (fused: no A buffers)
+enum class Schedule : char { PerConv, Merged, Fused };
+
 // byte offsets into the workspace of one forward (in training mode this is also the tape of the backward)
 struct Buffers {
     size_t mel = 0, pre = 0, har = 0, nsf = 0, sines = 0, wav = 0;
     size_t f0 = 0;                                           // [B][T] f0 of a ragged host call (clips unpacked)
-    std::vector<char> fused;                                 // per stage: its ResBlock steps run fused (no A buffers)
+    std::vector<Schedule> sched;                             // per stage
     std::vector<size_t> X, S;
     std::vector<std::vector<std::vector<size_t>>> A, R;      // [stage][ResBlock chain][dilation]
+};
+
+// Step m of ResBlock chain j of a stage: it reads x (also its residual) and leaves its result in dst, the stage sum S on
+// the last step (scaled by 1 / nk and, after the first chain, accumulated), else the next step's x.  t: c1's output of a
+// ResBlock1 step; nullptr for ResBlock2 and in fused stages.
+struct StepBufs {
+    float *x, *t, *dst;
+    float scale;
+    int accumulate;
 };
 
 // dgrad twins of the ResBlock convs of one stage (flipped taps, transposed channels) + upsampler weights
@@ -175,4 +188,5 @@ int gen_upload(svb_gen *g, const std::vector<float> &h, float **out);
 int gen_get_w(svb_gen *g, const std::string &name, std::vector<int64_t> want, const HostTensor **out);
 int gen_build_layers(svb_gen *g);
 int gen_build_bwd_layers(svb_gen *g);      // generator_bwd.cu
+StepBufs step_bufs(const svb_gen *g, int stage, int chain, int m);     // in the layout of the last forward (svb_gen::bf)
 }  // namespace svb

@@ -364,7 +364,6 @@ extern "C" int svb_gen_backward(svb_gen_t *g, const float *dwav_dev, void *strea
         const BwdStage &bs = g->bwd[i];
         const int C = s.C;
         const size_t n = c4t_floats(B, C, Ti), n4 = n / 4;
-        const float *X = F(bf.X[i]);
         SVB_CUDA(cudaMemsetAsync(Y1, 0, n * 4, st));
         SVB_CUDA(cudaMemsetAsync(Y2, 0, n * 4, st));
         for (int j = 0; j < nk; ++j) {
@@ -373,9 +372,9 @@ extern "C" int svb_gen_backward(svb_gen_t *g, const float *dwav_dev, void *strea
             SVB_TRY(launch_ew(G, dS, nullptr, nullptr, 1.f, 1.f / nk, n4, st));          // chain output enters S as x / nk
             for (int m = nd - 1; m >= 0; --m) {
                 const int d = c.resblock_dilation_sizes[j][m];
+                const StepBufs sb = step_bufs(g, i, j, m);
+                const float *xm = sb.x, *tm = sb.t;
                 if (c.resblock == 1) {
-                    const float *xm = m == 0 ? X : F(bf.R[i][j][m - 1]);
-                    const float *tm = F(bf.A[i][j][m]);
                     SVB_TRY(conv_wgrad(tm, G, C, C, Tip, Ti, rk, 1, 0.1f, base + ".convs2." + std::to_string(m)));
                     SVB_TRY(run_dgrad(g, bs.d2[j][m], G, Y1, Tip, B, Ti, st));
                     SVB_TRY(launch_ew(Y1, Y1, nullptr, tm, 0.1f, 1.f, n4, st));           // through leaky_relu(t_m)
@@ -384,7 +383,6 @@ extern "C" int svb_gen_backward(svb_gen_t *g, const float *dwav_dev, void *strea
                     SVB_TRY(launch_ew(G, Y2, G, xm, 0.1f, 1.f, n4, st));                  // skip connection + leaky_relu(x_m)
                     g->bwd_launches += 2;
                 } else {
-                    const float *xm = m == 0 ? X : (m % 2 ? F(bf.R[i][j][m - 1]) : F(bf.A[i][j][m - 1]));
                     SVB_TRY(conv_wgrad(xm, G, C, C, Tip, Ti, rk, d, 0.1f, base + ".convs." + std::to_string(m)));
                     SVB_TRY(run_dgrad(g, bs.d1[j][m], G, Y1, Tip, B, Ti, st));
                     SVB_TRY(launch_ew(G, Y1, G, xm, 0.1f, 1.f, n4, st));
