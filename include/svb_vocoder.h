@@ -398,6 +398,17 @@ int64_t svb_wav2spec_host(const svb_stft_config *cfg, const float *wav_host, int
 int64_t svb_wav2spec_batch_host(const svb_stft_config *cfg, const float *wav_concat_host, const int64_t *lengths,
                                 int32_t n_clips, const float *mel_basis_host, float *mel_concat_host, int64_t *frames_out,
                                 int device, void *stream);
+/* The same on device memory, with no copy of the samples and no synchronisation (the host form above is its H2D + call + D2H
+ * wrapper).  wav_concat_dev: the clips back to back (lengths: host array); mel_basis_dev [n_mels, n_fft/2+1]; mel_concat_dev
+ * receives the mels back to back, wav_out_dev (NULL = not wanted) every clip zero-padded to frames_c * hop samples, back to back
+ * (what wav2spec returns as its waveform, in the layout svb_pitch_ac_batch takes).  The only copy is the small clip table, into
+ * the caller-owned workspace of svb_wav2spec_workspace_bytes bytes.  Both reject before any launch (SVB_ERR_INVALID) a bad config,
+ * an empty clip, a null buffer or a short workspace; frames_out (NULL = not wanted) receives the frame counts.  svb_wav2spec_batch
+ * returns the total frame count, svb_wav2spec_workspace_bytes the workspace size, or a negative status. */
+int64_t svb_wav2spec_workspace_bytes(const svb_stft_config *cfg, const int64_t *lengths, int32_t n_clips, int64_t *frames_out);
+int64_t svb_wav2spec_batch(const svb_stft_config *cfg, const float *wav_concat_dev, const int64_t *lengths, int32_t n_clips,
+                           const float *mel_basis_dev, float *mel_concat_dev, float *wav_out_dev, int64_t *frames_out,
+                           void *workspace_dev, int64_t workspace_bytes, void *stream);
 
 /* ---- SVB acoustic step, first piece (SURVEY 8(f) N1): the WN gated dilated-conv stack of the GlobalFVAE
  * (modules/fastspeech/fs2_vae.py:19-91; built by modules/voice_conversion/vae_models.py:81-146 with hidden 192,

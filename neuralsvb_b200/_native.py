@@ -161,6 +161,8 @@ _PROTOS = {
     'svb_denoise': (ctypes.c_int, [ctypes.POINTER(StftConfig), _P, _I32, _I64, ctypes.c_float, _P, _P]),
     'svb_wav2spec_host': (_I64, [ctypes.POINTER(StftConfig), _P, _I64, _P, _P, _P, ctypes.c_int, _P]),
     'svb_wav2spec_batch_host': (_I64, [ctypes.POINTER(StftConfig), _P, _P, _I32, _P, _P, _P, ctypes.c_int, _P]),
+    'svb_wav2spec_workspace_bytes': (_I64, [ctypes.POINTER(StftConfig), _P, _I32, _P]),
+    'svb_wav2spec_batch': (_I64, [ctypes.POINTER(StftConfig), _P, _P, _I32, _P, _P, _P, _P, _P, _I64, _P]),
     'svb_gen_spec2wav_host_i16': (ctypes.c_int, [_P, _P, _P, _U64, _I32, _I32, _I32, _P, _P]),
     'svb_wav_to_int16': (ctypes.c_int, [_P, _I32, _I64, _I32, _P, _P]),
     'svb_gen_forward_ragged': (ctypes.c_int, [_P, _P, _P, _P, _P, _U64, _I32, _I32, _P, _P, _P]),

@@ -525,8 +525,12 @@ int fill_args(const svb_stft_config *cfg, const float *wav_dev, const float *mel
     return SVB_OK;
 }
 
-// launch of the v2 forward: `ct` = per-clip table on the device (nullptr members: B equal-length clips)
-int launch_stft_v2(const StftArgs &a, bool want_mel, const ClipTable &ct, int n_clips, int total_blocks, cudaStream_t st) {
+// launch of the v2 forward: `ct` = per-clip table on the device (nullptr members: B equal-length clips); `pack_ws` = caller-owned
+// room for the packed mel filters (mel_pack_bytes), nullptr: allocated on the stream
+size_t mel_pack_bytes(int n_mels, int n_bins) { return ((size_t)3 * n_mels + 4) * sizeof(int) + (size_t)n_mels * n_bins * sizeof(float); }
+
+int launch_stft_v2(const StftArgs &a, bool want_mel, const ClipTable &ct, int n_clips, int total_blocks, cudaStream_t st,
+                   char *pack_ws = nullptr) {
     MelPack mp = {};
     char *ws = nullptr;
     int pack_cap = 0;
@@ -534,10 +538,11 @@ int launch_stft_v2(const StftArgs &a, bool want_mel, const ClipTable &ct, int n_
         SVB_CHECK(a.n_mels <= 1024, SVB_ERR_INVALID, "stft: n_mels %d > 1024", a.n_mels);
         const size_t n_val = (size_t)a.n_mels * a.n_bins;
         const size_t ints = (size_t)3 * a.n_mels + 4;
-        SVB_CUDA(cudaMallocAsync((void **)&ws, ints * sizeof(int) + n_val * sizeof(float), st));
-        int *ip = reinterpret_cast<int *>(ws);
+        if (!pack_ws) SVB_CUDA(cudaMallocAsync((void **)&ws, mel_pack_bytes(a.n_mels, a.n_bins), st));
+        char *p = pack_ws ? pack_ws : ws;
+        int *ip = reinterpret_cast<int *>(p);
         mp.lo = ip, mp.hi = ip + a.n_mels, mp.off = ip + 2 * a.n_mels, mp.total = ip + 3 * a.n_mels;
-        float *val = reinterpret_cast<float *>(ws + ints * sizeof(int));
+        float *val = reinterpret_cast<float *>(p + ints * sizeof(int));
         mp.val = val;
         mel_pack_kernel<<<1, 256, 0, st>>>(a.mel_basis, a.n_mels, a.n_bins, ip, ip + a.n_mels, ip + 2 * a.n_mels, val, ip + 3 * a.n_mels);
         pack_cap = (int)std::min<size_t>(n_val, 4096);
@@ -566,52 +571,106 @@ extern "C" int svb_stft_forward(const svb_stft_config *cfg, const float *wav_dev
     return launch_stft_v2(a, want_mel, ClipTable{nullptr, nullptr, nullptr}, B, B * bpc, as_stream(stream));
 }
 
-// wav2spec of one clip or of a ragged batch: one H2D of the concatenated waveforms + the clip table, ONE kernel
-// launch over all frames of all clips, one D2H of the concatenated mels.
-static int64_t wav2spec_batch_impl(const svb_stft_config *cfg, const float *wav_host, const int64_t *lengths, int32_t n_clips,
-                                   const float *mel_basis_host, float *mel_host, int64_t *frames_out, int device, cudaStream_t st) {
-    SVB_CHECK(cfg && wav_host && lengths && mel_basis_host && mel_host && n_clips > 0, SVB_ERR_INVALID, "wav2spec: null buffer or no clips");
-    std::vector<long long> wav_off(n_clips + 1, 0), frm_off(n_clips + 1, 0);
-    std::vector<int> blk_off(n_clips + 1, 0);
+// The ragged batch of wav2spec: per clip c, the first CTA, the waveform offset and the output frame offset (1 + lengths[c] / hop
+// frames each, the centre-zero-padded STFT of data_gen_utils.process_utterance).  Checks every clip; frames_out (nullable) receives
+// the frame counts.
+struct Wav2SpecPlan {
+    std::vector<long long> wav_off, frm_off;
+    std::vector<int> blk_off;
+    size_t tab_bytes, pack_off, total;
+};
+
+static int plan_wav2spec(const svb_stft_config *cfg, const int64_t *lengths, int32_t n_clips, int64_t *frames_out, Wav2SpecPlan *p) {
+    SVB_CHECK(cfg && lengths && n_clips > 0, SVB_ERR_INVALID, "wav2spec: null config / lengths or no clips");
+    p->wav_off.assign(n_clips + 1, 0), p->frm_off.assign(n_clips + 1, 0), p->blk_off.assign(n_clips + 1, 0);
     for (int c = 0; c < n_clips; ++c) {
         SVB_TRY(validate_stft(cfg, lengths[c], true));
         const int64_t fr = svb_stft_num_frames(cfg, lengths[c]);
-        wav_off[c + 1] = wav_off[c] + lengths[c];
-        frm_off[c + 1] = frm_off[c] + fr;
-        blk_off[c + 1] = blk_off[c] + (int)((fr + kFPB - 1) / kFPB);
+        p->wav_off[c + 1] = p->wav_off[c] + lengths[c];
+        p->frm_off[c + 1] = p->frm_off[c] + fr;
+        p->blk_off[c + 1] = p->blk_off[c] + (int)((fr + kFPB - 1) / kFPB);
         if (frames_out) frames_out[c] = fr;
     }
-    SVB_CUDA(cudaSetDevice(device));
-    const int n_bins = cfg->n_fft / 2 + 1;
-    const size_t n_wav = (size_t)wav_off[n_clips], n_frames = (size_t)frm_off[n_clips];
-    const size_t tab_bytes = (size_t)(n_clips + 1) * (2 * sizeof(long long) + sizeof(int));
-    float *d_wav = nullptr, *d_basis = nullptr, *d_mel = nullptr;
-    char *d_tab = nullptr;
-    SVB_CUDA(cudaMallocAsync((void **)&d_wav, n_wav * sizeof(float), st));
-    SVB_CUDA(cudaMallocAsync((void **)&d_basis, (size_t)cfg->n_mels * n_bins * sizeof(float), st));
-    SVB_CUDA(cudaMallocAsync((void **)&d_mel, n_frames * cfg->n_mels * sizeof(float), st));
-    SVB_CUDA(cudaMallocAsync((void **)&d_tab, tab_bytes, st));
-    std::vector<char> tab(tab_bytes);
-    memcpy(tab.data(), wav_off.data(), (n_clips + 1) * sizeof(long long));
-    memcpy(tab.data() + (n_clips + 1) * sizeof(long long), frm_off.data(), (n_clips + 1) * sizeof(long long));
-    memcpy(tab.data() + 2 * (n_clips + 1) * sizeof(long long), blk_off.data(), (n_clips + 1) * sizeof(int));
-    SVB_CUDA(cudaMemcpyAsync(d_wav, wav_host, n_wav * sizeof(float), cudaMemcpyHostToDevice, st));
-    SVB_CUDA(cudaMemcpyAsync(d_basis, mel_basis_host, (size_t)cfg->n_mels * n_bins * sizeof(float), cudaMemcpyHostToDevice, st));
-    SVB_CUDA(cudaMemcpyAsync(d_tab, tab.data(), tab_bytes, cudaMemcpyHostToDevice, st));
+    SVB_CHECK(cfg->n_mels <= 1024, SVB_ERR_INVALID, "stft: n_mels %d > 1024", cfg->n_mels);
+    p->tab_bytes = (size_t)(n_clips + 1) * (2 * sizeof(long long) + sizeof(int));
+    p->pack_off = (p->tab_bytes + 255) / 256 * 256;
+    p->total = p->pack_off + mel_pack_bytes(cfg->n_mels, cfg->n_fft / 2 + 1);
+    return SVB_OK;
+}
+
+// every clip's waveform zero-padded (or cut) to frames * hop samples, back to back (audio.librosa_pad_lr + wav[:T * hop])
+__global__ void pad_to_frames_kernel(const float *__restrict__ wav, const long long *__restrict__ wav_off,
+                                     const long long *__restrict__ frm_off, int hop, float *__restrict__ out) {
+    const int c = blockIdx.y;
+    const long long w0 = wav_off[c], n = wav_off[c + 1] - w0;
+    const long long o0 = frm_off[c] * hop, m = (frm_off[c + 1] - frm_off[c]) * hop;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += (long long)gridDim.x * blockDim.x)
+        out[o0 + i] = i < n ? wav[w0 + i] : 0.f;
+}
+
+extern "C" int64_t svb_wav2spec_workspace_bytes(const svb_stft_config *cfg, const int64_t *lengths, int32_t n_clips, int64_t *frames_out) {
+    Wav2SpecPlan p;
+    SVB_TRY(plan_wav2spec(cfg, lengths, n_clips, frames_out, &p));
+    return (int64_t)p.total;
+}
+
+extern "C" int64_t svb_wav2spec_batch(const svb_stft_config *cfg, const float *wav_concat_dev, const int64_t *lengths, int32_t n_clips,
+                                      const float *mel_basis_dev, float *mel_concat_dev, float *wav_out_dev, int64_t *frames_out,
+                                      void *workspace_dev, int64_t workspace_bytes, void *stream) {
+    Wav2SpecPlan p;
+    SVB_TRY(plan_wav2spec(cfg, lengths, n_clips, frames_out, &p));
+    SVB_CHECK(wav_concat_dev && mel_basis_dev && mel_concat_dev && workspace_dev, SVB_ERR_INVALID, "wav2spec: null buffer");
+    SVB_CHECK(workspace_bytes >= (int64_t)p.total, SVB_ERR_INVALID, "wav2spec: workspace of %lld bytes, %lld needed",
+              (long long)workspace_bytes, (long long)p.total);
+    cudaStream_t st = as_stream(stream);
+    char *ws = static_cast<char *>(workspace_dev);
+    std::vector<char> tab(p.tab_bytes);
+    memcpy(tab.data(), p.wav_off.data(), (n_clips + 1) * sizeof(long long));
+    memcpy(tab.data() + (n_clips + 1) * sizeof(long long), p.frm_off.data(), (n_clips + 1) * sizeof(long long));
+    memcpy(tab.data() + 2 * (n_clips + 1) * sizeof(long long), p.blk_off.data(), (n_clips + 1) * sizeof(int));
+    SVB_CUDA(cudaMemcpyAsync(ws, tab.data(), p.tab_bytes, cudaMemcpyHostToDevice, st));
     svb_stft_config c = *cfg;
     c.frames_major = 1;
     StftArgs a;
-    int rc = fill_args(&c, d_wav, d_basis, d_mel, lengths[0], &a);
+    SVB_TRY(fill_args(&c, wav_concat_dev, mel_basis_dev, mel_concat_dev, lengths[0], &a));
     ClipTable ct;
-    ct.wav_off = reinterpret_cast<const long long *>(d_tab);
+    ct.wav_off = reinterpret_cast<const long long *>(ws);
     ct.frm_off = ct.wav_off + (n_clips + 1);
-    ct.blk_off = reinterpret_cast<const int *>(d_tab + 2 * (n_clips + 1) * sizeof(long long));
-    if (rc == SVB_OK) rc = launch_stft_v2(a, true, ct, n_clips, blk_off[n_clips], st);
-    if (rc == SVB_OK)
+    ct.blk_off = reinterpret_cast<const int *>(ws + 2 * (n_clips + 1) * sizeof(long long));
+    SVB_TRY(launch_stft_v2(a, true, ct, n_clips, p.blk_off[n_clips], st, ws + p.pack_off));
+    if (wav_out_dev) {
+        long long longest = 0;
+        for (int k = 0; k < n_clips; ++k) longest = std::max(longest, (p.frm_off[k + 1] - p.frm_off[k]) * cfg->hop);
+        const dim3 grid((unsigned)std::min<long long>((longest + 255) / 256, 132 * 4), (unsigned)n_clips);
+        pad_to_frames_kernel<<<grid, 256, 0, st>>>(wav_concat_dev, ct.wav_off, ct.frm_off, cfg->hop, wav_out_dev);
+        SVB_CUDA(cudaGetLastError());
+    }
+    return (int64_t)p.frm_off[n_clips];
+}
+
+// the host form: one H2D of the concatenated waveforms and the filters, svb_wav2spec_batch, one D2H of the mels; synchronises
+static int64_t wav2spec_batch_impl(const svb_stft_config *cfg, const float *wav_host, const int64_t *lengths, int32_t n_clips,
+                                   const float *mel_basis_host, float *mel_host, int64_t *frames_out, int device, cudaStream_t st) {
+    Wav2SpecPlan p;
+    SVB_TRY(plan_wav2spec(cfg, lengths, n_clips, nullptr, &p));
+    SVB_CHECK(wav_host && mel_basis_host && mel_host, SVB_ERR_INVALID, "wav2spec: null buffer or no clips");
+    SVB_CUDA(cudaSetDevice(device));
+    const int n_bins = cfg->n_fft / 2 + 1;
+    const size_t n_wav = (size_t)p.wav_off[n_clips], n_frames = (size_t)p.frm_off[n_clips];
+    float *d_wav = nullptr, *d_basis = nullptr, *d_mel = nullptr;
+    char *d_ws = nullptr;
+    SVB_CUDA(cudaMallocAsync((void **)&d_wav, n_wav * sizeof(float), st));
+    SVB_CUDA(cudaMallocAsync((void **)&d_basis, (size_t)cfg->n_mels * n_bins * sizeof(float), st));
+    SVB_CUDA(cudaMallocAsync((void **)&d_mel, n_frames * cfg->n_mels * sizeof(float), st));
+    SVB_CUDA(cudaMallocAsync((void **)&d_ws, p.total, st));
+    SVB_CUDA(cudaMemcpyAsync(d_wav, wav_host, n_wav * sizeof(float), cudaMemcpyHostToDevice, st));
+    SVB_CUDA(cudaMemcpyAsync(d_basis, mel_basis_host, (size_t)cfg->n_mels * n_bins * sizeof(float), cudaMemcpyHostToDevice, st));
+    int64_t rc = svb_wav2spec_batch(cfg, d_wav, lengths, n_clips, d_basis, d_mel, nullptr, frames_out, d_ws, (int64_t)p.total, st);
+    if (rc >= 0)
         SVB_CUDA(cudaMemcpyAsync(mel_host, d_mel, n_frames * cfg->n_mels * sizeof(float), cudaMemcpyDeviceToHost, st));
-    cudaFreeAsync(d_wav, st), cudaFreeAsync(d_basis, st), cudaFreeAsync(d_mel, st), cudaFreeAsync(d_tab, st);
+    cudaFreeAsync(d_wav, st), cudaFreeAsync(d_basis, st), cudaFreeAsync(d_mel, st), cudaFreeAsync(d_ws, st);
     SVB_CUDA(cudaStreamSynchronize(st));
-    return rc != SVB_OK ? rc : (int64_t)n_frames;
+    return rc;
 }
 
 extern "C" int64_t svb_wav2spec_batch_host(const svb_stft_config *cfg, const float *wav_concat_host, const int64_t *lengths,

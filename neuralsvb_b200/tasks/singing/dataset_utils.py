@@ -22,6 +22,34 @@ from neuralsvb_b200.utils.pitch_utils import f0_to_coarse, norm_interp_f0
 BATCH_KEYS = ('mels', 'prof_mels', 'pitch', 'prof_pitch', 'f0', 'uv', 'prof_f0', 'prof_uv', 'a2p_f0_alignment', 'multi_spk_emb')
 
 
+def cropped_frames(n_frames, hp):
+    """Frames a take of ``n_frames`` keeps: at most ``max_frames``, then a multiple of ``frames_multiple``."""
+    return min(n_frames, hp['max_frames']) // hp['frames_multiple'] * hp['frames_multiple']
+
+
+def take_conditioning(n_frames, f0, pitch, hp, f0_clip):
+    """(T, pitch, f0, uv) of one take of ``n_frames`` mel frames, from its binarized f0 (Hz) and pitch ids: T = cropped_frames,
+    ``normalize_pitch`` (``f0_clip``: 500 for the amateur take, 900 for the professional one), then norm_interp_f0 on the first T
+    frames.  The dataset's items and the beautifier's takes both go through it."""
+    T = cropped_frames(n_frames, hp)
+    if hp.get('normalize_pitch', False):
+        # the voiced frames moved to the dataset's f0 statistics; f0 / uv below come from the moved contour, as in the reference
+        f0 = np.array(f0, copy=True)
+        v = f0 > 0
+        if v.any() and f0[v].std() > 0:
+            f0[v] = ((f0[v] - f0[v].mean()) / f0[v].std() * hp['f0_std'] + hp['f0_mean']).clip(min=60, max=f0_clip)
+        pitch = torch.LongTensor(f0_to_coarse(f0)[:T])
+    else:
+        pitch = torch.LongTensor(pitch)[:T]
+    f0, uv = norm_interp_f0(f0[:T], hp)
+    return T, pitch, f0, uv
+
+
+def clip_alignment(a2p_f0_alignment, prof_T, amateur_T):
+    """The a2p alignment of the cropped takes: its first ``prof_T`` frames, never past the cropped amateur take."""
+    return torch.LongTensor(a2p_f0_alignment)[:prof_T].clip(max=amateur_T - 1)
+
+
 class MultiSpkEmbDataset(torch.utils.data.Dataset):
     def __init__(self, prefix, hparams, shuffle=False, data_dir=None):
         """Reads ``{prefix}_lengths.npy`` and the f0 statistics; sets ``hparams['f0_mean']`` / ``['f0_std']`` from
@@ -66,30 +94,16 @@ class MultiSpkEmbDataset(torch.utils.data.Dataset):
     def _take(self, item, prefix, f0_clip):
         """(mel, pitch, f0, uv) of one take (``prefix`` '' = amateur, 'prof_' = professional): cropped to ``max_frames``, then to a
         multiple of ``frames_multiple``."""
-        hp = self.hparams
-        mel = torch.Tensor(item[f'{prefix}mel'])[:hp['max_frames']]
-        T = mel.shape[0] // hp['frames_multiple'] * hp['frames_multiple']
-        mel = mel[:T]
-        f0 = item[f'{prefix}f0']
-        if hp.get('normalize_pitch', False):
-            # the voiced frames moved to the dataset's f0 statistics; f0 / uv below come from the moved contour, as in the reference
-            f0 = np.array(f0, copy=True)
-            v = f0 > 0
-            if v.any() and f0[v].std() > 0:
-                f0[v] = ((f0[v] - f0[v].mean()) / f0[v].std() * hp['f0_std'] + hp['f0_mean']).clip(min=60, max=f0_clip)
-            pitch = torch.LongTensor(f0_to_coarse(f0)[:T])
-        else:
-            pitch = torch.LongTensor(item[f'{prefix}pitch'])[:T]
-        f0, uv = norm_interp_f0(f0[:T], hp)
-        return mel, pitch, f0, uv
+        mel = item[f'{prefix}mel']
+        T, pitch, f0, uv = take_conditioning(len(mel), item[f'{prefix}f0'], item[f'{prefix}pitch'], self.hparams, f0_clip)
+        return torch.Tensor(mel)[:T], pitch, f0, uv
 
     def __getitem__(self, index):
         item = self._get_item(index)
         assert max(len(item['mel']), len(item['prof_mel'])) == self.sizes[index], (len(item['mel']), self.sizes[index])
         mel, pitch, f0, uv = self._take(item, '', 500)
         prof_mel, prof_pitch, prof_f0, prof_uv = self._take(item, 'prof_', 900)
-        # the alignment indexes amateur frames: never past the cropped amateur take
-        align = torch.LongTensor(item['a2p_f0_alignment'])[:prof_pitch.shape[0]].clip(max=pitch.shape[0] - 1)
+        align = clip_alignment(item['a2p_f0_alignment'], prof_pitch.shape[0], pitch.shape[0])
         assert align.shape == prof_pitch.shape, ('a2p F0 alignment with unmatched shape: ', align.shape, prof_pitch.shape)
         return {'item_name': item['item_name'], 'mel': mel, 'pitch': pitch, 'f0': f0, 'uv': uv, 'prof_mel': prof_mel,
                 'prof_pitch': prof_pitch, 'prof_f0': prof_f0, 'prof_uv': prof_uv, 'a2p_f0_alignment': align,

@@ -203,6 +203,35 @@ def resample_batch(wavs, orig_srs, target_sr):
     return res
 
 
+def resample_device(wav_concat, lengths, orig_srs, target_sr):
+    """``resample_batch`` on device memory (svb_resample_batch): a float32 CUDA tensor of the clips back to back, their host
+    ``lengths`` and rates -> a CUDA tensor of the resampled clips back to back (``resample_lengths``' second array gives their
+    lengths)."""
+    import torch
+
+    from neuralsvb_b200 import _native
+    srs, lens = _resample_args(orig_srs, lengths)
+    if int(lens.sum()) != wav_concat.numel():
+        raise ValueError(f'lengths sum to {int(lens.sum())}, the waveform tensor has {wav_concat.numel()} samples')
+    win, num_table = kaiser_best_window()
+    lib = _native.lib()
+    ws_bytes = lib.svb_resample_plan(int(target_sr), srs.ctypes.data_as(ctypes.c_void_p), lens.ctypes.data_as(ctypes.c_void_p),
+                                     len(lens), len(win), num_table, None, None)
+    if ws_bytes < 0:
+        raise ValueError(lib.svb_last_error().decode('utf-8', 'replace'))
+    _, out_lens = resample_lengths(lens, srs, target_sr)
+    x = wav_concat.contiguous()
+    out = torch.empty(max(int(out_lens.sum()), 1), device=x.device)
+    ws = torch.empty(max(int(ws_bytes), 1), dtype=torch.uint8, device=x.device)
+    with torch.cuda.device(x.device):
+        _native.check(lib.svb_resample_batch(int(target_sr), srs.ctypes.data_as(ctypes.c_void_p), lens.ctypes.data_as(ctypes.c_void_p),
+                                             len(lens), win.ctypes.data_as(ctypes.c_void_p), len(win), num_table,
+                                             ctypes.c_void_p(x.data_ptr()), ctypes.c_void_p(out.data_ptr()),
+                                             ctypes.c_void_p(ws.data_ptr()), int(ws_bytes), None,
+                                             _native.current_stream_ptr(x.device)), 'resample')
+    return out[:int(out_lens.sum())]
+
+
 def load_wav(path, sr=22050):
     """``librosa.core.load(path, sr=sr)`` for a WAV file: (float32 mono samples at ``sr``, sr); ``sr=None`` keeps the file's rate."""
     data, file_sr = read_wav(path)

@@ -65,16 +65,20 @@ def _load_wav(wav_fn, sr):
     return audio.load_wav(wav_fn, sr)[0]
 
 
-def _load_wavs(wav_fns, sr):
-    """Decode every path (arrays are taken to be at sr already), then resample all off-rate files in ONE device call."""
-    wavs, rates = [], []
+def decode_wavs(wav_fns, sr):
+    """[(float32 mono samples, rate)] of each path, decoded as utils/audio.read_wav does; arrays are taken to be at sr already."""
+    out = []
     for w in wav_fns:
         if isinstance(w, str):
-            data, file_sr = audio.read_wav(w)
+            out.append(audio.read_wav(w))
         else:
-            data, file_sr = np.ascontiguousarray(w, dtype=np.float32), sr
-        wavs.append(data)
-        rates.append(file_sr)
+            out.append((np.ascontiguousarray(w, dtype=np.float32), sr))
+    return out
+
+
+def _load_wavs(wav_fns, sr):
+    """Decode every path (arrays are taken to be at sr already), then resample all off-rate files in ONE device call."""
+    wavs, rates = [list(x) for x in zip(*decode_wavs(wav_fns, sr))] if wav_fns else ([], [])
     off = [i for i, r in enumerate(rates) if r != sr]
     if off:
         for i, y in zip(off, audio.resample_batch([wavs[i] for i in off], [rates[i] for i in off], sr)):
@@ -244,6 +248,40 @@ class HifiGAN(BaseVocoder):
             out.append((wo, mel[o:o + int(fr)]))
             o += int(fr)
         return out
+
+    @staticmethod
+    def wav2spec_device(wav_concat, lengths, hp=None, mel_basis=None):
+        """``wav2spec_batch`` on device memory (svb_wav2spec_batch: one launch, no copy of the samples): float32 CUDA tensor of the
+        clips back to back at audio_sample_rate, their host ``lengths`` -> (mels [sum T_c, n_mel] log10, waveforms [sum T_c * hop]
+        zero-padded per clip, frame counts T_c as an int64 numpy array), device tensors back to back as wav2spec_batch returns
+        them clip by clip.  ``mel_basis``: the [n_mel, n_fft / 2 + 1] filters already on the device (default: uploaded here)."""
+        hp = hparams if hp is None else hp
+        if not (torch.is_tensor(wav_concat) and wav_concat.is_cuda and wav_concat.dtype == torch.float32):
+            raise TypeError('wav2spec_device takes a float32 CUDA tensor')
+        wav_concat = wav_concat.contiguous()
+        device = wav_concat.device
+        lib = _native.lib()
+        cfg = stft_config(hp, _native.PAD_CENTER_ZERO, _native.OUT_LOG10_MEL, float(hp.get('wav2spec_eps', 1e-10)))
+        lens = np.ascontiguousarray(lengths, dtype=np.int64)
+        if int(lens.sum()) != wav_concat.numel():
+            raise ValueError(f'lengths sum to {int(lens.sum())}, the waveform tensor has {wav_concat.numel()} samples')
+        frames = np.zeros(len(lens), np.int64)
+        ws_bytes = lib.svb_wav2spec_workspace_bytes(ctypes.byref(cfg), lens.ctypes.data_as(ctypes.c_void_p), len(lens),
+                                                    frames.ctypes.data_as(ctypes.c_void_p))
+        if ws_bytes < 0:
+            raise ValueError(f'wav2spec: {lib.svb_last_error().decode("utf-8", "replace")}')
+        if mel_basis is None:
+            mel_basis = torch.tensor(audio.build_mel_basis(hp), dtype=torch.float32, device=device)
+        n = int(frames.sum())
+        mel = torch.empty(n, cfg.n_mels, device=device)
+        wav = torch.empty(n * cfg.hop, device=device)
+        ws = torch.empty(int(ws_bytes), dtype=torch.uint8, device=device)
+        with torch.cuda.device(device):
+            _native.check(lib.svb_wav2spec_batch(ctypes.byref(cfg), _native.ptr(wav_concat), lens.ctypes.data_as(ctypes.c_void_p),
+                                                 len(lens), _native.ptr(mel_basis.contiguous()), _native.ptr(mel), _native.ptr(wav),
+                                                 None, ctypes.c_void_p(ws.data_ptr()), int(ws_bytes),
+                                                 _native.current_stream_ptr(device)), 'wav2spec_batch')
+        return mel, wav, frames
 
     @staticmethod
     def wav2spec(wav_fn, return_linear=False, hp=None):

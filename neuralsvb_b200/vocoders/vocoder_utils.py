@@ -12,11 +12,16 @@ def denoise(wav, v=0.1, hp=None):
     """Spectral subtraction: STFT(fft_size, hop_size, win_size, pad 'constant') -> max(|X| - v, 0), phase kept -> iSTFT.
     ``wav``: 1-D float array (host) -> float32 array of length hop * (len // hop), like the reference
     (librosa.stft / istft); computed by ``svb_denoise`` on the current CUDA device."""
-    hp = hparams if hp is None else hp
     if not torch.cuda.is_available():
         raise RuntimeError('denoise needs a CUDA device: there is no CPU fallback')
+    return denoise_device(torch.from_numpy(np.ascontiguousarray(wav, np.float32)).cuda(), v, hp).cpu().numpy()
+
+
+def denoise_device(wav, v=0.1, hp=None):
+    """``denoise`` of a 1-D float32 CUDA tensor, left on its device."""
+    hp = hparams if hp is None else hp
     lib = _native.lib()
-    x = torch.from_numpy(np.ascontiguousarray(wav, np.float32)).cuda()[None]
+    x = wav.contiguous()[None]
     n = x.shape[1]
     hop = int(hp['hop_size'])
     c = _native.StftConfig(int(hp['fft_size']), hop, int(hp['win_size']), _native.PAD_CENTER_ZERO, _native.OUT_MAG_RAW, 0, 0, 1, 0.0)
@@ -24,7 +29,7 @@ def denoise(wav, v=0.1, hp=None):
     with torch.cuda.device(x.device):
         _native.check(lib.svb_denoise(ctypes.byref(c), _native.ptr(x), 1, n, ctypes.c_float(float(v)), _native.ptr(out),
                                       _native.current_stream_ptr(x.device)), 'denoise')
-    return out[0].cpu().numpy()
+    return out[0]
 
 
 def wav_to_int16(wav, norm=False):
