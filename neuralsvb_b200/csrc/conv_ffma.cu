@@ -8,6 +8,8 @@
 // scaling / ResBlock-sum accumulation are fused in the epilogue.
 #include "conv_ffma.cuh"
 
+#include <algorithm>
+
 namespace svb {
 
 constexpr int kRowsPerThread = 8;   // 8 rows x 32 lanes = 256-row tile
@@ -180,12 +182,17 @@ __global__ void c4t_to_nct_kernel(const float4 *__restrict__ c4t, float *__restr
     p[0] = v.x, p[T] = v.y, p[2 * (size_t)T] = v.z, p[3 * (size_t)T] = v.w;
 }
 
+// Frame-major conversions: one thread per (t, quad) reads 16 B of the frame-major row and writes one C4T row.  The frames
+// are strided over gridDim.y (at most kMaxGridY blocks), so a mel of any length launches: a whole song at hop 128 passes
+// the 65 535-block limit of gridDim.y after 6.3 minutes.
+constexpr int kMaxGridY = 65535;
+
 __global__ void btc_to_c4t_kernel(const float4 *__restrict__ btc, float4 *__restrict__ c4t, int C, int T, int Tp) {
-    // one thread per (t, quad): reads 16 B of the frame-major row, writes one C4T row
     const int cq = blockIdx.x * blockDim.x + threadIdx.x;
-    const int t = blockIdx.y, b = blockIdx.z;
+    const int b = blockIdx.z;
     if (cq >= (C >> 2)) return;
-    c4t[act_q4(b, C, Tp, cq, kPad + t)] = btc[((size_t)b * T + t) * (C >> 2) + cq];
+    for (int t = blockIdx.y; t < T; t += gridDim.y)
+        c4t[act_q4(b, C, Tp, cq, kPad + t)] = btc[((size_t)b * T + t) * (C >> 2) + cq];
 }
 
 // ragged batches: frames at or past len[b] are written as zeros without reading the input
@@ -205,11 +212,15 @@ __global__ void nct_to_c4t_ragged_kernel(const float *__restrict__ nct, float4 *
 __global__ void btc_to_c4t_ragged_kernel(const float4 *__restrict__ btc, float4 *__restrict__ c4t, int C, int T, int Tp,
                                          const int *__restrict__ len, const int *__restrict__ off) {
     const int cq = blockIdx.x * blockDim.x + threadIdx.x;
-    const int t = blockIdx.y, b = blockIdx.z;
+    const int b = blockIdx.z;
     if (cq >= (C >> 2)) return;
-    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (t < len[b]) v = btc[((off ? (size_t)off[b] : (size_t)b * T) + t) * (C >> 2) + cq];
-    c4t[act_q4(b, C, Tp, cq, kPad + t)] = v;
+    const int Lb = len[b];
+    const size_t row0 = off ? (size_t)off[b] : (size_t)b * T;
+    for (int t = blockIdx.y; t < T; t += gridDim.y) {
+        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (t < Lb) v = btc[(row0 + t) * (C >> 2) + cq];
+        c4t[act_q4(b, C, Tp, cq, kPad + t)] = v;
+    }
 }
 
 int launch_nct_to_c4t(const float *nct, float *c4t, int B, int C, int T, int Tp, cudaStream_t st) {
@@ -225,7 +236,7 @@ int launch_c4t_to_nct(const float *c4t, float *nct, int B, int C, int T, int Tp,
     return SVB_OK;
 }
 int launch_btc_to_c4t(const float *btc, float *c4t, int B, int C, int T, int Tp, cudaStream_t st) {
-    dim3 grid((C / 4 + 31) / 32, T, B);
+    dim3 grid((C / 4 + 31) / 32, std::min(T, kMaxGridY), B);
     btc_to_c4t_kernel<<<grid, 32, 0, st>>>(reinterpret_cast<const float4 *>(btc), reinterpret_cast<float4 *>(c4t), C,
                                            T, Tp);
     SVB_CUDA(cudaGetLastError());
@@ -239,7 +250,7 @@ int launch_nct_to_c4t_ragged(const float *nct, float *c4t, int B, int C, int T, 
 }
 int launch_btc_to_c4t_ragged(const float *btc, float *c4t, int B, int C, int T, int Tp, const int *len, const int *off,
                              cudaStream_t st) {
-    dim3 grid((C / 4 + 31) / 32, T, B);
+    dim3 grid((C / 4 + 31) / 32, std::min(T, kMaxGridY), B);
     btc_to_c4t_ragged_kernel<<<grid, 32, 0, st>>>(reinterpret_cast<const float4 *>(btc), reinterpret_cast<float4 *>(c4t), C,
                                                   T, Tp, len, off);
     SVB_CUDA(cudaGetLastError());

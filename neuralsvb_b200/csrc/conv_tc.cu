@@ -1197,8 +1197,30 @@ int launch_conv_tc(const TcWeights &w, const ConvArgs &a, int precision, cudaStr
     if ((p.total_groups + grid - 1) / grid > kMaxItems) {
         // more items per CTA than the shared-memory list holds: run the batch in slices of clips
         const int per_b = p.groups_per_b * p.col_blocks;
+        if (per_b > kMaxItems * grid) {
+            // One clip alone has more items than one launch lists (a whole song): run each clip on its own, in slices of
+            // rows that start on 256-row boundaries, so the tiles are those of one launch over the clip.  A slice's slabs
+            // read its halo rows from the clip's neighbouring rows in memory, and it stores only its own rows, so every
+            // row is computed as one launch would compute it.  A slice of `rows` input rows is at most rows / 128 items per
+            // column block.
+            const int rows = std::max(2 * kTcM, kMaxItems * grid / p.col_blocks / 2 * 2 * kTcM);
+            const int u = a.ups_u > 0 ? a.ups_u : 1;                  // output rows per input row
+            const size_t in_clip = (size_t)c4t_groups(a.Cin) * a.in_Tp * 32, out_clip = (size_t)c4t_groups(a.Cout) * a.out_Tp * 32;
+            for (int b = 0; b < a.B; ++b) {
+                const int Tb = clip_rows(a, b);
+                for (int r0 = 0; r0 < Tb; r0 += rows) {
+                    ConvArgs s = a;
+                    s.B = 1, s.Tq = std::min(rows, Tb - r0);
+                    s.len = nullptr, s.len_host = nullptr;
+                    s.in = a.in + b * in_clip + (size_t)r0 * 32;
+                    s.out = a.out + b * out_clip + (size_t)r0 * u * 32;
+                    if (a.res) s.res = a.res + b * out_clip + (size_t)r0 * u * 32;
+                    SVB_TRY(launch_conv_tc(w, s, precision, st));
+                }
+            }
+            return SVB_OK;
+        }
         const int nb = std::max(1, kMaxItems * grid / per_b);
-        SVB_CHECK(per_b <= kMaxItems * grid, SVB_ERR_INVALID, "tc conv: one clip alone has %d work items", per_b);
         for (int b0 = 0; b0 < a.B; b0 += nb) {
             ConvArgs s = a;
             s.B = std::min(nb, a.B - b0);
