@@ -137,6 +137,11 @@ int svb_wav_to_int16(const float *wav_dev, int32_t B, int64_t n, int32_t norm, i
 int svb_gen_forward_ragged(svb_gen_t *g, const float *mel_dev, const float *f0_dev, const float *rand_ini_dev,
                            const float *noise_dev, uint64_t seed, int32_t B, int32_t T_max, const int32_t *lengths_host,
                            float *wav_dev, void *stream);
+/* svb_gen_forward_ragged with the Philox draws of clip b keyed by (seed, first_clip + b, t): a batch vocoded in several calls
+ * draws what one call over all its clips would (first_clip >= 0; 0 is svb_gen_forward_ragged). */
+int svb_gen_forward_ragged_from(svb_gen_t *g, const float *mel_dev, const float *f0_dev, const float *rand_ini_dev,
+                                const float *noise_dev, uint64_t seed, int32_t first_clip, int32_t B, int32_t T_max,
+                                const int32_t *lengths_host, float *wav_dev, void *stream);
 /* spec2wav over a ragged batch from HOST memory (vocoders/hifigan.py:55-69, clip by clip): mel_host holds the clips' [T_b, n_mel]
  * mels back to back ([sum T_b, n_mel], as svb_wav2spec_batch_host returns them), f0_host their [T_b] f0 back to back or NULL;
  * wav_host receives sum(T_b) * hop samples, clip after clip.  One H2D copy, one forward, one D2H copy, one synchronisation. */
@@ -514,6 +519,20 @@ int64_t svb_sadtw_workspace_bytes(int32_t n_pairs, const int32_t *src_len_host, 
 int svb_sadtw_align(const void *src_f0_dev, const void *tgt_f0_dev, int32_t dtype, int32_t variant, int32_t n_pairs,
                     const int32_t *src_len_host, const int32_t *tgt_len_host, const double *tgt_scale_host, void *workspace_dev,
                     int64_t workspace_bytes, int64_t *alignment_dev, float *path_cost_dev, float *stage_ms_host, void *stream);
+/* Whole songs: svb_sadtw_long_workspace_bytes / svb_sadtw_align_long take the arguments of svb_sadtw_workspace_bytes /
+ * svb_sadtw_align and compute the same results, with each take of a pair at most 65536 frames (6.3 min at 22.05 kHz / hop 128)
+ * and no bound on min(S, T) below that.  A pair with min(S, T) <= 8192 runs on the one-CTA DTW kernel as in svb_sadtw_align; a
+ * longer one on ceil(min(S, T) / 8192) CTAs (at most 8) of a thread-block cluster, each holding its share of the three live
+ * anti-diagonals and reading its neighbours' edge cells through distributed shared memory.  Alignment and path cost are
+ * bit-identical to the one-CTA kernel's on any pair both can run.  The workspace is the same layout, 4 B of cost plus 1 B of
+ * direction per cell: 8.5 GB for a 4-minute pair (41 344 x 41 344 frames), 21.5 GB at 65536 x 65536.  A pair over 65536 frames
+ * on either side is refused (SVB_ERR_INVALID, -1 from the size query) before any launch.  The environment variable
+ * SVB_DTW_CTA_CELLS=<1 .. 8192>, read per call, replaces the 8192-cell share (clusters still at most 8 CTAs, so a share grows to
+ * ceil(min(S, T) / 8) when it would need more): a test and measurement hook that puts shorter pairs on clusters. */
+int64_t svb_sadtw_long_workspace_bytes(int32_t n_pairs, const int32_t *src_len_host, const int32_t *tgt_len_host, int64_t *offsets_host);
+int svb_sadtw_align_long(const void *src_f0_dev, const void *tgt_f0_dev, int32_t dtype, int32_t variant, int32_t n_pairs,
+                         const int32_t *src_len_host, const int32_t *tgt_len_host, const double *tgt_scale_host, void *workspace_dev,
+                         int64_t workspace_bytes, int64_t *alignment_dev, float *path_cost_dev, float *stage_ms_host, void *stream);
 /* The histogram kernel alone (cal_hist_of_f0(f, max_window=64, scale_factor=scale[k])): n_seq sequences concatenated in f0_dev,
  * hist_dev float32 [sum len, 48] = k / total (normalize_hist=True), counts_dev int32 [sum len, 48] = k (NULL = not wanted).
  * The workspace holds the per-sequence metadata (svb_sadtw_histogram_workspace_bytes). */

@@ -166,6 +166,7 @@ _PROTOS = {
     'svb_gen_spec2wav_host_i16': (ctypes.c_int, [_P, _P, _P, _U64, _I32, _I32, _I32, _P, _P]),
     'svb_wav_to_int16': (ctypes.c_int, [_P, _I32, _I64, _I32, _P, _P]),
     'svb_gen_forward_ragged': (ctypes.c_int, [_P, _P, _P, _P, _P, _U64, _I32, _I32, _P, _P, _P]),
+    'svb_gen_forward_ragged_from': (ctypes.c_int, [_P, _P, _P, _P, _P, _U64, _I32, _I32, _I32, _P, _P, _P]),
     'svb_gen_spec2wav_ragged_host': (ctypes.c_int, [_P, _P, _P, _U64, _I32, _P, _P, _P]),
     'svb_gen_spec2wav_ragged_host_i16': (ctypes.c_int, [_P, _P, _P, _U64, _I32, _P, _I32, _P, _P]),
     'svb_wn_create': (ctypes.c_int, [_I32, _I32, _I32, _I32, _I32, _I32, _I32, ctypes.POINTER(_P)]),
@@ -206,6 +207,8 @@ _PROTOS = {
     'svb_linear1_backward': (ctypes.c_int, [_P, _P, _P, _I32, _I32, _P, _P, _P, _P]),
     'svb_sadtw_workspace_bytes': (_I64, [_I32, _P, _P, _P]),
     'svb_sadtw_align': (ctypes.c_int, [_P, _P, _I32, _I32, _I32, _P, _P, _P, _P, _I64, _P, _P, _P, _P]),
+    'svb_sadtw_long_workspace_bytes': (_I64, [_I32, _P, _P, _P]),
+    'svb_sadtw_align_long': (ctypes.c_int, [_P, _P, _I32, _I32, _I32, _P, _P, _P, _P, _I64, _P, _P, _P, _P]),
     'svb_sadtw_histogram_workspace_bytes': (_I64, [_I32]),
     'svb_sadtw_histogram': (ctypes.c_int, [_P, _I32, _I32, _I32, _P, _P, _P, _I64, _P, _P, _P]),
     'svb_sadtw_cost': (ctypes.c_int, [_P, _I32, _P, _I32, _P, _P]),

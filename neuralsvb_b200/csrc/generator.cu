@@ -419,7 +419,7 @@ int prepare(svb_gen *g, int B, int T, const int *lens, const int *packed_tab, cu
 
 // mel -> G32T (and a host call's f0 unpacked); har_source = m_source(f0)   hifigan.py:145-149; x = conv_pre(x)   :151
 int front_end(svb_gen *g, const float *mel, bool mel_frame_major, const float *f0, const float *rand_ini, const float *noise,
-              uint64_t seed, int B, int T, const int *packed_tab, cudaStream_t st) {
+              uint64_t seed, int B, int T, const int *packed_tab, cudaStream_t st, int clip0) {
     const Buffers &bf = g->bf;
     const bool ragged = !g->rg_len.empty();
     const int n_mel = g->cfg.n_mel, Tp0 = c4t_rows(T), Tw = T * g->hop;
@@ -452,7 +452,7 @@ int front_end(svb_gen *g, const float *mel, bool mel_frame_major, const float *f
             ProfScope ps(g, ns, "nsf source (4 kernels)", 4.0 * B * (T + (double)Tw * (noise ? 10 : 1)), 60.0 * B * Tw * 9);
             SVB_TRY(launch_nsf_source(f0, rand_ini, noise, seed, B, T, g->hop, (float)g->cfg.audio_sample_rate, g->lin_w,
                                       g->lin_b_dev, g->ws + bf.nsf, ws_at(g, bf.har), g->training ? ws_at(g, bf.sines) : nullptr, ns,
-                                      &l, g->rg_dev));
+                                      &l, g->rg_dev, clip0));
         }
         if (side) SVB_CUDA(cudaEventRecord(g->ev_side, ns));
         g->last_launches += l;
@@ -545,7 +545,7 @@ int run_stage(svb_gen *g, int i, int B, int Tin, cudaStream_t st) {
 // ragged_table, and mel / f0 hold the clips back to back (mel frame-major).
 int forward_impl(svb_gen *g, const float *mel, bool mel_frame_major, const float *f0, const float *rand_ini,
                  const float *noise, uint64_t seed, int B, int T, float *wav, cudaStream_t st, const int *lens = nullptr,
-                 const int *packed_tab = nullptr) {
+                 const int *packed_tab = nullptr, int clip0 = 0) {
     SVB_CHECK(g && g->finalized, SVB_ERR_STATE, "generator: forward before finalize");
     SVB_CHECK(!g->dirty, SVB_ERR_STATE, "generator: weights were set after finalize; call svb_gen_update_weights first");
     SVB_CHECK(mel && wav && B > 0 && T > 0, SVB_ERR_INVALID, "generator: null buffer or empty batch (B %d T %d)", B, T);
@@ -556,7 +556,7 @@ int forward_impl(svb_gen *g, const float *mel, bool mel_frame_major, const float
     SVB_CUDA(cudaSetDevice(g->device));
     SVB_TRY(prepare(g, B, T, lens, packed_tab, st));
     g->last_nsf = f0 != nullptr;
-    SVB_TRY(front_end(g, mel, mel_frame_major, f0, rand_ini, noise, seed, B, T, packed_tab, st));
+    SVB_TRY(front_end(g, mel, mel_frame_major, f0, rand_ini, noise, seed, B, T, packed_tab, st, clip0));
     int Ti = T;
     for (int i = 0; i < (int)g->stages.size(); ++i) {
         SVB_TRY(run_stage(g, i, B, Ti, st));
@@ -959,6 +959,14 @@ extern "C" float svb_gen_last_ms(svb_gen_t *g) {
 extern "C" int svb_gen_forward_ragged(svb_gen_t *g, const float *mel_dev, const float *f0_dev, const float *rand_ini_dev,
                                       const float *noise_dev, uint64_t seed, int32_t B, int32_t T_max, const int32_t *lengths_host,
                                       float *wav_dev, void *stream) {
+    return svb_gen_forward_ragged_from(g, mel_dev, f0_dev, rand_ini_dev, noise_dev, seed, 0, B, T_max, lengths_host, wav_dev, stream);
+}
+
+extern "C" int svb_gen_forward_ragged_from(svb_gen_t *g, const float *mel_dev, const float *f0_dev, const float *rand_ini_dev,
+                                           const float *noise_dev, uint64_t seed, int32_t first_clip, int32_t B, int32_t T_max,
+                                           const int32_t *lengths_host, float *wav_dev, void *stream) {
+    SVB_CHECK(first_clip >= 0, SVB_ERR_INVALID, "generator: first_clip %d < 0", first_clip);
     SVB_TRY(check_lengths(g, B, T_max, lengths_host));
-    return forward_impl(g, mel_dev, false, f0_dev, rand_ini_dev, noise_dev, seed, B, T_max, wav_dev, as_stream(stream), lengths_host);
+    return forward_impl(g, mel_dev, false, f0_dev, rand_ini_dev, noise_dev, seed, B, T_max, wav_dev, as_stream(stream), lengths_host,
+                        nullptr, first_clip);
 }

@@ -52,14 +52,16 @@ struct NsfDims {
     int nchunk;         // ceil(T / 32)
     float sr;
     const int *len;     // frames of each clip (ragged batches) or nullptr: F
+    int clip0;          // the Philox draws of clip b are keyed by clip index clip0 + b
     __device__ int frames(int b) const { return len ? len[b] : F; }
 };
 
 // initial phase: rand_ini[b][k] (k = 0 forced to 0, :54) or Philox uniform
-__device__ __forceinline__ float rand_ini_of(const float *rand_ini, uint64_t seed, int b, int k) {
+// (Philox keyed by clip index b + clip0)
+__device__ __forceinline__ float rand_ini_of(const float *rand_ini, uint64_t seed, int b, int k, int clip0) {
     if (k == 0) return 0.f;
     if (rand_ini) return rand_ini[b * kH + k];
-    const uint4 r = philox4x32_10(make_uint4((uint32_t)b, (uint32_t)k, 0x1234u, 0u),
+    const uint4 r = philox4x32_10(make_uint4((uint32_t)(b + clip0), (uint32_t)k, 0x1234u, 0u),
                                   make_uint2((uint32_t)seed, (uint32_t)(seed >> 32) ^ 0x5eedu));
     return u01(r.x);
 }
@@ -76,7 +78,7 @@ __global__ void nsf_frame_prefix_kernel(NsfDims d, const float *__restrict__ f0,
     const float *f0b = f0 + (size_t)b * d.F;
     double *out = base1 + (size_t)wid * d.F;
     const float rad0 = rad_of(f0b[0], k, d.sr);
-    const float r0p = rad0 + rand_ini_of(rand_ini, seed, b, k);   // fp32 add (:56)
+    const float r0p = rad0 + rand_ini_of(rand_ini, seed, b, k, d.clip0);   // fp32 add (:56)
     double carry = (double)r0p - (double)rad0;
     const int Fb = d.frames(b);
     for (int f0i = 0; f0i < Fb; f0i += 32) {
@@ -117,7 +119,7 @@ __global__ void nsf_chunk_sum_kernel(NsfDims d, const float *__restrict__ f0, co
     const int chunk = (int)(wid % d.nchunk);
     const int bk = (int)(wid / d.nchunk), b = bk / kH, k = bk % kH;
     const float *f0b = f0 + (size_t)b * d.F;
-    const float r0p = rad_of(f0b[0], k, d.sr) + rand_ini_of(rand_ini, seed, b, k);
+    const float r0p = rad_of(f0b[0], k, d.sr) + rand_ini_of(rand_ini, seed, b, k, d.clip0);
     const int t = chunk * 32 + lane;
     double v = (t < d.frames(b) * d.U) ? nsf_v(d, f0b, base1 + (size_t)bk * d.F, k, t, r0p) : 0.0;
 #pragma unroll
@@ -169,7 +171,7 @@ __global__ void nsf_synth_kernel(NsfDims d, const float *__restrict__ f0, const 
         const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
 #pragma unroll
         for (int g = 0; g < 3; ++g) {
-            const uint4 r = philox4x32_10(make_uint4((uint32_t)t, (uint32_t)b, (uint32_t)g, 0x4e5346u), key);
+            const uint4 r = philox4x32_10(make_uint4((uint32_t)t, (uint32_t)(b + d.clip0), (uint32_t)g, 0x4e5346u), key);
             float n0, n1, n2, n3;
             box_muller(r.x, r.y, n0, n1);
             box_muller(r.z, r.w, n2, n3);
@@ -181,7 +183,7 @@ __global__ void nsf_synth_kernel(NsfDims d, const float *__restrict__ f0, const 
 #pragma unroll 1
     for (int k = 0; k < kH; ++k) {
         const int bk = b * kH + k;
-        const float r0p = rad_of(f0b[0], k, d.sr) + rand_ini_of(rand_ini, seed, b, k);
+        const float r0p = rad_of(f0b[0], k, d.sr) + rand_ini_of(rand_ini, seed, b, k, d.clip0);
         const double v = valid ? nsf_v(d, f0b, base1 + (size_t)bk * d.F, k, t, r0p) : 0.0;
         double incl = v;
 #pragma unroll
@@ -206,9 +208,9 @@ size_t nsf_workspace_bytes(int B, int F, int U) {
 
 int launch_nsf_source(const float *f0, const float *rand_ini, const float *noise, uint64_t seed, int B, int F, int U,
                       float sr, const float *lin_w_dev, const float *lin_b_dev, void *workspace, float *har, float *sines,
-                      cudaStream_t st, int *launches, const int *len) {
+                      cudaStream_t st, int *launches, const int *len, int clip0) {
     NsfDims d;
-    d.B = B, d.F = F, d.U = U, d.T = F * U, d.nchunk = (d.T + 31) / 32, d.sr = sr, d.len = len;
+    d.B = B, d.F = F, d.U = U, d.T = F * U, d.nchunk = (d.T + 31) / 32, d.sr = sr, d.len = len, d.clip0 = clip0;
     double *base1 = reinterpret_cast<double *>(workspace);
     double *csum = base1 + (size_t)B * kH * F;
     const int tpb = 128;

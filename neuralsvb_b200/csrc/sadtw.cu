@@ -7,7 +7,8 @@
 //   2. cost[i, j] = sum_m 0.5 (b_m - a_m)^2 / (b_m + a_m + 1e-8), a = amateur histogram j, b = professional histogram i, summed
 //      sequentially over m, written in anti-diagonal-major ("skewed") order so the wavefront reads contiguous memory;
 //   3. DTW over the [T, S] matrix: one CTA per pair walks the anti-diagonals with the three live diagonals in shared memory and
-//      writes one direction byte per cell (0 up, 1 left, 2 diagonal: the first minimum in the backtrack's order);
+//      writes one direction byte per cell (0 up, 1 left, 2 diagonal: the first minimum in the backtrack's order).  A longer pair
+//      of svb_sadtw_align_long (min(S, T) > 8192) walks them on a thread-block cluster instead (dtw_cluster_kernel);
 //   4. backtrack: one thread per pair follows the direction bytes from the last cell (align_from_distances).
 // The float DTW matrix never goes to HBM on this path.  Nothing is accumulated across pairs and there are no atomics, so a pair's
 // result does not depend on the batch it is in.
@@ -241,6 +242,7 @@ __global__ void __launch_bounds__(kDtwMaxThreads) dtw_kernel(const T *__restrict
     extern __shared__ __align__(16) unsigned char dtw_smem[];
     const PairMeta p = pairs ? pairs[blockIdx.x] : single;
     const int R = p.R, C = p.C, D = R + C - 1, nt = blockDim.x;
+    if (min(R, C) > maxdiag) return;            // a long pair of svb_sadtw_align_long: dtw_cluster_kernel's
     const T *cp = cost + p.cell_off;
     uint8_t *dp = dirs + p.cell_off;
     T *b2 = reinterpret_cast<T *>(dtw_smem), *b1 = b2 + maxdiag, *b0 = b1 + maxdiag;
@@ -296,6 +298,121 @@ __global__ void __launch_bounds__(kDtwMaxThreads) dtw_kernel(const T *__restrict
     }
 }
 
+// ---- the long-pair DTW: one thread-block cluster per pair ----------------------------------------------------------------------
+// A pair whose anti-diagonal (min(R, C) cells) exceeds one CTA's share runs on a cluster of G <= 8 CTAs.  CTA r owns the diagonal
+// positions c = i - lo(d) in [r W, r W + W) of every diagonal and keeps them of the three live diagonals in its own shared memory.
+// Cell c reads positions c - 1 + (lo(d) - lo(d-1)) and c + (lo(d) - lo(d-1)) of diagonal d - 1 and c - 1 + (lo(d) - lo(d-2)) of
+// d - 2, all in [c - 1, c + 1]: only a CTA's first and last cells (its edges) read a neighbour, through distributed shared
+// memory, and only they are read by one.  Per diagonal a CTA computes its interior cells, waits on the cluster barrier the edges
+// of the previous diagonal arrived on, computes its edges and arrives: the interior hides the barrier.  An edge is written only
+// after that wait, when the neighbours have finished the previous diagonal, the last one that read the slot it overwrites.
+constexpr int kLongMaxLen = 65536;          // frames per take of svb_sadtw_align_long
+constexpr int kMaxCluster = 8;              // the portable cluster size
+constexpr int kLongPerLaunch = 256;         // pairs per cluster launch (their indices travel as a kernel parameter)
+
+struct LongPairs {
+    int32_t idx[kLongPerLaunch];
+};
+
+// a CTA's share of a diagonal of m cells: `cells`, or more when `cells` would need more than 8 CTAs
+__host__ __device__ __forceinline__ int cluster_share(int m, int cells) {
+    return max(cells, (m + kMaxCluster - 1) / kMaxCluster);
+}
+
+__device__ __forceinline__ unsigned cluster_rank() {
+    unsigned r;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return r;
+}
+__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release;" ::: "memory"); }
+__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire;" ::: "memory"); }
+// the float at this CTA's shared address p in the shared memory of cluster CTA `rank`
+__device__ __forceinline__ float ld_cluster(const float *p, unsigned rank) {
+    unsigned a = (unsigned)__cvta_generic_to_shared(p), r;
+    float v;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(a), "r"(rank));
+    asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(r) : "memory");
+    return v;
+}
+
+// grid G x (pairs of the launch), cluster (G, 1, 1): cluster q runs pair list.idx[q] on its first ceil(min(R, C) / W) CTAs
+// (W = cluster_share); the rest hold no cells.  Same cells, directions, tie order and path cost as dtw_kernel<float, false>,
+// bit for bit.
+__global__ void __launch_bounds__(kDtwMaxThreads) dtw_cluster_kernel(const float *__restrict__ cost, const PairMeta *__restrict__ pairs,
+                                                                     LongPairs list, int G, int cells, uint8_t *__restrict__ dirs,
+                                                                     float *__restrict__ path_cost) {
+    extern __shared__ __align__(16) unsigned char dtw_smem[];
+    const int pid = list.idx[blockIdx.x / G];
+    const unsigned rank = cluster_rank();
+    const PairMeta p = pairs[pid];
+    const int R = p.R, C = p.C, D = R + C - 1, nt = blockDim.x, tid = threadIdx.x;
+    const int W = cluster_share(min(R, C), cells), c0 = (int)rank * W, tl = (W - 1) % nt;
+    const float *cp = cost + p.cell_off;
+    uint8_t *dp = dirs + p.cell_off;
+    float *b2 = reinterpret_cast<float *>(dtw_smem), *b1 = b2 + W, *b0 = b1 + W;
+    float nxt[kDtwPer];
+#pragma unroll
+    for (int k = 0; k < kDtwPer; ++k) nxt[k] = (c0 == 0 && tid + k * nt == 0) ? cp[0] : 0.f;
+    cluster_arrive();                           // every CTA of the cluster runs: its shared memory may be read
+    cluster_wait();
+    for (int d = 0; d < D; ++d) {
+        float cur[kDtwPer];
+#pragma unroll
+        for (int k = 0; k < kDtwPer; ++k) cur[k] = nxt[k];
+        const int lo = diag_lo(d, C), n = min(d, R - 1) - lo + 1, nloc = min(W, n - c0);
+        const int64_t start = diag_start(d, R, C);
+        if (d + 1 < D) {
+            const int n1 = min(min(d + 1, R - 1) - diag_lo(d + 1, C) + 1 - c0, W);
+            const int64_t s1 = start + n + c0;
+#pragma unroll
+            for (int k = 0; k < kDtwPer; ++k) {
+                const int c = tid + k * nt;
+                if (c < n1) nxt[k] = cp[s1 + c];
+            }
+        }
+        const int lo1 = diag_lo(d - 1, C), lo2 = diag_lo(d - 2, C);
+        // local cell c (global position c0 + c) from its cost; an edge may read a neighbour's cells
+        auto cell = [&](int c, float cv, bool edge) {
+            const int i = lo + c0 + c, j = d - i;
+            float v;
+            if (i == 0 || j == 0) {
+                v = (i == 0 && j == 0) ? 0.f : inf_of<float>();
+            } else {
+                const int lu = i - 1 - lo1 - c0, ll = i - lo1 - c0, lg = i - 1 - lo2 - c0;
+                auto at = [&](const float *b, int l) {
+                    return l < 0 ? ld_cluster(b + l + W, rank - 1) : l >= W ? ld_cluster(b + l - W, rank + 1) : b[l];
+                };
+                const float up = edge ? at(b1, lu) : b1[lu], left = edge ? at(b1, ll) : b1[ll], dg = edge ? at(b2, lg) : b2[lg];
+                float m = up;
+                uint8_t dir = 0;
+                if (left < m) m = left, dir = 1;
+                if (dg < m) m = dg, dir = 2;
+                v = add_rn(cv, m);
+                dp[start + c0 + c] = dir;
+            }
+            b0[c] = v;
+            if (i == R - 1 && j == C - 1 && path_cost) path_cost[pid] = v;
+        };
+        float e0 = 0.f, el = 0.f;
+#pragma unroll
+        for (int k = 0; k < kDtwPer; ++k) {
+            const int c = tid + k * nt;
+            if (c >= nloc) break;
+            if (c == 0) e0 = cur[k];
+            else if (c == W - 1) el = cur[k];
+            else cell(c, cur[k], false);
+        }
+        if (d > 0) cluster_wait();              // the neighbours' edges of diagonal d - 1
+        if (tid == 0 && nloc > 0) cell(0, e0, true);
+        if (W > 1 && tid == tl && nloc > W - 1) cell(W - 1, el, true);
+        cluster_arrive();
+        __syncthreads();
+        float *t = b2;
+        b2 = b1, b1 = b0, b0 = t;
+    }
+    cluster_wait();                             // no CTA leaves while a neighbour may still read its shared memory
+}
+
 // one thread per pair: align_from_distances.  results[i] = j while i > 0 and j > 0, then the first minimum of up, left, diagonal
 // (the direction byte); rows the walk never reached stay 0.
 __global__ void backtrack_kernel(const uint8_t *__restrict__ dirs, const PairMeta *__restrict__ pairs, PairMeta single, int n_pairs,
@@ -346,16 +463,22 @@ struct Layout {
     int64_t rows_src, rows_tgt, cells;
 };
 
-int sadtw_layout(int32_t n, const int32_t *src_len, const int32_t *tgt_len, Layout &L) {
+// long_pairs: svb_sadtw_align_long's bound (each take at most kLongMaxLen frames) instead of the one-CTA kernel's anti-diagonal
+int sadtw_layout(int32_t n, const int32_t *src_len, const int32_t *tgt_len, bool long_pairs, Layout &L) {
     SVB_CHECK(n > 0 && n <= kMaxPairs, SVB_ERR_INVALID, "sadtw: %d pairs (1 .. %d)", n, kMaxPairs);
     SVB_CHECK(src_len && tgt_len, SVB_ERR_INVALID, "sadtw: null length array");
     L.rows_src = L.rows_tgt = L.cells = 0;
     for (int p = 0; p < n; ++p) {
         SVB_CHECK(src_len[p] >= 2 && tgt_len[p] >= 2, SVB_ERR_INVALID,
                   "sadtw: pair %d has %d amateur and %d professional frames (at least 2 each are needed)", p, src_len[p], tgt_len[p]);
-        SVB_CHECK(std::min(src_len[p], tgt_len[p]) <= kMaxDiag, SVB_ERR_INVALID,
-                  "sadtw: pair %d: min(%d, %d) frames exceeds the %d-cell anti-diagonal of the DTW kernel", p, src_len[p], tgt_len[p],
-                  kMaxDiag);
+        if (long_pairs)
+            SVB_CHECK(std::max(src_len[p], tgt_len[p]) <= kLongMaxLen, SVB_ERR_INVALID,
+                      "sadtw_long: pair %d has %d amateur and %d professional frames: at most %d each", p, src_len[p], tgt_len[p],
+                      kLongMaxLen);
+        else
+            SVB_CHECK(std::min(src_len[p], tgt_len[p]) <= kMaxDiag, SVB_ERR_INVALID,
+                      "sadtw: pair %d: min(%d, %d) frames exceeds the %d-cell anti-diagonal of the DTW kernel", p, src_len[p],
+                      tgt_len[p], kMaxDiag);
         L.rows_src += src_len[p], L.rows_tgt += tgt_len[p], L.cells += (int64_t)src_len[p] * tgt_len[p];
     }
     L.off[0] = 0;
@@ -392,34 +515,73 @@ struct StageTimer {
     }
 };
 
-}  // namespace
-
-extern "C" int64_t svb_sadtw_workspace_bytes(int32_t n_pairs, const int32_t *src_len_host, const int32_t *tgt_len_host,
-                                             int64_t *offsets_host) {
-    Layout L;
-    if (sadtw_layout(n_pairs, src_len_host, tgt_len_host, L) != SVB_OK) return -1;
-    if (offsets_host)
-        for (int k = 0; k < 5; ++k) offsets_host[k] = (int64_t)L.off[k];
-    return (int64_t)L.total;
+// a cluster CTA's share of a diagonal: kMaxDiag, or SVB_DTW_CTA_CELLS (read per call; a test and measurement hook that puts
+// shorter pairs on clusters)
+int cta_cells(int &cells) {
+    cells = kMaxDiag;
+    if (const char *e = getenv("SVB_DTW_CTA_CELLS")) {
+        cells = atoi(e);
+        SVB_CHECK(cells >= 1 && cells <= kMaxDiag, SVB_ERR_INVALID, "sadtw_long: SVB_DTW_CTA_CELLS=%s (1 .. %d)", e, kMaxDiag);
+    }
+    return SVB_OK;
 }
 
-extern "C" int svb_sadtw_align(const void *src_f0_dev, const void *tgt_f0_dev, int32_t dtype, int32_t variant, int32_t n_pairs,
-                               const int32_t *src_len_host, const int32_t *tgt_len_host, const double *tgt_scale_host,
-                               void *workspace_dev, int64_t workspace_bytes, int64_t *alignment_dev, float *path_cost_dev,
-                               float *stage_ms_host, void *stream) {
+int cluster_ctas(int m, int cells) { const int w = cluster_share(m, cells); return (m + w - 1) / w; }
+
+// the pairs whose anti-diagonal exceeds `cells`, all at one cluster size (per kLongPerLaunch pairs), so that pairs needing
+// different cluster sizes run at the same time: the launch's G is the largest a pair needs, and a pair keeps its own share
+// (cluster_share), its CTAs past ceil(min(R, C) / share) holding no cells and only taking part in the barriers
+int launch_dtw_cluster(const float *cost, const PairMeta *d_pairs, const std::vector<PairMeta> &pairs, int cells, uint8_t *dirs,
+                       float *path_cost, cudaStream_t st) {
+    std::vector<int> ids;
+    for (int p = 0; p < (int)pairs.size(); ++p)
+        if (std::min(pairs[p].R, pairs[p].C) > cells) ids.push_back(p);
+    for (size_t q0 = 0; q0 < ids.size(); q0 += kLongPerLaunch) {
+        const int cnt = (int)std::min<size_t>(kLongPerLaunch, ids.size() - q0);
+        LongPairs list{};
+        int maxw = 0, G = 0;
+        for (int q = 0; q < cnt; ++q) {
+            const int m = std::min(pairs[ids[q0 + q]].R, pairs[ids[q0 + q]].C);
+            list.idx[q] = ids[q0 + q];
+            maxw = std::max(maxw, cluster_share(m, cells));
+            G = std::max(G, cluster_ctas(m, cells));
+        }
+        const size_t smem = (size_t)3 * maxw * sizeof(float);
+        static size_t configured[kSmemCacheDevices] = {};
+        SVB_TRY(raise_smem_limit(dtw_cluster_kernel, smem, configured));
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3((unsigned)(G * cnt)), cfg.blockDim = dim3(dtw_threads(maxw)), cfg.dynamicSmemBytes = smem;
+        cfg.stream = st;
+        cudaLaunchAttribute attr[1];
+        attr[0].id = cudaLaunchAttributeClusterDimension;
+        attr[0].val.clusterDim.x = G, attr[0].val.clusterDim.y = 1, attr[0].val.clusterDim.z = 1;
+        cfg.attrs = attr, cfg.numAttrs = 1;
+        SVB_CUDA(cudaLaunchKernelEx(&cfg, dtw_cluster_kernel, cost, d_pairs, list, G, cells, dirs, path_cost));
+    }
+    return SVB_OK;
+}
+
+// svb_sadtw_align and svb_sadtw_align_long: one validation, layout, histogram, cost and backtrack; long_pairs sends the pairs
+// whose anti-diagonal exceeds a CTA's share to dtw_cluster_kernel and the rest to dtw_kernel
+int sadtw_run(const void *src_f0_dev, const void *tgt_f0_dev, int32_t dtype, int32_t variant, int32_t n_pairs, const int32_t *src_len_host,
+              const int32_t *tgt_len_host, const double *tgt_scale_host, void *workspace_dev, int64_t workspace_bytes,
+              int64_t *alignment_dev, float *path_cost_dev, float *stage_ms_host, bool long_pairs, void *stream) {
     SVB_CHECK(src_f0_dev && tgt_f0_dev && workspace_dev && alignment_dev, SVB_ERR_INVALID, "sadtw: null argument");
     SVB_CHECK(dtype == SVB_SADTW_F32 || dtype == SVB_SADTW_F64, SVB_ERR_INVALID, "sadtw: bad f0 dtype %d", dtype);
     SVB_CHECK(variant == SVB_SADTW || variant == SVB_EHSADTW, SVB_ERR_INVALID, "sadtw: bad variant %d", variant);
     Layout L;
-    SVB_TRY(sadtw_layout(n_pairs, src_len_host, tgt_len_host, L));
+    SVB_TRY(sadtw_layout(n_pairs, src_len_host, tgt_len_host, long_pairs, L));
     SVB_CHECK(workspace_bytes >= (int64_t)L.total, SVB_ERR_INVALID, "sadtw: workspace of %lld bytes, %lld needed",
               (long long)workspace_bytes, (long long)L.total);
+    int share = kMaxDiag;
+    if (long_pairs) SVB_TRY(cta_cells(share));
     const int n = n_pairs;
     std::vector<SeqMeta> seqs(2 * (size_t)n);
     std::vector<PairMeta> pairs(n);
     int64_t fs = 0, ft = 0, cells = 0;
     int maxlen = 0, maxdiag = 0;
     int64_t maxtiles = 0;
+    bool has_long = false;
     for (int p = 0; p < n; ++p) {
         const int S = src_len_host[p], T = tgt_len_host[p];
         const double scale = tgt_scale_host ? tgt_scale_host[p] : (double)T / (double)S;
@@ -428,7 +590,8 @@ extern "C" int svb_sadtw_align(const void *src_f0_dev, const void *tgt_f0_dev, i
         pairs[p] = PairMeta{fs, L.rows_src + ft, cells, ft, T, S};
         fs += S, ft += T, cells += (int64_t)S * T;
         maxlen = std::max(maxlen, std::max(S, T));
-        maxdiag = std::max(maxdiag, std::min(S, T));
+        if (std::min(S, T) <= share) maxdiag = std::max(maxdiag, std::min(S, T));
+        else has_long = true;
         maxtiles = std::max(maxtiles, (int64_t)((S + kTileJ - 1) / kTileJ) * ((T + kTileI - 1) / kTileI));
     }
     // everything is validated: from here on, launches
@@ -458,12 +621,49 @@ extern "C" int svb_sadtw_align(const void *src_f0_dev, const void *tgt_f0_dev, i
     sadtw_cost_kernel<<<cgrid, kCostThreads, 0, st>>>(d_hist, d_pairs, d_cost);
     SVB_CUDA(cudaGetLastError());
     SVB_TRY(tm.mark(2, st));
-    SVB_TRY(launch_dtw<float>(d_cost, d_pairs, PairMeta{}, n, maxdiag, d_dirs, path_cost_dev, nullptr, st));
+    if (has_long) SVB_TRY(launch_dtw_cluster(d_cost, d_pairs, pairs, share, d_dirs, path_cost_dev, st));
+    if (maxdiag > 0) SVB_TRY(launch_dtw<float>(d_cost, d_pairs, PairMeta{}, n, maxdiag, d_dirs, path_cost_dev, nullptr, st));
     SVB_TRY(tm.mark(3, st));
     backtrack_kernel<<<(n + 127) / 128, 128, 0, st>>>(d_dirs, d_pairs, PairMeta{}, n, alignment_dev);
     SVB_CUDA(cudaGetLastError());
     SVB_TRY(tm.mark(4, st));
     return tm.read(stage_ms_host);
+}
+
+}  // namespace
+
+extern "C" int64_t svb_sadtw_workspace_bytes(int32_t n_pairs, const int32_t *src_len_host, const int32_t *tgt_len_host,
+                                             int64_t *offsets_host) {
+    Layout L;
+    if (sadtw_layout(n_pairs, src_len_host, tgt_len_host, false, L) != SVB_OK) return -1;
+    if (offsets_host)
+        for (int k = 0; k < 5; ++k) offsets_host[k] = (int64_t)L.off[k];
+    return (int64_t)L.total;
+}
+
+extern "C" int svb_sadtw_align(const void *src_f0_dev, const void *tgt_f0_dev, int32_t dtype, int32_t variant, int32_t n_pairs,
+                               const int32_t *src_len_host, const int32_t *tgt_len_host, const double *tgt_scale_host,
+                               void *workspace_dev, int64_t workspace_bytes, int64_t *alignment_dev, float *path_cost_dev,
+                               float *stage_ms_host, void *stream) {
+    return sadtw_run(src_f0_dev, tgt_f0_dev, dtype, variant, n_pairs, src_len_host, tgt_len_host, tgt_scale_host, workspace_dev,
+                     workspace_bytes, alignment_dev, path_cost_dev, stage_ms_host, false, stream);
+}
+
+extern "C" int64_t svb_sadtw_long_workspace_bytes(int32_t n_pairs, const int32_t *src_len_host, const int32_t *tgt_len_host,
+                                                  int64_t *offsets_host) {
+    Layout L;
+    if (sadtw_layout(n_pairs, src_len_host, tgt_len_host, true, L) != SVB_OK) return -1;
+    if (offsets_host)
+        for (int k = 0; k < 5; ++k) offsets_host[k] = (int64_t)L.off[k];
+    return (int64_t)L.total;
+}
+
+extern "C" int svb_sadtw_align_long(const void *src_f0_dev, const void *tgt_f0_dev, int32_t dtype, int32_t variant, int32_t n_pairs,
+                                    const int32_t *src_len_host, const int32_t *tgt_len_host, const double *tgt_scale_host,
+                                    void *workspace_dev, int64_t workspace_bytes, int64_t *alignment_dev, float *path_cost_dev,
+                                    float *stage_ms_host, void *stream) {
+    return sadtw_run(src_f0_dev, tgt_f0_dev, dtype, variant, n_pairs, src_len_host, tgt_len_host, tgt_scale_host, workspace_dev,
+                     workspace_bytes, alignment_dev, path_cost_dev, stage_ms_host, true, stream);
 }
 
 extern "C" int64_t svb_sadtw_histogram_workspace_bytes(int32_t n_seq) {

@@ -17,8 +17,11 @@ pair's a2p mel depends on the batch it is in and can differ from the same pair b
 (batch size 1) computes.  Beautify one pair per call to get exactly that.  Every other stage is per pair: bit-identical alone and
 in any batch.
 
+``beautify_songs`` takes whole songs (up to 65536 frames a take): each song is aligned whole, run through the model in
+overlapping segments of at most max_frames and vocoded whole from the stitched mel.
+
 ``python -m neuralsvb_b200.inference.beautify --config C --exp_name X [--hparams ...] --amateur a.wav ... --prof p.wav ...
---spk_emb e.npy ... --out o.wav ...`` writes one file per pair."""
+--spk_emb e.npy ... --out o.wav ... [--song]`` writes one file per pair."""
 import argparse
 import os
 
@@ -27,15 +30,19 @@ import torch
 
 from neuralsvb_b200.data_gen.tts.data_gen_utils import pitch_ac_device, pitch_frames
 from neuralsvb_b200.modules.fastspeech.fs2_vae import check_frames
-from neuralsvb_b200.tasks.singing.dataset_utils import clip_alignment, cropped_frames, take_conditioning
+from neuralsvb_b200.inference.song_plan import plan_song, segment_sizes, stitch_mels
+from neuralsvb_b200.modules.voice_conversion.dtw.core import LONG_MAX_FRAMES
+from neuralsvb_b200.tasks.singing.dataset_utils import clip_alignment, cropped_frames, normalized_take_f0, take_conditioning
 from neuralsvb_b200.utils import audio, collate_1d
 from neuralsvb_b200.utils.ckpt_utils import get_all_ckpts
 from neuralsvb_b200.utils.hparams import hparams, set_hparams
-from neuralsvb_b200.utils.pitch_utils import denorm_f0, f0_to_coarse
+from neuralsvb_b200.utils.pitch_utils import denorm_f0, f0_to_coarse, norm_interp_f0
 
 WAYS = ('a2a', 'p2p', 'a2p')
 ALIGN_METHOD = 'EHSADTW'
 EMB_DIM = 256
+SONG_ALIGN_BYTES = 24 << 30     # beautify_songs aligns consecutive songs together up to this much DTW workspace (one at the limit)
+SONG_VOCODE_FRAMES = 1 << 17    # and vocodes them together up to this many padded frames (songs x the longest professional take)
 
 
 def newest_checkpoint(work_dir):
@@ -102,7 +109,10 @@ class _Stages:
         if not self.on:
             return None
         torch.cuda.synchronize()
-        return {n: a.elapsed_time(b) for (n, a), (_, b) in zip(self.marks[:-1], self.marks[1:])}
+        out = {}
+        for (n, a), (_, b) in zip(self.marks[:-1], self.marks[1:]):
+            out[n] = out.get(n, 0.0) + a.elapsed_time(b)         # a stage marked more than once: its total
+        return out
 
 
 class SVBBeautifier:
@@ -136,9 +146,9 @@ class SVBBeautifier:
         self.timing, self.stage_ms = False, None
 
     # ------------------------------------------------------------------ host checks
-    def _takes(self, amateur, professional, spk_emb):
+    def _takes(self, amateur, professional, spk_emb, songs=False):
         """Decoded takes (B amateur, then B professional), their lengths at audio_sample_rate and mel frame counts, and the B
-        embeddings; every pair checked before any device work."""
+        embeddings; every pair checked before any device work.  songs: takes up to LONG_MAX_FRAMES instead of max_frames."""
         from neuralsvb_b200.vocoders.hifigan import decode_wavs
         amateur, professional, spk_emb = list(amateur), list(professional), list(spk_emb)
         B = len(amateur)
@@ -159,10 +169,13 @@ class SVBBeautifier:
             lens[off] = audio.resample_lengths(lens[off], [rates[k] for k in off], sr)[1]
         frames = lens // hop + 1
         for k in range(2 * B):
-            what = f'pair {k % B}: the {"amateur" if k < B else "professional"} take'
-            if frames[k] > hp['max_frames']:
+            what = f'{"song" if songs else "pair"} {k % B}: the {"amateur" if k < B else "professional"} take'
+            if songs and frames[k] > LONG_MAX_FRAMES:
+                raise ValueError(f'{what} has {frames[k]} frames, more than the {LONG_MAX_FRAMES} a song may have '
+                                 f'({LONG_MAX_FRAMES * hop / sr:.1f} s)')
+            if not songs and frames[k] > hp['max_frames']:
                 raise ValueError(f'{what} has {frames[k]} frames, more than max_frames = {hp["max_frames"]} '
-                                 f'({hp["max_frames"] * hop / sr:.1f} s); split the song first')
+                                 f'({hp["max_frames"] * hop / sr:.1f} s); beautify_songs takes whole songs')
             if pitch_frames(frames[k] * hop, hp) < 1:
                 raise ValueError(f'{what} is shorter than one pitch window')
             try:
@@ -208,24 +221,31 @@ class SVBBeautifier:
         """MleSVBVAE on the collated batch -> a2p mel_out [B, max Tp, n_mel] (device)."""
         B = len(Ta)
         offs = np.concatenate([[0], np.cumsum(frames)])
+        return self._model_on(sample, mel, offs[:B], offs[B:2 * B], Ta, Tp, eps)
+
+    def _model_on(self, sample, mel, a_rows, p_rows, Ta, Tp, eps):
+        """MleSVBVAE on the collated batch whose amateur take b is mel rows [a_rows[b], a_rows[b] + Ta[b]) and professional take
+        b rows [p_rows[b], p_rows[b] + Tp[b]) -> a2p mel_out [B, max Tp, n_mel] (device)."""
+        B = len(Ta)
         d = self.device
 
-        def pad(takes, T):
+        def pad(rows, T):
             x = torch.zeros(B, max(T), mel.shape[1], device=d)
-            for b, (k, t) in enumerate(zip(takes, T)):
-                x[b, :t] = mel[offs[k]:offs[k] + t]
+            for b, (r, t) in enumerate(zip(rows, T)):
+                x[b, :t] = mel[int(r):int(r) + t]
             return x
-        out = self.model(amateur_mel=pad(range(B), Ta), prof_mel=pad(range(B, 2 * B), Tp), amateur_pitch=sample['pitch'].to(d),
+        out = self.model(amateur_mel=pad(a_rows, Ta), prof_mel=pad(p_rows, Tp), amateur_pitch=sample['pitch'].to(d),
                          prof_pitch=sample['prof_pitch'].to(d), amateur_spk_id=sample['spk'].to(d), prof_spk_id=sample['spk'].to(d),
                          a2p_alignment=sample['a2p_f0_alignment'].to(d), infer=False, concurrent_ways=list(WAYS),
                          disable_map=self.hp['disable_map'], eps=eps)
         return out['a2p']['mel_out']
 
-    def _vocode(self, mel_out, f0, Tp, seed):
+    def _vocode(self, mel_out, f0, Tp, seed, first_clip=0):
         """The ragged generator at the professional frame counts, the denoise post-filter per clip when vocoder_denoise_c > 0
-        -> device waveforms back to back."""
+        -> device waveforms back to back.  Clip b's NSF draws are keyed by (seed, first_clip + b)."""
         hop = int(self.hp['hop_size'])
-        y = self.vocoder.model(mel_out.transpose(1, 2).contiguous(), f0=f0.to(self.device), seed=seed, lengths=Tp)
+        y = self.vocoder.model(mel_out.transpose(1, 2).contiguous(), f0=f0.to(self.device), seed=seed, lengths=Tp,
+                               first_clip=first_clip)
         clips = [y[b, 0, :t * hop] for b, t in enumerate(Tp)]
         v = self.hp.get('vocoder_denoise_c', 0.0)
         if v > 0:
@@ -254,6 +274,126 @@ class SVBBeautifier:
     def beautify(self, amateur, professional, spk_emb, **kw):
         """``beautify_batch`` of one pair -> one float32 array."""
         return self.beautify_batch([amateur], [professional], [spk_emb], **kw)[0]
+
+    def beautify_songs(self, amateur, professional, spk_emb, seed=None, eps=None, segment_frames=None, overlap_frames=64):
+        """The a2p take of whole songs: ``beautify_batch``'s inputs, with each take up to LONG_MAX_FRAMES frames (6.3 min at
+        22.05 kHz / hop 128) instead of max_frames.  Returns one float32 array of Tp x hop samples per song, Tp the professional
+        frame count cropped to a multiple of frames_multiple.
+
+        Each song is aligned whole (align_long, EHSADTW on the device f0 in float64), cut by ``plan_song`` into professional
+        segments of at most ``segment_frames`` (default max_frames) overlapping by ``overlap_frames``, each with the amateur slice
+        its alignment reads; the segments are conditioned by ``condition()``'s rules on their slices of the whole takes' f0 and
+        pitch ids, with alignment a2p[s:e] - a_lo.  MleSVBVAE runs once per song on that song's segments as one batch, with the
+        song's embedding and eps[b] repeated, so a song's result does not depend on the other songs of the call.  The a2p mels
+        are stitched with a linear cross-fade over each overlap (``stitch_mels``) and the songs vocoded whole in one ragged
+        generator call per group, with the whole professional take's f0.
+
+        With ``normalize_pitch`` each take is normalised once over the whole take and then sliced: one key for the song, where
+        per-clip conditioning would move every segment to the statistics on its own.  A song that fits one segment (Tp <=
+        segment_frames and Ta <= max_frames) gives exactly ``beautify`` of the pair with the same seed and eps.
+
+        ``seed`` keys the NSF draws by (seed, song index) as spec2wav_batch does, however the songs are grouped for the vocoder
+        (consecutive songs up to SONG_VOCODE_FRAMES padded frames per generator call), and draws eps [n_songs, latent, 1]
+        unless given.  Bad segment_frames / overlap_frames raise before any device work; every song is checked and planned
+        before the model runs: a bad take, a take over LONG_MAX_FRAMES or a song that cannot be planned raises ValueError naming
+        the song."""
+        with torch.no_grad(), torch.cuda.device(self.device):
+            return self._run_songs(amateur, professional, spk_emb, seed, eps, segment_frames, overlap_frames)
+
+    def _song_conditioning(self, frames, f0s, B):
+        """Per take (B amateur, then B professional): the cropped frame count, the f0 the segments are conditioned on (moved by
+        normalize_pitch over the whole take) and its pitch ids."""
+        hp, fm = self.hp, int(self.hp['frames_multiple'])
+        out = []
+        for k, f in enumerate(f0s):
+            if hp.get('normalize_pitch', False):
+                f = normalized_take_f0(f, hp, 500 if k < B else 900)
+            out.append((int(frames[k]) // fm * fm, f, f0_to_coarse(f)))
+        return out
+
+    def _align_songs(self, f0_dev, frames, st):
+        """EHSADTW of every song on the device f0 (float64, as _align), consecutive songs together up to SONG_ALIGN_BYTES of
+        workspace -> host int64 alignments.  With timing on, align_ms holds each group's (histogram, cost, DTW, backtrack) times."""
+        from neuralsvb_b200.modules.voice_conversion.dtw.core import align_long, long_workspace_bytes
+        B = len(frames) // 2
+        ws = [long_workspace_bytes([int(frames[b])], [int(frames[B + b])]) for b in range(B)]
+        t = torch.split(f0_dev.double(), [int(x) for x in frames])
+        aligns, self.align_ms = [], []
+        for g0, g1 in _groups(ws, SONG_ALIGN_BYTES):
+            st.mark('alignment')
+            r = align_long(list(t[g0:g1]), list(t[B + g0:B + g1]), ALIGN_METHOD, stage_ms=self.timing)
+            aligns += r.split()
+            if self.timing:
+                self.align_ms.append(r.stage_ms)
+        return aligns
+
+    def _run_songs(self, amateur, professional, spk_emb, seed, eps, segment_frames, overlap_frames):
+        hp = self.hp
+        segment_sizes(hp, segment_frames, overlap_frames, 'beautify_songs')         # before any device work
+        dec, rates, lens, frames, spk = self._takes(amateur, professional, spk_emb, songs=True)
+        B = len(spk)
+        if eps is not None:
+            eps = torch.as_tensor(eps, dtype=torch.float32)
+            if tuple(eps.shape) != (B, hp['latent_size'], 1):
+                raise ValueError(f'eps must be [{B}, {hp["latent_size"]}, 1], got {tuple(eps.shape)}')
+        st = _Stages(self.timing)
+        st.mark('h2d')
+        mel, wav = self._front_end(dec, rates, lens, st)
+        st.mark('pitch')
+        f0_dev, f0s = self._pitch(wav, frames)
+        for k, f in enumerate(f0s):
+            if sum(f) == 0:
+                raise ValueError(f'song {k % B}: the {"amateur" if k < B else "professional"} take has no voiced f0 '
+                                 '(the alignment is undefined)')
+        aligns = self._align_songs(f0_dev, frames, st)
+        torch.cuda.empty_cache()        # the DTW workspace's cached blocks: the generator allocates its workspace outside torch
+        st.mark('plan_conditioning')
+        takes = self._song_conditioning(frames, f0s, B)
+        hp_seg = dict(hp, normalize_pitch=False)        # the segments' f0 is already the whole take's normalised one
+        songs = []
+        for b in range(B):
+            (Ta, fa, pa), (Tp, fp, pp) = takes[b], takes[B + b]
+            a2p = clip_alignment(aligns[b], Tp, Ta).numpy()
+            pf0, puv = norm_interp_f0(fp[:Tp], hp)
+            plan = plan_song(Tp, Ta, a2p, puv.numpy(), hp, segment_frames, overlap_frames, name=f'song {b}')
+            K = len(plan)
+            sample, sa, sp = condition([a1 - a0 for _, _, a0, a1 in plan] + [e - s for s, e, _, _ in plan],
+                                       [fa[a0:a1] for _, _, a0, a1 in plan] + [fp[s:e] for s, e, _, _ in plan],
+                                       [pa[a0:a1] for _, _, a0, a1 in plan] + [pp[s:e] for s, e, _, _ in plan],
+                                       [a2p[s:e] - a0 for s, e, a0, _ in plan], [spk[b]] * K, hp_seg)
+            songs.append((plan, sample, sa, sp, denorm_f0(pf0, puv, hp)))
+        if seed is None:
+            self.vocoder.model.seed += 1
+            seed = self.vocoder.model.seed
+        if eps is None:
+            eps = torch.randn(B, hp['latent_size'], 1, device=self.device, generator=torch.Generator(self.device).manual_seed(seed))
+        eps = eps.to(self.device)
+        offs = np.concatenate([[0], np.cumsum(frames)])
+        song_mels = []
+        for b, (plan, sample, sa, sp, _) in enumerate(songs):
+            st.mark('acoustic_model')
+            K = len(plan)
+            out = self._model_on(sample, mel, [offs[b] + a0 for _, _, a0, _ in plan], [offs[B + b] + s for s, _, _, _ in plan],
+                                 sa, sp, eps[b:b + 1].expand(K, -1, -1).contiguous())
+            st.mark('stitch')
+            song_mels.append(stitch_mels([out[k] for k in range(K)], plan, overlap_frames))
+        clips = []
+        Tps = [songs[b][0][-1][1] for b in range(B)]
+        for g0, g1 in _groups([1] * B, SONG_VOCODE_FRAMES, lambda a, b: (b - a) * max(Tps[a:b])):
+            st.mark('vocoder')
+            x = torch.zeros(g1 - g0, max(Tps[g0:g1]), mel.shape[1], device=self.device)
+            f0 = torch.zeros(g1 - g0, max(Tps[g0:g1]))
+            for q, b in enumerate(range(g0, g1)):
+                x[q, :Tps[b]] = song_mels[b]
+                f0[q, :Tps[b]] = songs[b][4]
+            clips.append(self._vocode(x, f0, Tps[g0:g1], seed, first_clip=g0))
+        st.mark('d2h')
+        out = torch.cat(clips).cpu().numpy()
+        st.mark('end')
+        self.stage_ms = st.ms()
+        self.song_mels, self.song_plans = song_mels, [s[0] for s in songs]
+        hop = int(hp['hop_size'])
+        return np.split(out, np.cumsum([t * hop for t in Tps])[:-1])
 
     def _run(self, amateur, professional, spk_emb, seed, eps):
         hp = self.hp
@@ -294,6 +434,18 @@ class SVBBeautifier:
         return np.split(out, np.cumsum([t * hop for t in Tp])[:-1])
 
 
+def _groups(sizes, limit, size_of=None):
+    """Consecutive [g0, g1) ranges of items whose size (size_of(g0, g1), default the sum of sizes) stays within limit; an item
+    over the limit alone is a group."""
+    size_of = size_of or (lambda a, b: sum(sizes[a:b]))
+    out, g0 = [], 0
+    for g1 in range(1, len(sizes) + 1):
+        if g1 - g0 > 1 and size_of(g0, g1) > limit:
+            out.append((g0, g1 - 1))
+            g0 = g1 - 1
+    return out + [(g0, len(sizes))]
+
+
 def parse_args(argv=None):
     p = argparse.ArgumentParser(description='Beautify amateur singing with an SVB experiment: one output WAV per '
                                             '(amateur, professional, embedding) triple.')
@@ -304,6 +456,8 @@ def parse_args(argv=None):
     p.add_argument('--prof', nargs='+', required=True)
     p.add_argument('--spk_emb', nargs='+', required=True)
     p.add_argument('--out', nargs='+', required=True)
+    p.add_argument('--song', action='store_true', help='whole songs (beautify_songs): takes longer than max_frames are aligned '
+                                                       'whole, run through the model in overlapping segments and vocoded whole')
     args = p.parse_args(argv)
     counts = {k: len(getattr(args, k)) for k in ('amateur', 'prof', 'spk_emb', 'out')}
     if len(set(counts.values())) != 1:
@@ -318,7 +472,7 @@ def main(argv=None):
     hp = set_hparams(config=args.config, exp_name=args.exp_name, hparams_str=args.hparams, print_hparams=False)
     hp['infer'] = True
     b = SVBBeautifier(work_dir, hp=hparams)
-    wavs = b.beautify_batch(args.amateur, args.prof, args.spk_emb)
+    wavs = (b.beautify_songs if args.song else b.beautify_batch)(args.amateur, args.prof, args.spk_emb)
     for w, fn in zip(wavs, args.out):
         if os.path.dirname(fn):
             os.makedirs(os.path.dirname(fn), exist_ok=True)

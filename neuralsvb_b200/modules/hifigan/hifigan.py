@@ -174,14 +174,15 @@ class HifiGanGenerator(nn.Module):
         self._drop_handle()
         return r
 
-    def forward(self, x, f0=None, rand_ini=None, noise=None, seed=None, lengths=None):
+    def forward(self, x, f0=None, rand_ini=None, noise=None, seed=None, lengths=None, first_clip=0):
         """x [B, n_mel, T] fp32 on a CUDA device, f0 [B, T] Hz or None -> [B, 1, T*hop].
         ``rand_ini`` [B,9] / ``noise`` [B,T*hop,9] inject the NSF source's random draws
         (parity testing); otherwise they are drawn in-kernel from ``seed``.
 
         ``lengths`` (host sequence of B ints, 1 <= lengths[b] <= T): a ragged batch, inference only.  Clip b is vocoded as
         if it were run alone on its first lengths[b] frames (svb_gen_forward_ragged); its frames past that are never read and
-        its samples from lengths[b] * hop on are 0.
+        its samples from lengths[b] * hop on are 0.  ``first_clip`` (ragged batches only): the in-kernel draws of clip b are keyed
+        by clip index first_clip + b, so a batch vocoded in several calls draws what one call over all of it would.
 
         In ``train()`` mode with grad enabled the result carries a grad_fn: ``backward`` runs
         ``svb_gen_backward`` (native data / weight gradients) and hands every parameter its gradient
@@ -196,14 +197,16 @@ class HifiGanGenerator(nn.Module):
         if seed is None:
             self.seed += 1
             seed = self.seed
+        if first_clip and lengths is None:
+            raise ValueError('HifiGanGenerator.forward: first_clip applies to ragged batches (lengths=...) only')
         if lengths is not None:
-            return self._run_forward(x, f0, rand_ini, noise, seed, train=False, lengths=lengths)
+            return self._run_forward(x, f0, rand_ini, noise, seed, train=False, lengths=lengths, first_clip=first_clip)
         if train:
             entries = self._param_entries()
             return _GenTrainFn.apply(self, x, f0, rand_ini, noise, seed, *[p for e in entries for p in e[2]])
         return self._run_forward(x, f0, rand_ini, noise, seed, train=False)
 
-    def _run_forward(self, x, f0, rand_ini, noise, seed, train, lengths=None):
+    def _run_forward(self, x, f0, rand_ini, noise, seed, train, lengths=None, first_clip=0):
         lib = _native.lib()
         B, C, T = x.shape
         if lengths is not None:
@@ -223,9 +226,10 @@ class HifiGanGenerator(nn.Module):
         with torch.cuda.device(x.device):
             st = _native.current_stream_ptr(x.device)
             if lengths is not None:
-                _native.check(lib.svb_gen_forward_ragged(g, _native.ptr(x), _native.ptr(f0), _native.ptr(ri), _native.ptr(nz),
-                                                         ctypes.c_uint64(seed), B, T, lengths.ctypes.data_as(ctypes.c_void_p),
-                                                         _native.ptr(y), st), 'gen_forward_ragged')
+                _native.check(lib.svb_gen_forward_ragged_from(g, _native.ptr(x), _native.ptr(f0), _native.ptr(ri), _native.ptr(nz),
+                                                              ctypes.c_uint64(seed), int(first_clip), B, T,
+                                                              lengths.ctypes.data_as(ctypes.c_void_p), _native.ptr(y), st),
+                              'gen_forward_ragged')
             else:
                 _native.check(lib.svb_gen_forward(g, _native.ptr(x), _native.ptr(f0), _native.ptr(ri), _native.ptr(nz),
                                                   ctypes.c_uint64(seed), B, T, _native.ptr(y), st), 'gen_forward')

@@ -103,6 +103,33 @@ def align_batch(srcs, tgts, method='EHSADTW', scales=None, stage_ms=False, keep_
     methods (BASELINES) go to baseline_batch."""
     if method in BASELINES:
         return baseline_batch(srcs, tgts, method, stage_ms)
+    return _sadtw(srcs, tgts, method, scales, stage_ms, keep_workspace, 'sadtw')
+
+
+LONG_MAX_FRAMES = 65536
+
+
+def align_long(srcs, tgts, method='EHSADTW', scales=None, stage_ms=False, keep_workspace=False):
+    """align_batch for whole songs: each take of a pair up to LONG_MAX_FRAMES frames (6.3 min at 22.05 kHz / hop 128).  A pair
+    whose shorter take exceeds 8192 frames runs its DTW on a thread-block cluster; the others on the one-CTA kernel of
+    align_batch, in the same call.  Same results as align_batch on any pair both accept.  The workspace holds every pair's cost
+    matrix (5 bytes per cell: 8.5 GB for a 4-minute pair), long_workspace_bytes."""
+    if method not in VARIANTS:
+        raise ValueError(f'align_long runs {sorted(VARIANTS)}, got {method!r}')
+    return _sadtw(srcs, tgts, method, scales, stage_ms, keep_workspace, 'sadtw_long')
+
+
+def long_workspace_bytes(src_len, tgt_len):
+    """Bytes of align_long's device workspace for pairs of these amateur / professional frame counts (ValueError past its
+    limits)."""
+    s_arr, s_p = _i32(src_len)
+    t_arr, t_p = _i32(tgt_len)
+    if s_arr.shape != t_arr.shape or s_arr.ndim != 1:
+        raise ValueError(f'{s_arr.shape} amateur and {t_arr.shape} professional lengths')
+    return _check(_native.lib().svb_sadtw_long_workspace_bytes(len(s_arr), s_p, t_p, None), 'sadtw_long_workspace_bytes')
+
+
+def _sadtw(srcs, tgts, method, scales, stage_ms, keep_workspace, entry):
     if method not in VARIANTS:
         raise ValueError(f'method must be one of {sorted(METHODS)}, got {method!r}')
     if len(srcs) != len(tgts) or len(srcs) == 0:
@@ -116,7 +143,9 @@ def align_batch(srcs, tgts, method='EHSADTW', scales=None, stage_ms=False, keep_
     s_arr, s_p = _i32(S)
     t_arr, t_p = _i32(T)
     sec = (ctypes.c_int64 * 5)()
-    ws_bytes = _check(lib.svb_sadtw_workspace_bytes(n, s_p, t_p, sec), 'sadtw_workspace_bytes')
+    size_fn = lib.svb_sadtw_workspace_bytes if entry == 'sadtw' else lib.svb_sadtw_long_workspace_bytes
+    align_fn = lib.svb_sadtw_align if entry == 'sadtw' else lib.svb_sadtw_align_long
+    ws_bytes = _check(size_fn(n, s_p, t_p, sec), f'{entry}_workspace_bytes')
     sc = None
     if scales is not None:
         sc = np.ascontiguousarray(scales, dtype=np.float64)
@@ -127,9 +156,9 @@ def align_batch(srcs, tgts, method='EHSADTW', scales=None, stage_ms=False, keep_
     pc = torch.empty(n, dtype=torch.float32, device=device)
     ms = (ctypes.c_float * 4)() if stage_ms else None
     with torch.cuda.device(device):
-        _check(lib.svb_sadtw_align(_vp(src), _vp(tgt), DTYPES[dt], VARIANTS[method], n, s_p, t_p,
-                                   None if sc is None else ctypes.c_void_p(sc.ctypes.data), _vp(ws), ws_bytes, _vp(out), _vp(pc), ms,
-                                   _native.current_stream_ptr(device)), 'sadtw_align')
+        _check(align_fn(_vp(src), _vp(tgt), DTYPES[dt], VARIANTS[method], n, s_p, t_p,
+                        None if sc is None else ctypes.c_void_p(sc.ctypes.data), _vp(ws), ws_bytes, _vp(out), _vp(pc), ms,
+                        _native.current_stream_ptr(device)), f'{entry.replace("sadtw", "sadtw_align")}')
     return AlignResult(alignment=out, offsets=np.concatenate([[0], np.cumsum(T)]).astype(np.int64), path_cost=pc,
                        stage_ms=tuple(ms) if stage_ms else None, src_len=S, tgt_len=T,
                        workspace=ws if keep_workspace else None, sections=list(sec) if keep_workspace else None)

@@ -33,16 +33,23 @@ def take_conditioning(n_frames, f0, pitch, hp, f0_clip):
     frames.  The dataset's items and the beautifier's takes both go through it."""
     T = cropped_frames(n_frames, hp)
     if hp.get('normalize_pitch', False):
-        # the voiced frames moved to the dataset's f0 statistics; f0 / uv below come from the moved contour, as in the reference
-        f0 = np.array(f0, copy=True)
-        v = f0 > 0
-        if v.any() and f0[v].std() > 0:
-            f0[v] = ((f0[v] - f0[v].mean()) / f0[v].std() * hp['f0_std'] + hp['f0_mean']).clip(min=60, max=f0_clip)
+        # f0 / uv below come from the moved contour, as in the reference
+        f0 = normalized_take_f0(f0, hp, f0_clip)
         pitch = torch.LongTensor(f0_to_coarse(f0)[:T])
     else:
         pitch = torch.LongTensor(pitch)[:T]
     f0, uv = norm_interp_f0(f0[:T], hp)
     return T, pitch, f0, uv
+
+
+def normalized_take_f0(f0, hp, f0_clip):
+    """``normalize_pitch``'s contour (a copy): the take's voiced frames moved to the dataset's f0 statistics, clipped to
+    [60, f0_clip]."""
+    f0 = np.array(f0, copy=True)
+    v = f0 > 0
+    if v.any() and f0[v].std() > 0:
+        f0[v] = ((f0[v] - f0[v].mean()) / f0[v].std() * hp['f0_std'] + hp['f0_mean']).clip(min=60, max=f0_clip)
+    return f0
 
 
 def clip_alignment(a2p_f0_alignment, prof_T, amateur_T):
