@@ -631,6 +631,25 @@ int svb_resample_batch(int32_t target_sr, const int32_t *src_sr, const int64_t *
 int svb_resample_batch_host(int32_t target_sr, const int32_t *src_sr, const int64_t *lengths, int32_t n_clips, const double *win_host,
                             int32_t nwin, int32_t num_table, const float *wav_concat_host, float *out_host, int device, void *stream);
 
+/* ---- FLAC decoding (csrc/flac.cu): a ragged batch of native FLAC streams (RFC 9639; oracle/flac.py is the reference) to float32
+ * mono, one call.  Stream s is nbytes[s] bytes of data_dev (streams back to back, normally whole files), its first frame at byte
+ * first_frame[s] (where the metadata ends), with STREAMINFO's sample_rate, channels, bits and total_samples (host arrays; the
+ * caller parses the metadata).  Output: total_samples[s] float32 samples per stream, back to back: sample / 2^(bits - 1), channels
+ * averaged as numpy's float32 mean(axis=1) over a C-ordered [n, ch] array (in order; 8 channels pairwise, as numpy adds exactly 8
+ * elements) -- bit-identical to utils.audio.read_wav of a WAV holding the same PCM.  The last frame must end where the stream does.
+ * svb_flac_plan: size of the caller-owned workspace and each stream's output sample count, -1 (svb_last_error names the stream) on
+ *   bits outside 4..24, total_samples 0 (unknown), more than 8 channels, or 2 GiB of input or more.  No CUDA call.
+ * svb_flac_decode_batch: finds the frames (sync code, header, CRC-8; a candidate is a frame only when the CRC-16 of the span to the
+ *   next accepted frame checks out and its number continues the chain), checks each frame against STREAMINFO and the chain against
+ *   its total, decodes every subframe with a reader bounded by its frame, and writes out_dev.  Synchronises the stream; a damaged
+ *   stream returns SVB_ERR_INVALID with the stream and byte offset in svb_last_error.  stage_ms_host (NULL = not wanted) receives
+ *   the CUDA-event time of the decode launches. */
+int64_t svb_flac_plan(int32_t n_streams, const int64_t *nbytes, const int64_t *first_frame, const int32_t *sample_rate,
+                      const int32_t *channels, const int32_t *bits, const int64_t *total_samples, int64_t *out_samples);
+int svb_flac_decode_batch(int32_t n_streams, const int64_t *nbytes, const int64_t *first_frame, const int32_t *sample_rate,
+                          const int32_t *channels, const int32_t *bits, const int64_t *total_samples, const void *data_dev,
+                          float *out_dev, void *workspace_dev, int64_t workspace_bytes, float *stage_ms_host, void *stream);
+
 /* Host-only view of the schedule of a merged tensor-core launch (csrc/conv_tc.cu: tc_schedule; no CUDA call, usable without a GPU):
  * `n_layers` convolutions of one shape class (taps KS[l], residual / accumulate flags) over B clips x Tq rows, tiles of 128 rows in
  * items of up to MT tiles, `col_blocks` column blocks, `grid` CTAs.  items_out receives 5 ints per item (layer, column block, clip,

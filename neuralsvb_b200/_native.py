@@ -17,7 +17,7 @@ LIB_PATH = os.path.join(_HERE, 'libsvb_vocoder.so')
 HEADER = os.path.join(_ROOT, 'include', 'svb_vocoder.h')
 SOURCES = ['wn.cu', 'conformer.cu', 'api.cu', 'conv_ffma.cu', 'conv_tc.cu', 'nsf_source.cu', 'frontend.cu', 'generator.cu', 'layer_api.cu', 'disc_ops.cu',
            'train_ops.cu', 'generator_bwd.cu', 'disc_bwd.cu', 'tc_layer.cu', 'wgrad_tc.cu', 'mel_loss.cu', 'mel_disc.cu', 'sadtw.cu',
-           'pitch_ac.cu', 'resample.cu']
+           'pitch_ac.cu', 'resample.cu', 'flac.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '-Xcompiler', '-fPIC', '-shared']
 
@@ -223,6 +223,8 @@ _PROTOS = {
     'svb_resample_plan': (_I64, [_I32, _P, _P, _I32, _I32, _I32, _P, _P]),
     'svb_resample_batch': (ctypes.c_int, [_I32, _P, _P, _I32, _P, _I32, _I32, _P, _P, _P, _I64, _P, _P]),
     'svb_resample_batch_host': (ctypes.c_int, [_I32, _P, _P, _I32, _P, _I32, _I32, _P, _P, ctypes.c_int, _P]),
+    'svb_flac_plan': (_I64, [_I32, _P, _P, _P, _P, _P, _P, _P]),
+    'svb_flac_decode_batch': (ctypes.c_int, [_I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I64, _P, _P]),
 }
 
 

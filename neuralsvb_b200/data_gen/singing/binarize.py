@@ -1,8 +1,8 @@
 """The singing binarizer's item bookkeeping (reference data_gen/singing/binarize.py over data_gen/tts/base_binarizer.py): scan
-``{processed_data_dir}/data/*/*.wav``, keep the items of ``hparams['datasets']``, split them by ``test_prefixes`` and write
+``{processed_data_dir}/data/*/*.wav`` and ``*.flac``, keep the items of ``hparams['datasets']``, split them by ``test_prefixes`` and write
 ``spk_map.json``.  ``process_data`` is the subclass's (binarize_para.py).
 
-The reference reads PopBuTFy's mp3 files through librosa; here the input is WAV at any rate and channel count (folded to mono and
+The reference reads PopBuTFy's mp3 files through librosa; here the input is WAV or FLAC at any rate and channel count (folded to mono and
 resampled to ``audio_sample_rate`` on the GPU as ``librosa.core.load`` does), so mp3 files are decoded to WAV once beforehand (for
 example ``ffmpeg -i x.mp3 x.wav``)."""
 import glob
@@ -44,9 +44,19 @@ class SingingBinarizer:
         its first '#'), sorted names, then only the items of hparams['datasets'], then the train / test split."""
         for ds_id, processed_data_dir in enumerate(self.processed_data_dirs):
             wav_fns = sorted(glob.glob(f'{processed_data_dir}/data/*/*.wav'))
-            if not wav_fns and glob.glob(f'{processed_data_dir}/data/*/*.mp3'):
+            flac_fns = sorted(glob.glob(f'{processed_data_dir}/data/*/*.flac'))
+            if not wav_fns and not flac_fns and glob.glob(f'{processed_data_dir}/data/*/*.mp3'):
                 raise ValueError(f'{processed_data_dir}/data holds mp3 files only: the binarizer reads WAV (any rate; it resamples '
-                                 f'to {hparams["audio_sample_rate"]} Hz itself); decode them once, e.g. ffmpeg -i x.mp3 x.wav')
+                                 f'to {hparams["audio_sample_rate"]} Hz itself); decode them once, e.g. ffmpeg -i x.mp3 x.wav '
+                                 '(FLAC is also accepted)')
+            if flac_fns:
+                seen = {os.path.splitext(os.path.basename(w))[0]: w for w in wav_fns}
+                for fn in flac_fns:
+                    name = os.path.splitext(os.path.basename(fn))[0]
+                    if name in seen:
+                        raise ValueError(f'item {name!r} is both {seen[name]} and {fn}: keep one of the two')
+                    seen[name] = fn
+                wav_fns = sorted(wav_fns + flac_fns)
             for wav_fn in wav_fns:
                 item_name = os.path.splitext(os.path.basename(wav_fn))[0]
                 if len(self.processed_data_dirs) > 1:

@@ -1,5 +1,5 @@
 """Beautify raw singing: an amateur take and a professional take of the same song in, the a2p (amateur-to-professional) take
-out, as ``SVBVAEMleTask --infer`` computes it for a binarized pair, but straight from WAV files and for a ragged batch of pairs
+out, as ``SVBVAEMleTask --infer`` computes it for a binarized pair, but straight from WAV or FLAC files and for a ragged batch of pairs
 in one call.
 
 For every pair the chain is the existing route's, stage by stage: ``PopBuTFyENBinarizer.process_batch`` (``wav2spec``, the
@@ -157,11 +157,11 @@ class SVBBeautifier:
                              'one of each per pair, at least one pair')
         spk = [_embedding(e, i) for i, e in enumerate(spk_emb)]
         hp, sr, hop = self.hp, int(self.hp['audio_sample_rate']), int(self.hp['hop_size'])
-        dec = decode_wavs(amateur + professional, sr)
+        dec = decode_wavs(amateur + professional, sr, self.device)
         for k, (w, _) in enumerate(dec):
             if w.ndim != 1 or len(w) == 0:
                 raise ValueError(f'pair {k % B}: the {"amateur" if k < B else "professional"} take must be 1-D samples, '
-                                 f'got shape {w.shape}')
+                                 f'got shape {tuple(w.shape)}')
         rates = [r for _, r in dec]
         lens = np.array([len(w) for w, _ in dec], np.int64)
         off = [k for k, r in enumerate(rates) if r != sr]
@@ -186,15 +186,20 @@ class SVBBeautifier:
 
     # ------------------------------------------------------------------ device stages
     def _front_end(self, dec, rates, lens, st):
-        """One H2D copy of every decoded sample, the resampler over the off-rate takes, the front end -> (mels, padded waveforms)."""
+        """One H2D copy of the decoded host samples (WAV files and arrays; FLAC takes were decoded on the device and stay there),
+        the takes assembled on the device, the resampler over the off-rate takes, the front end -> (mels, padded waveforms)."""
         from neuralsvb_b200.vocoders.hifigan import HifiGAN
         sr = int(self.hp['audio_sample_rate'])
-        raw = torch.from_numpy(np.concatenate([w for w, _ in dec])).to(self.device)
+        host = [k for k, (w, _) in enumerate(dec) if not torch.is_tensor(w)]
+        pieces = [w for w, _ in dec]
+        if host:
+            up = torch.from_numpy(np.concatenate([dec[k][0] for k in host])).to(self.device)
+            for k, p in zip(host, torch.split(up, [len(dec[k][0]) for k in host])):
+                pieces[k] = p
+        raw = up if len(host) == len(dec) else pieces[0] if len(pieces) == 1 else torch.cat(pieces)
         st.mark('resample')
         off = [k for k, r in enumerate(rates) if r != sr]
         if off:
-            starts = np.concatenate([[0], np.cumsum([len(w) for w, _ in dec])])
-            pieces = [raw[starts[k]:starts[k + 1]] for k in range(len(dec))]
             y = audio.resample_device(torch.cat([pieces[k] for k in off]), [len(dec[k][0]) for k in off], [rates[k] for k in off], sr)
             for k, p in zip(off, torch.split(y, [int(lens[k]) for k in off])):
                 pieces[k] = p

@@ -3,7 +3,8 @@ sites of librosa.filters.mel in data_gen/tts/data_gen_utils.py:130, modules/hifi
 The STFT / magnitude / mel projection / log themselves run in the fused CUDA kernel
 (csrc/frontend.cu); what stays on the host is the constant mel filterbank and index arithmetic.
 
-Loading audio (``load_wav``, ``resample_batch``): the reference's ``librosa.core.load(path, sr=sr)`` for WAV files -- decode,
+Loading audio (``load_wav``, ``resample_batch``): the reference's ``librosa.core.load(path, sr=sr)`` for WAV and FLAC files -- decode
+(FLAC on the GPU, csrc/flac.cu),
 fold to mono, resample with resampy's ``kaiser_best`` filter -- with the resampling in csrc/resample.cu (oracle/resample.py
 states the algorithm)."""
 import ctypes
@@ -101,12 +102,55 @@ def kaiser_best_window():
     return win, num_bits
 
 
+def is_flac(path):
+    """True when the file starts with the native FLAC marker ``fLaC`` (a path, or a WAV path: False)."""
+    with open(path, 'rb') as f:
+        return f.read(4) == b'fLaC'
+
+
+def flac_info(data, name='stream'):
+    """STREAMINFO of FLAC bytes (a whole file, or at least its metadata): dict(sample_rate, channels, bits, total_samples,
+    first_frame), first_frame being the byte where the metadata blocks end.  Raises ValueError naming ``name`` for a stream that is
+    not native FLAC (Ogg-encapsulated FLAC is refused) or whose metadata is cut short."""
+    data = memoryview(data)
+    if bytes(data[:4]) == b'OggS':
+        raise ValueError(f'{name}: Ogg-encapsulated FLAC is not supported; store it as native FLAC (.flac)')
+    if bytes(data[:4]) != b'fLaC':
+        raise ValueError(f'{name}: not a FLAC stream (no fLaC marker)')
+    off, info = 4, None
+    while True:
+        if off + 4 > len(data):
+            raise ValueError(f'{name}: FLAC metadata runs past the end of the file at byte {off}')
+        head = bytes(data[off:off + 4])
+        last, btype, n = head[0] >> 7, head[0] & 0x7F, int.from_bytes(head[1:], 'big')
+        if btype == 127 or off + 4 + n > len(data) or (btype == 0) != (info is None) or (btype == 0 and n != 34):
+            raise ValueError(f'{name}: bad FLAC metadata block (type {btype}, {n} bytes) at byte {off}')
+        if btype == 0:
+            v = int.from_bytes(bytes(data[off + 14:off + 22]), 'big')
+            info = dict(sample_rate=v >> 44, channels=((v >> 41) & 7) + 1, bits=((v >> 36) & 31) + 1, total_samples=v & ((1 << 36) - 1))
+        off += 4 + n
+        if last:
+            info['first_frame'] = off
+            return info
+
+
 def wav_info(path):
-    """(sample rate, frames, channels) from a WAV file's header, without reading its samples."""
+    """(sample rate, frames, channels) from a WAV file's header or a FLAC file's STREAMINFO, without reading its samples."""
     with open(path, 'rb') as f:
         riff = f.read(12)
+        if riff[:4] == b'fLaC':
+            head, off, last = bytearray(riff), 4, False      # read the metadata blocks only, header by header
+            while not last:
+                head += f.read(max(0, off + 4 - len(head)))
+                if len(head) < off + 4:
+                    break
+                last = head[off] >> 7
+                off += 4 + int.from_bytes(head[off + 1:off + 4], 'big')
+                head += f.read(max(0, off - len(head)))
+            i = flac_info(bytes(head), path)
+            return i['sample_rate'], i['total_samples'], i['channels']
         if len(riff) < 12 or riff[:4] != b'RIFF' or riff[8:12] != b'WAVE':
-            raise ValueError(f'{path}: not a RIFF/WAVE file')
+            raise ValueError(f'{path}: not a RIFF/WAVE file (FLAC files are also accepted)')
         fmt = None
         while True:
             head = f.read(8)
@@ -132,9 +176,63 @@ def wav_seconds(path):
     return frames / sr
 
 
+def flac_decode_device(blobs, names=None, device=None, stage_ms=None):
+    """Decode FLAC files held in memory (``blobs``: bytes of whole files) in ONE device call (svb_flac_decode_batch): the bytes go to
+    the device in one copy -> (float32 CUDA tensor of every stream's mono samples back to back, int64 numpy lengths, rates).  The
+    samples are bit-identical to ``read_wav`` of a WAV file holding the same PCM.  Raises ValueError naming the file (``names``) and
+    byte offset for a stream that does not decode.  ``stage_ms`` (a list): the CUDA-event time of the decode launches is appended."""
+    import torch
+
+    from neuralsvb_b200 import _native
+    names = [f'stream {i}' for i in range(len(blobs))] if names is None else list(names)
+    infos = [flac_info(b, n) for b, n in zip(blobs, names)]
+    nbytes = np.array([len(b) for b in blobs], np.int64)
+    first = np.array([i['first_frame'] for i in infos], np.int64)
+    srs = np.array([i['sample_rate'] for i in infos], np.int32)
+    chans = np.array([i['channels'] for i in infos], np.int32)
+    bits = np.array([i['bits'] for i in infos], np.int32)
+    total = np.array([i['total_samples'] for i in infos], np.int64)
+    lib = _native.lib()
+    args = [len(blobs)] + [a.ctypes.data_as(ctypes.c_void_p) for a in (nbytes, first, srs, chans, bits, total)]
+    lens = np.zeros(len(blobs), np.int64)
+    ws_bytes = lib.svb_flac_plan(*args, lens.ctypes.data_as(ctypes.c_void_p))
+    if ws_bytes < 0:
+        raise ValueError(_flac_error(lib.svb_last_error().decode('utf-8', 'replace'), names))
+    if not torch.cuda.is_available():
+        raise RuntimeError('FLAC decoding runs on CUDA: neuralsvb_b200 has no CPU fallback')
+    device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
+    host = torch.from_numpy(np.frombuffer(b''.join(bytes(b) for b in blobs), np.uint8).copy())
+    data = host.to(device)
+    out = torch.empty(max(int(lens.sum()), 1), device=device)
+    ws = torch.empty(int(ws_bytes), dtype=torch.uint8, device=device)
+    ms = ctypes.c_float(0.0)
+    with torch.cuda.device(device):
+        rc = lib.svb_flac_decode_batch(*args, ctypes.c_void_p(data.data_ptr()), ctypes.c_void_p(out.data_ptr()),
+                                       ctypes.c_void_p(ws.data_ptr()), int(ws_bytes), None if stage_ms is None else ctypes.byref(ms),
+                                       _native.current_stream_ptr(device))
+    if stage_ms is not None and rc == 0:
+        stage_ms.append(ms.value)
+    if rc == -1:
+        raise ValueError(_flac_error(lib.svb_last_error().decode('utf-8', 'replace'), names))
+    _native.check(rc, 'flac_decode_batch')
+    return out[:int(lens.sum())], lens, [int(r) for r in srs]
+
+
+def _flac_error(msg, names):
+    """'flac: stream 3: ...' -> the same message naming the file."""
+    import re
+    m = re.match(r'flac: stream (\d+): (.*)', msg)
+    return f'{names[int(m.group(1))]}: {m.group(2)}' if m else msg
+
+
 def read_wav(path):
-    """(float32 mono samples, file rate) of a WAV file, decoded as ``librosa.load`` documents: integer PCM / 2^(bits - 1) (scipy
-    returns 24-bit as left-justified int32), uint8 as (x - 128) / 128, float as is; channels averaged in float32."""
+    """(float32 mono samples, file rate) of a WAV or FLAC file (recognised by its magic bytes), decoded as ``librosa.load``
+    documents: integer PCM / 2^(bits - 1) (scipy returns 24-bit WAV as left-justified int32; FLAC 8-bit is signed), uint8 WAV as
+    (x - 128) / 128, float as is; channels averaged in float32.  A FLAC file is decoded on the GPU (``flac_decode_device``)."""
+    if is_flac(path):
+        with open(path, 'rb') as f:
+            y, _, rates = flac_decode_device([f.read()], [path])
+        return y.cpu().numpy(), rates[0]
     from scipy.io import wavfile
     sr, data = wavfile.read(path)
     if data.dtype.kind == 'i':
@@ -233,7 +331,8 @@ def resample_device(wav_concat, lengths, orig_srs, target_sr):
 
 
 def load_wav(path, sr=22050):
-    """``librosa.core.load(path, sr=sr)`` for a WAV file: (float32 mono samples at ``sr``, sr); ``sr=None`` keeps the file's rate."""
+    """``librosa.core.load(path, sr=sr)`` for a WAV or FLAC file: (float32 mono samples at ``sr``, sr); ``sr=None`` keeps the file's
+    rate."""
     data, file_sr = read_wav(path)
     if sr is None or file_sr == sr:
         return data, file_sr

@@ -60,19 +60,35 @@ def stft_config(hp, pad_mode, out_kind, eps, frames_major=1, clamp=0):
 
 
 def _load_wav(wav_fn, sr):
-    """librosa.core.load(wav_fn, sr=sr) for a WAV file (utils/audio.load_wav): decoded, mono, resampled on the GPU when the file's
+    """librosa.core.load(wav_fn, sr=sr) for a WAV or FLAC file (utils/audio.load_wav): decoded, mono, resampled on the GPU when the file's
     rate is not sr."""
     return audio.load_wav(wav_fn, sr)[0]
 
 
-def decode_wavs(wav_fns, sr):
-    """[(float32 mono samples, rate)] of each path, decoded as utils/audio.read_wav does; arrays are taken to be at sr already."""
-    out = []
-    for w in wav_fns:
+def decode_wavs(wav_fns, sr, device=None):
+    """[(float32 mono samples, rate)] of each path, decoded as utils/audio.read_wav does; arrays are taken to be at sr already.
+    The FLAC paths of a call are read into one host buffer and decoded together: one copy of the compressed bytes to the device and
+    one svb_flac_decode_batch.  ``device`` given: a FLAC take's samples stay there (a CUDA tensor, for callers that assemble their
+    input on the device); otherwise they come back to the host as numpy arrays like every other take."""
+    out = [None] * len(wav_fns)
+    flac = [i for i, w in enumerate(wav_fns) if isinstance(w, str) and audio.is_flac(w)]
+    for i, w in enumerate(wav_fns):
         if isinstance(w, str):
-            out.append(audio.read_wav(w))
+            if i not in flac:
+                out[i] = audio.read_wav(w)
         else:
-            out.append((np.ascontiguousarray(w, dtype=np.float32), sr))
+            out[i] = (np.ascontiguousarray(w, dtype=np.float32), sr)
+    if flac:
+        blobs = []
+        for i in flac:
+            with open(wav_fns[i], 'rb') as f:
+                blobs.append(f.read())
+        y, lens, rates = audio.flac_decode_device(blobs, [wav_fns[i] for i in flac], device)
+        if device is None:
+            y = y.cpu().numpy()
+        for i, piece, r in zip(flac, torch.split(y, [int(n) for n in lens]) if device is not None else np.split(y, np.cumsum(lens)[:-1]),
+                               rates):
+            out[i] = (piece, r)
     return out
 
 
