@@ -143,7 +143,7 @@ int svb_gen_forward_ragged_from(svb_gen_t *g, const float *mel_dev, const float 
                                 const float *noise_dev, uint64_t seed, int32_t first_clip, int32_t B, int32_t T_max,
                                 const int32_t *lengths_host, float *wav_dev, void *stream);
 /* spec2wav over a ragged batch from HOST memory (vocoders/hifigan.py:55-69, clip by clip): mel_host holds the clips' [T_b, n_mel]
- * mels back to back ([sum T_b, n_mel], as svb_wav2spec_batch_host returns them), f0_host their [T_b] f0 back to back or NULL;
+ * mels back to back ([sum T_b, n_mel], as svb_wav2spec_batch returns them), f0_host their [T_b] f0 back to back or NULL;
  * wav_host receives sum(T_b) * hop samples, clip after clip.  One H2D copy, one forward, one D2H copy, one synchronisation. */
 int svb_gen_spec2wav_ragged_host(svb_gen_t *g, const float *mel_host, const float *f0_host, uint64_t seed, int32_t B,
                                  const int32_t *lengths_host, float *wav_host, void *stream);
@@ -390,26 +390,13 @@ int svb_stft_backward(const svb_stft_config *cfg, const float *wav_dev, int32_t 
  * Only n_fft / hop / win of cfg are read. */
 int svb_denoise(const svb_stft_config *cfg, const float *wav_dev, int32_t B, int64_t n, float v, float *out_dev, void *stream);
 
-/* PWG.wav2spec / process_utterance (vocoders/pwg.py:105-122, data_gen_utils.py:93-147) from HOST
- * memory: wav_host [n] -> mel_host [frames, n_mels] (log10), wav_out_host [frames*hop] (zero padded
- * on the right, audio.librosa_pad_lr, utils/audio.py:67-76).  mel_basis_host [n_mels, n_fft/2+1].
- * Returns the frame count (>= 0) or a negative status. */
-int64_t svb_wav2spec_host(const svb_stft_config *cfg, const float *wav_host, int64_t n,
-                          const float *mel_basis_host, float *mel_host, float *wav_out_host, int device,
-                          void *stream);
-
-/* The binarizer's call site (data_gen/tts/base_binarizer.py:168-178, data_gen/singing/binarize_para.py:116-217 call
- * wav2spec once per file from a CPU process pool) as ONE call over a ragged batch: `n_clips` waveforms concatenated in
- * wav_concat_host with their lengths; mel_concat_host receives the [frames_c, n_mels] log10-mels back to back and
- * frames_out[c] their frame counts (1 + lengths[c] / hop each).  One H2D, one kernel launch over all frames of all
- * clips, one D2H.  Returns the total frame count or a negative status. */
-int64_t svb_wav2spec_batch_host(const svb_stft_config *cfg, const float *wav_concat_host, const int64_t *lengths,
-                                int32_t n_clips, const float *mel_basis_host, float *mel_concat_host, int64_t *frames_out,
-                                int device, void *stream);
-/* The same on device memory, with no copy of the samples and no synchronisation (the host form above is its H2D + call + D2H
- * wrapper).  wav_concat_dev: the clips back to back (lengths: host array); mel_basis_dev [n_mels, n_fft/2+1]; mel_concat_dev
- * receives the mels back to back, wav_out_dev (NULL = not wanted) every clip zero-padded to frames_c * hop samples, back to back
- * (what wav2spec returns as its waveform, in the layout svb_pitch_ac_batch takes).  The only copy is the small clip table, into
+/* PWG.wav2spec / process_utterance (vocoders/pwg.py:105-122, data_gen_utils.py:93-147) at the binarizer's call site
+ * (data_gen/tts/base_binarizer.py:168-178, data_gen/singing/binarize_para.py:116-217 call wav2spec once per file from a CPU
+ * process pool) as ONE call over a ragged batch on device memory, with no copy of the samples and no synchronisation.
+ * wav_concat_dev: the clips back to back (lengths: host array); mel_basis_dev [n_mels, n_fft/2+1]; mel_concat_dev receives the
+ * [frames_c, n_mels] log10-mels back to back (1 + lengths[c] / hop frames each), wav_out_dev (NULL = not wanted) every clip
+ * zero-padded on the right to frames_c * hop samples (audio.librosa_pad_lr, utils/audio.py:67-76), back to back (what wav2spec
+ * returns as its waveform, in the layout svb_pitch_ac_batch takes).  One kernel launch over all frames of all clips.  The only copy is the small clip table, into
  * the caller-owned workspace of svb_wav2spec_workspace_bytes bytes.  Both reject before any launch (SVB_ERR_INVALID) a bad config,
  * an empty clip, a null buffer or a short workspace; frames_out (NULL = not wanted) receives the frame counts.  svb_wav2spec_batch
  * returns the total frame count, svb_wav2spec_workspace_bytes the workspace size, or a negative status. */
@@ -587,7 +574,6 @@ int svb_dtw_baselines_cost(const void *src_dev, const void *tgt_dev, int32_t dty
  *   (frequency, strength) of the unvoiced candidate then the voiced ones strongest first (unused: (0, -inf)); count_dev int32 [frames];
  *   r_dev float32 [frames, tau_max + 2] = the normalised autocorrelation r(tau); stage_ms_host (NULL = not wanted) receives 3 CUDA-event
  *   times (clip statistics, candidates, path) and makes the call synchronise.
- * svb_pitch_ac_batch_host: the same from host memory: one H2D copy, the three launches, one D2H copy; synchronises.
  * All reject before any launch (SVB_ERR_INVALID): a null pointer, a bad config, a clip shorter than one window, a short workspace. */
 typedef struct svb_pitch_config {
     int32_t sr;
@@ -607,8 +593,6 @@ int64_t svb_pitch_ac_workspace_bytes(const svb_pitch_config *cfg, const int64_t 
 int svb_pitch_ac_batch(const svb_pitch_config *cfg, const float *wav_concat_dev, const int64_t *lengths, int32_t n_clips,
                        const int64_t *mel_frames, float *f0_out_dev, void *workspace_dev, int64_t workspace_bytes, float *cand_dev,
                        int32_t *count_dev, float *r_dev, float *stage_ms_host, void *stream);
-int svb_pitch_ac_batch_host(const svb_pitch_config *cfg, const float *wav_concat_host, const int64_t *lengths, int32_t n_clips,
-                            const int64_t *mel_frames, float *f0_out_host, int device, void *stream);
 
 /* ---- Resampling (csrc/resample.cu): librosa.core.load(path, sr=target)'s resampy kaiser_best resampler (reference
  * data_gen/tts/data_gen_utils.py:111); oracle/resample.py states every step.  A batch is ragged: n_clips float32 waveforms concatenated
@@ -621,15 +605,12 @@ int svb_pitch_ac_batch_host(const svb_pitch_config *cfg, const float *wav_concat
  *   No CUDA call.
  * svb_resample_batch (device pointers): out_dev float32 [sum out_lengths]; stage_ms_host (NULL = not wanted) receives 2 CUDA-event
  *   times (time register, filter) and makes the call synchronise.
- * svb_resample_batch_host: the same from host memory: one H2D copy of the samples, the launches, one D2H copy; synchronises.
  * All reject before any launch (SVB_ERR_INVALID): a null pointer, a bad rate or length, a short workspace. */
 int64_t svb_resample_plan(int32_t target_sr, const int32_t *src_sr, const int64_t *lengths, int32_t n_clips, int32_t nwin,
                           int32_t num_table, int64_t *res_lengths_out, int64_t *out_lengths_out);
 int svb_resample_batch(int32_t target_sr, const int32_t *src_sr, const int64_t *lengths, int32_t n_clips, const double *win_host,
                        int32_t nwin, int32_t num_table, const float *wav_concat_dev, float *out_dev, void *workspace_dev,
                        int64_t workspace_bytes, float *stage_ms_host, void *stream);
-int svb_resample_batch_host(int32_t target_sr, const int32_t *src_sr, const int64_t *lengths, int32_t n_clips, const double *win_host,
-                            int32_t nwin, int32_t num_table, const float *wav_concat_host, float *out_host, int device, void *stream);
 
 /* ---- FLAC decoding (csrc/flac.cu): a ragged batch of native FLAC streams (RFC 9639; oracle/flac.py is the reference) to float32
  * mono, one call.  Stream s is nbytes[s] bytes of data_dev (streams back to back, normally whole files), its first frame at byte

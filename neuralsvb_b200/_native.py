@@ -159,8 +159,6 @@ _PROTOS = {
     'svb_stft_forward': (ctypes.c_int, [ctypes.POINTER(StftConfig), _P, _I32, _I64, _P, _P, _P]),
     'svb_stft_backward': (ctypes.c_int, [ctypes.POINTER(StftConfig), _P, _I32, _I64, _P, _P, _P, _P]),
     'svb_denoise': (ctypes.c_int, [ctypes.POINTER(StftConfig), _P, _I32, _I64, ctypes.c_float, _P, _P]),
-    'svb_wav2spec_host': (_I64, [ctypes.POINTER(StftConfig), _P, _I64, _P, _P, _P, ctypes.c_int, _P]),
-    'svb_wav2spec_batch_host': (_I64, [ctypes.POINTER(StftConfig), _P, _P, _I32, _P, _P, _P, ctypes.c_int, _P]),
     'svb_wav2spec_workspace_bytes': (_I64, [ctypes.POINTER(StftConfig), _P, _I32, _P]),
     'svb_wav2spec_batch': (_I64, [ctypes.POINTER(StftConfig), _P, _P, _I32, _P, _P, _P, _P, _P, _I64, _P]),
     'svb_gen_spec2wav_host_i16': (ctypes.c_int, [_P, _P, _P, _U64, _I32, _I32, _I32, _P, _P]),
@@ -219,10 +217,8 @@ _PROTOS = {
     'svb_dtw_baselines_cost': (ctypes.c_int, [_P, _P, _I32, _I32, _I32, _P, _P, _I32, _P, _I64, _P, _P]),
     'svb_pitch_ac_workspace_bytes': (_I64, [ctypes.POINTER(PitchConfig), _P, _I32, _P]),
     'svb_pitch_ac_batch': (ctypes.c_int, [ctypes.POINTER(PitchConfig), _P, _P, _I32, _P, _P, _P, _I64, _P, _P, _P, _P, _P]),
-    'svb_pitch_ac_batch_host': (ctypes.c_int, [ctypes.POINTER(PitchConfig), _P, _P, _I32, _P, _P, ctypes.c_int, _P]),
     'svb_resample_plan': (_I64, [_I32, _P, _P, _I32, _I32, _I32, _P, _P]),
     'svb_resample_batch': (ctypes.c_int, [_I32, _P, _P, _I32, _P, _I32, _I32, _P, _P, _P, _I64, _P, _P]),
-    'svb_resample_batch_host': (ctypes.c_int, [_I32, _P, _P, _I32, _P, _I32, _I32, _P, _P, ctypes.c_int, _P]),
     'svb_flac_plan': (_I64, [_I32, _P, _P, _P, _P, _P, _P, _P]),
     'svb_flac_decode_batch': (ctypes.c_int, [_I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I64, _P, _P]),
 }

@@ -7,7 +7,7 @@
 // staged once per CTA in shared memory; the mel filters come in a span-compressed form (mel_pack_kernel: first / last
 // non-zero bin of every row + the values in between, ~2 values per frequency bin for triangular filters), so the
 // projection walks only the non-zero span of each filter.  Clips of different lengths are served by one launch
-// through a per-clip table (ragged batches of the binarizer, svb_wav2spec_batch_host).
+// through a per-clip table (ragged batches of the binarizer, svb_wav2spec_batch).
 // Backward / denoise keep the one-CTA-per-frame complex FFT below (they need the full inverse transform).
 //
 // Replaces (see include/svb_vocoder.h for the per-mode citations):
@@ -646,53 +646,6 @@ extern "C" int64_t svb_wav2spec_batch(const svb_stft_config *cfg, const float *w
         SVB_CUDA(cudaGetLastError());
     }
     return (int64_t)p.frm_off[n_clips];
-}
-
-// the host form: one H2D of the concatenated waveforms and the filters, svb_wav2spec_batch, one D2H of the mels; synchronises
-static int64_t wav2spec_batch_impl(const svb_stft_config *cfg, const float *wav_host, const int64_t *lengths, int32_t n_clips,
-                                   const float *mel_basis_host, float *mel_host, int64_t *frames_out, int device, cudaStream_t st) {
-    Wav2SpecPlan p;
-    SVB_TRY(plan_wav2spec(cfg, lengths, n_clips, nullptr, &p));
-    SVB_CHECK(wav_host && mel_basis_host && mel_host, SVB_ERR_INVALID, "wav2spec: null buffer or no clips");
-    SVB_CUDA(cudaSetDevice(device));
-    const int n_bins = cfg->n_fft / 2 + 1;
-    const size_t n_wav = (size_t)p.wav_off[n_clips], n_frames = (size_t)p.frm_off[n_clips];
-    float *d_wav = nullptr, *d_basis = nullptr, *d_mel = nullptr;
-    char *d_ws = nullptr;
-    SVB_CUDA(cudaMallocAsync((void **)&d_wav, n_wav * sizeof(float), st));
-    SVB_CUDA(cudaMallocAsync((void **)&d_basis, (size_t)cfg->n_mels * n_bins * sizeof(float), st));
-    SVB_CUDA(cudaMallocAsync((void **)&d_mel, n_frames * cfg->n_mels * sizeof(float), st));
-    SVB_CUDA(cudaMallocAsync((void **)&d_ws, p.total, st));
-    SVB_CUDA(cudaMemcpyAsync(d_wav, wav_host, n_wav * sizeof(float), cudaMemcpyHostToDevice, st));
-    SVB_CUDA(cudaMemcpyAsync(d_basis, mel_basis_host, (size_t)cfg->n_mels * n_bins * sizeof(float), cudaMemcpyHostToDevice, st));
-    int64_t rc = svb_wav2spec_batch(cfg, d_wav, lengths, n_clips, d_basis, d_mel, nullptr, frames_out, d_ws, (int64_t)p.total, st);
-    if (rc >= 0)
-        SVB_CUDA(cudaMemcpyAsync(mel_host, d_mel, n_frames * cfg->n_mels * sizeof(float), cudaMemcpyDeviceToHost, st));
-    cudaFreeAsync(d_wav, st), cudaFreeAsync(d_basis, st), cudaFreeAsync(d_mel, st), cudaFreeAsync(d_ws, st);
-    SVB_CUDA(cudaStreamSynchronize(st));
-    return rc;
-}
-
-extern "C" int64_t svb_wav2spec_batch_host(const svb_stft_config *cfg, const float *wav_concat_host, const int64_t *lengths,
-                                           int32_t n_clips, const float *mel_basis_host, float *mel_concat_host,
-                                           int64_t *frames_out, int device, void *stream) {
-    return wav2spec_batch_impl(cfg, wav_concat_host, lengths, n_clips, mel_basis_host, mel_concat_host, frames_out, device,
-                               as_stream(stream));
-}
-
-extern "C" int64_t svb_wav2spec_host(const svb_stft_config *cfg, const float *wav_host, int64_t n,
-                                     const float *mel_basis_host, float *mel_host, float *wav_out_host, int device,
-                                     void *stream) {
-    SVB_TRY(validate_stft(cfg, n, true));
-    SVB_CHECK(wav_host && mel_basis_host && mel_host, SVB_ERR_INVALID, "wav2spec: null buffer");
-    const int64_t frames = wav2spec_batch_impl(cfg, wav_host, &n, 1, mel_basis_host, mel_host, nullptr, device, as_stream(stream));
-    if (frames < 0) return frames;
-    if (wav_out_host) {
-        // audio.librosa_pad_lr(wav, fft, hop, 1): right-pad to (n // hop + 1) * hop, then wav[:frames * hop]
-        const int64_t out_len = frames * cfg->hop;
-        for (int64_t i = 0; i < out_len; ++i) wav_out_host[i] = i < n ? wav_host[i] : 0.f;
-    }
-    return frames;
 }
 
 extern "C" int svb_stft_backward(const svb_stft_config *cfg, const float *wav_dev, int32_t B, int64_t n,

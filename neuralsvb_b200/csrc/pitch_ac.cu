@@ -87,7 +87,7 @@ int validate(const svb_pitch_config *cfg) {
 // ---- workspace ----------------------------------------------------------------------------------------------------------------
 struct Layout {
     size_t off_clip, off_stats, off_win, off_rwn, off_cand, off_count, off_bp, total;
-    long long frames, out_frames;
+    long long frames;
     int blocks, L, tau_max;
 };
 
@@ -112,7 +112,7 @@ int plan(const svb_pitch_config *cfg, const int64_t *lengths, const int64_t *mel
         L = g.L, tau_max = g.tau_max;
     }
     SVB_CHECK(blk < (1 << 30), SVB_ERR_INVALID, "pitch_ac: %lld frames are too many for one call", fr);
-    lay->frames = fr, lay->out_frames = out, lay->blocks = blk, lay->L = L, lay->tau_max = tau_max;
+    lay->frames = fr, lay->blocks = blk, lay->L = L, lay->tau_max = tau_max;
     lay->off_clip = 0;
     lay->off_stats = align_up((size_t)n_clips * sizeof(PitchClip));
     lay->off_win = lay->off_stats + align_up((size_t)n_clips * 2 * sizeof(float));
@@ -501,35 +501,4 @@ extern "C" int svb_pitch_ac_batch(const svb_pitch_config *cfg, const float *wav_
                                   float *cand_dev, int32_t *count_dev, float *r_dev, float *stage_ms_host, void *stream) {
     return run(cfg, wav_concat_dev, lengths, n_clips, mel_frames, f0_out_dev, workspace_dev, workspace_bytes, cand_dev, count_dev, r_dev,
                stage_ms_host, as_stream(stream));
-}
-
-extern "C" int svb_pitch_ac_batch_host(const svb_pitch_config *cfg, const float *wav_concat_host, const int64_t *lengths, int32_t n_clips,
-                                       const int64_t *mel_frames, float *f0_out_host, int device, void *stream) {
-    std::vector<PitchClip> clips;
-    Layout lay;
-    SVB_TRY(plan(cfg, lengths, mel_frames, n_clips, &clips, &lay));
-    SVB_CHECK(wav_concat_host && mel_frames && f0_out_host, SVB_ERR_INVALID, "pitch_ac: null buffer");
-    SVB_CUDA(cudaSetDevice(device));
-    cudaStream_t st = as_stream(stream);
-    long long n_wav = 0;
-    for (int c = 0; c < n_clips; ++c) n_wav += lengths[c];
-    float *d_wav = nullptr, *d_f0 = nullptr;
-    void *d_ws = nullptr;
-    SVB_CUDA(cudaMallocAsync((void **)&d_wav, (size_t)n_wav * sizeof(float), st));
-    SVB_CUDA(cudaMallocAsync((void **)&d_f0, std::max<size_t>(1, (size_t)lay.out_frames) * sizeof(float), st));
-    SVB_CUDA(cudaMallocAsync(&d_ws, lay.total, st));
-    int rc = SVB_OK;
-    if (cudaMemcpyAsync(d_wav, wav_concat_host, (size_t)n_wav * sizeof(float), cudaMemcpyHostToDevice, st) != cudaSuccess) {
-        set_error("pitch_ac: host-to-device copy failed");
-        rc = SVB_ERR_CUDA;
-    }
-    if (rc == SVB_OK) rc = run(cfg, d_wav, lengths, n_clips, mel_frames, d_f0, d_ws, (int64_t)lay.total, nullptr, nullptr, nullptr, nullptr, st);
-    if (rc == SVB_OK && lay.out_frames > 0 &&
-        cudaMemcpyAsync(f0_out_host, d_f0, (size_t)lay.out_frames * sizeof(float), cudaMemcpyDeviceToHost, st) != cudaSuccess) {
-        set_error("pitch_ac: device-to-host copy failed");
-        rc = SVB_ERR_CUDA;
-    }
-    cudaFreeAsync(d_wav, st), cudaFreeAsync(d_f0, st), cudaFreeAsync(d_ws, st);
-    SVB_CUDA(cudaStreamSynchronize(st));
-    return rc;
 }

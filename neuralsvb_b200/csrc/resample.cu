@@ -52,7 +52,7 @@ struct Layout {
     std::vector<ResClip> clips;
     std::vector<ResRate> rates;
     size_t off_clip, off_rate, off_tab, off_tr, total, smem;
-    long long in_total, out_total;
+    long long out_total;
     int blocks;
 };
 
@@ -101,7 +101,7 @@ int plan(int32_t target_sr, const int32_t *src_sr, const int64_t *lengths, int32
     }
     SVB_CHECK(blk < (1LL << 31), SVB_ERR_INVALID, "resample: %lld output samples are too many for one call", out);
     for (auto &R : lay->rates) R.tr_off = tr, tr += R.n_max;
-    lay->in_total = in, lay->out_total = out, lay->blocks = (int)blk, lay->smem = smem;
+    lay->out_total = out, lay->blocks = (int)blk, lay->smem = smem;
     lay->off_clip = 0;
     lay->off_rate = align_up((size_t)n_clips * sizeof(ResClip));
     lay->off_tab = lay->off_rate + align_up(std::max<size_t>(1, lay->rates.size()) * sizeof(ResRate));
@@ -263,35 +263,4 @@ extern "C" int svb_resample_batch(int32_t target_sr, const int32_t *src_sr, cons
                                   int64_t workspace_bytes, float *stage_ms_host, void *stream) {
     return run(target_sr, src_sr, lengths, n_clips, win_host, nwin, num_table, wav_concat_dev, out_dev, workspace_dev, workspace_bytes,
                stage_ms_host, as_stream(stream));
-}
-
-extern "C" int svb_resample_batch_host(int32_t target_sr, const int32_t *src_sr, const int64_t *lengths, int32_t n_clips,
-                                       const double *win_host, int32_t nwin, int32_t num_table, const float *wav_concat_host,
-                                       float *out_host, int device, void *stream) {
-    Layout lay;
-    SVB_TRY(plan(target_sr, src_sr, lengths, n_clips, nwin, num_table, &lay));
-    SVB_CHECK(win_host && wav_concat_host && out_host, SVB_ERR_INVALID, "resample: null buffer");
-    SVB_CUDA(cudaSetDevice(device));
-    cudaStream_t st = as_stream(stream);
-    float *d_wav = nullptr, *d_out = nullptr;
-    void *d_ws = nullptr;
-    SVB_CUDA(cudaMallocAsync((void **)&d_wav, std::max<size_t>(1, (size_t)lay.in_total) * sizeof(float), st));
-    SVB_CUDA(cudaMallocAsync((void **)&d_out, std::max<size_t>(1, (size_t)lay.out_total) * sizeof(float), st));
-    SVB_CUDA(cudaMallocAsync(&d_ws, lay.total, st));
-    int rc = SVB_OK;
-    if (lay.in_total > 0 &&
-        cudaMemcpyAsync(d_wav, wav_concat_host, (size_t)lay.in_total * sizeof(float), cudaMemcpyHostToDevice, st) != cudaSuccess) {
-        set_error("resample: host-to-device copy failed");
-        rc = SVB_ERR_CUDA;
-    }
-    if (rc == SVB_OK)
-        rc = run(target_sr, src_sr, lengths, n_clips, win_host, nwin, num_table, d_wav, d_out, d_ws, (int64_t)lay.total, nullptr, st);
-    if (rc == SVB_OK && lay.out_total > 0 &&
-        cudaMemcpyAsync(out_host, d_out, (size_t)lay.out_total * sizeof(float), cudaMemcpyDeviceToHost, st) != cudaSuccess) {
-        set_error("resample: device-to-host copy failed");
-        rc = SVB_ERR_CUDA;
-    }
-    cudaFreeAsync(d_wav, st), cudaFreeAsync(d_out, st), cudaFreeAsync(d_ws, st);
-    SVB_CUDA(cudaStreamSynchronize(st));
-    return rc;
 }

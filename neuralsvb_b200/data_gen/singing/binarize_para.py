@@ -5,7 +5,8 @@ Pairing, splits, the speaker map, the ``max_mel_tech_gap`` skip (logged to ``bad
 written follow the reference.  The reference processes one pair per CPU worker; here the pairs of a split are grouped by seconds of
 audio (``batch_seconds``, VocoderBinarizer's grouping) and each group costs three device calls: ``wav2spec_batch`` over both takes of
 every pair, ``get_pitch_batch`` over the takes that passed the gap check, and ``align_pitch`` (EHSADTW, the reference's choice) over
-the pairs that kept a voiced f0.  Items are written in metadata order.
+the pairs that kept a voiced f0.  The takes reach the device through ``utils.audio.load_takes`` (one copy, off-rate files resampled
+there); ``wav2spec_batch`` and ``get_pitch_batch`` copy their results back.  Items are written in metadata order.
 
 Each item holds exactly what ``MultiSpkEmbDataset`` reads: ``item_name``, ``mel`` / ``prof_mel`` [T, 80], ``f0`` / ``prof_f0`` (Hz),
 ``pitch`` / ``prof_pitch`` (coarse ids), ``a2p_f0_alignment`` [T_prof] and ``multi_spk_emb`` [1 + spk_emb_num, 256].  Per split:

@@ -3,7 +3,7 @@
 The reference packs a dataset by calling ``get_vocoder_cls(hparams).wav2spec(wav_fn)`` once per file from a pool of
 single-threaded CPU workers (data_gen/tts/base_binarizer.py:128-178, data_gen/singing/binarize_para.py:116-217,
 ``OMP_NUM_THREADS=1`` at data_gen/tts/bin/binarize.py:3).  Here the files of a split are grouped into ragged batches
-and every batch is ONE device call (``HifiGAN.wav2spec_batch`` -> ``svb_wav2spec_batch_host``); the items written are
+and every batch is ONE device call (``HifiGAN.wav2spec_batch``: ``audio.load_takes`` -> ``svb_wav2spec_batch``); the items written are
 the reference's: ``item_name, wav_fn, spk_id, mel [T, 80] (log10), wav float16 [T*hop], sec, len`` (+ ``f0`` when a
 pitch function is supplied: ``data_gen.tts.data_gen_utils.get_pitch`` is this package's GPU tracker, and the reference's
 parselmouth extractor can be passed instead),

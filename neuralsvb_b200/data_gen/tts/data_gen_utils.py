@@ -4,7 +4,8 @@ The reference runs Praat's autocorrelation tracker through parselmouth, once per
 this package's own CUDA implementation (csrc/pitch_ac.cu) of the algorithm oracle/pitch_ac.py states: the reference's settings
 (time step hop / sr, floor 80 Hz, ceiling 750 Hz, voicing threshold 0.6) and Praat's documented defaults for the rest.  It is not
 Praat, and agreement with parselmouth has not been measured; a user who has parselmouth can pass the reference extractor as a
-binarizer's ``pitch_fn`` instead.
+binarizer's ``pitch_fn`` instead.  ``pitch_ac_device`` is the entry point; ``get_pitch_batch`` / ``get_pitch`` copy host waveforms
+to the device, call it and copy the f0 back.
 
 Placement follows the reference: ``2 * pad_size`` zero frames in front (pad_size 4 at hop 128, 2 at hop 256), then the track is cut
 to ``len(mel)`` or extended with its last value.  The reference's ``np.pad`` would receive a negative right pad on this grid (its
@@ -77,22 +78,14 @@ def analysis_frames(lengths, hparams):
 
 def get_pitch_batch(wavs, mels, hparams):
     """[(f0 [len(mel)] float64 Hz, pitch ids [len(mel)] int64)] for each (wav, mel) pair: ONE device call over the ragged batch
-    (svb_pitch_ac_batch_host: one H2D copy, three launches, one D2H copy).  ``mels`` may also be frame counts."""
+    (one H2D copy of the waveforms, ``pitch_ac_device``, one D2H copy of the f0).  ``mels`` may also be frame counts."""
     wavs = [np.ascontiguousarray(w, dtype=np.float32) for w in wavs]
     if not wavs:
         return []
     n_mel = np.array([m if np.isscalar(m) else len(m) for m in mels], np.int64)
     assert len(n_mel) == len(wavs), (len(n_mel), len(wavs))
-    cfg = pitch_config(hparams)
-    device = _device()
-    lengths = np.array([len(w) for w in wavs], np.int64)
-    cat = np.ascontiguousarray(np.concatenate(wavs))
-    out = np.zeros(max(int(n_mel.sum()), 1), np.float32)
-    with torch.cuda.device(device):
-        _check(_native.lib().svb_pitch_ac_batch_host(ctypes.byref(cfg), cat.ctypes.data_as(ctypes.c_void_p),
-                                                     lengths.ctypes.data_as(ctypes.c_void_p), len(wavs),
-                                                     n_mel.ctypes.data_as(ctypes.c_void_p), out.ctypes.data_as(ctypes.c_void_p),
-                                                     device.index, _native.current_stream_ptr(device)), 'pitch_ac')
+    x = torch.from_numpy(np.concatenate(wavs)).to(_device())
+    out = pitch_ac_device(x, [len(w) for w in wavs], n_mel, hparams).f0.cpu().numpy()
     res, o = [], 0
     for T in n_mel:
         f0 = out[o:o + int(T)].astype(np.float64)

@@ -10,7 +10,8 @@ the a2p mel with the professional take's denormalised f0.  Each stage runs once 
     decoded samples --H2D--> resampler (off-rate takes) -> front end (svb_wav2spec_batch) -> pitch tracker -> EHSADTW
         -> [host: crop, f0 normalisation, collate] -> MleSVBVAE -> ragged generator -> [denoise] --D2H--> waveforms
 
-The samples cross PCIe once each way; in between only the per-frame f0, pitch ids and alignments do.
+The takes reach the device through ``utils.audio.load_takes``, the one loading route of the package.  The samples cross PCIe once
+each way; in between only the per-frame f0, pitch ids and alignments do.
 
 The acoustic model runs on the zero-padded batch, as the task's collated batches do, and the model is not blind to padding: a
 pair's a2p mel depends on the batch it is in and can differ from the same pair beautified alone, which is what ``--infer``
@@ -147,9 +148,9 @@ class SVBBeautifier:
 
     # ------------------------------------------------------------------ host checks
     def _takes(self, amateur, professional, spk_emb, songs=False):
-        """Decoded takes (B amateur, then B professional), their lengths at audio_sample_rate and mel frame counts, and the B
-        embeddings; every pair checked before any device work.  songs: takes up to LONG_MAX_FRAMES instead of max_frames."""
-        from neuralsvb_b200.vocoders.hifigan import decode_wavs
+        """Decoded takes (B amateur, then B professional; ``audio.decode_wavs``), their rates, their lengths at audio_sample_rate
+        and mel frame counts, and the B embeddings; every pair checked before any device work.  songs: takes up to LONG_MAX_FRAMES
+        instead of max_frames."""
         amateur, professional, spk_emb = list(amateur), list(professional), list(spk_emb)
         B = len(amateur)
         if B == 0 or len(professional) != B or len(spk_emb) != B:
@@ -157,7 +158,7 @@ class SVBBeautifier:
                              'one of each per pair, at least one pair')
         spk = [_embedding(e, i) for i, e in enumerate(spk_emb)]
         hp, sr, hop = self.hp, int(self.hp['audio_sample_rate']), int(self.hp['hop_size'])
-        dec = decode_wavs(amateur + professional, sr, self.device)
+        dec = audio.decode_wavs(amateur + professional, sr, self.device)
         for k, (w, _) in enumerate(dec):
             if w.ndim != 1 or len(w) == 0:
                 raise ValueError(f'pair {k % B}: the {"amateur" if k < B else "professional"} take must be 1-D samples, '
@@ -186,26 +187,12 @@ class SVBBeautifier:
 
     # ------------------------------------------------------------------ device stages
     def _front_end(self, dec, rates, lens, st):
-        """One H2D copy of the decoded host samples (WAV files and arrays; FLAC takes were decoded on the device and stay there),
-        the takes assembled on the device, the resampler over the off-rate takes, the front end -> (mels, padded waveforms)."""
+        """``audio.load_takes`` of what ``_takes`` returned (``dec`` holds each take's rate; one H2D copy of the host samples, the
+        resampler over the off-rate takes), then the front end on the ``lens`` samples of each take -> (mels, padded waveforms)."""
         from neuralsvb_b200.vocoders.hifigan import HifiGAN
-        sr = int(self.hp['audio_sample_rate'])
-        host = [k for k, (w, _) in enumerate(dec) if not torch.is_tensor(w)]
-        pieces = [w for w, _ in dec]
-        if host:
-            up = torch.from_numpy(np.concatenate([dec[k][0] for k in host])).to(self.device)
-            for k, p in zip(host, torch.split(up, [len(dec[k][0]) for k in host])):
-                pieces[k] = p
-        raw = up if len(host) == len(dec) else pieces[0] if len(pieces) == 1 else torch.cat(pieces)
-        st.mark('resample')
-        off = [k for k, r in enumerate(rates) if r != sr]
-        if off:
-            y = audio.resample_device(torch.cat([pieces[k] for k in off]), [len(dec[k][0]) for k in off], [rates[k] for k in off], sr)
-            for k, p in zip(off, torch.split(y, [int(lens[k]) for k in off])):
-                pieces[k] = p
-            raw = torch.cat(pieces)
+        x, _ = audio.load_takes(dec, int(self.hp['audio_sample_rate']), self.device)
         st.mark('front_end')
-        mel, wav, frames = HifiGAN.wav2spec_device(raw, lens, self.hp, self.mel_basis)
+        mel, wav, _ = HifiGAN.wav2spec_device(x, lens, self.hp, self.mel_basis)
         return mel, wav
 
     def _pitch(self, wav, frames):
@@ -342,7 +329,7 @@ class SVBBeautifier:
             if tuple(eps.shape) != (B, hp['latent_size'], 1):
                 raise ValueError(f'eps must be [{B}, {hp["latent_size"]}, 1], got {tuple(eps.shape)}')
         st = _Stages(self.timing)
-        st.mark('h2d')
+        st.mark('load')
         mel, wav = self._front_end(dec, rates, lens, st)
         st.mark('pitch')
         f0_dev, f0s = self._pitch(wav, frames)
@@ -409,7 +396,7 @@ class SVBBeautifier:
             if tuple(eps.shape) != (B, hp['latent_size'], 1):
                 raise ValueError(f'eps must be [{B}, {hp["latent_size"]}, 1], got {tuple(eps.shape)}')
         st = _Stages(self.timing)
-        st.mark('h2d')
+        st.mark('load')
         mel, wav = self._front_end(dec, rates, lens, st)
         st.mark('pitch')
         f0_dev, f0s = self._pitch(wav, frames)

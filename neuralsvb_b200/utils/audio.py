@@ -3,10 +3,11 @@ sites of librosa.filters.mel in data_gen/tts/data_gen_utils.py:130, modules/hifi
 The STFT / magnitude / mel projection / log themselves run in the fused CUDA kernel
 (csrc/frontend.cu); what stays on the host is the constant mel filterbank and index arithmetic.
 
-Loading audio (``load_wav``, ``resample_batch``): the reference's ``librosa.core.load(path, sr=sr)`` for WAV and FLAC files -- decode
-(FLAC on the GPU, csrc/flac.cu),
-fold to mono, resample with resampy's ``kaiser_best`` filter -- with the resampling in csrc/resample.cu (oracle/resample.py
-states the algorithm)."""
+Loading audio (``load_takes``, ``load_wav``): the reference's ``librosa.core.load(path, sr=sr)`` for WAV and FLAC files -- decode
+(WAV on the host, FLAC on the GPU, csrc/flac.cu), fold to mono, resample with resampy's ``kaiser_best`` filter -- with the
+resampling in csrc/resample.cu (oracle/resample.py states the algorithm).  ``load_takes`` is the one route to the device: one
+host-to-device copy of the samples decoded on the host, FLAC samples left where they were decoded, and one resampler call over the
+off-rate takes.  ``load_wav``, ``read_wav``'s FLAC branch and ``resample_batch`` are that route with a copy back to the host."""
 import ctypes
 import functools
 import struct
@@ -228,11 +229,10 @@ def _flac_error(msg, names):
 def read_wav(path):
     """(float32 mono samples, file rate) of a WAV or FLAC file (recognised by its magic bytes), decoded as ``librosa.load``
     documents: integer PCM / 2^(bits - 1) (scipy returns 24-bit WAV as left-justified int32; FLAC 8-bit is signed), uint8 WAV as
-    (x - 128) / 128, float as is; channels averaged in float32.  A FLAC file is decoded on the GPU (``flac_decode_device``)."""
+    (x - 128) / 128, float as is; channels averaged in float32.  A FLAC file is decoded on the GPU (``load_wav`` at its own rate);
+    a WAV file needs no device."""
     if is_flac(path):
-        with open(path, 'rb') as f:
-            y, _, rates = flac_decode_device([f.read()], [path])
-        return y.cpu().numpy(), rates[0]
+        return load_wav(path, None)
     from scipy.io import wavfile
     sr, data = wavfile.read(path)
     if data.dtype.kind == 'i':
@@ -269,12 +269,10 @@ def resample_lengths(lengths, orig_srs, target_sr):
 
 def resample_batch(wavs, orig_srs, target_sr):
     """Resample each float32 clip from its own rate to ``target_sr`` with resampy's kaiser_best filter, zero-padded to
-    ceil(n target_sr / sr) samples like ``librosa.resample(..., fix=True)``: ONE device call over the ragged batch
-    (svb_resample_batch_host).  A clip already at target_sr comes back unchanged.  Raises ValueError for a clip too short to
+    ceil(n target_sr / sr) samples like ``librosa.resample(..., fix=True)``: the clips go to the device in one copy, through
+    ``resample_device`` and back.  A clip already at target_sr comes back unchanged.  Raises ValueError for a clip too short to
     yield a sample or a bad rate."""
     import torch
-
-    from neuralsvb_b200 import _native
     wavs = [np.ascontiguousarray(w, dtype=np.float32) for w in wavs]
     if not wavs:
         return []
@@ -284,19 +282,11 @@ def resample_batch(wavs, orig_srs, target_sr):
     _, out_lens = resample_lengths(lens, srs, target_sr)
     if not torch.cuda.is_available():
         raise RuntimeError('resample_batch runs on CUDA: neuralsvb_b200 has no CPU fallback')
-    device = torch.device('cuda', torch.cuda.current_device())
-    win, num_table = kaiser_best_window()
-    cat = np.ascontiguousarray(np.concatenate(wavs))
-    out = np.empty(max(int(out_lens.sum()), 1), np.float32)
-    lib = _native.lib()
-    with torch.cuda.device(device):
-        _native.check(lib.svb_resample_batch_host(int(target_sr), srs.ctypes.data_as(ctypes.c_void_p), lens.ctypes.data_as(ctypes.c_void_p),
-                                                  len(wavs), win.ctypes.data_as(ctypes.c_void_p), len(win), num_table,
-                                                  cat.ctypes.data_as(ctypes.c_void_p), out.ctypes.data_as(ctypes.c_void_p),
-                                                  device.index, _native.current_stream_ptr(device)), 'resample')
+    x = torch.from_numpy(np.concatenate(wavs)).to(torch.device('cuda', torch.cuda.current_device()))
+    out = resample_device(x, lens, srs, target_sr).cpu().numpy()
     res, o = [], 0
     for w, sr, n in zip(wavs, srs, out_lens):
-        res.append(w if int(sr) == int(target_sr) else out[o:o + int(n)].copy())
+        res.append(w if int(sr) == int(target_sr) else out[o:o + int(n)])
         o += int(n)
     return res
 
@@ -308,16 +298,18 @@ def resample_device(wav_concat, lengths, orig_srs, target_sr):
     import torch
 
     from neuralsvb_b200 import _native
+    if not (torch.is_tensor(wav_concat) and wav_concat.is_cuda and wav_concat.dtype == torch.float32):
+        raise TypeError('resample_device takes a float32 CUDA tensor')
     srs, lens = _resample_args(orig_srs, lengths)
     if int(lens.sum()) != wav_concat.numel():
         raise ValueError(f'lengths sum to {int(lens.sum())}, the waveform tensor has {wav_concat.numel()} samples')
     win, num_table = kaiser_best_window()
     lib = _native.lib()
+    out_lens = np.zeros(len(lens), np.int64)
     ws_bytes = lib.svb_resample_plan(int(target_sr), srs.ctypes.data_as(ctypes.c_void_p), lens.ctypes.data_as(ctypes.c_void_p),
-                                     len(lens), len(win), num_table, None, None)
+                                     len(lens), len(win), num_table, None, out_lens.ctypes.data_as(ctypes.c_void_p))
     if ws_bytes < 0:
         raise ValueError(lib.svb_last_error().decode('utf-8', 'replace'))
-    _, out_lens = resample_lengths(lens, srs, target_sr)
     x = wav_concat.contiguous()
     out = torch.empty(max(int(out_lens.sum()), 1), device=x.device)
     ws = torch.empty(max(int(ws_bytes), 1), dtype=torch.uint8, device=x.device)
@@ -330,10 +322,66 @@ def resample_device(wav_concat, lengths, orig_srs, target_sr):
     return out[:int(out_lens.sum())]
 
 
+def decode_wavs(takes, sr, device=None):
+    """[(float32 mono samples, rate)] of each take, decoded as ``read_wav`` does; a float32 array is taken to be at sr already, and a
+    (samples, rate) pair, as this function returns it, is passed through.  WAV files and arrays stay numpy arrays and make no CUDA
+    call.  The FLAC files of a call are read into one host buffer and decoded together (``flac_decode_device``: one copy of the
+    compressed bytes to ``device``, one svb_flac_decode_batch); their samples stay there as CUDA tensors."""
+    import torch
+    out = [None] * len(takes)
+    flac = [i for i, w in enumerate(takes) if isinstance(w, str) and is_flac(w)]
+    for i, w in enumerate(takes):
+        if isinstance(w, tuple):
+            out[i] = w
+        elif isinstance(w, str):
+            if i not in flac:
+                out[i] = read_wav(w)
+        else:
+            out[i] = (np.ascontiguousarray(w, dtype=np.float32), sr)
+    if flac:
+        blobs = []
+        for i in flac:
+            with open(takes[i], 'rb') as f:
+                blobs.append(f.read())
+        y, lens, rates = flac_decode_device(blobs, [takes[i] for i in flac], device)
+        for i, piece, r in zip(flac, torch.split(y, [int(n) for n in lens]), rates):
+            out[i] = (piece, r)
+    return out
+
+
+def load_takes(takes, sr, device=None):
+    """The takes -- WAV or FLAC paths at any rate, float32 arrays at ``sr``, or ``decode_wavs``' (samples, rate) pairs -- as
+    ``librosa.core.load(path, sr=sr)`` reads them, on the device: (float32 CUDA tensor of the takes back to back at ``sr``, int64
+    numpy lengths).  One host-to-device copy of all samples decoded on the host; FLAC takes are decoded on the device and stay
+    there; the off-rate takes go through one ``resample_device`` call."""
+    import torch
+    if not torch.cuda.is_available():
+        raise RuntimeError('load_takes runs on CUDA: neuralsvb_b200 has no CPU fallback')
+    device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
+    dec = decode_wavs(takes, sr, device)
+    pieces = [w for w, _ in dec]
+    host = [k for k, w in enumerate(pieces) if not torch.is_tensor(w)]
+    if host:
+        up = torch.from_numpy(np.concatenate([pieces[k] for k in host])).to(device)
+        for k, p in zip(host, torch.split(up, [len(pieces[k]) for k in host])):
+            pieces[k] = p
+    off = [k for k, (_, r) in enumerate(dec) if r != sr]
+    if off:
+        n_in, rates = [len(pieces[k]) for k in off], [dec[k][1] for k in off]
+        y = resample_device(torch.cat([pieces[k] for k in off]), n_in, rates, sr)
+        for k, p in zip(off, torch.split(y, [int(n) for n in resample_lengths(n_in, rates, sr)[1]])):
+            pieces[k] = p
+    lens = np.array([len(p) for p in pieces], np.int64)
+    if len(host) == len(dec) and not off:
+        return up, lens                             # already back to back
+    return torch.cat(pieces), lens
+
+
 def load_wav(path, sr=22050):
     """``librosa.core.load(path, sr=sr)`` for a WAV or FLAC file: (float32 mono samples at ``sr``, sr); ``sr=None`` keeps the file's
-    rate."""
-    data, file_sr = read_wav(path)
+    rate.  A WAV file at ``sr`` needs no device; a file at another rate goes through ``load_takes`` and back."""
+    dec = decode_wavs([path], sr)
+    y, file_sr = dec[0]
     if sr is None or file_sr == sr:
-        return data, file_sr
-    return resample_batch([data], [file_sr], sr)[0], sr
+        return (y if isinstance(y, np.ndarray) else y.cpu().numpy()), file_sr
+    return load_takes(dec, sr)[0].cpu().numpy(), sr

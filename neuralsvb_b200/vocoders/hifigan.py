@@ -3,7 +3,8 @@
 Same surface as the reference class (vocoders/hifigan.py:39-69 + PWG.wav2spec,
 vocoders/pwg.py:105-122): no-arg constructor reading ``hparams['vocoder_ckpt']``,
 ``spec2wav(mel[T,80], f0=[T]) -> np.float32[T*hop]``, static ``wav2spec(wav_fn)``,
-registered under the names ``HifiGAN`` / ``hifigan``.
+registered under the names ``HifiGAN`` / ``hifigan``.  ``wav2spec`` / ``wav2spec_batch`` load their takes with
+``utils.audio.load_takes`` and run ``wav2spec_device`` (svb_wav2spec_batch) on them.
 """
 import ctypes
 import glob
@@ -57,49 +58,6 @@ def stft_config(hp, pad_mode, out_kind, eps, frames_major=1, clamp=0):
     c.pad_mode, c.out_kind, c.clamp_input = pad_mode, out_kind, clamp
     c.n_mels, c.frames_major, c.eps = int(hp['audio_num_mel_bins']), frames_major, float(eps)
     return c
-
-
-def _load_wav(wav_fn, sr):
-    """librosa.core.load(wav_fn, sr=sr) for a WAV or FLAC file (utils/audio.load_wav): decoded, mono, resampled on the GPU when the file's
-    rate is not sr."""
-    return audio.load_wav(wav_fn, sr)[0]
-
-
-def decode_wavs(wav_fns, sr, device=None):
-    """[(float32 mono samples, rate)] of each path, decoded as utils/audio.read_wav does; arrays are taken to be at sr already.
-    The FLAC paths of a call are read into one host buffer and decoded together: one copy of the compressed bytes to the device and
-    one svb_flac_decode_batch.  ``device`` given: a FLAC take's samples stay there (a CUDA tensor, for callers that assemble their
-    input on the device); otherwise they come back to the host as numpy arrays like every other take."""
-    out = [None] * len(wav_fns)
-    flac = [i for i, w in enumerate(wav_fns) if isinstance(w, str) and audio.is_flac(w)]
-    for i, w in enumerate(wav_fns):
-        if isinstance(w, str):
-            if i not in flac:
-                out[i] = audio.read_wav(w)
-        else:
-            out[i] = (np.ascontiguousarray(w, dtype=np.float32), sr)
-    if flac:
-        blobs = []
-        for i in flac:
-            with open(wav_fns[i], 'rb') as f:
-                blobs.append(f.read())
-        y, lens, rates = audio.flac_decode_device(blobs, [wav_fns[i] for i in flac], device)
-        if device is None:
-            y = y.cpu().numpy()
-        for i, piece, r in zip(flac, torch.split(y, [int(n) for n in lens]) if device is not None else np.split(y, np.cumsum(lens)[:-1]),
-                               rates):
-            out[i] = (piece, r)
-    return out
-
-
-def _load_wavs(wav_fns, sr):
-    """Decode every path (arrays are taken to be at sr already), then resample all off-rate files in ONE device call."""
-    wavs, rates = [list(x) for x in zip(*decode_wavs(wav_fns, sr))] if wav_fns else ([], [])
-    off = [i for i, r in enumerate(rates) if r != sr]
-    if off:
-        for i, y in zip(off, audio.resample_batch([wavs[i] for i in off], [rates[i] for i in off], sr)):
-            wavs[i] = y
-    return wavs
 
 
 @register_vocoder
@@ -230,40 +188,20 @@ class HifiGAN(BaseVocoder):
     def wav2spec_batch(wav_fns, hp=None):
         """The binarizer's per-file ``wav2spec`` loop (data_gen/tts/base_binarizer.py:168-178,
         data_gen/singing/binarize_para.py:116-217) as ONE device call over a ragged batch: list of paths / float arrays
-        -> list of (wav [T*hop], mel [T, n_mel] log10), identical to ``wav2spec`` clip by clip
-        (svb_wav2spec_batch_host: one H2D, one launch over all frames of all clips, one D2H).  Files at another rate than
-        audio_sample_rate are first resampled together in one ``audio.resample_batch`` call."""
+        -> list of host (wav [T*hop], mel [T, n_mel] log10), identical to ``wav2spec`` clip by clip.  The takes reach the device
+        through ``audio.load_takes`` (files at another rate than audio_sample_rate resampled together there), then
+        ``wav2spec_device``; the mels and the padded waveforms come back in one copy each."""
         hp = hparams if hp is None else hp
         device = _require_cuda()
         if hp.get('loud_norm', False):
             raise NotImplementedError('loud_norm (pyloudnorm BS.1770) is data preparation, outside this path')
-        wavs = _load_wavs(wav_fns, hp['audio_sample_rate'])
-        if not wavs:
+        if not wav_fns:
             return []
-        lib = _native.lib()
-        cfg = stft_config(hp, _native.PAD_CENTER_ZERO, _native.OUT_LOG10_MEL, float(hp.get('wav2spec_eps', 1e-10)))
-        lengths = np.array([len(w) for w in wavs], np.int64)
-        frames = lengths // cfg.hop + 1
-        cat = np.ascontiguousarray(np.concatenate(wavs))
-        basis = np.ascontiguousarray(audio.build_mel_basis(hp))
-        mel = np.empty((int(frames.sum()), cfg.n_mels), np.float32)
-        got = np.zeros(len(wavs), np.int64)
-        with torch.cuda.device(device):
-            rc = lib.svb_wav2spec_batch_host(ctypes.byref(cfg), cat.ctypes.data_as(ctypes.c_void_p),
-                                             lengths.ctypes.data_as(ctypes.c_void_p), len(wavs),
-                                             basis.ctypes.data_as(ctypes.c_void_p), mel.ctypes.data_as(ctypes.c_void_p),
-                                             got.ctypes.data_as(ctypes.c_void_p), device.index,
-                                             _native.current_stream_ptr(device))
-            _native.check(rc, 'wav2spec_batch')
-        assert np.array_equal(got, frames), (got, frames)
-        out, o = [], 0
-        for w, fr in zip(wavs, frames):
-            n_out = int(fr) * cfg.hop                       # audio.librosa_pad_lr + wav[:T * hop] (data_gen_utils.py:138-140)
-            wo = np.zeros(n_out, np.float32)
-            wo[:min(len(w), n_out)] = w[:n_out]
-            out.append((wo, mel[o:o + int(fr)]))
-            o += int(fr)
-        return out
+        x, lengths = audio.load_takes(wav_fns, hp['audio_sample_rate'], device)
+        mel, wav, frames = HifiGAN.wav2spec_device(x, lengths, hp)
+        mel, wav = mel.cpu().numpy(), wav.cpu().numpy()
+        offs, hop = np.concatenate([[0], np.cumsum(frames)]), int(hp['hop_size'])
+        return [(wav[a * hop:b * hop], mel[a:b]) for a, b in zip(offs[:-1], offs[1:])]
 
     @staticmethod
     def wav2spec_device(wav_concat, lengths, hp=None, mel_basis=None):
@@ -303,32 +241,15 @@ class HifiGAN(BaseVocoder):
     def wav2spec(wav_fn, return_linear=False, hp=None):
         """wav file path (any sample rate: resampled like librosa.core.load) or float array at audio_sample_rate ->
         (wav [T*hop], mel [T, n_mel] log10)
-        [+ normalised dB linear spectrogram [T, n_fft/2+1]]   (vocoders/pwg.py:105-122)."""
+        [+ normalised dB linear spectrogram [T, n_fft/2+1]]   (vocoders/pwg.py:105-122): ``wav2spec_batch`` of one take."""
         hp = hparams if hp is None else hp
-        device = _require_cuda()
-        if hp.get('loud_norm', False):
-            raise NotImplementedError('loud_norm (pyloudnorm BS.1770) is data preparation, outside this path')
-        wav = _load_wav(wav_fn, hp['audio_sample_rate']) if isinstance(wav_fn, str) \
-            else np.ascontiguousarray(wav_fn, dtype=np.float32)
-        eps = float(hp.get('wav2spec_eps', 1e-10))
-        lib = _native.lib()
-        cfg = stft_config(hp, _native.PAD_CENTER_ZERO, _native.OUT_LOG10_MEL, eps)
-        frames = int(lib.svb_stft_num_frames(ctypes.byref(cfg), len(wav)))
-        basis = np.ascontiguousarray(audio.build_mel_basis(hp))
-        mel = np.empty((frames, cfg.n_mels), np.float32)
-        wav_out = np.empty(frames * cfg.hop, np.float32)
-        with torch.cuda.device(device):
-            st = _native.current_stream_ptr(device)
-            rc = lib.svb_wav2spec_host(ctypes.byref(cfg), wav.ctypes.data_as(ctypes.c_void_p), len(wav),
-                                       basis.ctypes.data_as(ctypes.c_void_p), mel.ctypes.data_as(ctypes.c_void_p),
-                                       wav_out.ctypes.data_as(ctypes.c_void_p), device.index, st)
-            _native.check(rc, 'wav2spec')
-            if not return_linear:
-                return wav_out, mel
-            cfg2 = stft_config(hp, _native.PAD_CENTER_ZERO, _native.OUT_MAG_RAW, 0.0)
-            w = torch.from_numpy(wav).to(device)
-            lin = torch.empty(frames, cfg.n_fft // 2 + 1, device=device)
-            _native.check(lib.svb_stft_forward(ctypes.byref(cfg2), _native.ptr(w), 1, len(wav), None,
-                                               _native.ptr(lin), st), 'stft_forward')
-            lin = audio.normalize(audio.amp_to_db(lin.cpu().numpy()), hp)
-        return wav_out, mel, lin
+        wav, mel = HifiGAN.wav2spec_batch([wav_fn], hp)[0]
+        if not return_linear:
+            return wav, mel
+        x, n = audio.load_takes([wav_fn], hp['audio_sample_rate'])     # the linear spectrogram is of the unpadded samples
+        cfg = stft_config(hp, _native.PAD_CENTER_ZERO, _native.OUT_MAG_RAW, 0.0)
+        lin = torch.empty(len(mel), cfg.n_fft // 2 + 1, device=x.device)
+        with torch.cuda.device(x.device):
+            _native.check(_native.lib().svb_stft_forward(ctypes.byref(cfg), _native.ptr(x), 1, int(n[0]), None, _native.ptr(lin),
+                                                         _native.current_stream_ptr(x.device)), 'stft_forward')
+        return wav, mel, audio.normalize(audio.amp_to_db(lin.cpu().numpy()), hp)

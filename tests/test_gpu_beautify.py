@@ -212,7 +212,7 @@ def test_cli_writes_what_save_wav_writes_from_the_api(exp22, tmp_path):
         assert open(fn, 'rb').read() == open(ref, 'rb').read(), fn
 
 
-def test_device_front_end_matches_the_host_entry_on_a_ragged_batch():
+def test_device_front_end_matches_per_clip_calls_and_the_host_wrapper_on_a_ragged_batch():
     from neuralsvb_b200.vocoders.hifigan import HifiGAN, stft_config
     hp = {'fft_size': 512, 'hop_size': 128, 'win_size': 512, 'audio_num_mel_bins': 80, 'audio_sample_rate': 22050, 'fmin': 50,
           'fmax': 11025}
@@ -223,15 +223,17 @@ def test_device_front_end_matches_the_host_entry_on_a_ragged_batch():
     lib = _native.lib()
     cfg = stft_config(hp, _native.PAD_CENTER_ZERO, _native.OUT_LOG10_MEL, 1e-10)
     lens = np.array(lengths, np.int64)
-    mel_h = np.full((int(frames.sum()), 80), np.nan, np.float32)
-    basis = np.ascontiguousarray(audio.build_mel_basis(hp))
-    assert lib.svb_wav2spec_batch_host(ctypes.byref(cfg), cat.ctypes.data_as(ctypes.c_void_p), lens.ctypes.data_as(ctypes.c_void_p),
-                                       len(lens), basis.ctypes.data_as(ctypes.c_void_p), mel_h.ctypes.data_as(ctypes.c_void_p), None, 0,
-                                       None) == frames.sum()
     assert frames.tolist() == [1 + n // 128 for n in lengths]
-    assert np.array_equal(mel_d.cpu().numpy(), mel_h)
+    offs = np.concatenate([[0], np.cumsum(frames)])
+    for k, c in enumerate(clips):
+        mel1, wav1, _ = HifiGAN.wav2spec_device(torch.from_numpy(c).cuda(), lengths[k:k + 1], hp)
+        assert torch.equal(mel_d[offs[k]:offs[k + 1]], mel1) and torch.equal(wav_d[offs[k] * 128:offs[k + 1] * 128], wav1), k
+    host = HifiGAN.wav2spec_batch(clips, hp)
+    assert np.array_equal(np.concatenate([m for _, m in host]), mel_d.cpu().numpy())
+    assert np.array_equal(np.concatenate([w for w, _ in host]), wav_d.cpu().numpy())
     pad = np.concatenate([np.concatenate([c, np.zeros(f * 128 - len(c), np.float32)]) for c, f in zip(clips, frames)])
     assert np.array_equal(wav_d.cpu().numpy(), pad)
+    basis = np.ascontiguousarray(audio.build_mel_basis(hp))
     ws = lib.svb_wav2spec_workspace_bytes(ctypes.byref(cfg), lens.ctypes.data_as(ctypes.c_void_p), len(lens), None)
     assert ws > 0
     buf = torch.empty(int(ws), dtype=torch.uint8, device='cuda')

@@ -37,7 +37,7 @@ from tests import gpu_util as U
 from tests.test_gpu_generator_forward import (BARS, MARGIN, compare, describe, group_errors, judge, make_model, ref_weights,
                                               say, schedules)
 from tests.test_gpu_generator_ragged import alone, bits_equal, clip_errors, run
-from tests.test_gpu_stft_kernels import (FWD_TOL, LOG10_MEL, ZERO, assert_clear_of_eps, errors, make_wave,
+from tests.test_gpu_stft_kernels import (FWD_TOL, LOG10_MEL, ZERO, assert_clear_of_eps, errors, make_wave, run_wav2spec,
                                          stft_reference)
 
 pytestmark = pytest.mark.gpu
@@ -73,8 +73,7 @@ def hop_of(h):
 
 
 # ------------------------------------------------------------------ 1. the singing front end
-def test_singing_front_end_on_a_long_ragged_batch_matches_float64_and_single_clip_calls(capfd):
-    lib = _native.lib()
+def test_singing_front_end_on_a_long_ragged_batch_matches_float64_and_single_clip_device_calls(capfd):
     cfg = (HP['fft_size'], HOP, HP['win_size'], ZERO, LOG10_MEL, 0, HP['audio_num_mel_bins'], 1, EPS)
     c = _native.StftConfig(*cfg)
     # 1 sample; 127 / 128 / 129 samples (around one hop); a 60-frame take; 8 s; exactly max_frames frames; one clip beyond
@@ -103,10 +102,10 @@ def test_singing_front_end_on_a_long_ragged_batch_matches_float64_and_single_cli
         fr = int(frames[i])
         m, w = mel[off:off + fr], wav[off * HOP:(off + fr) * HOP]
         off += fr
-        single = torch.full((fr, cfg[6]), float('nan'))
-        single_wav = torch.full((fr * HOP,), float('nan'))
-        assert lib.svb_wav2spec_host(ctypes.byref(c), _native.ptr(x.contiguous()), L, _native.ptr(basis), _native.ptr(single),
-                                     _native.ptr(single_wav), 0, None) == fr
+        single = torch.full((fr, cfg[6]), float('nan'), device='cuda')
+        single_wav = torch.full((fr * HOP,), float('nan'), device='cuda')
+        assert run_wav2spec(c, x.cuda(), [L], basis.cuda(), single, single_wav) == fr
+        single, single_wav = single.cpu(), single_wav.cpu()
         assert torch.equal(m, single), f'clip {i} (length {L}): the batch differs from its single-clip call'
         lpad, rpad = FE.librosa_pad_lr(x.numpy(), HP['fft_size'], HOP)
         want = np.pad(x.numpy(), (lpad, rpad))[:fr * HOP]

@@ -1,5 +1,5 @@
 """-m gpu: the fused STFT front end (svb_stft_forward = stft_mel_v2_kernel, svb_stft_backward = stft_mel_bwd_kernel,
-svb_wav2spec_batch_host) against float64 torch.stft on the same fp32 waveform, per output kind and padding mode as
+svb_wav2spec_batch) against float64 torch.stft on the same fp32 waveform, per output kind and padding mode as
 include/svb_vocoder.h documents them, at the product configurations and at the edges of the kernels: n_fft 64 / 4096,
 mel filters read from global memory, hops that do not divide n_fft, partial last CTAs, the shortest legal reflect clips,
 input clamping, empty mel rows, silence (magnitude floor and log clamps) and ragged batches.  The backward is compared
@@ -199,6 +199,19 @@ def run_forward(cfg, wav, basis):
     return out
 
 
+def run_wav2spec(c, wav, lengths, basis, mel, wav_out=None, frames=None):
+    """svb_wav2spec_batch (StftConfig c) of the clips back to back in the CUDA tensor wav, into the CUDA tensors mel / wav_out and
+    the host int64 array frames (both may be None), with a workspace of the size svb_wav2spec_workspace_bytes gives -> its return
+    value."""
+    lib = _native.lib()
+    lens = np.ascontiguousarray(lengths, np.int64)
+    ws = lib.svb_wav2spec_workspace_bytes(ctypes.byref(c), lens.ctypes.data_as(ctypes.c_void_p), len(lens), None)
+    buf = torch.empty(int(ws), dtype=torch.uint8, device='cuda')
+    return lib.svb_wav2spec_batch(ctypes.byref(c), _native.ptr(wav), lens.ctypes.data_as(ctypes.c_void_p), len(lens), _native.ptr(basis),
+                                  _native.ptr(mel), _native.ptr(wav_out), None if frames is None else frames.ctypes.data_as(ctypes.c_void_p),
+                                  ctypes.c_void_p(buf.data_ptr()), int(ws), None)
+
+
 def run_backward(cfg, wav, basis, dout):
     B, n = wav.shape
     dwav = torch.zeros_like(wav)
@@ -242,22 +255,19 @@ def test_stft_forward_and_backward_match_float64_torch(case):
     assert not backward or _within(e['dwav'], BWD_TOL_ILL.get(tag, BWD_TOL)), (tag, e)
 
 
-def test_wav2spec_ragged_batch_matches_single_clip_calls_and_float64_torch():
+def test_wav2spec_ragged_batch_matches_single_clip_device_calls_and_float64_torch():
     """Clips of 1-5 frames between long ones in ONE launch: every clip's block range is found by the binary search over the
     clip table; each clip must equal its own single-clip call (bit for bit) and the float64 reference."""
-    lib = _native.lib()
     cfg = (1024, 256, 1024, ZERO, LOG10_MEL, 0, 80, 1, 1e-10)
     c = _native.StftConfig(*cfg)
     lengths = [8192, 1, 300, 5000, 600, 773, 1024, 7001, 17, 1280, 4096]
     clips = [make_wave(1, L, ('ragged', i))[0] for i, L in enumerate(lengths)]
-    basis = make_basis('loss80', 1024, 80)
-    wav_cat = torch.cat(clips).contiguous()
-    lens = np.asarray(lengths, np.int64)
+    basis = make_basis('loss80', 1024, 80).cuda()
+    wav_cat = torch.cat(clips).cuda()
     fr = np.zeros(len(lengths), np.int64)
     total = sum(1 + L // 256 for L in lengths)
-    mel = torch.full((total, 80), float('nan'))
-    got = lib.svb_wav2spec_batch_host(ctypes.byref(c), _native.ptr(wav_cat), lens.ctypes.data_as(ctypes.c_void_p), len(lengths),
-                                      _native.ptr(basis), _native.ptr(mel), fr.ctypes.data_as(ctypes.c_void_p), 0, None)
+    mel = torch.full((total, 80), float('nan'), device='cuda')
+    got = run_wav2spec(c, wav_cat, lengths, basis, mel, frames=fr)
     assert _native.check(got, 'wav2spec_batch') == total
     assert fr.tolist() == [1 + L // 256 for L in lengths] and {1, 2, 3, 4, 5} <= set(fr.tolist())
     off = 0
@@ -265,13 +275,12 @@ def test_wav2spec_ragged_batch_matches_single_clip_calls_and_float64_torch():
     for i, (L, x) in enumerate(zip(lengths, clips)):
         m = mel[off:off + fr[i]]
         off += fr[i]
-        single = torch.full((fr[i], 80), float('nan'))
-        assert lib.svb_wav2spec_host(ctypes.byref(c), _native.ptr(x.contiguous()), L, _native.ptr(basis), _native.ptr(single), None, 0,
-                                     None) == fr[i]
+        single = torch.full((fr[i], 80), float('nan'), device='cuda')
+        assert run_wav2spec(c, x.cuda(), [L], basis, single) == fr[i]
         assert torch.equal(m, single), f'clip {i} (length {L}) differs from its single-clip call'
-        ref, ratio = stft_reference(x[None].cuda(), cfg, basis.cuda())
+        ref, ratio = stft_reference(x[None].cuda(), cfg, basis)
         assert_clear_of_eps(ratio, f'clip {i}')
-        e = errors(m.cuda(), ref[0])
+        e = errors(m, ref[0])
         worst = max(worst, e)
         assert _within(e, FWD_TOL), (i, L, e)
     print('MEASURED ragged', f'{worst[0]:.2e}/{worst[1]:.2e}')
