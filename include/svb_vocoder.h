@@ -520,6 +520,40 @@ int64_t svb_sadtw_long_workspace_bytes(int32_t n_pairs, const int32_t *src_len_h
 int svb_sadtw_align_long(const void *src_f0_dev, const void *tgt_f0_dev, int32_t dtype, int32_t variant, int32_t n_pairs,
                          const int32_t *src_len_host, const int32_t *tgt_len_host, const double *tgt_scale_host, void *workspace_dev,
                          int64_t workspace_bytes, int64_t *alignment_dev, float *path_cost_dev, float *stage_ms_host, void *stream);
+/* Whole songs in bounded device memory: svb_sadtw_align_striped computes what svb_sadtw_align_long computes, bit for bit (same
+ * arguments and limits, plus budget_bytes), in a workspace of at most budget_bytes.  Every pair's anti-diagonals are cut into
+ * stripes of K diagonals; a stripe's cost is computed into one of two stripe buffers (K x min(S, T) floats per pair) on a side
+ * stream while the DTW runs the stripe before it on the caller's stream, starting from the two diagonals before the stripe (a
+ * checkpoint slot of 2 x min(S, T) floats per pair).
+ *   SVB_SADTW_SINGLE_PASS: one forward pass writes every direction byte (S x T bytes per pair, the skewed layout), then the
+ *     backtrack runs once.  Chosen when it fits the budget, at K = min(512, longest S + T - 1).
+ *   SVB_SADTW_CHECKPOINTED: the forward pass keeps the last two diagonals of every stripe and no direction; the backward pass
+ *     recomputes each stripe's cost and DTW from the last stripe to the first, with stripe-local directions (K x min(S, T) bytes
+ *     per pair), and continues the backtrack over it.  About twice the work; memory linear in length.  K is the largest power of
+ *     two <= 8192 that fits the budget.
+ * svb_sadtw_striped_plan (host only, no CUDA call) fills *plan for these lengths and budget: the mode, K, the stripe count
+ *   ceil(max(S + T - 1) / K), the section offsets [seq metas, pair metas, stripe metas, histograms, 2 stripe cost buffers,
+ *   directions, checkpoint slots (ceil((S + T - 1) / K) per pair, 1 in single pass), walk states (16 B per pair)], the total
+ *   (the workspace svb_sadtw_align_striped needs) and the smallest budget it would accept.  It validates the lengths as
+ *   svb_sadtw_long_workspace_bytes does and refuses (SVB_ERR_INVALID) a budget below that minimum, naming it.  The environment
+ *   variable SVB_DTW_STRIPE_DIAGS=<1 .. 131072>, read per call, forces the checkpointed mode at that K (a test and measurement
+ *   hook); a forced K whose workspace exceeds the budget is refused.  SVB_DTW_CTA_CELLS acts as in svb_sadtw_align_long.
+ * svb_sadtw_align_striped refuses a workspace smaller than the plan's total.  stage_ms_host receives (histogram, forward,
+ *   backward, backtrack): forward is the caller's stream from the end of the histograms to the last stripe's DTW, which includes
+ *   waiting for stripe costs not hidden under the DTW; backward is the checkpointed backward pass (costs, DTW and backtrack
+ *   stripe by stripe; 0 in single pass), backtrack the single pass's backtrack (0 when checkpointed). */
+typedef enum svb_sadtw_stripe_mode { SVB_SADTW_SINGLE_PASS = 0, SVB_SADTW_CHECKPOINTED = 1 } svb_sadtw_stripe_mode;
+typedef struct svb_sadtw_stripe_plan {
+    int32_t mode, stripe_diags, stripes, reserved;
+    int64_t offsets[8];
+    int64_t total_bytes, min_budget_bytes;
+} svb_sadtw_stripe_plan;
+int svb_sadtw_striped_plan(int32_t n_pairs, const int32_t *src_len_host, const int32_t *tgt_len_host, int64_t budget_bytes,
+                           svb_sadtw_stripe_plan *plan);
+int svb_sadtw_align_striped(const void *src_f0_dev, const void *tgt_f0_dev, int32_t dtype, int32_t variant, int32_t n_pairs,
+                            const int32_t *src_len_host, const int32_t *tgt_len_host, const double *tgt_scale_host, void *workspace_dev,
+                            int64_t workspace_bytes, int64_t budget_bytes, int64_t *alignment_dev, float *path_cost_dev,
+                            float *stage_ms_host, void *stream);
 /* The histogram kernel alone (cal_hist_of_f0(f, max_window=64, scale_factor=scale[k])): n_seq sequences concatenated in f0_dev,
  * hist_dev float32 [sum len, 48] = k / total (normalize_hist=True), counts_dev int32 [sum len, 48] = k (NULL = not wanted).
  * The workspace holds the per-sequence metadata (svb_sadtw_histogram_workspace_bytes). */

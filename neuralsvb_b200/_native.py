@@ -207,6 +207,8 @@ _PROTOS = {
     'svb_sadtw_align': (ctypes.c_int, [_P, _P, _I32, _I32, _I32, _P, _P, _P, _P, _I64, _P, _P, _P, _P]),
     'svb_sadtw_long_workspace_bytes': (_I64, [_I32, _P, _P, _P]),
     'svb_sadtw_align_long': (ctypes.c_int, [_P, _P, _I32, _I32, _I32, _P, _P, _P, _P, _I64, _P, _P, _P, _P]),
+    'svb_sadtw_striped_plan': (ctypes.c_int, [_I32, _P, _P, _I64, _P]),
+    'svb_sadtw_align_striped': (ctypes.c_int, [_P, _P, _I32, _I32, _I32, _P, _P, _P, _P, _I64, _I64, _P, _P, _P, _P]),
     'svb_sadtw_histogram_workspace_bytes': (_I64, [_I32]),
     'svb_sadtw_histogram': (ctypes.c_int, [_P, _I32, _I32, _I32, _P, _P, _P, _I64, _P, _P, _P]),
     'svb_sadtw_cost': (ctypes.c_int, [_P, _I32, _P, _I32, _P, _P]),

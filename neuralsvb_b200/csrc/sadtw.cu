@@ -11,7 +11,8 @@
 //      of svb_sadtw_align_long (min(S, T) > 8192) walks them on a thread-block cluster instead (dtw_cluster_kernel);
 //   4. backtrack: one thread per pair follows the direction bytes from the last cell (align_from_distances).
 // The float DTW matrix never goes to HBM on this path.  Nothing is accumulated across pairs and there are no atomics, so a pair's
-// result does not depend on the batch it is in.
+// result does not depend on the batch it is in.  svb_sadtw_align_striped runs steps 2-4 stripe by stripe of anti-diagonals in a
+// bounded workspace, with the same cells and results (the STRIPE variants of the cost and DTW kernels, backtrack_stripe_kernel).
 //
 // Numerics follow the reference's Python / numpy / torch arithmetic bit for bit: every division and product is an explicit
 // round-to-nearest intrinsic (no FMA contraction can move a slope across a region threshold), the f0 arithmetic runs in the input's
@@ -66,6 +67,30 @@ __host__ __device__ __forceinline__ int diag_lo(int d, int C) { return d - C + 1
 __host__ __device__ __forceinline__ int64_t skew_index(int i, int j, int R, int C) {
     return diag_start(i + j, R, C) + i - diag_lo(i + j, C);
 }
+// cells of anti-diagonal d (<= 0 for d < 0)
+__host__ __device__ __forceinline__ int diag_len(int d, int R, int C) { return min(d, R - 1) - diag_lo(d, C) + 1; }
+
+// ---- striped alignment (svb_sadtw_align_striped) ------------------------------------------------------------------------------
+// The anti-diagonals [0, D) of every pair are cut into stripes [d0, d1) of K diagonals, the same cuts for all pairs of a call.  A
+// stripe's costs go to a stripe buffer of K x min(R, C) floats per pair, at the skewed offset minus diag_start(d0); the DTW of a
+// stripe starts from the two diagonals before d0, read from a checkpoint slot (2 x min(R, C) floats, indexed by i - lo(d)), and
+// writes its own last two diagonals to a slot.
+struct StripePair {
+    int64_t cost_off;               // first float of the pair in each stripe cost buffer
+    int64_t dir_off;                // first direction byte of the pair (single pass: cell_off, the global skewed layout)
+    int64_t ckpt_off;               // first float of the pair's checkpoint slots
+};
+
+struct Stripe {
+    const StripePair *pairs;
+    float *ckpt;
+    int d0, d1;                     // a pair runs [d0, min(d1, D)), nothing when d0 >= D
+    int slot_in, slot_out;          // slot read when d0 > 0 / written with the stripe's last two diagonals (-1: none)
+    int local_dirs;                 // directions at stripe-local offsets (checkpointed backward pass), else global
+    int nj;                         // the cost launch's tiles per tile row
+};
+
+__host__ __device__ __forceinline__ int floor_div(int a, int b) { return a >= 0 ? a / b : -((-a + b - 1) / b); }
 
 // int(b * scale) (truncation toward zero), then a left boundary of 0 becomes 1 (cal_hist_of_f0)
 void scaled_windows(int variant, double scale, int32_t *lo, int32_t *hi) {
@@ -186,13 +211,42 @@ __device__ __forceinline__ float chi_square(const float *a, const float *b) {
 // [32 w, 32 w + 32) of the tile; at step dd lane k computes cell (k, (dd - k) mod 32), so a warp's 32 cells lie on two
 // anti-diagonals, consecutive rows on each: two contiguous runs of the skewed layout per store.
 constexpr int kTileI = 32, kTileJ = 128, kRowStride = 52;
+
+// the tile rows [lo, hi] of an R x C pair that meet the diagonals [d0, d1) (d0 < d1 <= R + C - 1): row t has a cell with
+// i + j >= d0 iff 32 t + 31 + C - 1 >= d0, and one with i + j < d1 iff 32 t < d1
+__host__ __device__ __forceinline__ void stripe_rows(int R, int C, int d0, int d1, int &lo, int &hi) {
+    lo = max(0, -floor_div(C + kTileI - 2 - d0, kTileI));
+    hi = min((R - 1) / kTileI, (d1 - 1) / kTileI);
+}
+// tiles per tile row of a stripe of K diagonals: a tile spans kTileI + kTileJ - 1 diagonals
+__host__ __device__ __forceinline__ int stripe_row_tiles(int K) { return (K + kTileI + kTileJ - 3) / kTileJ + 1; }
+
+// STRIPE: grid (tile rows meeting the stripe x s.nj, n_pairs), CTA x takes tile row lo + x / nj, tile column (the first that
+// meets the stripe) + x % nj, and writes only the cells with d0 <= i + j < d1, at stripe-local offsets.
+template <bool STRIPE>
 __global__ void __launch_bounds__(kCostThreads) sadtw_cost_kernel(const float *__restrict__ hist, const PairMeta *__restrict__ pairs,
-                                                                  float *__restrict__ cost) {
+                                                                  float *__restrict__ cost, Stripe s) {
     __shared__ __align__(16) float sb[kTileI * kRowStride], sa[kTileJ * kRowStride];
     const PairMeta p = pairs[blockIdx.y];
     const int R = p.R, C = p.C, tiles_j = (C + kTileJ - 1) / kTileJ;
-    if ((int)blockIdx.x >= tiles_j * ((R + kTileI - 1) / kTileI)) return;
-    const int i0 = (blockIdx.x / tiles_j) * kTileI, j0 = (blockIdx.x % tiles_j) * kTileJ;
+    int i0, j0, d0 = 0, d1 = 0;
+    int64_t base = p.cell_off;
+    if constexpr (STRIPE) {
+        d0 = s.d0, d1 = min(s.d1, R + C - 1);
+        if (d0 >= d1) return;
+        int lo, hi;
+        stripe_rows(R, C, d0, d1, lo, hi);
+        const int ti = lo + (int)blockIdx.x / s.nj;
+        if (ti > hi) return;
+        i0 = ti * kTileI;
+        const int tj = max(0, -floor_div(i0 + kTileI + kTileJ - 2 - d0, kTileJ)) + (int)blockIdx.x % s.nj;
+        if (tj > min(tiles_j - 1, (d1 - 1 - i0) / kTileJ)) return;
+        j0 = tj * kTileJ;
+        base = s.pairs[blockIdx.y].cost_off - diag_start(d0, R, C);
+    } else {
+        if ((int)blockIdx.x >= tiles_j * ((R + kTileI - 1) / kTileI)) return;
+        i0 = (blockIdx.x / tiles_j) * kTileI, j0 = (blockIdx.x % tiles_j) * kTileJ;
+    }
     const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
     for (int q = threadIdx.x; q < (kTileI + kTileJ) * (kBins / 4); q += kCostThreads) {
         const int r = q / (kBins / 4), c = q - r * (kBins / 4);
@@ -207,7 +261,8 @@ __global__ void __launch_bounds__(kCostThreads) sadtw_cost_kernel(const float *_
     if (i >= R) return;
     for (int dd = 0; dd < 32; ++dd) {
         const int jj = w * 32 + ((dd - lane) & 31), j = j0 + jj;
-        if (j < C) cost[p.cell_off + skew_index(i, j, R, C)] = chi_square(sa + jj * kRowStride, sb + lane * kRowStride);
+        if (j < C && (!STRIPE || (i + j >= d0 && i + j < d1)))
+            cost[base + skew_index(i, j, R, C)] = chi_square(sa + jj * kRowStride, sb + lane * kRowStride);
     }
 }
 
@@ -235,19 +290,48 @@ __global__ void skew_kernel(const T *__restrict__ src, int R, int C, T *__restri
 // Shared memory: the anti-diagonals d - 2, d - 1 and d (indexed by i - lo(d)), 3 x maxdiag elements.  Each thread keeps the costs
 // of its cells of the next diagonal in registers, so the load is in flight during the current step.  dirs: one byte per cell
 // (i, j >= 1), skewed.  path_cost[pair] = dtw[R-1, C-1].  FULL: also the whole matrix, row-major, to dtw_full (time_warp).
-template <typename T, bool FULL>
+// STRIPE: the diagonals [s.d0, min(s.d1, D)) only, from the stripe cost buffer, the directions at s.pairs' offsets (none when
+// dirs is null) and the two diagonals before d0 from checkpoint slot s.slot_in; the last two go to slot s.slot_out.  Thread t
+// reads and writes the slot positions t, t + nt, ..., so a slot may be read and written by the same launch.
+template <typename T, bool FULL, bool STRIPE>
 __global__ void __launch_bounds__(kDtwMaxThreads) dtw_kernel(const T *__restrict__ cost, const PairMeta *__restrict__ pairs, PairMeta single,
                                                              int maxdiag, uint8_t *__restrict__ dirs, T *__restrict__ path_cost,
-                                                             T *__restrict__ dtw_full) {
+                                                             T *__restrict__ dtw_full, Stripe s) {
     extern __shared__ __align__(16) unsigned char dtw_smem[];
     const PairMeta p = pairs ? pairs[blockIdx.x] : single;
     const int R = p.R, C = p.C, D = R + C - 1, nt = blockDim.x;
     if (min(R, C) > maxdiag) return;            // a long pair of svb_sadtw_align_long: dtw_cluster_kernel's
-    const T *cp = cost + p.cell_off;
-    uint8_t *dp = dirs + p.cell_off;
+    const T *cp;
+    uint8_t *dp;
     T *b2 = reinterpret_cast<T *>(dtw_smem), *b1 = b2 + maxdiag, *b0 = b1 + maxdiag;
     T nxt[kDtwPer];
-    {
+    int dbeg = 0, dend = D;
+    int64_t corg = 0, dorg = 0;                 // skewed offset of the first cell of the cost / direction buffer
+    float *ck = nullptr;
+    if constexpr (STRIPE) {
+        const StripePair q = s.pairs[blockIdx.x];
+        dbeg = s.d0, dend = min(s.d1, D);
+        if (dbeg >= dend) return;
+        corg = diag_start(dbeg, R, C), dorg = s.local_dirs ? corg : 0;
+        cp = cost + q.cost_off;
+        dp = dirs ? dirs + q.dir_off : nullptr;
+        ck = s.ckpt + q.ckpt_off;
+        const int m = min(R, C);
+        if (dbeg > 0) {
+            const float *in = ck + (int64_t)s.slot_in * 2 * m;
+            for (int c = threadIdx.x; c < diag_len(dbeg - 2, R, C); c += nt) b2[c] = in[c];
+            for (int c = threadIdx.x; c < diag_len(dbeg - 1, R, C); c += nt) b1[c] = in[m + c];
+        }
+        const int n = diag_len(dbeg, R, C);
+#pragma unroll
+        for (int k = 0; k < kDtwPer; ++k) {
+            const int c = threadIdx.x + k * nt;
+            nxt[k] = c < n ? cp[c] : (T)0;
+        }
+        __syncthreads();
+    } else {
+        cp = cost + p.cell_off;
+        dp = dirs + p.cell_off;
         const int n = min(0, R - 1) - diag_lo(0, C) + 1;
 #pragma unroll
         for (int k = 0; k < kDtwPer; ++k) {
@@ -255,15 +339,15 @@ __global__ void __launch_bounds__(kDtwMaxThreads) dtw_kernel(const T *__restrict
             nxt[k] = c < n ? cp[c] : (T)0;
         }
     }
-    for (int d = 0; d < D; ++d) {
+    for (int d = dbeg; d < dend; ++d) {
         T cur[kDtwPer];
 #pragma unroll
         for (int k = 0; k < kDtwPer; ++k) cur[k] = nxt[k];
         const int lo = diag_lo(d, C), n = min(d, R - 1) - lo + 1;
         const int64_t start = diag_start(d, R, C);
-        if (d + 1 < D) {
+        if (d + 1 < dend) {
             const int n1 = min(d + 1, R - 1) - diag_lo(d + 1, C) + 1;
-            const int64_t s1 = start + n;
+            const int64_t s1 = start + n - corg;
 #pragma unroll
             for (int k = 0; k < kDtwPer; ++k) {
                 const int c = threadIdx.x + k * nt;
@@ -286,7 +370,7 @@ __global__ void __launch_bounds__(kDtwMaxThreads) dtw_kernel(const T *__restrict
                 if (left < m) m = left, dir = 1;
                 if (dg < m) m = dg, dir = 2;
                 v = add_rn(cur[k], m);
-                dp[start + c] = dir;
+                if (!STRIPE || dp) dp[start - dorg + c] = dir;
             }
             b0[c] = v;
             if (FULL) dtw_full[(int64_t)i * C + j] = v;
@@ -295,6 +379,14 @@ __global__ void __launch_bounds__(kDtwMaxThreads) dtw_kernel(const T *__restrict
         __syncthreads();
         T *t = b2;
         b2 = b1, b1 = b0, b0 = t;
+    }
+    if constexpr (STRIPE) {
+        if (s.slot_out >= 0) {
+            const int m = min(R, C);
+            float *out = ck + (int64_t)s.slot_out * 2 * m;
+            for (int c = threadIdx.x; c < diag_len(dend - 2, R, C); c += nt) out[c] = b2[c];
+            for (int c = threadIdx.x; c < diag_len(dend - 1, R, C); c += nt) out[m + c] = b1[c];
+        }
     }
 }
 
@@ -337,33 +429,59 @@ __device__ __forceinline__ float ld_cluster(const float *p, unsigned rank) {
 
 // grid G x (pairs of the launch), cluster (G, 1, 1): cluster q runs pair list.idx[q] on its first ceil(min(R, C) / W) CTAs
 // (W = cluster_share); the rest hold no cells.  Same cells, directions, tie order and path cost as dtw_kernel<float, false>,
-// bit for bit.
+// bit for bit.  STRIPE: as dtw_kernel's, each CTA reading and writing its own positions of the checkpoint slots (all CTAs of a
+// cluster leave together when the stripe is past the pair).
+template <bool STRIPE>
 __global__ void __launch_bounds__(kDtwMaxThreads) dtw_cluster_kernel(const float *__restrict__ cost, const PairMeta *__restrict__ pairs,
                                                                      LongPairs list, int G, int cells, uint8_t *__restrict__ dirs,
-                                                                     float *__restrict__ path_cost) {
+                                                                     float *__restrict__ path_cost, Stripe s) {
     extern __shared__ __align__(16) unsigned char dtw_smem[];
     const int pid = list.idx[blockIdx.x / G];
     const unsigned rank = cluster_rank();
     const PairMeta p = pairs[pid];
     const int R = p.R, C = p.C, D = R + C - 1, nt = blockDim.x, tid = threadIdx.x;
     const int W = cluster_share(min(R, C), cells), c0 = (int)rank * W, tl = (W - 1) % nt;
-    const float *cp = cost + p.cell_off;
-    uint8_t *dp = dirs + p.cell_off;
+    const float *cp;
+    uint8_t *dp;
     float *b2 = reinterpret_cast<float *>(dtw_smem), *b1 = b2 + W, *b0 = b1 + W;
     float nxt[kDtwPer];
+    int dbeg = 0, dend = D;
+    int64_t corg = 0, dorg = 0;
+    float *ck = nullptr;
+    if constexpr (STRIPE) {
+        const StripePair q = s.pairs[pid];
+        dbeg = s.d0, dend = min(s.d1, D);
+        if (dbeg >= dend) return;
+        corg = diag_start(dbeg, R, C), dorg = s.local_dirs ? corg : 0;
+        cp = cost + q.cost_off;
+        dp = dirs ? dirs + q.dir_off : nullptr;
+        ck = s.ckpt + q.ckpt_off + c0;
+        const int m = min(R, C);
+        if (dbeg > 0) {
+            const float *in = ck + (int64_t)s.slot_in * 2 * m;
+            for (int c = tid; c < min(W, diag_len(dbeg - 2, R, C) - c0); c += nt) b2[c] = in[c];
+            for (int c = tid; c < min(W, diag_len(dbeg - 1, R, C) - c0); c += nt) b1[c] = in[m + c];
+        }
+        const int n = min(W, diag_len(dbeg, R, C) - c0);
 #pragma unroll
-    for (int k = 0; k < kDtwPer; ++k) nxt[k] = (c0 == 0 && tid + k * nt == 0) ? cp[0] : 0.f;
+        for (int k = 0; k < kDtwPer; ++k) nxt[k] = tid + k * nt < n ? cp[c0 + tid + k * nt] : 0.f;
+    } else {
+        cp = cost + p.cell_off;
+        dp = dirs + p.cell_off;
+#pragma unroll
+        for (int k = 0; k < kDtwPer; ++k) nxt[k] = (c0 == 0 && tid + k * nt == 0) ? cp[0] : 0.f;
+    }
     cluster_arrive();                           // every CTA of the cluster runs: its shared memory may be read
     cluster_wait();
-    for (int d = 0; d < D; ++d) {
+    for (int d = dbeg; d < dend; ++d) {
         float cur[kDtwPer];
 #pragma unroll
         for (int k = 0; k < kDtwPer; ++k) cur[k] = nxt[k];
         const int lo = diag_lo(d, C), n = min(d, R - 1) - lo + 1, nloc = min(W, n - c0);
         const int64_t start = diag_start(d, R, C);
-        if (d + 1 < D) {
+        if (d + 1 < dend) {
             const int n1 = min(min(d + 1, R - 1) - diag_lo(d + 1, C) + 1 - c0, W);
-            const int64_t s1 = start + n + c0;
+            const int64_t s1 = start + n + c0 - corg;
 #pragma unroll
             for (int k = 0; k < kDtwPer; ++k) {
                 const int c = tid + k * nt;
@@ -388,7 +506,7 @@ __global__ void __launch_bounds__(kDtwMaxThreads) dtw_cluster_kernel(const float
                 if (left < m) m = left, dir = 1;
                 if (dg < m) m = dg, dir = 2;
                 v = add_rn(cv, m);
-                dp[start + c0 + c] = dir;
+                if (!STRIPE || dp) dp[start - dorg + c0 + c] = dir;
             }
             b0[c] = v;
             if (i == R - 1 && j == C - 1 && path_cost) path_cost[pid] = v;
@@ -402,13 +520,21 @@ __global__ void __launch_bounds__(kDtwMaxThreads) dtw_cluster_kernel(const float
             else if (c == W - 1) el = cur[k];
             else cell(c, cur[k], false);
         }
-        if (d > 0) cluster_wait();              // the neighbours' edges of diagonal d - 1
+        if (d > dbeg) cluster_wait();           // the neighbours' edges of diagonal d - 1
         if (tid == 0 && nloc > 0) cell(0, e0, true);
         if (W > 1 && tid == tl && nloc > W - 1) cell(W - 1, el, true);
         cluster_arrive();
         __syncthreads();
         float *t = b2;
         b2 = b1, b1 = b0, b0 = t;
+    }
+    if constexpr (STRIPE) {
+        if (s.slot_out >= 0) {
+            const int m = min(R, C);
+            float *out = ck + (int64_t)s.slot_out * 2 * m;
+            for (int c = tid; c < min(W, diag_len(dend - 2, R, C) - c0); c += nt) out[c] = b2[c];
+            for (int c = tid; c < min(W, diag_len(dend - 1, R, C) - c0); c += nt) out[m + c] = b1[c];
+        }
     }
     cluster_wait();                             // no CTA leaves while a neighbour may still read its shared memory
 }
@@ -434,6 +560,36 @@ __global__ void backtrack_kernel(const uint8_t *__restrict__ dirs, const PairMet
     for (int r = 0; r < first; ++r) res[r] = 0;
 }
 
+struct WalkState {
+    int32_t i, j, first, pad_;
+};
+
+// one thread per pair: backtrack_kernel's walk over the cells of stripe [s.d0, s.d1) (stripe-local directions), from where the
+// walk left the stripe after it (from the last cell in the pair's last stripe), until it leaves this one; stripe 0 zeroes the
+// rows the walk never reached
+__global__ void backtrack_stripe_kernel(const uint8_t *__restrict__ dirs, const PairMeta *__restrict__ pairs, Stripe s, int n_pairs,
+                                        WalkState *__restrict__ state, int64_t *__restrict__ out) {
+    const int pid = blockIdx.x * blockDim.x + threadIdx.x;
+    if (pid >= n_pairs) return;
+    const PairMeta p = pairs[pid];
+    const int R = p.R, C = p.C, D = R + C - 1, d0 = s.d0;
+    if (d0 >= D) return;
+    WalkState w = d0 <= D - 1 && D - 1 < s.d1 ? WalkState{R - 1, C - 1, R, 0} : state[pid];
+    const uint8_t *dp = dirs + s.pairs[pid].dir_off;
+    const int64_t org = diag_start(d0, R, C);
+    int64_t *res = out + p.out_row;
+    while (w.i > 0 && w.j > 0 && w.i + w.j >= d0) {
+        res[w.i] = w.j;
+        w.first = w.i;
+        const uint8_t dir = dp[skew_index(w.i, w.j, R, C) - org];
+        if (dir != 1) --w.i;
+        if (dir != 0) --w.j;
+    }
+    if (d0 == 0)
+        for (int r = 0; r < w.first; ++r) res[r] = 0;
+    state[pid] = w;
+}
+
 int dtw_threads(int maxdiag) {
     const int t = (maxdiag + kDtwPer - 1) / kDtwPer;
     return std::min(kDtwMaxThreads, std::max(64, (t + 31) / 32 * 32));
@@ -446,13 +602,25 @@ int launch_dtw(const T *cost, const PairMeta *pairs, const PairMeta &single, int
     const int threads = dtw_threads(maxdiag);
     if (dtw_full) {
         static size_t configured[kSmemCacheDevices] = {};
-        SVB_TRY(raise_smem_limit(dtw_kernel<T, true>, smem, configured));
-        dtw_kernel<T, true><<<n_pairs, threads, smem, st>>>(cost, pairs, single, maxdiag, dirs, path_cost, dtw_full);
+        SVB_TRY(raise_smem_limit(dtw_kernel<T, true, false>, smem, configured));
+        dtw_kernel<T, true, false><<<n_pairs, threads, smem, st>>>(cost, pairs, single, maxdiag, dirs, path_cost, dtw_full, Stripe{});
     } else {
         static size_t configured[kSmemCacheDevices] = {};
-        SVB_TRY(raise_smem_limit(dtw_kernel<T, false>, smem, configured));
-        dtw_kernel<T, false><<<n_pairs, threads, smem, st>>>(cost, pairs, single, maxdiag, dirs, path_cost, nullptr);
+        SVB_TRY(raise_smem_limit(dtw_kernel<T, false, false>, smem, configured));
+        dtw_kernel<T, false, false><<<n_pairs, threads, smem, st>>>(cost, pairs, single, maxdiag, dirs, path_cost, nullptr, Stripe{});
     }
+    SVB_CUDA(cudaGetLastError());
+    return SVB_OK;
+}
+
+// the one-CTA kernel on one stripe of every pair with min(R, C) <= maxdiag
+int launch_dtw_stripe(const float *cost, const PairMeta *pairs, int n_pairs, int maxdiag, uint8_t *dirs, float *path_cost,
+                      const Stripe &s, cudaStream_t st) {
+    const size_t smem = (size_t)3 * maxdiag * sizeof(float);
+    static size_t configured[kSmemCacheDevices] = {};
+    SVB_TRY(raise_smem_limit(dtw_kernel<float, false, true>, smem, configured));
+    dtw_kernel<float, false, true><<<n_pairs, dtw_threads(maxdiag), smem, st>>>(cost, pairs, PairMeta{}, maxdiag, dirs, path_cost,
+                                                                               nullptr, s);
     SVB_CUDA(cudaGetLastError());
     return SVB_OK;
 }
@@ -532,10 +700,10 @@ int cluster_ctas(int m, int cells) { const int w = cluster_share(m, cells); retu
 // different cluster sizes run at the same time: the launch's G is the largest a pair needs, and a pair keeps its own share
 // (cluster_share), its CTAs past ceil(min(R, C) / share) holding no cells and only taking part in the barriers
 int launch_dtw_cluster(const float *cost, const PairMeta *d_pairs, const std::vector<PairMeta> &pairs, int cells, uint8_t *dirs,
-                       float *path_cost, cudaStream_t st) {
+                       float *path_cost, cudaStream_t st, const Stripe *stripe = nullptr) {
     std::vector<int> ids;
     for (int p = 0; p < (int)pairs.size(); ++p)
-        if (std::min(pairs[p].R, pairs[p].C) > cells) ids.push_back(p);
+        if (std::min(pairs[p].R, pairs[p].C) > cells && (!stripe || stripe->d0 < pairs[p].R + pairs[p].C - 1)) ids.push_back(p);
     for (size_t q0 = 0; q0 < ids.size(); q0 += kLongPerLaunch) {
         const int cnt = (int)std::min<size_t>(kLongPerLaunch, ids.size() - q0);
         LongPairs list{};
@@ -547,8 +715,6 @@ int launch_dtw_cluster(const float *cost, const PairMeta *d_pairs, const std::ve
             G = std::max(G, cluster_ctas(m, cells));
         }
         const size_t smem = (size_t)3 * maxw * sizeof(float);
-        static size_t configured[kSmemCacheDevices] = {};
-        SVB_TRY(raise_smem_limit(dtw_cluster_kernel, smem, configured));
         cudaLaunchConfig_t cfg = {};
         cfg.gridDim = dim3((unsigned)(G * cnt)), cfg.blockDim = dim3(dtw_threads(maxw)), cfg.dynamicSmemBytes = smem;
         cfg.stream = st;
@@ -556,56 +722,59 @@ int launch_dtw_cluster(const float *cost, const PairMeta *d_pairs, const std::ve
         attr[0].id = cudaLaunchAttributeClusterDimension;
         attr[0].val.clusterDim.x = G, attr[0].val.clusterDim.y = 1, attr[0].val.clusterDim.z = 1;
         cfg.attrs = attr, cfg.numAttrs = 1;
-        SVB_CUDA(cudaLaunchKernelEx(&cfg, dtw_cluster_kernel, cost, d_pairs, list, G, cells, dirs, path_cost));
+        if (stripe) {
+            static size_t configured[kSmemCacheDevices] = {};
+            SVB_TRY(raise_smem_limit(dtw_cluster_kernel<true>, smem, configured));
+            SVB_CUDA(cudaLaunchKernelEx(&cfg, dtw_cluster_kernel<true>, cost, d_pairs, list, G, cells, dirs, path_cost, *stripe));
+        } else {
+            static size_t configured[kSmemCacheDevices] = {};
+            SVB_TRY(raise_smem_limit(dtw_cluster_kernel<false>, smem, configured));
+            SVB_CUDA(cudaLaunchKernelEx(&cfg, dtw_cluster_kernel<false>, cost, d_pairs, list, G, cells, dirs, path_cost, Stripe{}));
+        }
     }
     return SVB_OK;
 }
 
-// svb_sadtw_align and svb_sadtw_align_long: one validation, layout, histogram, cost and backtrack; long_pairs sends the pairs
-// whose anti-diagonal exceeds a CTA's share to dtw_cluster_kernel and the rest to dtw_kernel
-int sadtw_run(const void *src_f0_dev, const void *tgt_f0_dev, int32_t dtype, int32_t variant, int32_t n_pairs, const int32_t *src_len_host,
-              const int32_t *tgt_len_host, const double *tgt_scale_host, void *workspace_dev, int64_t workspace_bytes,
-              int64_t *alignment_dev, float *path_cost_dev, float *stage_ms_host, bool long_pairs, void *stream) {
+int check_run_args(const void *src_f0_dev, const void *tgt_f0_dev, int32_t dtype, int32_t variant, const void *workspace_dev,
+                   const int64_t *alignment_dev) {
     SVB_CHECK(src_f0_dev && tgt_f0_dev && workspace_dev && alignment_dev, SVB_ERR_INVALID, "sadtw: null argument");
     SVB_CHECK(dtype == SVB_SADTW_F32 || dtype == SVB_SADTW_F64, SVB_ERR_INVALID, "sadtw: bad f0 dtype %d", dtype);
     SVB_CHECK(variant == SVB_SADTW || variant == SVB_EHSADTW, SVB_ERR_INVALID, "sadtw: bad variant %d", variant);
-    Layout L;
-    SVB_TRY(sadtw_layout(n_pairs, src_len_host, tgt_len_host, long_pairs, L));
-    SVB_CHECK(workspace_bytes >= (int64_t)L.total, SVB_ERR_INVALID, "sadtw: workspace of %lld bytes, %lld needed",
-              (long long)workspace_bytes, (long long)L.total);
-    int share = kMaxDiag;
-    if (long_pairs) SVB_TRY(cta_cells(share));
-    const int n = n_pairs;
-    std::vector<SeqMeta> seqs(2 * (size_t)n);
-    std::vector<PairMeta> pairs(n);
+    return SVB_OK;
+}
+
+// the host metadata of a call: sequence and pair metas (histogram rows: the amateur frames of all pairs, then the professional
+// ones from rows_src on), and the launch bounds.  Validates the scale factors and windows.
+struct Metas {
+    std::vector<SeqMeta> seqs;
+    std::vector<PairMeta> pairs;
+    int maxlen = 0, maxdiag = 0;        // longest take; longest anti-diagonal of the pairs the one-CTA kernel runs
+    int64_t maxtiles = 0;               // cost tiles of the largest pair
+    bool has_long = false;              // a pair for the cluster kernel
+};
+
+int make_metas(int32_t variant, int n, const int32_t *src_len_host, const int32_t *tgt_len_host, const double *tgt_scale_host,
+               int64_t rows_src, int share, Metas &M) {
+    M.seqs.resize(2 * (size_t)n);
+    M.pairs.resize(n);
     int64_t fs = 0, ft = 0, cells = 0;
-    int maxlen = 0, maxdiag = 0;
-    int64_t maxtiles = 0;
-    bool has_long = false;
     for (int p = 0; p < n; ++p) {
         const int S = src_len_host[p], T = tgt_len_host[p];
         const double scale = tgt_scale_host ? tgt_scale_host[p] : (double)T / (double)S;
-        SVB_TRY(make_seq(variant, fs, fs, S, 1.0, "amateur sequence", p, seqs[p]));
-        SVB_TRY(make_seq(variant, ft, L.rows_src + ft, T, scale, "professional sequence", p, seqs[n + p]));
-        pairs[p] = PairMeta{fs, L.rows_src + ft, cells, ft, T, S};
+        SVB_TRY(make_seq(variant, fs, fs, S, 1.0, "amateur sequence", p, M.seqs[p]));
+        SVB_TRY(make_seq(variant, ft, rows_src + ft, T, scale, "professional sequence", p, M.seqs[n + p]));
+        M.pairs[p] = PairMeta{fs, rows_src + ft, cells, ft, T, S};
         fs += S, ft += T, cells += (int64_t)S * T;
-        maxlen = std::max(maxlen, std::max(S, T));
-        if (std::min(S, T) <= share) maxdiag = std::max(maxdiag, std::min(S, T));
-        else has_long = true;
-        maxtiles = std::max(maxtiles, (int64_t)((S + kTileJ - 1) / kTileJ) * ((T + kTileI - 1) / kTileI));
+        M.maxlen = std::max(M.maxlen, std::max(S, T));
+        if (std::min(S, T) <= share) M.maxdiag = std::max(M.maxdiag, std::min(S, T));
+        else M.has_long = true;
+        M.maxtiles = std::max(M.maxtiles, (int64_t)((S + kTileJ - 1) / kTileJ) * ((T + kTileI - 1) / kTileI));
     }
-    // everything is validated: from here on, launches
-    cudaStream_t st = as_stream(stream);
-    char *ws = static_cast<char *>(workspace_dev);
-    SeqMeta *d_seqs = reinterpret_cast<SeqMeta *>(ws + L.off[0]);
-    PairMeta *d_pairs = reinterpret_cast<PairMeta *>(ws + L.off[1]);
-    float *d_hist = reinterpret_cast<float *>(ws + L.off[2]), *d_cost = reinterpret_cast<float *>(ws + L.off[3]);
-    uint8_t *d_dirs = reinterpret_cast<uint8_t *>(ws + L.off[4]);
-    SVB_CUDA(cudaMemcpyAsync(d_seqs, seqs.data(), seqs.size() * sizeof(SeqMeta), cudaMemcpyHostToDevice, st));
-    SVB_CUDA(cudaMemcpyAsync(d_pairs, pairs.data(), pairs.size() * sizeof(PairMeta), cudaMemcpyHostToDevice, st));
-    StageTimer tm(stage_ms_host != nullptr);
-    SVB_TRY(tm.create());
-    SVB_TRY(tm.mark(0, st));
+    return SVB_OK;
+}
+
+int launch_hist(const void *src_f0_dev, const void *tgt_f0_dev, int32_t dtype, int32_t variant, int n, int maxlen,
+                const SeqMeta *d_seqs, float *d_hist, cudaStream_t st) {
     const dim3 hgrid((maxlen + kHistThreads / 8 - 1) / (kHistThreads / 8), 2 * n);
     if (dtype == SVB_SADTW_F32)
         sadtw_hist_kernel<float><<<hgrid, kHistThreads, 0, st>>>(static_cast<const float *>(src_f0_dev),
@@ -616,16 +785,238 @@ int sadtw_run(const void *src_f0_dev, const void *tgt_f0_dev, int32_t dtype, int
                                                                  static_cast<const double *>(tgt_f0_dev), n, d_seqs, variant, d_hist,
                                                                  nullptr);
     SVB_CUDA(cudaGetLastError());
+    return SVB_OK;
+}
+
+// svb_sadtw_align and svb_sadtw_align_long: one validation, layout, histogram, cost and backtrack; long_pairs sends the pairs
+// whose anti-diagonal exceeds a CTA's share to dtw_cluster_kernel and the rest to dtw_kernel
+int sadtw_run(const void *src_f0_dev, const void *tgt_f0_dev, int32_t dtype, int32_t variant, int32_t n_pairs, const int32_t *src_len_host,
+              const int32_t *tgt_len_host, const double *tgt_scale_host, void *workspace_dev, int64_t workspace_bytes,
+              int64_t *alignment_dev, float *path_cost_dev, float *stage_ms_host, bool long_pairs, void *stream) {
+    SVB_TRY(check_run_args(src_f0_dev, tgt_f0_dev, dtype, variant, workspace_dev, alignment_dev));
+    Layout L;
+    SVB_TRY(sadtw_layout(n_pairs, src_len_host, tgt_len_host, long_pairs, L));
+    SVB_CHECK(workspace_bytes >= (int64_t)L.total, SVB_ERR_INVALID, "sadtw: workspace of %lld bytes, %lld needed",
+              (long long)workspace_bytes, (long long)L.total);
+    int share = kMaxDiag;
+    if (long_pairs) SVB_TRY(cta_cells(share));
+    const int n = n_pairs;
+    Metas M;
+    SVB_TRY(make_metas(variant, n, src_len_host, tgt_len_host, tgt_scale_host, L.rows_src, share, M));
+    // everything is validated: from here on, launches
+    cudaStream_t st = as_stream(stream);
+    char *ws = static_cast<char *>(workspace_dev);
+    SeqMeta *d_seqs = reinterpret_cast<SeqMeta *>(ws + L.off[0]);
+    PairMeta *d_pairs = reinterpret_cast<PairMeta *>(ws + L.off[1]);
+    float *d_hist = reinterpret_cast<float *>(ws + L.off[2]), *d_cost = reinterpret_cast<float *>(ws + L.off[3]);
+    uint8_t *d_dirs = reinterpret_cast<uint8_t *>(ws + L.off[4]);
+    SVB_CUDA(cudaMemcpyAsync(d_seqs, M.seqs.data(), M.seqs.size() * sizeof(SeqMeta), cudaMemcpyHostToDevice, st));
+    SVB_CUDA(cudaMemcpyAsync(d_pairs, M.pairs.data(), M.pairs.size() * sizeof(PairMeta), cudaMemcpyHostToDevice, st));
+    StageTimer tm(stage_ms_host != nullptr);
+    SVB_TRY(tm.create());
+    SVB_TRY(tm.mark(0, st));
+    SVB_TRY(launch_hist(src_f0_dev, tgt_f0_dev, dtype, variant, n, M.maxlen, d_seqs, d_hist, st));
     SVB_TRY(tm.mark(1, st));
-    const dim3 cgrid((unsigned)maxtiles, n);
-    sadtw_cost_kernel<<<cgrid, kCostThreads, 0, st>>>(d_hist, d_pairs, d_cost);
+    const dim3 cgrid((unsigned)M.maxtiles, n);
+    sadtw_cost_kernel<false><<<cgrid, kCostThreads, 0, st>>>(d_hist, d_pairs, d_cost, Stripe{});
     SVB_CUDA(cudaGetLastError());
     SVB_TRY(tm.mark(2, st));
-    if (has_long) SVB_TRY(launch_dtw_cluster(d_cost, d_pairs, pairs, share, d_dirs, path_cost_dev, st));
-    if (maxdiag > 0) SVB_TRY(launch_dtw<float>(d_cost, d_pairs, PairMeta{}, n, maxdiag, d_dirs, path_cost_dev, nullptr, st));
+    if (M.has_long) SVB_TRY(launch_dtw_cluster(d_cost, d_pairs, M.pairs, share, d_dirs, path_cost_dev, st));
+    if (M.maxdiag > 0) SVB_TRY(launch_dtw<float>(d_cost, d_pairs, PairMeta{}, n, M.maxdiag, d_dirs, path_cost_dev, nullptr, st));
     SVB_TRY(tm.mark(3, st));
     backtrack_kernel<<<(n + 127) / 128, 128, 0, st>>>(d_dirs, d_pairs, PairMeta{}, n, alignment_dev);
     SVB_CUDA(cudaGetLastError());
+    SVB_TRY(tm.mark(4, st));
+    return tm.read(stage_ms_host);
+}
+
+// ---- svb_sadtw_align_striped: the planner and the run -----------------------------------------------------------------------
+constexpr int kSinglePassDiags = 512;       // stripe width of the single pass
+constexpr int kMaxStripeDiags = 8192;       // the widest stripe the planner picks for the checkpointed passes
+constexpr int kMaxForcedDiags = 1 << 17;    // SVB_DTW_STRIPE_DIAGS: at most this (more than any pair's R + C - 1)
+
+// workspace of svb_sadtw_align_striped: [seq metas | pair metas | stripe metas | histograms | 2 stripe cost buffers | directions |
+// checkpoint slots | walk states]
+struct StripePlan {
+    int mode = SVB_SADTW_SINGLE_PASS, diags = 0, stripes = 0;
+    size_t off[8] = {}, total = 0, minimum = 0;
+    Layout L;                       // sadtw_layout(long_pairs = true): the validation and the histogram rows
+    int64_t sum_min = 0;            // sum over pairs of min(R, C)
+    int max_d = 0;                  // the longest R + C - 1
+};
+
+int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
+
+// the memory model: the sections of the workspace at stripe width K, single pass or checkpointed
+size_t stripe_sections(int n, const int32_t *src_len, const int32_t *tgt_len, const StripePlan &P, int K, bool single, size_t *off) {
+    int64_t slots = 0;              // checkpoint slots x min(R, C), summed over pairs: one slot each in single pass
+    for (int p = 0; p < n; ++p) {
+        const int64_t m = std::min(src_len[p], tgt_len[p]);
+        slots += (single ? 1 : ceil_div(src_len[p] + tgt_len[p] - 1, K)) * m;
+    }
+    off[0] = 0;
+    off[1] = align_up(off[0] + (size_t)2 * n * sizeof(SeqMeta));
+    off[2] = align_up(off[1] + (size_t)n * sizeof(PairMeta));
+    off[3] = align_up(off[2] + (size_t)n * sizeof(StripePair));
+    off[4] = align_up(off[3] + (size_t)(P.L.rows_src + P.L.rows_tgt) * kBins * sizeof(float));
+    off[5] = align_up(off[4] + (size_t)2 * K * P.sum_min * sizeof(float));
+    off[6] = align_up(off[5] + (single ? (size_t)P.L.cells : (size_t)K * P.sum_min));
+    off[7] = align_up(off[6] + (size_t)slots * 2 * sizeof(float));
+    return align_up(off[7] + (size_t)n * sizeof(WalkState));
+}
+
+// single pass at kSinglePassDiags when it fits the budget, else checkpointed at the largest power of two K <= kMaxStripeDiags
+// that fits; SVB_DTW_STRIPE_DIAGS=<K> (read per call; a test and measurement hook) forces checkpointed at K.  minimum: the
+// smallest budget any of these choices fits.
+int stripe_plan(int32_t n, const int32_t *src_len, const int32_t *tgt_len, int64_t budget, StripePlan &P) {
+    SVB_TRY(sadtw_layout(n, src_len, tgt_len, true, P.L));
+    P.sum_min = 0, P.max_d = 0;
+    for (int p = 0; p < n; ++p) {
+        P.sum_min += std::min(src_len[p], tgt_len[p]);
+        P.max_d = std::max(P.max_d, src_len[p] + tgt_len[p] - 1);
+    }
+    int forced = 0;
+    if (const char *e = getenv("SVB_DTW_STRIPE_DIAGS")) {
+        forced = atoi(e);
+        SVB_CHECK(forced >= 1 && forced <= kMaxForcedDiags, SVB_ERR_INVALID, "sadtw_striped: SVB_DTW_STRIPE_DIAGS=%s (1 .. %d)", e,
+                  kMaxForcedDiags);
+    }
+    size_t off[8];
+    const int ks = std::min(kSinglePassDiags, P.max_d);
+    const size_t single = stripe_sections(n, src_len, tgt_len, P, ks, true, off);
+    P.minimum = single;
+    int best = 0;                   // the largest power of two that fits
+    for (int K = 1; K <= kMaxStripeDiags; K *= 2) {
+        const size_t t = stripe_sections(n, src_len, tgt_len, P, K, false, off);
+        P.minimum = std::min(P.minimum, t);
+        if ((int64_t)t <= budget) best = K;
+        if (K >= P.max_d) break;
+    }
+    if (forced) {
+        P.mode = SVB_SADTW_CHECKPOINTED, P.diags = forced;
+    } else if ((int64_t)single <= budget) {
+        P.mode = SVB_SADTW_SINGLE_PASS, P.diags = ks;
+    } else {
+        SVB_CHECK(best > 0, SVB_ERR_INVALID,
+                  "sadtw_striped: a budget of %lld bytes is below the minimum of %lld bytes for these %d pairs", (long long)budget,
+                  (long long)P.minimum, n);
+        P.mode = SVB_SADTW_CHECKPOINTED, P.diags = best;
+    }
+    P.total = stripe_sections(n, src_len, tgt_len, P, P.diags, P.mode == SVB_SADTW_SINGLE_PASS, P.off);
+    SVB_CHECK((int64_t)P.total <= budget, SVB_ERR_INVALID,
+              "sadtw_striped: SVB_DTW_STRIPE_DIAGS=%d needs %lld bytes, more than the budget of %lld bytes", forced,
+              (long long)P.total, (long long)budget);
+    P.stripes = (int)ceil_div(P.max_d, P.diags);
+    return SVB_OK;
+}
+
+// a side stream for the stripe costs and the events that order it with the DTW on the caller's stream
+struct SideStream {
+    cudaStream_t s = nullptr;
+    cudaEvent_t ev[5] = {};         // [0, 1]: cost of buffer b written; [2, 3]: DTW done with buffer b; [4]: histograms written
+    ~SideStream() {
+        for (auto e : ev)
+            if (e) cudaEventDestroy(e);
+        if (s) cudaStreamDestroy(s);
+    }
+    int create() {
+        SVB_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+        for (auto &e : ev) SVB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+        return SVB_OK;
+    }
+};
+
+int sadtw_striped_run(const void *src_f0_dev, const void *tgt_f0_dev, int32_t dtype, int32_t variant, int32_t n_pairs,
+                      const int32_t *src_len_host, const int32_t *tgt_len_host, const double *tgt_scale_host, void *workspace_dev,
+                      int64_t workspace_bytes, int64_t budget_bytes, int64_t *alignment_dev, float *path_cost_dev,
+                      float *stage_ms_host, void *stream) {
+    SVB_TRY(check_run_args(src_f0_dev, tgt_f0_dev, dtype, variant, workspace_dev, alignment_dev));
+    StripePlan P;
+    SVB_TRY(stripe_plan(n_pairs, src_len_host, tgt_len_host, budget_bytes, P));
+    SVB_CHECK(workspace_bytes >= (int64_t)P.total, SVB_ERR_INVALID, "sadtw_striped: workspace of %lld bytes, the plan needs %lld",
+              (long long)workspace_bytes, (long long)P.total);
+    int share;
+    SVB_TRY(cta_cells(share));
+    const int n = n_pairs, K = P.diags;
+    const bool single = P.mode == SVB_SADTW_SINGLE_PASS;
+    Metas M;
+    SVB_TRY(make_metas(variant, n, src_len_host, tgt_len_host, tgt_scale_host, P.L.rows_src, share, M));
+    std::vector<StripePair> sp(n);
+    int64_t mins = 0, slots = 0;
+    int max_tiles_j = 0;
+    for (int p = 0; p < n; ++p) {
+        const PairMeta &q = M.pairs[p];
+        const int m = std::min(q.R, q.C);
+        sp[p] = StripePair{(int64_t)K * mins, single ? q.cell_off : (int64_t)K * mins, 2 * slots};
+        mins += m, slots += (single ? 1 : ceil_div(q.R + q.C - 1, K)) * m;
+        max_tiles_j = std::max(max_tiles_j, (q.C + kTileJ - 1) / kTileJ);
+    }
+    // everything is validated: from here on, launches
+    cudaStream_t st = as_stream(stream);
+    char *ws = static_cast<char *>(workspace_dev);
+    SeqMeta *d_seqs = reinterpret_cast<SeqMeta *>(ws + P.off[0]);
+    PairMeta *d_pairs = reinterpret_cast<PairMeta *>(ws + P.off[1]);
+    StripePair *d_sp = reinterpret_cast<StripePair *>(ws + P.off[2]);
+    float *d_hist = reinterpret_cast<float *>(ws + P.off[3]);
+    float *d_cost[2] = {reinterpret_cast<float *>(ws + P.off[4]), reinterpret_cast<float *>(ws + P.off[4]) + (size_t)K * P.sum_min};
+    uint8_t *d_dirs = reinterpret_cast<uint8_t *>(ws + P.off[5]);
+    float *d_ckpt = reinterpret_cast<float *>(ws + P.off[6]);
+    WalkState *d_walk = reinterpret_cast<WalkState *>(ws + P.off[7]);
+    SVB_CUDA(cudaMemcpyAsync(d_seqs, M.seqs.data(), M.seqs.size() * sizeof(SeqMeta), cudaMemcpyHostToDevice, st));
+    SVB_CUDA(cudaMemcpyAsync(d_pairs, M.pairs.data(), M.pairs.size() * sizeof(PairMeta), cudaMemcpyHostToDevice, st));
+    SVB_CUDA(cudaMemcpyAsync(d_sp, sp.data(), sp.size() * sizeof(StripePair), cudaMemcpyHostToDevice, st));
+    SideStream side;
+    SVB_TRY(side.create());
+    StageTimer tm(stage_ms_host != nullptr);
+    SVB_TRY(tm.create());
+    SVB_TRY(tm.mark(0, st));
+    SVB_TRY(launch_hist(src_f0_dev, tgt_f0_dev, dtype, variant, n, M.maxlen, d_seqs, d_hist, st));
+    SVB_CUDA(cudaEventRecord(side.ev[4], st));
+    SVB_CUDA(cudaStreamWaitEvent(side.s, side.ev[4], 0));
+    SVB_TRY(tm.mark(1, st));
+    const int nj = std::min(max_tiles_j, stripe_row_tiles(K));
+    int seq = 0;
+    // stripe k: its cost on the side stream into buffer seq % 2 once the DTW two stripes back is done with it, then its DTW on the
+    // caller's stream; forward: checkpoint slot k - 1 in, k out (single pass: slot 0 both ways, global directions); backward:
+    // stripe-local directions and the walk over them
+    auto run_stripe = [&](int k, bool forward) -> int {
+        const int b = seq++ & 1;
+        Stripe s{d_sp, d_ckpt, k * K, k * K + K, single ? 0 : k - 1, single ? 0 : forward ? k : -1, !single, nj};
+        int64_t gx = 0;
+        for (const PairMeta &q : M.pairs) {
+            const int d1 = std::min(s.d1, q.R + q.C - 1);
+            if (s.d0 >= d1) continue;
+            int lo, hi;
+            stripe_rows(q.R, q.C, s.d0, d1, lo, hi);
+            gx = std::max<int64_t>(gx, (int64_t)(hi - lo + 1) * nj);
+        }
+        SVB_CUDA(cudaStreamWaitEvent(side.s, side.ev[2 + b], 0));
+        if (gx > 0) {
+            sadtw_cost_kernel<true><<<dim3((unsigned)gx, n), kCostThreads, 0, side.s>>>(d_hist, d_pairs, d_cost[b], s);
+            SVB_CUDA(cudaGetLastError());
+        }
+        SVB_CUDA(cudaEventRecord(side.ev[b], side.s));
+        SVB_CUDA(cudaStreamWaitEvent(st, side.ev[b], 0));
+        uint8_t *dirs = single || !forward ? d_dirs : nullptr;
+        float *pc = forward ? path_cost_dev : nullptr;
+        if (M.has_long) SVB_TRY(launch_dtw_cluster(d_cost[b], d_pairs, M.pairs, share, dirs, pc, st, &s));
+        if (M.maxdiag > 0) SVB_TRY(launch_dtw_stripe(d_cost[b], d_pairs, n, M.maxdiag, dirs, pc, s, st));
+        if (!forward) {
+            backtrack_stripe_kernel<<<(n + 127) / 128, 128, 0, st>>>(d_dirs, d_pairs, s, n, d_walk, alignment_dev);
+            SVB_CUDA(cudaGetLastError());
+        }
+        SVB_CUDA(cudaEventRecord(side.ev[2 + b], st));
+        return SVB_OK;
+    };
+    for (int k = 0; k < P.stripes; ++k) SVB_TRY(run_stripe(k, true));
+    SVB_TRY(tm.mark(2, st));
+    if (!single)
+        for (int k = P.stripes - 1; k >= 0; --k) SVB_TRY(run_stripe(k, false));
+    SVB_TRY(tm.mark(3, st));
+    if (single) {
+        backtrack_kernel<<<(n + 127) / 128, 128, 0, st>>>(d_dirs, d_pairs, PairMeta{}, n, alignment_dev);
+        SVB_CUDA(cudaGetLastError());
+    }
     SVB_TRY(tm.mark(4, st));
     return tm.read(stage_ms_host);
 }
@@ -664,6 +1055,25 @@ extern "C" int svb_sadtw_align_long(const void *src_f0_dev, const void *tgt_f0_d
                                     float *stage_ms_host, void *stream) {
     return sadtw_run(src_f0_dev, tgt_f0_dev, dtype, variant, n_pairs, src_len_host, tgt_len_host, tgt_scale_host, workspace_dev,
                      workspace_bytes, alignment_dev, path_cost_dev, stage_ms_host, true, stream);
+}
+
+extern "C" int svb_sadtw_striped_plan(int32_t n_pairs, const int32_t *src_len_host, const int32_t *tgt_len_host, int64_t budget_bytes,
+                                      svb_sadtw_stripe_plan *plan) {
+    SVB_CHECK(plan, SVB_ERR_INVALID, "sadtw_striped: null argument");
+    StripePlan P;
+    SVB_TRY(stripe_plan(n_pairs, src_len_host, tgt_len_host, budget_bytes, P));
+    plan->mode = P.mode, plan->stripe_diags = P.diags, plan->stripes = P.stripes, plan->reserved = 0;
+    for (int k = 0; k < 8; ++k) plan->offsets[k] = (int64_t)P.off[k];
+    plan->total_bytes = (int64_t)P.total, plan->min_budget_bytes = (int64_t)P.minimum;
+    return SVB_OK;
+}
+
+extern "C" int svb_sadtw_align_striped(const void *src_f0_dev, const void *tgt_f0_dev, int32_t dtype, int32_t variant, int32_t n_pairs,
+                                       const int32_t *src_len_host, const int32_t *tgt_len_host, const double *tgt_scale_host,
+                                       void *workspace_dev, int64_t workspace_bytes, int64_t budget_bytes, int64_t *alignment_dev,
+                                       float *path_cost_dev, float *stage_ms_host, void *stream) {
+    return sadtw_striped_run(src_f0_dev, tgt_f0_dev, dtype, variant, n_pairs, src_len_host, tgt_len_host, tgt_scale_host, workspace_dev,
+                             workspace_bytes, budget_bytes, alignment_dev, path_cost_dev, stage_ms_host, stream);
 }
 
 extern "C" int64_t svb_sadtw_histogram_workspace_bytes(int32_t n_seq) {

@@ -18,11 +18,11 @@ pair's a2p mel depends on the batch it is in and can differ from the same pair b
 (batch size 1) computes.  Beautify one pair per call to get exactly that.  Every other stage is per pair: bit-identical alone and
 in any batch.
 
-``beautify_songs`` takes whole songs (up to 65536 frames a take): each song is aligned whole, run through the model in
-overlapping segments of at most max_frames and vocoded whole from the stitched mel.
+``beautify_songs`` takes whole songs (up to 65536 frames a take): each song is aligned whole (within a device-memory budget,
+``align_bytes``), run through the model in overlapping segments of at most max_frames and vocoded whole from the stitched mel.
 
 ``python -m neuralsvb_b200.inference.beautify --config C --exp_name X [--hparams ...] --amateur a.wav ... --prof p.wav ...
---spk_emb e.npy ... --out o.wav ... [--song]`` writes one file per pair."""
+--spk_emb e.npy ... --out o.wav ... [--song [--align_gb G]]`` writes one file per pair."""
 import argparse
 import os
 
@@ -42,7 +42,7 @@ from neuralsvb_b200.utils.pitch_utils import denorm_f0, f0_to_coarse, norm_inter
 WAYS = ('a2a', 'p2p', 'a2p')
 ALIGN_METHOD = 'EHSADTW'
 EMB_DIM = 256
-SONG_ALIGN_BYTES = 24 << 30     # beautify_songs aligns consecutive songs together up to this much DTW workspace (one at the limit)
+SONG_ALIGN_BYTES = 24 << 30     # beautify_songs' default budget for the alignment workspace of all songs of a call (align_songs)
 SONG_VOCODE_FRAMES = 1 << 17    # and vocodes them together up to this many padded frames (songs x the longest professional take)
 
 
@@ -267,12 +267,15 @@ class SVBBeautifier:
         """``beautify_batch`` of one pair -> one float32 array."""
         return self.beautify_batch([amateur], [professional], [spk_emb], **kw)[0]
 
-    def beautify_songs(self, amateur, professional, spk_emb, seed=None, eps=None, segment_frames=None, overlap_frames=64):
+    def beautify_songs(self, amateur, professional, spk_emb, seed=None, eps=None, segment_frames=None, overlap_frames=64,
+                       align_bytes=None):
         """The a2p take of whole songs: ``beautify_batch``'s inputs, with each take up to LONG_MAX_FRAMES frames (6.3 min at
         22.05 kHz / hop 128) instead of max_frames.  Returns one float32 array of Tp x hop samples per song, Tp the professional
         frame count cropped to a multiple of frames_multiple.
 
-        Each song is aligned whole (align_long, EHSADTW on the device f0 in float64), cut by ``plan_song`` into professional
+        All songs are aligned whole in one ``align_songs`` call (EHSADTW on the device f0 in float64, align_long's results) within
+        ``align_bytes`` of device workspace (default SONG_ALIGN_BYTES; a lower budget trades about twice the alignment time for
+        memory linear in the songs' lengths, with the same results), then each song is cut by ``plan_song`` into professional
         segments of at most ``segment_frames`` (default max_frames) overlapping by ``overlap_frames``, each with the amateur slice
         its alignment reads; the segments are conditioned by ``condition()``'s rules on their slices of the whole takes' f0 and
         pitch ids, with alignment a2p[s:e] - a_lo.  MleSVBVAE runs once per song on that song's segments as one batch, with the
@@ -286,11 +289,12 @@ class SVBBeautifier:
 
         ``seed`` keys the NSF draws by (seed, song index) as spec2wav_batch does, however the songs are grouped for the vocoder
         (consecutive songs up to SONG_VOCODE_FRAMES padded frames per generator call), and draws eps [n_songs, latent, 1]
-        unless given.  Bad segment_frames / overlap_frames raise before any device work; every song is checked and planned
+        unless given.  Bad segment_frames / overlap_frames and an align_bytes below the smallest workable alignment budget (the
+        message names it) raise before any device work; every song is checked and planned
         before the model runs: a bad take, a take over LONG_MAX_FRAMES or a song that cannot be planned raises ValueError naming
         the song."""
         with torch.no_grad(), torch.cuda.device(self.device):
-            return self._run_songs(amateur, professional, spk_emb, seed, eps, segment_frames, overlap_frames)
+            return self._run_songs(amateur, professional, spk_emb, seed, eps, segment_frames, overlap_frames, align_bytes)
 
     def _song_conditioning(self, frames, f0s, B):
         """Per take (B amateur, then B professional): the cropped frame count, the f0 the segments are conditioned on (moved by
@@ -304,26 +308,27 @@ class SVBBeautifier:
         return out
 
     def _align_songs(self, f0_dev, frames, st):
-        """EHSADTW of every song on the device f0 (float64, as _align), consecutive songs together up to SONG_ALIGN_BYTES of
-        workspace -> host int64 alignments.  With timing on, align_ms holds each group's (histogram, cost, DTW, backtrack) times."""
-        from neuralsvb_b200.modules.voice_conversion.dtw.core import align_long, long_workspace_bytes
+        """EHSADTW of every song on the device f0 (float64, as _align) in one align_songs call within the call's alignment budget
+        -> host int64 alignments.  With timing on, align_ms holds the call's (histogram, forward, backward, backtrack) times."""
+        from neuralsvb_b200.modules.voice_conversion.dtw.core import align_songs
         B = len(frames) // 2
-        ws = [long_workspace_bytes([int(frames[b])], [int(frames[B + b])]) for b in range(B)]
         t = torch.split(f0_dev.double(), [int(x) for x in frames])
-        aligns, self.align_ms = [], []
-        for g0, g1 in _groups(ws, SONG_ALIGN_BYTES):
-            st.mark('alignment')
-            r = align_long(list(t[g0:g1]), list(t[B + g0:B + g1]), ALIGN_METHOD, stage_ms=self.timing)
-            aligns += r.split()
-            if self.timing:
-                self.align_ms.append(r.stage_ms)
-        return aligns
+        st.mark('alignment')
+        r = align_songs(list(t[:B]), list(t[B:]), ALIGN_METHOD, workspace_bytes=self._align_bytes, stage_ms=self.timing)
+        self.align_ms = [r.stage_ms] if self.timing else []
+        return r.split()
 
-    def _run_songs(self, amateur, professional, spk_emb, seed, eps, segment_frames, overlap_frames):
+    def _run_songs(self, amateur, professional, spk_emb, seed, eps, segment_frames, overlap_frames, align_bytes=None):
+        from neuralsvb_b200.modules.voice_conversion.dtw.core import striped_plan
         hp = self.hp
         segment_sizes(hp, segment_frames, overlap_frames, 'beautify_songs')         # before any device work
         dec, rates, lens, frames, spk = self._takes(amateur, professional, spk_emb, songs=True)
         B = len(spk)
+        self._align_bytes = SONG_ALIGN_BYTES if align_bytes is None else int(align_bytes)
+        try:
+            striped_plan(frames[:B], frames[B:], self._align_bytes)                  # a budget below the minimum: before any device work
+        except ValueError as e:
+            raise ValueError(f'beautify_songs: align_bytes = {self._align_bytes}: {e}') from None
         if eps is not None:
             eps = torch.as_tensor(eps, dtype=torch.float32)
             if tuple(eps.shape) != (B, hp['latent_size'], 1):
@@ -450,6 +455,9 @@ def parse_args(argv=None):
     p.add_argument('--out', nargs='+', required=True)
     p.add_argument('--song', action='store_true', help='whole songs (beautify_songs): takes longer than max_frames are aligned '
                                                        'whole, run through the model in overlapping segments and vocoded whole')
+    p.add_argument('--align_gb', type=float, default=None,
+                   help='with --song: device memory budget of the alignment in GiB (default 24); a lower one aligns in about '
+                        'twice the time with the same results')
     args = p.parse_args(argv)
     counts = {k: len(getattr(args, k)) for k in ('amateur', 'prof', 'spk_emb', 'out')}
     if len(set(counts.values())) != 1:
@@ -464,7 +472,11 @@ def main(argv=None):
     hp = set_hparams(config=args.config, exp_name=args.exp_name, hparams_str=args.hparams, print_hparams=False)
     hp['infer'] = True
     b = SVBBeautifier(work_dir, hp=hparams)
-    wavs = (b.beautify_songs if args.song else b.beautify_batch)(args.amateur, args.prof, args.spk_emb)
+    if args.song:
+        align_bytes = None if args.align_gb is None else int(args.align_gb * (1 << 30))
+        wavs = b.beautify_songs(args.amateur, args.prof, args.spk_emb, align_bytes=align_bytes)
+    else:
+        wavs = b.beautify_batch(args.amateur, args.prof, args.spk_emb)
     for w, fn in zip(wavs, args.out):
         if os.path.dirname(fn):
             os.makedirs(os.path.dirname(fn), exist_ok=True)

@@ -129,6 +129,76 @@ def long_workspace_bytes(src_len, tgt_len):
     return _check(_native.lib().svb_sadtw_long_workspace_bytes(len(s_arr), s_p, t_p, None), 'sadtw_long_workspace_bytes')
 
 
+SONGS_WORKSPACE_BYTES = 24 << 30
+STRIPE_MODES = ('single_pass', 'checkpointed')
+
+
+class StripePlan(ctypes.Structure):
+    """svb_sadtw_stripe_plan: the mode (index into STRIPE_MODES), the stripe width K in anti-diagonals, the stripe count, the byte
+    offsets of the workspace sections, the workspace size and the smallest budget the planner accepts."""
+    _fields_ = [('mode', ctypes.c_int32), ('stripe_diags', ctypes.c_int32), ('stripes', ctypes.c_int32),
+                ('reserved', ctypes.c_int32), ('offsets', ctypes.c_int64 * 8), ('total_bytes', ctypes.c_int64),
+                ('min_budget_bytes', ctypes.c_int64)]
+
+
+def striped_plan(src_len, tgt_len, budget):
+    """The plan of align_songs for pairs of these amateur / professional frame counts within ``budget`` bytes of workspace
+    (host only; ValueError past align_long's limits or below the smallest workable budget, which the message names)."""
+    s_arr, s_p = _i32(src_len)
+    t_arr, t_p = _i32(tgt_len)
+    if s_arr.shape != t_arr.shape or s_arr.ndim != 1:
+        raise ValueError(f'{s_arr.shape} amateur and {t_arr.shape} professional lengths')
+    plan = StripePlan()
+    _check(_native.lib().svb_sadtw_striped_plan(len(s_arr), s_p, t_p, int(budget), ctypes.byref(plan)), 'sadtw_striped_plan')
+    return plan
+
+
+def striped_workspace_bytes(src_len, tgt_len, budget):
+    """Bytes of align_songs' device workspace for these frame counts within ``budget`` (<= budget; ValueError as striped_plan)."""
+    return striped_plan(src_len, tgt_len, budget).total_bytes
+
+
+def _frames(f):
+    t = as_tensor(f)
+    if t.dim() == 1 or (t.dim() == 2 and t.shape[1] == 1):
+        return int(t.shape[0])
+    raise ValueError(f'an f0 contour must be [S] or [S, 1], got {tuple(t.shape)}')
+
+
+def align_songs(srcs, tgts, method='EHSADTW', workspace_bytes=SONGS_WORKSPACE_BYTES, stage_ms=False):
+    """align_long's results, bit for bit, in at most ``workspace_bytes`` of device workspace: a budget, not a choice of
+    algorithm.  The planner (striped_plan) runs a single pass that keeps every direction byte (1 byte per cell instead of
+    align_long's 5) when that fits, else a checkpointed forward and backward pass over stripes of K anti-diagonals whose memory
+    is linear in the takes' lengths.  The result also carries ``mode`` (one of STRIPE_MODES), ``stripe_diags`` (K),
+    ``stripes`` and ``workspace_bytes``; stage_ms: (histogram, forward, backward, backtrack) CUDA-event times.  Lengths,
+    method and budget are checked before any device work."""
+    if method not in VARIANTS:
+        raise ValueError(f'align_songs runs {sorted(VARIANTS)}, got {method!r}')
+    if len(srcs) != len(tgts) or len(srcs) == 0:
+        raise ValueError(f'{len(srcs)} amateur and {len(tgts)} professional contours')
+    plan = striped_plan([_frames(f) for f in srcs], [_frames(f) for f in tgts], workspace_bytes)
+    device = device_of(*srcs, *tgts)
+    src, S, dt = _batch_f0(srcs, device, 'amateur')
+    tgt, T, dt2 = _batch_f0(tgts, device, 'professional')
+    if dt != dt2:
+        raise TypeError('amateur and professional f0 must have the same type')
+    n, lib = len(S), _native.lib()
+    s_arr, s_p = _i32(S)
+    t_arr, t_p = _i32(T)
+    ws = torch.empty(plan.total_bytes, dtype=torch.uint8, device=device)
+    out = torch.empty(int(t_arr.sum()), dtype=torch.int64, device=device)
+    pc = torch.empty(n, dtype=torch.float32, device=device)
+    ms = (ctypes.c_float * 4)() if stage_ms else None
+    with torch.cuda.device(device):
+        _check(lib.svb_sadtw_align_striped(_vp(src), _vp(tgt), DTYPES[dt], VARIANTS[method], n, s_p, t_p, None, _vp(ws),
+                                           plan.total_bytes, int(workspace_bytes), _vp(out), _vp(pc), ms,
+                                           _native.current_stream_ptr(device)), 'sadtw_align_striped')
+    return AlignResult(alignment=out, offsets=np.concatenate([[0], np.cumsum(T)]).astype(np.int64), path_cost=pc,
+                       stage_ms=tuple(ms) if stage_ms else None, src_len=S, tgt_len=T, workspace=None, sections=None,
+                       mode=STRIPE_MODES[plan.mode], stripe_diags=plan.stripe_diags, stripes=plan.stripes,
+                       workspace_bytes=plan.total_bytes)
+
+
 def _sadtw(srcs, tgts, method, scales, stage_ms, keep_workspace, entry):
     if method not in VARIANTS:
         raise ValueError(f'method must be one of {sorted(METHODS)}, got {method!r}')

@@ -6,8 +6,8 @@ resampler runs, the others are float32 arrays.  Weights are random draws of the 
 tools/beautify_bench.py: the timings do not depend on what the weights have learnt.
 
 Reports, with the card's name and power limit read in the same run:
-  * CUDA-event times per stage of one call (h2d, resample, front_end, pitch, alignment = histogram + cost + DTW + backtrack
-    with their own event times, plan_conditioning = host planning and conditioning, acoustic_model, stitch, vocoder, d2h);
+  * CUDA-event times per stage of one call (h2d, resample, front_end, pitch, alignment = align_songs' histogram + forward +
+    backward + backtrack with their own event times, plan_conditioning = host planning and conditioning, acoustic_model, stitch, vocoder, d2h);
   * DTW microseconds per anti-diagonal step: the cluster kernel on each song aligned alone, and on a 5000 x 5000 pair the cluster
     kernel forced by SVB_DTW_CTA_CELLS (2 and 8 CTAs) against the one-CTA kernel, alternated in this process;
   * peak device memory of one call (torch.cuda.max_memory_allocated) and the alignment workspace of each song;
@@ -135,7 +135,7 @@ def main():
     print(f"{N} songs, {audio_s:.1f} s of input audio (both takes); call {wall:.3f} s (median of {args.repeats}), "
           f"{audio_s / wall:.1f} audio-s/s, peak device memory {peak / 1e9:.2f} GB")
     print('  stage (device time, ms): ' + ', '.join(f'{k} {v:.1f}' for k, v in res['stage_ms'].items()))
-    print('  alignment groups (histogram, cost, dtw, backtrack ms): ' + str(res['align_groups_ms']))
+    print('  alignment (histogram, forward, backward, backtrack ms): ' + str(res['align_groups_ms']))
     for i, s in enumerate(per_song):
         print(f"  song {i}: {s['frames']} frames, {s['ctas']} CTAs, {s['workspace_GB']} GB workspace, {s['segments']} segments, "
               f"DTW {s['dtw_us_per_step']:.3f} us/step (stages {s['stage_ms']} ms)")
