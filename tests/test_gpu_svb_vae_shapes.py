@@ -122,10 +122,13 @@ def _outputs(r, c):
     return out
 
 
-def _oracle_forward(batch, eps):
+def _oracle_forward(batch, eps, sd=None):
+    """The float64 oracle's outputs, keyed as _native_forward keys them, at ``sd`` (a model's state_dict; default the weights
+    _model loads)."""
     from oracle import fs2_vae as OF
     from oracle import svb_vae as OS
-    w = {k: (v.cuda().double() if v.is_floating_point() else v.cuda()) for k, v in S.make_svb_state_dict(1234).items()}
+    sd = S.make_svb_state_dict(1234) if sd is None else sd
+    w = {k: (v.cuda().double() if v.is_floating_point() else v.cuda()) for k, v in sd.items()}
     b = {k: (v.cuda().double() if v.is_floating_point() else v.cuda()) for k, v in batch.items()}
     with torch.no_grad(), torch.device('cuda'):            # oracle/vc_asr.py builds its position table on the default device
         r = OS.mle_svb_vae_forward(w, b, eps.cuda().double())
