@@ -236,6 +236,12 @@ int svb_tc_layer_forward(svb_tc_layer_t *layer, const float *x_dev, int32_t B, i
                          float *y_dev, void *stream);
 int svb_tc_layer_backward(svb_tc_layer_t *layer, const float *x_dev, const float *y_dev, const float *dy_dev, int32_t B,
                           int32_t T, int32_t W, float out_slope, float *dx_dev, float *dw_dev, float *db_dev, void *stream);
+/* Ragged batches (inference; dense stride-1 layers of svb_tc_layer_create, W = 1): clip b is x[b][:, :len[b]] (1 <= len[b] <= T),
+ * its frames past len[b] read as zero whatever they hold, as the clip alone and unpadded sees its padding; y[b][:, len[b]:] is
+ * written as zeros.  Only each clip's live 128-row tiles run.  A clip's result is the same bits in any batch, at any row and padded
+ * length.  len_host / len_dev: the same int32 [B] on the host (checked, planned) and on the device (read by the kernels). */
+int svb_tc_layer_forward_ragged(svb_tc_layer_t *layer, const float *x_dev, int32_t B, int32_t T, const int32_t *len_host,
+                                const int32_t *len_dev, float out_slope, float *y_dev, void *stream);
 
 /* ---- mel discriminator (modules/fastspeech/multi_window_disc.py): fp32 operators ------------------------------------
  * svb_conv2d_forward: y[b, co] = scale[b, co] * leaky_relu(conv2d(x, w) + bias, out_slope) on [B, C, H, W] device tensors,
@@ -329,6 +335,11 @@ int svb_conv1d_backward_run(const float *x_nct_dev, const float *w_host, const f
 int svb_conv_nct_forward(const float *x_dev, const float *w_dev, const float *bias_dev, float *y_dev, int32_t B,
                          int32_t Cin, int32_t Cout, int32_t Tin, int32_t W, int32_t K, int32_t stride, int32_t dil,
                          int32_t pad, int32_t groups, float out_slope, void *stream);
+/* svb_conv_nct_forward on a ragged batch (inference, W = 1), with svb_tc_layer_forward_ragged's contract: clip b is
+ * x[b][:, :len[b]]; its output has (len[b] + 2*pad - dil*(K-1) - 1)/stride + 1 frames (>= 1), the frames after them are zeros. */
+int svb_conv_nct_forward_ragged(const float *x_dev, const float *w_dev, const float *bias_dev, float *y_dev, int32_t B, int32_t Cin,
+                                int32_t Cout, int32_t Tin, int32_t K, int32_t stride, int32_t dil, int32_t pad, int32_t groups,
+                                float out_slope, const int32_t *len_host, const int32_t *len_dev, void *stream);
 /* AvgPool1d(4, 2, padding=1) over the last dim of [rows, Tin] (MultiScaleDiscriminator.meanpools, hifigan.py:304-307) */
 int svb_avgpool1d_4_2_1(const float *x_dev, float *y_dev, int64_t rows, int32_t Tin, void *stream);
 /* F.pad(x, (0, Tpad - T), 'reflect') over the last dim of [rows, T] (DiscriminatorP.forward, hifigan.py:209-212) */
@@ -468,6 +479,26 @@ int svb_layer_norm_nct(const float *x_dev, const float *gamma_dev, const float *
 int svb_relpos_attention_nct(const float *q_dev, const float *k_dev, const float *v_dev, const float *p_dev, const float *bias_u_dev,
                              const float *bias_v_dev, const float *mask_dev, int32_t B, int32_t C, int32_t T, int32_t n_head,
                              float *out_dev, void *stream);
+/* The same on a ragged batch: clip b is computed as alone at T = len[b] (1 <= len[b] <= T; its keys, queries and position rows),
+ * its rows past len[b] are written as zeros.  len_host / len_dev as svb_tc_layer_forward_ragged. */
+int svb_relpos_attention_nct_ragged(const float *q_dev, const float *k_dev, const float *v_dev, const float *p_dev,
+                                    const float *bias_u_dev, const float *bias_v_dev, const float *mask_dev, int32_t B, int32_t C,
+                                    int32_t T, int32_t n_head, const int32_t *len_host, const int32_t *len_dev, float *out_dev,
+                                    void *stream);
+
+/* ---- Length-aware reductions of the SVB acoustic model (MleSVBVAE with per-clip frame counts; csrc/acoustic_ragged.cu).  Each
+ * clip is reduced over its own frames in an order that depends only on its frame count and the channel shape.
+ * y = x + relu(GroupNorm(groups, C)(h)) over clip b's first len[b] frames of [B, C, T] tensors (ConvStacks' ConvBlock, norm 'gn'),
+ * statistics in float32 over those frames only; y[b][:, len[b]:] = 0. */
+int svb_group_norm_relu_add_ragged(const float *x_dev, const float *h_dev, const float *gamma_dev, const float *beta_dev, int32_t B,
+                                   int32_t C, int32_t T, int32_t groups, float eps, const int32_t *len_host, const int32_t *len_dev,
+                                   float *y_dev, void *stream);
+/* The GlobalFVAEEncoder's head (vae_models.py:102-104) on the last pooling's output x [B, 2*latent, T]: per clip the mean over its
+ * first n3 frames, n3 = its encoder frame count enc_len[b] through three valid k = 3 stride-2 convolutions (n -> (n - 3)/2 + 1,
+ * 1 <= n3 <= T), split into m / logs [B, latent] and z = m + eps * exp(logs) (eps [B, latent]). */
+int svb_global_latent_head_ragged(const float *x_dev, int32_t B, int32_t latent, int32_t T, const int32_t *enc_len_host,
+                                  const int32_t *enc_len_dev, const float *eps_dev, float *m_dev, float *logs_dev, float *z_dev,
+                                  void *stream);
 
 /* ---- Mel reconstruction loss of the SVB acoustic step (the `ssim:0.5|l1:0.5` recipe: FastSpeech2Task.l1_loss and
  * ssim_loss(bias), tasks/tts/fs2.py:158-175, ssim(..., size_average=False), modules/commons/ssim.py:319-351).

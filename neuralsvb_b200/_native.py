@@ -17,7 +17,7 @@ LIB_PATH = os.path.join(_HERE, 'libsvb_vocoder.so')
 HEADER = os.path.join(_ROOT, 'include', 'svb_vocoder.h')
 SOURCES = ['wn.cu', 'conformer.cu', 'api.cu', 'conv_ffma.cu', 'conv_tc.cu', 'nsf_source.cu', 'frontend.cu', 'generator.cu', 'layer_api.cu', 'disc_ops.cu',
            'train_ops.cu', 'generator_bwd.cu', 'disc_bwd.cu', 'tc_layer.cu', 'wgrad_tc.cu', 'mel_loss.cu', 'mel_disc.cu', 'sadtw.cu',
-           'pitch_ac.cu', 'resample.cu', 'flac.cu']
+           'pitch_ac.cu', 'resample.cu', 'flac.cu', 'acoustic_ragged.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '-Xcompiler', '-fPIC', '-shared']
 
@@ -131,6 +131,12 @@ _PROTOS = {
     'svb_tc_layer_out_len': (_I64, [_P, _I64]),
     'svb_tc_layer_forward': (ctypes.c_int, [_P, _P, _I32, _I32, _I32, ctypes.c_float, _P, _P]),
     'svb_tc_layer_backward': (ctypes.c_int, [_P, _P, _P, _P, _I32, _I32, _I32, ctypes.c_float, _P, _P, _P, _P]),
+    'svb_tc_layer_forward_ragged': (ctypes.c_int, [_P, _P, _I32, _I32, _P, _P, ctypes.c_float, _P, _P]),
+    'svb_conv_nct_forward_ragged': (ctypes.c_int, [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _I32, ctypes.c_float,
+                                                   _P, _P, _P]),
+    'svb_relpos_attention_nct_ragged': (ctypes.c_int, [_P, _P, _P, _P, _P, _P, _P, _I32, _I32, _I32, _I32, _P, _P, _P, _P]),
+    'svb_group_norm_relu_add_ragged': (ctypes.c_int, [_P, _P, _P, _P, _I32, _I32, _I32, _I32, ctypes.c_float, _P, _P, _P, _P]),
+    'svb_global_latent_head_ragged': (ctypes.c_int, [_P, _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P]),
     'svb_gen_set_training': (ctypes.c_int, [_P, _I32]),
     'svb_gen_update_weights': (ctypes.c_int, [_P]),
     'svb_gen_zero_grad': (ctypes.c_int, [_P, _P]),

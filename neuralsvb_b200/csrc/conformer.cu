@@ -53,28 +53,36 @@ __global__ void __launch_bounds__(256) layer_norm_nct_kernel(const float *__rest
 // rel_shift written as the index map it performs (oracle/vc_asr.py:shifted_bd):
 //   bd[i][j] = (q_i + v) . p[T-1-(i-j)]  for j <= i ;  0 for j == i+1 ;  (q_{i+1} + v) . p[j-i-2]  for j >= i+2
 // masked keys get finfo(float32).min before the softmax and 0 after it; out_i = sum_j attn[i][j] v_j.
+// RAGGED: clip b is computed as alone at T = len[b] (queries, keys and the position table's T - 1 - (i - j) rows); its rows at
+// or past len[b] are written as zeros.  The row stride of q, k, v and out stays T (Tr below).
 constexpr int kAttWarps = 8;
+template <bool RAGGED>
 __global__ void __launch_bounds__(32 * kAttWarps) relpos_attention_nct_kernel(const float *__restrict__ q, const float *__restrict__ k,
                                                                               const float *__restrict__ v, const float *__restrict__ p,
                                                                               const float *__restrict__ bias_u, const float *__restrict__ bias_v,
-                                                                              const float *__restrict__ mask, int C, int T, int dk,
-                                                                              float *__restrict__ out) {
+                                                                              const float *__restrict__ mask, int C, int Tr, int dk,
+                                                                              float *__restrict__ out, const int *__restrict__ len) {
     extern __shared__ float sm[];                   // per warp: qu[dk], qv[dk], qv_next[dk], scores[T]
     const int lane = threadIdx.x & 31, wrp = threadIdx.x >> 5;
     const int h = blockIdx.y, b = blockIdx.z, i = blockIdx.x * kAttWarps + wrp;
-    if (i >= T) return;
-    float *qu = sm + (size_t)wrp * (3 * dk + T), *qv = qu + dk, *qn = qv + dk, *sc = qn + dk;
-    const size_t base = ((size_t)b * C + (size_t)h * dk) * T;
-    const float *kb = k + base, *vb = v + base, *pb = p + (size_t)h * dk * T;
+    if (i >= Tr) return;
+    const size_t base = ((size_t)b * C + (size_t)h * dk) * Tr;
+    const int T = RAGGED ? min(Tr, __ldg(len + b)) : Tr;
+    if (RAGGED && i >= T) {
+        for (int d = lane; d < dk; d += 32) out[base + (size_t)d * Tr + i] = 0.f;
+        return;
+    }
+    float *qu = sm + (size_t)wrp * (3 * dk + Tr), *qv = qu + dk, *qn = qv + dk, *sc = qn + dk;
+    const float *kb = k + base, *vb = v + base, *pb = p + (size_t)h * dk * Tr;
     for (int d = lane; d < dk; d += 32) {
-        const float qi = q[base + (size_t)d * T + i];
+        const float qi = q[base + (size_t)d * Tr + i];
         qu[d] = qi + __ldg(bias_u + h * dk + d);
         qv[d] = qi + __ldg(bias_v + h * dk + d);
-        qn[d] = (i + 1 < T ? q[base + (size_t)d * T + i + 1] : 0.f) + __ldg(bias_v + h * dk + d);
+        qn[d] = (i + 1 < T ? q[base + (size_t)d * Tr + i + 1] : 0.f) + __ldg(bias_v + h * dk + d);
     }
     __syncwarp();
     const float scale = rsqrtf((float)dk);
-    const float *mb = mask ? mask + (size_t)b * T : nullptr;
+    const float *mb = mask ? mask + (size_t)b * Tr : nullptr;
     float mx = -FLT_MAX;
     for (int j = lane; j < T; j += 32) {
         float ac = 0.f, bd = 0.f;
@@ -82,8 +90,8 @@ __global__ void __launch_bounds__(32 * kAttWarps) relpos_attention_nct_kernel(co
         const int col = past ? T - 1 - (i - j) : (zero ? 0 : j - i - 2);
         const float *qsel = past ? qv : qn;
         for (int d = 0; d < dk; ++d) {
-            ac = fmaf(qu[d], kb[(size_t)d * T + j], ac);
-            bd = fmaf(qsel[d], __ldg(pb + (size_t)d * T + col), bd);
+            ac = fmaf(qu[d], kb[(size_t)d * Tr + j], ac);
+            bd = fmaf(qsel[d], __ldg(pb + (size_t)d * Tr + col), bd);
         }
         float s = (ac + (zero ? 0.f : bd)) * scale;
         if (mb && !(mb[j] > 0.f)) s = -FLT_MAX;
@@ -105,10 +113,10 @@ __global__ void __launch_bounds__(32 * kAttWarps) relpos_attention_nct_kernel(co
     __syncwarp();
     for (int d = 0; d < dk; ++d) {
         float acc = 0.f;
-        for (int j = lane; j < T; j += 32) acc = fmaf(sc[j], vb[(size_t)d * T + j], acc);
+        for (int j = lane; j < T; j += 32) acc = fmaf(sc[j], vb[(size_t)d * Tr + j], acc);
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-        if (lane == 0) out[base + (size_t)d * T + i] = acc;
+        if (lane == 0) out[base + (size_t)d * Tr + i] = acc;
     }
 }
 
@@ -135,9 +143,30 @@ extern "C" int svb_relpos_attention_nct(const float *q_dev, const float *k_dev, 
     const size_t smem = (size_t)kAttWarps * (3 * dk + T) * 4;
     SVB_CHECK(smem <= 200 * 1024, SVB_ERR_INVALID, "relpos_attention_nct: T %d does not fit the score rows in shared memory", T);
     static size_t configured[kSmemCacheDevices] = {};
-    SVB_TRY(raise_smem_limit(relpos_attention_nct_kernel, smem, configured));
-    relpos_attention_nct_kernel<<<dim3((T + kAttWarps - 1) / kAttWarps, n_head, B), 32 * kAttWarps, smem, as_stream(stream)>>>(
-        q_dev, k_dev, v_dev, p_dev, bias_u_dev, bias_v_dev, mask_dev, C, T, dk, out_dev);
+    SVB_TRY(raise_smem_limit(relpos_attention_nct_kernel<false>, smem, configured));
+    relpos_attention_nct_kernel<false><<<dim3((T + kAttWarps - 1) / kAttWarps, n_head, B), 32 * kAttWarps, smem, as_stream(stream)>>>(
+        q_dev, k_dev, v_dev, p_dev, bias_u_dev, bias_v_dev, mask_dev, C, T, dk, out_dev, nullptr);
+    SVB_CUDA(cudaGetLastError());
+    return SVB_OK;
+}
+
+extern "C" int svb_relpos_attention_nct_ragged(const float *q_dev, const float *k_dev, const float *v_dev, const float *p_dev,
+                                               const float *bias_u_dev, const float *bias_v_dev, const float *mask_dev, int32_t B,
+                                               int32_t C, int32_t T, int32_t n_head, const int32_t *len_host, const int32_t *len_dev,
+                                               float *out_dev, void *stream) {
+    SVB_CHECK(q_dev && k_dev && v_dev && p_dev && bias_u_dev && bias_v_dev && out_dev && len_host && len_dev && B > 0 && T > 0 &&
+                  n_head > 0 && C % n_head == 0,
+              SVB_ERR_INVALID, "relpos_attention_nct_ragged: bad argument");
+    for (int b = 0; b < B; ++b)
+        SVB_CHECK(len_host[b] >= 1 && len_host[b] <= T, SVB_ERR_INVALID, "relpos_attention_nct_ragged: clip %d has %d frames (T %d)", b,
+                  len_host[b], T);
+    const int dk = C / n_head;
+    const size_t smem = (size_t)kAttWarps * (3 * dk + T) * 4;
+    SVB_CHECK(smem <= 200 * 1024, SVB_ERR_INVALID, "relpos_attention_nct_ragged: T %d does not fit the score rows in shared memory", T);
+    static size_t configured[kSmemCacheDevices] = {};
+    SVB_TRY(raise_smem_limit(relpos_attention_nct_kernel<true>, smem, configured));
+    relpos_attention_nct_kernel<true><<<dim3((T + kAttWarps - 1) / kAttWarps, n_head, B), 32 * kAttWarps, smem, as_stream(stream)>>>(
+        q_dev, k_dev, v_dev, p_dev, bias_u_dev, bias_v_dev, mask_dev, C, T, dk, out_dev, len_dev);
     SVB_CUDA(cudaGetLastError());
     return SVB_OK;
 }

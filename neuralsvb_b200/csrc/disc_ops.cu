@@ -28,8 +28,10 @@ constexpr int kGCI = 4;   // input channels per shared-memory chunk
 
 // Block = COQ output-channel quads (4*COQ = the group's output channels, up to 64) x 4*TX outputs, TX = 256 / COQ:
 // the narrow groups of the MSD (8-32 channels per group) keep every thread busy.
-template <int COQ>
-__global__ void __launch_bounds__(256) gconv_kernel(GConvArgs a) {
+// RAGGED (inference): clip b's input frames at or past len[b] read as zero, as the clip alone and unpadded; its output frames
+// at or past its own output length are written as zeros, and blocks wholly past it skip the arithmetic.
+template <int COQ, bool RAGGED>
+__global__ void __launch_bounds__(256) gconv_kernel(GConvArgs a, const int *__restrict__ len) {
     constexpr int TX = 256 / COQ, kGT = 4 * TX, kGC = 4 * COQ;
     extern __shared__ float sm[];
     const int span = (kGT - 1) * a.stride + (a.K - 1) * a.dil + 1;
@@ -41,6 +43,15 @@ __global__ void __launch_bounds__(256) gconv_kernel(GConvArgs a) {
     const int bw = blockIdx.z, b = bw / a.W, wcol = bw % a.W;
     const int to0 = blockIdx.x * kGT;
     const int tid = threadIdx.x, tx = tid % TX, ty = tid / TX;       // tx: outputs tx + TX j ; ty: couts 4 ty ..
+    const int Tin = RAGGED ? min(a.Tin, __ldg(len + b)) : a.Tin;
+    const int Tout = RAGGED ? min(a.Tout, (Tin + 2 * a.pad - a.dil * (a.K - 1) - 1) / a.stride + 1) : a.Tout;
+    if (RAGGED && to0 >= Tout) {
+        for (int idx = tid; idx < kGC * kGT; idx += 256) {
+            const int cog = co_t * kGC + idx / kGT, to = to0 + idx % kGT;
+            if (cog < cout_g && to < a.Tout) a.y[(((size_t)b * a.Cout + g * cout_g + cog) * a.Tout + to) * a.W + wcol] = 0.f;
+        }
+        return;
+    }
     float acc[4][4];
 #pragma unroll
     for (int i = 0; i < 4; ++i)
@@ -53,7 +64,7 @@ __global__ void __launch_bounds__(256) gconv_kernel(GConvArgs a) {
             const int ci = idx / span, s = idx - ci * span;
             const int t = t_in0 + s;
             float v = 0.f;
-            if (c0 + ci < cin_g && t >= 0 && t < a.Tin)
+            if (c0 + ci < cin_g && t >= 0 && t < Tin)
                 v = __ldg(a.x + (((size_t)b * a.Cin + g * cin_g + c0 + ci) * a.Tin + t) * a.W + wcol);
             xs[idx] = v;
         }
@@ -88,7 +99,7 @@ __global__ void __launch_bounds__(256) gconv_kernel(GConvArgs a) {
             const int to = to0 + tx + TX * j;
             if (to >= a.Tout) continue;
             const float v = acc[i][j] + bv;
-            a.y[(((size_t)b * a.Cout + co) * a.Tout + to) * a.W + wcol] = lrelu(v, a.out_slope);
+            a.y[(((size_t)b * a.Cout + co) * a.Tout + to) * a.W + wcol] = (RAGGED && to >= Tout) ? 0.f : lrelu(v, a.out_slope);
         }
     }
 }
@@ -164,16 +175,16 @@ __global__ void matvec_rows_kernel(const float *__restrict__ Wm, const float *__
 
 using namespace svb;
 
-template <int COQ>
-static int launch_gconv(const GConvArgs &a, cudaStream_t st) {
+template <int COQ, bool RAGGED = false>
+static int launch_gconv(const GConvArgs &a, cudaStream_t st, const int *len = nullptr) {
     constexpr int TX = 256 / COQ, kGT = 4 * TX, kGC = 4 * COQ;
     const int span = (kGT - 1) * a.stride + (a.K - 1) * a.dil + 1;
     const size_t smem = ((size_t)kGCI * span + (size_t)kGCI * a.K * kGC) * 4;
     static size_t configured[kSmemCacheDevices] = {};
-    SVB_TRY(raise_smem_limit(gconv_kernel<COQ>, smem, configured));
+    SVB_TRY(raise_smem_limit(gconv_kernel<COQ, RAGGED>, smem, configured));
     const int cout_g = a.Cout / a.groups;
     dim3 grid((a.Tout + kGT - 1) / kGT, ((cout_g + kGC - 1) / kGC) * a.groups, a.B * a.W);
-    gconv_kernel<COQ><<<grid, 256, smem, st>>>(a);
+    gconv_kernel<COQ, RAGGED><<<grid, 256, smem, st>>>(a, len);
     SVB_CUDA(cudaGetLastError());
     return SVB_OK;
 }
@@ -244,6 +255,33 @@ extern "C" int svb_conv_nct_forward(const float *x_dev, const float *w_dev, cons
     if (cout_g <= 16) return launch_gconv<4>(a, as_stream(stream));
     if (cout_g <= 32) return launch_gconv<8>(a, as_stream(stream));
     return launch_gconv<16>(a, as_stream(stream));
+}
+
+// Ragged batches (inference, W = 1): clip b is x[b][:, :len[b]]; its output has (len[b] + 2 pad - dil (K - 1) - 1) / stride + 1
+// frames, the frames after them are zeros.  The result of a clip does not depend on B, Tin, its row or its padding.
+extern "C" int svb_conv_nct_forward_ragged(const float *x_dev, const float *w_dev, const float *bias_dev, float *y_dev, int32_t B,
+                                           int32_t Cin, int32_t Cout, int32_t Tin, int32_t K, int32_t stride, int32_t dil, int32_t pad,
+                                           int32_t groups, float out_slope, const int32_t *len_host, const int32_t *len_dev,
+                                           void *stream) {
+    SVB_CHECK(x_dev && w_dev && y_dev && len_host && len_dev && B > 0 && Cin > 0 && Cout > 0 && Tin > 0 && K > 0 && stride > 0 &&
+                  dil > 0 && groups > 0 && Cin % groups == 0 && Cout % groups == 0 && pad >= 0,
+              SVB_ERR_INVALID, "conv_nct_ragged: bad argument");
+    GConvArgs a;
+    a.x = x_dev, a.w = w_dev, a.bias = bias_dev, a.y = y_dev;
+    a.B = B, a.Cin = Cin, a.Cout = Cout, a.Tin = Tin, a.W = 1, a.K = K, a.stride = stride, a.dil = dil, a.pad = pad;
+    a.groups = groups, a.out_slope = out_slope;
+    a.Tout = (Tin + 2 * pad - dil * (K - 1) - 1) / stride + 1;
+    for (int b = 0; b < B; ++b) {
+        const int n = len_host[b];
+        SVB_CHECK(n >= 1 && n <= Tin && (n + 2 * pad - dil * (K - 1) - 1) / stride + 1 >= 1 && n + 2 * pad - dil * (K - 1) - 1 >= 0,
+                  SVB_ERR_INVALID, "conv_nct_ragged: clip %d has %d frames (Tin %d, K %d, stride %d): no output frame", b, n, Tin, K, stride);
+    }
+    const int cout_g = Cout / groups;
+    cudaStream_t st = as_stream(stream);
+    if (cout_g <= 8) return launch_gconv<2, true>(a, st, len_dev);
+    if (cout_g <= 16) return launch_gconv<4, true>(a, st, len_dev);
+    if (cout_g <= 32) return launch_gconv<8, true>(a, st, len_dev);
+    return launch_gconv<16, true>(a, st, len_dev);
 }
 
 extern "C" int svb_avgpool1d_4_2_1(const float *x_dev, float *y_dev, int64_t rows, int32_t Tin, void *stream) {

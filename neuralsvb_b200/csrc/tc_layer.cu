@@ -26,9 +26,13 @@ namespace {
 // no memset): out[clip][(c*KE + j)][to] = x[b][c][to*s + j - p][w] * (mask ? lrelu'(mask) : 1)
 // grid (row blocks, channel groups, clips); a warp writes one 128-byte row per step, a thread keeps its (channel, tap):
 // no per-element index division, the gathered input lines are re-read from L1 by the neighbouring rows of the block.
+// RAGGED (len = frames per clip, W = 1): clip b's input frames at or past len[b] read as zero, as a clip alone and unpadded
+// sees its zero padding.
 constexpr int kExpRows = 64;
+template <bool RAGGED>
 __global__ void __launch_bounds__(256) expand_to_g32t_kernel(const float *__restrict__ x, const float *__restrict__ mask, float slope, int C,
-                                                             int T, int W, int KE, int s, int p, int Tq, int Tp, float *__restrict__ out) {
+                                                             int T, int W, int KE, int s, int p, int Tq, int Tp, float *__restrict__ out,
+                                                             const int *__restrict__ len) {
     const int lane = threadIdx.x & 31, wrp = threadIdx.x >> 5;
     const int grp = blockIdx.y, clip = blockIdx.z, groups = gridDim.y;
     const int cc = grp * 32 + lane;
@@ -39,13 +43,14 @@ __global__ void __launch_bounds__(256) expand_to_g32t_kernel(const float *__rest
     const float *xb = x + xoff;
     const float *mb = mask ? mask + xoff : nullptr;
     float *ob = out + ((size_t)clip * groups + grp) * Tp * 32 + lane;
+    const int Tb = RAGGED ? min(T, __ldg(len + b)) : T;
     const int r1 = min(Tp, (int)(blockIdx.x + 1) * kExpRows);
     for (int row = blockIdx.x * kExpRows + wrp; row < r1; row += 8) {
         const int to = row - kPad;
         float v = 0.f;
         if (ch_ok && to >= 0 && to < Tq) {
             const int t = to * s + j - p;
-            if (t >= 0 && t < T) {
+            if (t >= 0 && t < Tb) {
                 v = __ldg(xb + (size_t)t * W);
                 if (mb && !(__ldg(mb + (size_t)t * W) > 0.f)) v *= slope;
             }
@@ -56,16 +61,19 @@ __global__ void __launch_bounds__(256) expand_to_g32t_kernel(const float *__rest
 
 // y[b][c][t][w] = lrelu(g[clip][c][row0 + t], slope).  One block = (32 rows, one 32-channel group, one b, ALL w): the rows
 // come in as whole 128-byte lines into a padded smem tile, every channel then leaves as one contiguous run of 32*W floats.
+// RAGGED (W = 1): frames at or past len[b] are written as zeros.
 constexpr int kMaxTileW = 11;       // MPD periods 2..11; wider W fall back to W slices of this size
+template <bool RAGGED>
 __global__ void __launch_bounds__(256) g32t_to_nctw_kernel(const float *__restrict__ g, int C, int T, int W, int Tp, float slope,
-                                                           float *__restrict__ y, int row0, int w0, int wn) {
+                                                           float *__restrict__ y, int row0, int w0, int wn, const int *__restrict__ len) {
     __shared__ float tile[kMaxTileW][32][33];
     const int lane = threadIdx.x & 31, wrp = threadIdx.x >> 5;
     const int t0 = blockIdx.x * 32, grp = blockIdx.y, b = blockIdx.z, groups = gridDim.y;
+    const int Tb = RAGGED ? min(T, __ldg(len + b)) : T;
     for (int idx = wrp; idx < wn * 32; idx += 8) {          // (w, row) pairs: one coalesced 128-byte line each
         const int wi = idx >> 5, tr = idx & 31;
         float v = 0.f;
-        if (t0 + tr < T) v = g[((((size_t)b * W + w0 + wi) * groups + grp) * Tp + kPad + row0 + t0 + tr) * 32 + lane];
+        if (t0 + tr < Tb) v = g[((((size_t)b * W + w0 + wi) * groups + grp) * Tp + kPad + row0 + t0 + tr) * 32 + lane];
         tile[wi][tr][lane] = v >= 0.f ? v : v * slope;
     }
     __syncthreads();
@@ -180,14 +188,18 @@ int arena_get(int device, size_t bytes, char **out) {
 }
 
 void launch_expand(const float *x, const float *mask, float slope, int B, int C, int T, int W, int KE, int s, int p, int Tq, int Tp,
-                   float *out, cudaStream_t st) {
+                   float *out, cudaStream_t st, const int *len = nullptr) {
     const dim3 grid((Tp + kExpRows - 1) / kExpRows, c4t_groups(C * KE), B * W);
-    expand_to_g32t_kernel<<<grid, 256, 0, st>>>(x, mask, slope, C, T, W, KE, s, p, Tq, Tp, out);
+    if (len) expand_to_g32t_kernel<true><<<grid, 256, 0, st>>>(x, mask, slope, C, T, W, KE, s, p, Tq, Tp, out, len);
+    else expand_to_g32t_kernel<false><<<grid, 256, 0, st>>>(x, mask, slope, C, T, W, KE, s, p, Tq, Tp, out, nullptr);
 }
-void launch_g32t_to_nctw(const float *g, int B, int C, int T, int W, int Tp, float slope, float *y, int row0, cudaStream_t st) {
+void launch_g32t_to_nctw(const float *g, int B, int C, int T, int W, int Tp, float slope, float *y, int row0, cudaStream_t st,
+                         const int *len = nullptr) {
     const dim3 grid((T + 31) / 32, c4t_groups(C), B);
-    for (int w0 = 0; w0 < W; w0 += kMaxTileW)
-        g32t_to_nctw_kernel<<<grid, 256, 0, st>>>(g, C, T, W, Tp, slope, y, row0, w0, std::min(kMaxTileW, W - w0));
+    for (int w0 = 0; w0 < W; w0 += kMaxTileW) {
+        if (len) g32t_to_nctw_kernel<true><<<grid, 256, 0, st>>>(g, C, T, W, Tp, slope, y, row0, w0, std::min(kMaxTileW, W - w0), len);
+        else g32t_to_nctw_kernel<false><<<grid, 256, 0, st>>>(g, C, T, W, Tp, slope, y, row0, w0, std::min(kMaxTileW, W - w0), nullptr);
+    }
 }
 void launch_col2im(const float *g, int B, int C, int T, int W, int KE, int s, int p, int Tq, int Tp, float *dx, cudaStream_t st) {
     const dim3 grid((T * W + 255) / 256, C, B);
@@ -410,8 +422,9 @@ extern "C" int svb_tc_layer_set_weight_dev(svb_tc_layer_t *L, const float *w_dev
 }
 
 static int run_tc(const svb_tc_layer *L, const ConvLayer &cl, const float *in, float *out, int Tp, int clips, int Tq, cudaStream_t st,
-                  int cin_blk = 0) {
+                  int cin_blk = 0, const int *len_dev = nullptr, const int *len_host = nullptr) {
     ConvArgs a;
+    a.len = len_dev, a.len_host = len_host, a.len_mul = 1;
     a.in = in, a.w = cl.w, a.bias = cl.b, a.res = nullptr, a.out = out;
     a.B = clips, a.Cin = cl.Cin, a.in_Tp = Tp, a.Cout = cl.Cout, a.out_Tp = Tp, a.CoutP = cl.CoutP, a.Tq = Tq;
     a.KS = cl.KS, a.dil = 1, a.ups_u = 0, a.in_slope = 1.f, a.out_scale = 1.f, a.accumulate = 0;
@@ -469,6 +482,31 @@ extern "C" int svb_tc_layer_forward(svb_tc_layer_t *L, const float *x_dev, int32
                                                                          Tq, Tp, xe, st);
     SVB_TRY(run_tc(L, L->fwd, xe, yg, Tp, clips, Tq, st));
     launch_g32t_to_nctw(yg, B, L->Cout, Tq, W, Tp, out_slope, y_dev, 0, st);
+    SVB_CUDA(cudaGetLastError());
+    return SVB_OK;
+}
+
+// Ragged batches (inference): clip b is x[b][:, :len[b]], frames past it absent.  The planner's ragged route (ConvArgs::len)
+// runs only each clip's live 128-row tiles; a clip's result does not depend on B, T, its row or its padding.
+extern "C" int svb_tc_layer_forward_ragged(svb_tc_layer_t *L, const float *x_dev, int32_t B, int32_t T, const int32_t *len_host,
+                                           const int32_t *len_dev, float out_slope, float *y_dev, void *stream) {
+    SVB_CHECK(L && L->has_w && x_dev && y_dev && len_host && len_dev && B > 0 && T > 0, SVB_ERR_INVALID,
+              "tc_layer_forward_ragged: bad argument");
+    SVB_CHECK(!L->two_d && !L->poly && L->stride == 1, SVB_ERR_INVALID,
+              "tc_layer_forward_ragged: dense stride-1 layers only (stride %d%s)", L->stride, L->poly ? ", grouped" : L->two_d ? ", 2-D" : "");
+    for (int b = 0; b < B; ++b)
+        SVB_CHECK(len_host[b] >= 1 && len_host[b] <= T, SVB_ERR_INVALID, "tc_layer_forward_ragged: clip %d has %d frames (T %d)", b,
+                  len_host[b], T);
+    SVB_CUDA(cudaSetDevice(L->device));
+    cudaStream_t st = as_stream(stream);
+    const int Tp = c4t_rows(T);
+    const size_t n_x = c4t_floats(B, L->Cin, T), n_y = c4t_floats(B, L->Cout, T);
+    char *base;
+    SVB_TRY(arena_get(L->device, (n_x + n_y) * 4, &base));
+    float *xe = reinterpret_cast<float *>(base), *yg = xe + n_x;
+    launch_expand(x_dev, nullptr, 1.f, B, L->Cin, T, 1, 1, 1, 0, T, Tp, xe, st, len_dev);
+    SVB_TRY(run_tc(L, L->fwd, xe, yg, Tp, B, T, st, 0, len_dev, len_host));
+    launch_g32t_to_nctw(yg, B, L->Cout, T, 1, Tp, out_slope, y_dev, 0, st, len_dev);
     SVB_CUDA(cudaGetLastError());
     return SVB_OK;
 }

@@ -145,6 +145,7 @@ class SVBBeautifier:
             self.vocoder = get_vocoder_cls(self.hp)()
         self.mel_basis = torch.tensor(audio.build_mel_basis(self.hp), dtype=torch.float32, device=self.device)
         self.timing, self.stage_ms = False, None
+        self._batch_invariant = False       # the current call's batch_invariant (beautify_batch / beautify_songs)
 
     # ------------------------------------------------------------------ host checks
     def _takes(self, amateur, professional, spk_emb, songs=False):
@@ -217,7 +218,8 @@ class SVBBeautifier:
 
     def _model_on(self, sample, mel, a_rows, p_rows, Ta, Tp, eps):
         """MleSVBVAE on the collated batch whose amateur take b is mel rows [a_rows[b], a_rows[b] + Ta[b]) and professional take
-        b rows [p_rows[b], p_rows[b] + Tp[b]) -> a2p mel_out [B, max Tp, n_mel] (device)."""
+        b rows [p_rows[b], p_rows[b] + Tp[b]) -> a2p mel_out [B, max Tp, n_mel] (device).  With the call's batch_invariant, the
+        model runs in its length-aware mode on Ta / Tp."""
         B = len(Ta)
         d = self.device
 
@@ -229,7 +231,8 @@ class SVBBeautifier:
         out = self.model(amateur_mel=pad(a_rows, Ta), prof_mel=pad(p_rows, Tp), amateur_pitch=sample['pitch'].to(d),
                          prof_pitch=sample['prof_pitch'].to(d), amateur_spk_id=sample['spk'].to(d), prof_spk_id=sample['spk'].to(d),
                          a2p_alignment=sample['a2p_f0_alignment'].to(d), infer=False, concurrent_ways=list(WAYS),
-                         disable_map=self.hp['disable_map'], eps=eps)
+                         disable_map=self.hp['disable_map'], eps=eps,
+                         **(dict(amateur_lens=Ta, prof_lens=Tp) if self._batch_invariant else {}))
         return out['a2p']['mel_out']
 
     def _vocode(self, mel_out, f0, Tp, seed, first_clip=0):
@@ -246,7 +249,7 @@ class SVBBeautifier:
         return torch.cat(clips)
 
     # ------------------------------------------------------------------ public
-    def beautify_batch(self, amateur, professional, spk_emb, seed=None, eps=None):
+    def beautify_batch(self, amateur, professional, spk_emb, seed=None, eps=None, batch_invariant=False):
         """The a2p take of every (amateur, professional, embedding) triple: float32 arrays of T_prof x hop samples, T_prof the
         professional take's frame count after the dataset's crop.  A take is a WAV path (any rate) or a float32 array at
         audio_sample_rate; an embedding is the amateur take's own [256] vector or a .npy path (row 0 of multi_spk_emb).
@@ -259,16 +262,21 @@ class SVBBeautifier:
         a take shorter than one pitch window or than 60 frames after the frames_multiple crop, a take longer than max_frames
         (the task would crop it silently), a take without voiced f0 (the binarizer's "Empty f0" skip), lists of different
         lengths, or an embedding that is not 256 finite floats.  The binarizer's ``max_mel_tech_gap`` skip is dataset curation and
-        is not applied."""
+        is not applied.
+
+        ``batch_invariant``: the acoustic model runs in its length-aware mode (MleSVBVAE's amateur_lens / prof_lens), so each
+        pair's a2p mel is the same bits as that pair beautified alone with batch_invariant=True and the same eps row, and its
+        waveform too given the same NSF key.  The reference only ever runs one pair at a time.  The default (False) runs the model
+        on the zero-padded batch, as the task's collated batches do: a pair's mel then moves with the other pairs' lengths."""
         with torch.no_grad(), torch.cuda.device(self.device):
-            return self._run(amateur, professional, spk_emb, seed, eps)
+            return self._run(amateur, professional, spk_emb, seed, eps, batch_invariant)
 
     def beautify(self, amateur, professional, spk_emb, **kw):
         """``beautify_batch`` of one pair -> one float32 array."""
         return self.beautify_batch([amateur], [professional], [spk_emb], **kw)[0]
 
     def beautify_songs(self, amateur, professional, spk_emb, seed=None, eps=None, segment_frames=None, overlap_frames=64,
-                       align_bytes=None):
+                       align_bytes=None, batch_invariant=False):
         """The a2p take of whole songs: ``beautify_batch``'s inputs, with each take up to LONG_MAX_FRAMES frames (6.3 min at
         22.05 kHz / hop 128) instead of max_frames.  Returns one float32 array of Tp x hop samples per song, Tp the professional
         frame count cropped to a multiple of frames_multiple.
@@ -292,9 +300,14 @@ class SVBBeautifier:
         unless given.  Bad segment_frames / overlap_frames and an align_bytes below the smallest workable alignment budget (the
         message names it) raise before any device work; every song is checked and planned
         before the model runs: a bad take, a take over LONG_MAX_FRAMES or a song that cannot be planned raises ValueError naming
-        the song."""
+        the song.
+
+        ``batch_invariant``: each segment runs as it would alone (``beautify_batch``'s batch_invariant), so the short tail segment
+        no longer moves with the padding to the longest segment; a song that fits one segment then gives exactly
+        ``beautify(..., batch_invariant=True)`` of the pair."""
         with torch.no_grad(), torch.cuda.device(self.device):
-            return self._run_songs(amateur, professional, spk_emb, seed, eps, segment_frames, overlap_frames, align_bytes)
+            return self._run_songs(amateur, professional, spk_emb, seed, eps, segment_frames, overlap_frames, align_bytes,
+                                   batch_invariant)
 
     def _song_conditioning(self, frames, f0s, B):
         """Per take (B amateur, then B professional): the cropped frame count, the f0 the segments are conditioned on (moved by
@@ -318,12 +331,14 @@ class SVBBeautifier:
         self.align_ms = [r.stage_ms] if self.timing else []
         return r.split()
 
-    def _run_songs(self, amateur, professional, spk_emb, seed, eps, segment_frames, overlap_frames, align_bytes=None):
+    def _run_songs(self, amateur, professional, spk_emb, seed, eps, segment_frames, overlap_frames, align_bytes=None,
+                   batch_invariant=False):
         from neuralsvb_b200.modules.voice_conversion.dtw.core import striped_plan
         hp = self.hp
         segment_sizes(hp, segment_frames, overlap_frames, 'beautify_songs')         # before any device work
         dec, rates, lens, frames, spk = self._takes(amateur, professional, spk_emb, songs=True)
         B = len(spk)
+        self._batch_invariant = bool(batch_invariant)
         self._align_bytes = SONG_ALIGN_BYTES if align_bytes is None else int(align_bytes)
         try:
             striped_plan(frames[:B], frames[B:], self._align_bytes)                  # a budget below the minimum: before any device work
@@ -392,10 +407,11 @@ class SVBBeautifier:
         hop = int(hp['hop_size'])
         return np.split(out, np.cumsum([t * hop for t in Tps])[:-1])
 
-    def _run(self, amateur, professional, spk_emb, seed, eps):
+    def _run(self, amateur, professional, spk_emb, seed, eps, batch_invariant=False):
         hp = self.hp
         dec, rates, lens, frames, spk = self._takes(amateur, professional, spk_emb)
         B = len(spk)
+        self._batch_invariant = bool(batch_invariant)
         if eps is not None:
             eps = torch.as_tensor(eps, dtype=torch.float32)
             if tuple(eps.shape) != (B, hp['latent_size'], 1):
@@ -458,6 +474,9 @@ def parse_args(argv=None):
     p.add_argument('--align_gb', type=float, default=None,
                    help='with --song: device memory budget of the alignment in GiB (default 24); a lower one aligns in about '
                         'twice the time with the same results')
+    p.add_argument('--batch_invariant', action='store_true',
+                   help='run the acoustic model on each pair\'s (or song segment\'s) own frames only: every output is then the same '
+                        'as that pair beautified alone, whatever else is in the call')
     args = p.parse_args(argv)
     counts = {k: len(getattr(args, k)) for k in ('amateur', 'prof', 'spk_emb', 'out')}
     if len(set(counts.values())) != 1:
@@ -474,9 +493,9 @@ def main(argv=None):
     b = SVBBeautifier(work_dir, hp=hparams)
     if args.song:
         align_bytes = None if args.align_gb is None else int(args.align_gb * (1 << 30))
-        wavs = b.beautify_songs(args.amateur, args.prof, args.spk_emb, align_bytes=align_bytes)
+        wavs = b.beautify_songs(args.amateur, args.prof, args.spk_emb, align_bytes=align_bytes, batch_invariant=args.batch_invariant)
     else:
-        wavs = b.beautify_batch(args.amateur, args.prof, args.spk_emb)
+        wavs = b.beautify_batch(args.amateur, args.prof, args.spk_emb, batch_invariant=args.batch_invariant)
     for w, fn in zip(wavs, args.out):
         if os.path.dirname(fn):
             os.makedirs(os.path.dirname(fn), exist_ok=True)

@@ -404,8 +404,12 @@ class GlobalFVAEEncoder(nn.Module):
         scale = bn.weight / torch.sqrt(bn.running_var + bn.eps)
         return x * scale[None, :, None] + (bn.bias - bn.running_mean * scale)[None, :, None]
 
-    def forward(self, x, x_mask, g, eps=None):
+    def forward(self, x, x_mask, g, eps=None, lens=None):
+        """``lens`` (FrameLens of the mel frames; inference): each clip from its own frames only -- its convolutions treat the frames
+        past its end as absent, and its latent is the mean over its own pooled frames (svb_global_latent_head_ragged)."""
         from neuralsvb_b200.modules.hifigan.discriminators import conv_nct
+        if lens is not None:
+            return self._forward_ragged(x, x_mask, g, eps, lens)
         train = torch.is_grad_enabled() and self.training
         if train and not self.trainable:
             raise RuntimeError('neuralsvb_b200 GlobalFVAEEncoder is inference only: call .eval() and run under torch.no_grad() '
@@ -429,6 +433,29 @@ class GlobalFVAEEncoder(nn.Module):
         z = m + (torch.randn_like(m) if eps is None else eps) * torch.exp(logs)                         # :104
         return z, m, logs, x_mask
 
+    def _forward_ragged(self, x, x_mask, g, eps, lens):
+        from neuralsvb_b200.modules.hifigan.discriminators import conv_nct_ragged
+        s0 = self.strides[0]
+        c = self.pre_net[0]
+        enc = lens.map(lambda n: (n + 2 * (s0 // 2) - 2 * s0) // s0 + 1)
+        x = conv_nct_ragged(x.float(), c.weight, c.bias, 2 * s0, s0, s0 // 2, 1, 1.0, lens)
+        x_mask = x_mask[:, :, ::s0][:, :, :x.shape[-1]]
+        x = self.wn(x * x_mask, x_mask, g) * x_mask
+        x = conv_nct_ragged(x, self.out_proj.weight, self.out_proj.bias, 1, 1, 0, 1, 1.0, enc)
+        p, n = self.poolings, enc
+        for i, bn in ((0, p[2]), (3, p[5]), (6, None)):
+            x = conv_nct_ragged(x, p[i].weight, p[i].bias, 3, 2, 0, 1, 0.0 if bn is not None else 1.0, n)
+            n = n.map(lambda k: (k - 3) // 2 + 1)
+            if bn is not None:
+                x = self._bn_eval(bn, x).contiguous()
+        B, L = x.shape[0], self.latent_channels
+        eps = torch.randn(B, L, 1, device=x.device) if eps is None else eps.float().contiguous()
+        m, logs, z = (torch.empty(B, L, 1, device=x.device) for _ in range(3))
+        _native.check(_native.lib().svb_global_latent_head_ragged(
+            _native.ptr(x.contiguous()), B, L, x.shape[-1], enc.c_host, _native.ptr(enc.dev), _native.ptr(eps), _native.ptr(m),
+            _native.ptr(logs), _native.ptr(z), _native.current_stream_ptr(x.device)), 'global_latent_head_ragged')
+        return z, m, logs, x_mask
+
 
 class GlobalFVAE(nn.Module):
     """``modules/voice_conversion/vae_models.py:130-146`` (GlobalFVAE over TMPFVAE :11-52, FVAE fs2_vae.py:155-178) without the
@@ -449,20 +476,25 @@ class GlobalFVAE(nn.Module):
         self.decoder = GlobalFVAEDecoder(latent_size, hidden_channels, in_out_channels, kernel_size, dec_n_layers, gin_channels,
                                          strides=strides, precision=precision, trainable=trainable)
 
-    def forward(self, x=None, x_mask=None, g=None, infer=False, eps=None):
-        from neuralsvb_b200.modules.hifigan.discriminators import conv_nct
+    def forward(self, x=None, x_mask=None, g=None, infer=False, eps=None, lens=None):
+        """``lens`` (vc_modules.FrameLens of the mel frames; inference, infer=False): every clip from its own frames only (see
+        MleSVBVAE.forward), x_mask then the lengths' mask."""
+        from neuralsvb_b200.modules.hifigan.discriminators import conv_nct, conv_nct_ragged
         if not infer:
             check_frames(g.shape[-1], self.strides[0])
         g_sqz = g
         for c in self.g_pre_net:                                                                        # vae_models.py:20
-            g_sqz = conv_nct(g_sqz.float(), c.weight, c.bias, c.kernel_size[0], stride=c.stride[0], pad=c.padding[0])
+            if lens is None:
+                g_sqz = conv_nct(g_sqz.float(), c.weight, c.bias, c.kernel_size[0], stride=c.stride[0], pad=c.padding[0])
+            else:
+                g_sqz = conv_nct_ragged(g_sqz.float(), c.weight, c.bias, c.kernel_size[0], c.stride[0], c.padding[0], 1, 1.0, lens)
         if infer:                                                                                       # :45-52
             # the reference samples [B, latent, T / 4] here and its GlobalFVAEDecoder then repeats that T / 4 times (a shape
             # error: the SVB task never takes this branch, it calls vae_model.decoder directly, svb_vae.py:303); a GLOBAL
             # latent has one time step
             z_p = torch.randn(g_sqz.shape[0], self.latent_size, 1, device=g.device) if eps is None else eps
             return self.decoder(z_p, 1, g), z_p
-        z_q, m_q, logs_q, x_mask_sqz = self.encoder(x, x_mask, g_sqz, eps=eps)                          # :22
+        z_q, m_q, logs_q, x_mask_sqz = self.encoder(x, x_mask, g_sqz, eps=eps, lens=lens)               # :22
         x_recon = self.decoder(z_q, x_mask, g)                                                          # :23
         # validate_args=False: the argument check of torch.distributions is a device -> host synchronisation per call
         q_dist = torch.distributions.Normal(m_q, logs_q.exp(), validate_args=False)

@@ -186,6 +186,37 @@ class _TcConvFn(torch.autograd.Function):
         return dx, dw, db, None, None, None, None, None, None, None, None
 
 
+def conv_tc_ragged(x, w, b, layer, K, pad, slope, lens):
+    """Stride-1 dense conv through the tensor-core layer handle on a ragged batch (inference): clip b is x[b][:, :n_b], frames past
+    it absent; ``lens`` (vc_modules.FrameLens) holds n_b.  Output frames past n_b are zeros."""
+    lib = _native.lib()
+    x, w, b = _cuda(x), _cuda(w), _cuda(b)
+    B, Cin, T = x.shape
+    with torch.cuda.device(x.device):
+        st = _native.current_stream_ptr(x.device)
+        h = layer.get(Cin, w.shape[0], K, 1, pad, x.device)
+        _tc_sync_weight(layer, h, w, b, st)
+        y = torch.empty((B, w.shape[0], T), device=x.device, dtype=torch.float32)
+        _native.check(lib.svb_tc_layer_forward_ragged(h, _native.ptr(x), B, T, lens.c_host, _native.ptr(lens.dev), ctypes.c_float(slope),
+                                                      _native.ptr(y), st), 'tc_layer_forward_ragged')
+    return y
+
+
+def conv_nct_ragged(x, w, b, K, stride, pad, groups, slope, lens):
+    """conv_nct on a ragged batch (inference): clip b is x[b][:, :n_b] (``lens``), its output (n_b + 2 pad - K) // stride + 1
+    frames, zeros after them."""
+    x = _cuda(x)
+    B, Cin, Tin = x.shape
+    Tout = (Tin + 2 * pad - (K - 1) - 1) // stride + 1
+    y = torch.empty((B, w.shape[0], Tout), device=x.device, dtype=torch.float32)
+    with torch.cuda.device(x.device):
+        _native.check(_native.lib().svb_conv_nct_forward_ragged(_native.ptr(x), _native.ptr(_cuda(w)), _native.ptr(_cuda(b)), _native.ptr(y),
+                                                                B, Cin, w.shape[0], Tin, K, stride, 1, pad, groups, ctypes.c_float(slope),
+                                                                lens.c_host, _native.ptr(lens.dev), _native.current_stream_ptr(x.device)),
+                      'conv_nct_forward_ragged')
+    return y
+
+
 def _conv_nct_raw(x, w, b, K, stride=1, dil=1, pad=0, groups=1, slope=1.0, W=1):
     lib = _native.lib()
     x = _cuda(x)

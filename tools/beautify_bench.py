@@ -147,11 +147,31 @@ def copies(b, args):
                 'small': int(sum(1 for x in v if x < 1 << 20))} for d, v in res.items()}
 
 
+def time_modes(b, run, repeats):
+    """The acoustic_model stage (device ms) and the whole call (s) of ``run(batch_invariant)``, default and length-aware
+    alternated, after one warm-up call of each."""
+    out = {'default': {'acoustic_model_ms': [], 'call_s': []}, 'batch_invariant': {'acoustic_model_ms': [], 'call_s': []}}
+    b.timing = True
+    for mode in (False, True):
+        run(mode)
+    for _ in range(repeats):
+        for mode, key in ((False, 'default'), (True, 'batch_invariant')):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            run(mode)
+            out[key]['call_s'].append(round(time.perf_counter() - t0, 3))
+            out[key]['acoustic_model_ms'].append(round(b.stage_ms['acoustic_model'], 2))
+    b.timing = False
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--pairs', type=int, default=64)
     ap.add_argument('--repeats', type=int, default=3)
     ap.add_argument('--out', type=str, default='')
+    ap.add_argument('--modes', action='store_true',
+                    help='also time the acoustic model in both modes (batch_invariant False / True), alternated in this process')
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit('beautify_bench measures on a CUDA device; none is visible')
@@ -179,12 +199,17 @@ def main():
         stages = b.stage_ms
         b.timing = False
         cp = copies(b, call)
+        modes = time_modes(b, lambda m: b.beautify_batch(*call, seed=1, eps=eps, batch_invariant=m), args.repeats) if args.modes else None
     t1, t0 = float(np.median(one)), float(np.median(old))
     res = {'card': card(), 'pairs': N, 'input_audio_s': round(audio_s, 1), 'repeats': args.repeats,
            'one_call_s': [round(x, 3) for x in one], 'existing_route_s': [round(x, 3) for x in old],
            'one_call_pairs_per_s': round(N / t1, 2), 'one_call_audio_s_per_s': round(audio_s / t1, 1),
            'existing_pairs_per_s': round(N / t0, 2), 'existing_audio_s_per_s': round(audio_s / t0, 1),
            'stage_ms': {k: round(v, 2) for k, v in stages.items()}, 'copies': cp}
+    if modes:
+        res['modes'] = modes
+        for k, v in modes.items():
+            print(f"  acoustic model, {k:15s}: {v['acoustic_model_ms']} ms (calls {v['call_s']} s)")
     print(f"card: {res['card']}")
     print(f"{N} pairs, {audio_s:.1f} s of input audio (both takes), median of {args.repeats}")
     print(f"  one call      {t1:8.3f} s   {N / t1:7.2f} pairs/s   {audio_s / t1:8.1f} audio-s/s")

@@ -77,11 +77,31 @@ def dtw_us_per_step(srcs, tgts, cells=None):
     return r.stage_ms, 1e3 * r.stage_ms[2] / steps
 
 
+def time_modes(b, run, repeats):
+    """The acoustic_model stage (device ms) and the whole call (s) of ``run(batch_invariant)``, default and length-aware
+    alternated, after one warm-up call of each."""
+    out = {'default': {'acoustic_model_ms': [], 'call_s': []}, 'batch_invariant': {'acoustic_model_ms': [], 'call_s': []}}
+    b.timing = True
+    for mode in (False, True):
+        run(mode)
+    for _ in range(repeats):
+        for mode, key in ((False, 'default'), (True, 'batch_invariant')):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            run(mode)
+            out[key]['call_s'].append(round(time.perf_counter() - t0, 3))
+            out[key]['acoustic_model_ms'].append(round(b.stage_ms['acoustic_model'], 2))
+    b.timing = False
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--songs', type=int, default=4)
     ap.add_argument('--repeats', type=int, default=2)
     ap.add_argument('--out', type=str, default='')
+    ap.add_argument('--modes', action='store_true',
+                    help='also time the acoustic model in both modes (batch_invariant False / True), alternated in this process')
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit('song_bench measures on a CUDA device; none is visible')
@@ -105,6 +125,10 @@ def main():
         b.beautify_songs(*call, seed=1, eps=eps)
         stages, align_ms, plans = b.stage_ms, b.align_ms, b.song_plans
         b.timing = False
+        if args.modes:
+            res['modes'] = time_modes(b, lambda m: b.beautify_songs(*call, seed=1, eps=eps, batch_invariant=m), args.repeats)
+            for k, v in res['modes'].items():
+                print(f"  acoustic model, {k:15s}: {v['acoustic_model_ms']} ms (calls {v['call_s']} s)")
         # the songs' f0 as the call aligns it: each song alone on the cluster kernel
         f0_dev, f0s = b._pitch(*_front(b, call))
         frames = [len(f) for f in f0s]
